@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- BASELINE.json's metric on B200: decode tokens/s + RTF, Voxtral-Mini-4B Q4_0, 16 s audio.
+"""bench.py -- BASELINE.json's metric on H100: decode tokens/s + RTF, Voxtral-Mini-4B Q4_0, 16 s audio.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--streams B] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--streams B] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Workload (config.workload): BASELINE.json configs[4] -- concurrent 16 s streams, B=8 per GPU
@@ -16,6 +16,9 @@ call (pinned host PCM in, token ids out, copies inside the timed region).
 Weights are synthetic (random Q4_0 blocks with the real tensor names/shapes: no checkpoint exists
 offline) and the audio is a synthetic speech-like signal; token-count, shapes and bytes moved are
 identical to the real model's (the decode loop never stops at EOS).
+`--dump-outputs DIR`: after the timed steps, the token ids the timed calls returned in their last step are written as
+float64 `.npy` files (ids.npy: device-resident input, ids_e2e.npy: host-buffer call, ids_single_stream.npy: one
+stream); weights and audio are seeded, so two builds run with the same arguments can be compared output for output.
 
 `--impl reference`: the reference has no CPU backend and cannot be built here (Rust, SURVEY F1-F2),
 so the reference arm times the oracle port (oracle/: C q4 matvec with OpenMP on all host cores +
@@ -95,7 +98,7 @@ def measured_peaks():
             return json.load(open(p)), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return {"hbm_gbs": 6650.0}, "fallback (B200_PROFILING.md)"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet (700 W), not measured"
 
 
 def ensure_gguf(rank: int, barrier):
@@ -114,7 +117,7 @@ def make_audio(n_streams: int, rank: int) -> np.ndarray:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -284,6 +287,14 @@ def streaming_leg(vx, model, audio, B, max_ticks=260):
         pool.close()
 
 
+def dump_outputs(out_dir: str, rank: int, arrays: dict):
+    """Writes each array as <out_dir>/<name>.npy in float64 (token ids are exact there); ranks > 0 add a _rank<r> suffix."""
+    os.makedirs(out_dir, exist_ok=True)
+    sfx = f"_rank{rank}" if rank else ""
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}{sfx}.npy"), np.asarray(a, dtype=np.float64))
+
+
 # --------------------------------------------------------------------------------------------
 def run_ours(args, rank, local_rank, world):
     import voxtral_mini_realtime_rs_b200 as vx
@@ -329,7 +340,7 @@ def run_ours(args, rank, local_rank, world):
     wall0 = time.perf_counter()
     dec_ms = pre_ms = enc_ms = tot_ms = pf_ms = 0.0
     for _ in range(args.steps):
-        model.transcribe_pcm_dev(dev_audio, B, n, timings=tm)
+        ids = model.transcribe_pcm_dev(dev_audio, B, n, timings=tm)
         dec_ms += tm.decode_ms; pre_ms += tm.preprocess_ms; enc_ms += tm.encode_ms; tot_ms += tm.total_ms
         pf_ms += tm.prefill_ms
     vx.lib().vox_dev_sync(local_rank)
@@ -361,7 +372,7 @@ def run_ours(args, rank, local_rank, world):
         model.transcribe_pcm_dev(dev_audio, 1, n, timings=tm1)
     s_dec = s_tot = s_pf = 0.0
     for _ in range(K):
-        model.transcribe_pcm_dev(dev_audio, 1, n, timings=tm1)
+        ids_single = model.transcribe_pcm_dev(dev_audio, 1, n, timings=tm1)
         s_dec += tm1.decode_ms; s_tot += tm1.total_ms; s_pf += tm1.prefill_ms
     s_step_ms = (s_dec - s_pf) / K / max(n_tok - 1, 1)
     # single-stream end to end through the host-buffer C ABI (pinned PCM in, ids out)
@@ -371,6 +382,8 @@ def run_ours(args, rank, local_rank, world):
     for _ in range(K):
         model.transcribe_pcm(pinned.array[0], timings=tm1)
     s_e2e_wall = time.perf_counter() - e1
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, rank, {"ids": ids, "ids_e2e": ids_e2e, "ids_single_stream": ids_single})
     single = {"decode_tokens_per_sec": n_tok * K / (s_dec / 1e3), "rtf": (s_tot / K / 1e3) / AUDIO_SECONDS,
               "e2e": {"tokens_per_sec": n_tok * K / s_e2e_wall, "rtf": (s_e2e_wall / K) / AUDIO_SECONDS,
                       "h2d_bytes_per_step": int(n * 4), "d2h_bytes_per_step": int(n_tok * 4),
@@ -391,7 +404,7 @@ def run_ours(args, rank, local_rank, world):
             ms = vx.q4_matmul_bench(ws, 1, iters=480, warmup=48)
             mv_bytes = nn * kk * 18 // 32 + 4 * kk + 4 * nn
             mv[f"n{nn}"] = {"shape": f"[1,3072]x[{nn},3072]^T", "ms": ms, "bytes": mv_bytes, "gbs": mv_bytes / ms / 1e6,
-                            "l2": f"24 rotating weight copies ({24 * mv_bytes / 1e6:.0f} MB) > 126 MB L2"}
+                            "l2": f"24 rotating weight copies ({24 * mv_bytes / 1e6:.0f} MB) > 50 MB L2"}
             del ws
         mv.update(mv["n9216"])      # top-level keys = the reference's shape (as in round 1)
     except Exception as e:  # pragma: no cover
@@ -411,17 +424,8 @@ def run_ours(args, rank, local_rank, world):
     peaks, peak_src = measured_peaks()
     step_bytes = int(info["decode_step_bytes"])
     achieved = step_bytes / (step_ms_loop / 1e3) / 1e9
-    traffic = None
-    prof = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(prof):
-        try:
-            traffic = json.load(open(prof)).get("decode_step_dram_bytes")
-        except Exception:
-            traffic = None
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                "frac": achieved / peaks["hbm_gbs"], "traffic": traffic,
-                "traffic_source": "static: profiles/traffic.json (ncu --set full capture of this kernel; not re-measured in this run)",
-                "peak_source": peak_src,
+                "frac": achieved / peaks["hbm_gbs"], "peak_source": peak_src,
                 "launch": f"one decode step for B={B} streams = one launch of the persistent decode kernel (CUDA-graph replay)",
                 "algorithmic_bytes_per_launch": step_bytes, "ms_per_launch": step_ms_loop,
                 "single_stream": {"achieved": step_bytes / (s_step_ms / 1e3) / 1e9,
@@ -447,7 +451,7 @@ def run_ours(args, rank, local_rank, world):
                    "model": "Voxtral-Mini-4B-Realtime Q4_0 GGUF layout, synthetic weights (seed 42)",
                    "audio_seconds": AUDIO_SECONDS, "streams_per_gpu": B, "tokens_per_stream": int(n_tok),
                    "parallelism": f"replicas x{world}, no data-path collective",
-                   "l2": "decode reads 1.93 GB of weights per step >> 126 MB L2 (no flush needed)"},
+                   "l2": "decode reads 1.93 GB of weights per step >> 50 MB L2 (no flush needed)"},
         "rtf": (tot_s / K) / AUDIO_SECONDS, "rtf_per_stream_amortised": (tot_s / K) / (AUDIO_SECONDS * B),
         "stage_ms": {"preprocess": pre_ms / K, "encode": enc_ms / K, "decode": dec_ms / K, "prefill": pf_ms / K},
         "wall_s_timed_region": wall_s, "model_load_s": load_s,
@@ -457,10 +461,10 @@ def run_ours(args, rank, local_rank, world):
         "gpu_launches": int(launches), "clocks": clocks, "roofline": roofline, "cpu_baseline": cpu,
         "single_stream": single, "streaming": streaming,
         # SURVEY 8(d) config 3: encoder + adapter of the same streams, algorithmic 1.235 TFLOP per 16 s stream
-        # (f32-equivalent; the tcgen05 GEMM spends 5 bf16 MMAs per product for f32-grade accuracy)
+        # (f32-equivalent; the wgmma GEMM spends 3 f16 MMAs per product for f32-grade accuracy)
         "encoder": {"ms": enc_ms / K, "algorithmic_tflop": 1.235 * B,
                     "tflops": 1.235 * B / (enc_ms / K / 1e3) if enc_ms > 0 else None,
-                    "frac_of_bf16_dense_peak": (1.235 * B / (enc_ms / K / 1e3)) / peaks.get("bf16_tflops", 1700.9) if enc_ms > 0 else None},
+                    "frac_of_bf16_dense_peak": (1.235 * B / (enc_ms / K / 1e3)) / peaks.get("bf16_tflops", 989.0) if enc_ms > 0 else None},
     }
     print(json.dumps(line), flush=True)
     if dist is not None:
@@ -477,7 +481,13 @@ def main():
     ap.add_argument("--cpu-tokens", type=int, default=6)
     ap.add_argument("--no-streaming", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the timed path's outputs of its last step as DIR/<name>.npy (float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs applies to the GPU path only (--impl ours)")
     rank, local_rank, world = dist_env()
     if args.impl == "reference":
         run_reference(args, rank, world)

@@ -1,6 +1,6 @@
 /* voxtral.h -- C ABI of libvoxtral_b200.so
  *
- * B200-native (sm_100a) replacement for the Q4_0 GGUF hot path of
+ * H100-native (sm_90a) replacement for the Q4_0 GGUF hot path of
  * TrevorS/voxtral-mini-realtime-rs.  The reference exposes no C FFI; its seams are the Rust
  * functions cited beside each entry point below (paths relative to the reference repo).  A Rust
  * `extern "C"` binding for this header is shown in INTEGRATION.md.
@@ -14,7 +14,7 @@
  *     (NULL = the handle's own stream).
  *   - thread-compatibility: one thread per handle at a time; different sessions may run
  *     concurrently (they own their stream, KV cache and workspace).
- *   - there is NO CPU fallback: every compute entry point fails with VOX_ECUDA if no sm_100
+ *   - there is NO CPU fallback: every compute entry point fails with VOX_ECUDA if no sm_90
  *     device / driver is available.
  */
 #ifndef VOXTRAL_H
@@ -118,7 +118,7 @@ int32_t vox_q4_matmul_host(const vox_q4 *w, const float *x, float *y, int32_t b,
                            const float *bias /* nullable */);
 void vox_q4_tensor_free(vox_q4 *w);
 /* kernel selection of the operator seam (bit mask, default 0): bit 0 = SIMT warp-reduce matvec instead of
- * the tensor-core-assisted one (M <= 8); bit 1 = SIMT tiled GEMM instead of the tcgen05 GEMM (M > 8).
+ * the tensor-core-assisted one (M <= 8); bit 1 = SIMT tiled GEMM instead of the wgmma GEMM (M > 8).
  * All implement the same contract; exposed for A/B measurement and parity tests. */
 int32_t vox_q4_set_matvec_mode(int32_t mode);
 

@@ -1,6 +1,6 @@
 """All-CTA phase trace of the persistent decode-step kernel: skew vs fixed cost per phase.
 
-    VOX_MEGA_TRACE_ALL=1 python scripts/mega_trace_all.py [--streams B]      (GPU box)
+    VOX_MEGA_TRACE_ALL=1 python scripts/mega_trace_all.py [--streams B] [--save trace.npy]
 
 Every CTA stamps (SM clock) op start / first weights ready (or KV walk start) / body done / barrier passed; the CTAs are
 aligned on their exit from the first grid barrier (they leave it within one L2 round trip of each other).  Per op class:
@@ -26,6 +26,7 @@ GGUF = os.environ.get("VOX_BENCH_GGUF", "/dev/shm/voxtral_synth_s42.gguf")
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--streams", type=int, default=8)
+    ap.add_argument("--save", metavar="NPY", default=None, help="also write the raw trace [CTA][op][4] here")
     args = ap.parse_args()
     if not os.path.exists(GGUF):
         synth.write_synthetic_gguf(GGUF, synth.VoxtralConfig(), seed=42)
@@ -37,9 +38,8 @@ def main():
     model.transcribe_pcm(audio, timings=tm)
     model.transcribe_pcm(audio, timings=tm)
     tr = model.debug("mega_trace_all")
-    grid = 148
-    tr = tr.reshape(grid, -1, 4)
-    n = tr.shape[1]
+    n = 1 + 5 * model.info["dec_layers"] + 2         # embed, 5 phases per layer, lm_head, argmax
+    tr = tr.reshape(-1, n, 4)                        # one row per CTA: the grid is one CTA per SM of this device
     per_layer = ["qkv", "attn", "wo", "w13", "w2"]
     names = ["embed"] + per_layer * ((n - 3) // len(per_layer)) + ["lm_head", "argmax"]
     step = (tm.decode_ms - tm.prefill_ms) / max(1, tm.decode_tokens - 1)
@@ -47,7 +47,8 @@ def main():
     # SM clocks are not mutually synchronised (and drift): every CTA is measured against ITS OWN exit from the previous
     # grid barrier -- all CTAs leave a barrier within one L2 round trip of each other, so these offsets are comparable.
     agg = {}
-    np.save(os.path.join(ROOT, "gpurun_out", f"mega_trace_all_b{B}.npy"), tr)
+    if args.save:
+        np.save(args.save, tr)
     for i, nm in enumerate(names):
         start, done, exit_, ready = tr[:, i, 0], tr[:, i, 1], tr[:, i, 2], tr[:, i, 3]
         prev = tr[:, i - 1, 2] if i > 0 else start

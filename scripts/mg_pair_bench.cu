@@ -2,7 +2,7 @@
 // m16n8k16 + unpack + scale FMAs) timed in isolation: operands resident in shared memory, no TMA ring, no mbarriers,
 // 1 CTA per SM.  Cycles per call and warp for 4/8/16 resident warps and with parts of the body removed -- which pipe (or
 // which latency) sets the ~1300 cycles per ring stage seen in the kernel's warp trace?
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o mg_pair_bench mg_pair_bench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o mg_pair_bench mg_pair_bench.cu
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -121,14 +121,16 @@ template <int MODE>
 void run(const char *name) {
     unsigned long long *d;
     float *sink;
-    cudaMalloc(&d, 8 * 148 * 32);
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    cudaMalloc(&d, 8 * (size_t)sms * 32);
     cudaMalloc(&sink, 4);
     const int iters = 2000;
     const int smem = 4 * 2 * SLOT + 16 * 2 * 16 * MT * 8 + 16 * 2 * MT * 8;
     cudaFuncSetAttribute(body_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     printf("%-58s", name);
     for (int warps : {4, 8, 16}) {
-        body_kernel<MODE><<<148, warps * 32, smem>>>(d, iters, sink, 0);
+        body_kernel<MODE><<<sms, warps * 32, smem>>>(d, iters, sink, 0);
         cudaDeviceSynchronize();
         unsigned long long h[32];
         cudaMemcpy(h, d, sizeof(h), cudaMemcpyDeviceToHost);

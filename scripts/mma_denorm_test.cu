@@ -3,7 +3,7 @@
 //       A Q4 nibble n sitting in the low bits of a 16-bit lane is the f16 subnormal n * 2^-24
 //       (and n << 4 is 16 n * 2^-24), i.e. nibbles can feed the MMA with one LOP3 per two weights.
 //   (2) same with bf16 inputs built by the 0x4300|n magic (128 + n).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -o mma_denorm_test mma_denorm_test.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -o mma_denorm_test mma_denorm_test.cu
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cstdint>

@@ -1,6 +1,6 @@
-// mma_rate_bench.cu -- issue rate of the LEGACY warp-level MMA instructions on sm_100a (they are what the decode matvec's
+// mma_rate_bench.cu -- issue rate of the LEGACY warp-level MMA instructions on sm_90a (they are what the decode matvec's
 // arithmetic runs on): per SM sub-partition, cycles per instruction with 1..8 resident warps and 4 independent
-// accumulator chains per warp.  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o mma_rate_bench mma_rate_bench.cu
+// accumulator chains per warp.  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o mma_rate_bench mma_rate_bench.cu
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
@@ -49,15 +49,17 @@ __global__ void rate_kernel(unsigned long long *out, int iters, float *sink) {
 template <int KIND>
 void run(const char *name, int macs) {
     unsigned long long *d; float *sink;
-    cudaMalloc(&d, 8 * 148); cudaMalloc(&sink, 4);
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    cudaMalloc(&d, 8 * (size_t)sms); cudaMalloc(&sink, 4);
     const int iters = 4096;
     printf("%-28s", name);
     for (int warps : {4, 8, 16, 32}) {    // per CTA (1 CTA per SM): 1, 2, 4, 8 warps per sub-partition
-        rate_kernel<KIND><<<148, warps * 32>>>(d, iters, sink);
+        rate_kernel<KIND><<<sms, warps * 32>>>(d, iters, sink);
         cudaDeviceSynchronize();
-        unsigned long long h[148];
-        cudaMemcpy(h, d, sizeof(h), cudaMemcpyDeviceToHost);
-        double cyc = (double)h[0];
+        unsigned long long h0 = 0;   // CTA 0's cycle count
+        cudaMemcpy(&h0, d, sizeof(h0), cudaMemcpyDeviceToHost);
+        double cyc = (double)h0;
         const double per_smsp = (double)iters * 4 * (warps / 4);       // instructions issued per sub-partition
         printf("  %2d w/SMSP: %6.2f cyc/instr (%5.0f MAC/clk/SM)", warps / 4, cyc / per_smsp, macs * per_smsp * 4 / cyc);
     }

@@ -1,5 +1,5 @@
-"""Key metrics of an ncu report as a small CSV (runs here, no GPU):  python scripts/ncu_key.py rep.ncu-rep > profiles/x_ncu_key.csv
-Also summarises an `ncu --csv --log-file` launch list:               python scripts/ncu_key.py --launches launches.csv > profiles/y_summary.csv"""
+"""Key metrics of an ncu report as a small CSV (no GPU needed):  python scripts/ncu_key.py rep.ncu-rep > x_ncu_key.csv
+Also summarises an `ncu --csv --log-file` launch list:          python scripts/ncu_key.py --launches launches.csv > y_summary.csv"""
 import collections
 import csv
 import io

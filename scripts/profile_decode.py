@@ -1,7 +1,7 @@
 """Profiling harness: one single-stream (or B-stream) full transcribe on the full-size synthetic
-model, with the CUDA profiler API bracketing only the region of interest.  Meant to run under
-`ncu --profile-from-start off ...` (see scripts/gpu_profile.sh); numbers printed while under a
-profiler are never bench values.
+model, with the CUDA profiler API bracketing only the region of interest.  Meant to run under a
+profiler that honours cudaProfilerStart/Stop; numbers printed while under a profiler are never
+bench values.
 
     python scripts/profile_decode.py [--streams B] [--region decode|encode|all] [--eager]
 """

@@ -1,9 +1,9 @@
 """Per-kernel SASS evidence of the in-tree library (runs without a GPU):
 
-    python scripts/sass_summary.py > profiles/sass_r02.txt
+    python scripts/sass_summary.py > sass_summary.txt
 
-Counts, for every kernel in libvoxtral_b200.so (sm_100a only), the mnemonics B200_PROFILING.md names as proof of a
-Blackwell-native path: UTC*MMA (tcgen05.mma), LDTM/STTM (tcgen05.ld/st), UBLKCP (cp.async.bulk), UTMALDG/UTMASTG
+Counts, for every kernel in libvoxtral_b200.so (sm_90a only), the mnemonics that are proof of a
+Hopper-native path: HGMMA (wgmma), UBLKCP (cp.async.bulk), UTMALDG/UTMASTG
 (cp.async.bulk.tensor), HMMA (legacy mma.sync), plus registers per thread from the ELF.
 """
 import collections
@@ -14,7 +14,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "voxtral_mini_realtime_rs_b200", "libvoxtral_b200.so")
-KEYS = ["UTCHMMA", "UTCQMMA", "UTCIMMA", "UTCOMMA", "LDTM", "STTM", "UBLKCP", "UTMALDG", "UTMASTG", "UTCBAR", "HMMA", "IMMA", "SYNCS", "LDGSTS", "REDG", "ATOMG"]
+KEYS = ["HGMMA", "UBLKCP", "UTMALDG", "UTMASTG", "HMMA", "IMMA", "SYNCS", "LDGSTS", "REDG", "ATOMG"]
 
 
 def demangle(names):

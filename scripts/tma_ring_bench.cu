@@ -2,7 +2,7 @@
 // one producer thread streaming a large buffer through a ring of `nstage` stages (each filled by `ncopy`
 // cp.async.bulk copies), 16 consumer warps that only wait for a stage and release it (no arithmetic).
 // Tells which ring geometry the HBM stream needs, independent of the MMA loop.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tma_ring_bench tma_ring_bench.cu && ./tma_ring_bench
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tma_ring_bench tma_ring_bench.cu && ./tma_ring_bench
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>

@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     config.addinivalue_line("markers", "slow: long-running (full-size model)")
 
 
@@ -35,6 +35,15 @@ def tiny_gguf(tmp_path_factory):
     from oracle import gguf_synth
     p = str(tmp_path_factory.mktemp("gguf") / "tiny.gguf")
     gguf_synth.write_synthetic_gguf(p, gguf_synth.VoxtralConfig.tiny(), seed=3)
+    return p
+
+
+@pytest.fixture(scope="session")
+def full_gguf(tmp_path_factory):
+    """The full-size synthetic model (seed 42, 2.5 GB; the weights bench.py runs), written once per session."""
+    from voxtral_mini_realtime_rs_b200 import synth
+    p = str(tmp_path_factory.mktemp("gguf_full") / "voxtral_synth_s42.gguf")
+    synth.write_synthetic_gguf(p, synth.VoxtralConfig(), seed=42)
     return p
 
 

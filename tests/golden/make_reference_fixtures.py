@@ -1,11 +1,11 @@
-"""Pins the oracle to the REFERENCE'S OWN Python (run in the build container, where /root/reference exists):
+"""Pins the oracle to the REFERENCE'S OWN Python (needs a checkout of the reference crate):
 
-    python tests/golden/make_reference_fixtures.py [--full]
+    VOX_REFERENCE_DIR=<reference checkout> python tests/golden/make_reference_fixtures.py [--full]
 
 The reference validates its Rust layers against `.npy` files produced by its torch scripts
 (rms_norm.rs:156-211, rope.rs:168-253, swiglu.rs:100-187, conv.rs:113-215, rms_norm.rs:214-291,
 attention.rs:476-619, mel.rs:486-614).  Those scripts are imported here UNMODIFIED from
-/root/reference/scripts and run on our synthetic weights (dequantised to f32, served through a
+the reference's scripts/ directory and run on our synthetic weights (dequantised to f32, served through a
 `get_tensor` shim in place of `safe_open(consolidated.safetensors)`):
 
   A  ref_ops.npz       reference_forward.py  test_rms_norm / test_rope / test_swiglu / test_conv /
@@ -23,7 +23,7 @@ attention.rs:476-619, mel.rs:486-614).  Those scripts are imported here UNMODIFI
 
 Stored: inputs, reference outputs (or row subsets + checksums for the big ones).  Consumers:
 tests/test_oracle_vs_reference_py.py (CPU: oracle == reference Python) and tests/test_reference_py_gpu.py
-(-m gpu: CUDA == reference Python).  /root/reference is NOT needed to run those tests.
+(-m gpu: CUDA == reference Python).  The reference checkout is NOT needed to run those tests.
 """
 import ast
 import contextlib
@@ -42,7 +42,7 @@ from oracle import gguf_synth, mel as omel, q4 as oq4  # noqa: E402
 from voxtral_mini_realtime_rs_b200 import synth       # noqa: E402
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF_SCRIPTS = "/root/reference/scripts"
+REF_SCRIPTS = os.path.join(os.environ.get("VOX_REFERENCE_DIR", ""), "scripts")
 SEED_FULL = 42
 SEED_SMALL = 11
 AUDIO_SECONDS = 1.0

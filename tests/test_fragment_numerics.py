@@ -93,7 +93,7 @@ def test_tiny_and_huge_magnitudes():
 
 
 def test_gemm_f16_two_by_two_split_three_products():
-    """numpy model of the tcgen05 GEMM's operand split (csrc/gemm_tc5.cu, round 2): weights (q-8)*d*2^8 as f16 hi + the
+    """numpy model of the wgmma GEMM's operand split (csrc/gemm_tc5.cu): weights (q-8)*d*2^8 as f16 hi + the
     exact f16 residual, activations * 2^s_t as f16 hi + mid, products w_hi x_h + w_hi x_m + w_lo x_h in f64 (the MMA
     accumulates in f32).  Error relative to sum |w||x| stays at the f32 rounding level even with outlier activations and
     tiny / large block scales -- i.e. 3 MMAs per k-step carry f32-grade accuracy (round 1 spent 5 on bf16 pieces)."""

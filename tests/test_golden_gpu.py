@@ -17,7 +17,6 @@ from voxtral_mini_realtime_rs_b200 import synth
 
 pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
-FULL_GGUF = os.environ.get("VOX_BENCH_GGUF", "/dev/shm/voxtral_synth_s42.gguf")
 
 
 NEAR_TIE = 2e-3     # f32 summation-order noise on logits of O(1)
@@ -86,10 +85,8 @@ def test_tiny_golden(vx, tmp_path):
 
 
 @pytest.fixture(scope="module")
-def full_model(vx):
-    if not os.path.exists(FULL_GGUF):
-        synth.write_synthetic_gguf(FULL_GGUF, synth.VoxtralConfig(), seed=42)
-    m = vx.Q4ModelLoader.from_file(FULL_GGUF).load(0, max_batch=8, max_mel_frames=2400)
+def full_model(vx, full_gguf):
+    m = vx.Q4ModelLoader.from_file(full_gguf).load(0, max_batch=8, max_mel_frames=2400)
     yield m
     m.close()
 
@@ -136,14 +133,14 @@ def test_full_size_golden_16s_second_utterance(vx, full_model):
 
 
 @pytest.mark.slow
-def test_full_size_vs_live_oracle_3s(vx, full_model):
+def test_full_size_vs_live_oracle_3s(vx, full_model, full_gguf):
     """The oracle run live on the box's host cores (3 s audio -> 27 tokens): encoder hidden states
     and audio embeds within 1e-3 (north_star bound), ids per the near-tie rule."""
     from oracle import mel as omel
     from oracle.model import OracleModel
     audio = synth.speechlike(3.0, seed=77)
     mel = omel.mel_tensor_from_audio(omel.peak_normalize(audio))
-    om = OracleModel(FULL_GGUF)
+    om = OracleModel(full_gguf)
     cap, info = {}, {}
     emb = om.encode_audio(mel, cap)
     toks = om.transcribe_streaming(mel, omel.time_embedding(6.0, 3072), audio_embeds=emb, info=info)

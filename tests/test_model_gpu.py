@@ -181,8 +181,9 @@ def test_transcribe_pcm_pipeline_and_batch(vx, tiny_model, tiny_oracle):
 
 
 def test_batches_above_eight_streams(vx, tiny_gguf, tiny_oracle):
-    """More than 8 streams per GPU leave the persistent decode kernel (token capacity 8) for the per-op path whose
-    linears are the tcgen05 GEMM (M = B > 8 rows) -- same ids as the oracle, graph replay == eager."""
+    """More than 8 streams per GPU: each decode step runs the persistent decode kernel (token capacity 8) over
+    consecutive groups of up to 8 rows, and the prefill's linears (B x 38 rows) are the wgmma GEMM -- same ids as the
+    oracle, graph replay == eager."""
     m = vx.Q4ModelLoader.from_file(tiny_gguf).load(0, max_batch=20, max_mel_frames=1500)
     try:
         sigs = [omel.speechlike(3.0, seed=300 + i) for i in range(20)]

@@ -197,7 +197,7 @@ def test_tokenizer_semantics():           # mod.rs:170-208 (+ tests 216-270 with
 def test_tokenizer_reference_golden_if_available():        # mod.rs:255-268 (needs the real tekken.json)
     import os
     import pytest
-    p = os.environ.get("VOXTRAL_TEKKEN_JSON", "/root/reference/models/voxtral/tekken.json")
+    p = os.environ.get("VOXTRAL_TEKKEN_JSON", "models/voxtral/tekken.json")
     if not os.path.exists(p):
         pytest.skip("real tekken.json not available offline (SURVEY F3)")
     t = otok.VoxtralTokenizer.from_file(p)

@@ -1,7 +1,7 @@
-"""oracle/ == the REFERENCE'S OWN torch scripts (CPU; no GPU, no /root/reference needed at run time).
+"""oracle/ == the REFERENCE'S OWN torch scripts (CPU; no GPU, and no checkout of the reference needed at run time).
 
 The fixtures under tests/golden/ref_*.npz were produced by tests/golden/make_reference_fixtures.py, which imports,
-unmodified, /root/reference/scripts/{reference_forward,generate_padded_reference,compare_full_forward}.py -- the scripts
+unmodified, the reference's scripts/{reference_forward,generate_padded_reference,compare_full_forward}.py -- the scripts
 that write the `.npy` files the reference's Rust layer tests load (rms_norm.rs:156-211, rope.rs:168-253,
 swiglu.rs:100-187, conv.rs:113-215, rms_norm.rs:214-291, attention.rs:476-619, mel.rs:486-614) -- and runs them on
 our synthetic weights.  The Rust tests accept 1e-3 (mel: 1e-2) against those files; the oracle is held to 1e-5 per op
@@ -22,7 +22,6 @@ from voxtral_mini_realtime_rs_b200 import synth
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLD = os.path.join(HERE, "golden")
 ENC0 = f"{synth.ENC}.transformer.layers.0"
-FULL_GGUF = os.environ.get("VOX_BENCH_GGUF", "/dev/shm/voxtral_synth_s42.gguf")
 
 
 def maxdiff(a, b):
@@ -134,9 +133,8 @@ def test_chain_small_matches_reference_py():
 
 
 @pytest.mark.slow
-@pytest.mark.skipif(not os.path.exists(FULL_GGUF), reason="full-size synthetic GGUF not generated (tests/test_golden_gpu.py does it on the GPU box)")
-def test_chain_full_matches_reference_py():
+def test_chain_full_matches_reference_py(full_gguf):
     fx = np.load(os.path.join(GOLD, "ref_chain_full.npz"))
-    om = OracleModel(FULL_GGUF)
+    om = OracleModel(full_gguf)
     r = _check_chain(om, fx, False, tol_mel=2e-4, tol_act=2e-4, tol_logit=1e-3)
     print("oracle vs reference python (full):", r)

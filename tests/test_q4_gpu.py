@@ -18,7 +18,7 @@ pytestmark = pytest.mark.gpu
 
 @pytest.fixture(autouse=True, params=["tc", "simt"])
 def matvec_mode(request, vx):
-    """Every test runs with both kernel families: tensor-core paths (mma.sync matvec for M<=8, tcgen05
+    """Every test runs with both kernel families: tensor-core paths (mma.sync matvec for M<=8, wgmma
     GEMM for M>8; default) and the SIMT matvec / SIMT tiled GEMM."""
     assert vx.lib().vox_q4_set_matvec_mode(3 if request.param == "simt" else 0) == 0
     yield request.param
@@ -116,8 +116,8 @@ def test_q4_matmul_all_m_random_blocks(vx, m):
 
 @pytest.mark.parametrize("m,n,k", [(130, 256, 1280), (586, 1280, 2048), (38, 384, 3072), (257, 128, 64)])
 def test_q4_gemm_large_m_accuracy(vx, m, n, k):
-    """Encoder / prefill sized GEMMs (N % 128 == 0, K % 64 == 0 => tcgen05 path in 'tc' mode): the
-    3x2 bf16 split keeps f32-grade accuracy (error ~ f32 summation-order noise, far below 1e-3)."""
+    """Encoder / prefill sized GEMMs (N % 128 == 0, K % 64 == 0 => wgmma path in 'tc' mode): the
+    2x2 f16 split keeps f32-grade accuracy (error ~ f32 summation-order noise, far below 1e-3)."""
     rng = np.random.default_rng(m + n)
     raw = np.empty((n * k // 32, 18), np.uint8)
     raw[:, :2] = rng.uniform(0.002, 0.02, n * k // 32).astype(np.float16).view(np.uint8).reshape(-1, 2)

@@ -1,5 +1,5 @@
 """CUDA path == the REFERENCE'S OWN torch scripts (fixtures tests/golden/ref_*.npz, generator
-tests/golden/make_reference_fixtures.py: /root/reference/scripts/{reference_forward,generate_padded_reference,
+tests/golden/make_reference_fixtures.py: the reference's scripts/{reference_forward,generate_padded_reference,
 compare_full_forward}.py run unmodified on our synthetic weights).  Everything through the C ABI.
 
 Bounds: north_star -- encoder hidden states / audio embeddings within 1e-3 abs; logits of O(1) within 2e-3
@@ -16,7 +16,6 @@ from voxtral_mini_realtime_rs_b200 import synth
 pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLD = os.path.join(HERE, "golden")
-FULL_GGUF = os.environ.get("VOX_BENCH_GGUF", "/dev/shm/voxtral_synth_s42.gguf")
 ENC0 = f"{synth.ENC}.transformer.layers.0"
 
 
@@ -75,11 +74,9 @@ def test_chain_small_vs_reference_py(vx):
 
 
 @pytest.mark.slow
-def test_chain_full_vs_reference_py(vx):
+def test_chain_full_vs_reference_py(vx, full_gguf):
     fx = np.load(os.path.join(GOLD, "ref_chain_full.npz"))
-    if not os.path.exists(FULL_GGUF):
-        synth.write_synthetic_gguf(FULL_GGUF, synth.VoxtralConfig(), seed=42)
-    model = vx.Q4ModelLoader.from_file(FULL_GGUF).load(0, max_batch=1, max_mel_frames=1000)
+    model = vx.Q4ModelLoader.from_file(full_gguf).load(0, max_batch=1, max_mel_frames=1000)
     try:
         _check_chain(vx, model, fx, False, "full-size seed-42 model")
     finally:

@@ -1,4 +1,4 @@
-"""voxtral_mini_realtime_rs_b200 -- B200-native (sm_100a) Q4_0 Voxtral-Mini-4B streaming-ASR hot path.
+"""voxtral_mini_realtime_rs_b200 -- H100-native (sm_90a) Q4_0 Voxtral-Mini-4B streaming-ASR hot path.
 
 Host-side mirror (ctypes over the C ABI in ``include/voxtral.h``) of the reference crate's public
 surface for this path (TrevorS/voxtral-mini-realtime-rs, ``src/lib.rs:22-39``):

@@ -1,9 +1,9 @@
-"""In-tree build of libvoxtral_b200.so (sm_100a only; nvcc cross-compiles without a GPU).
+"""In-tree build of libvoxtral_b200.so (sm_90a only: H100; nvcc cross-compiles without a GPU).
 
     python -m voxtral_mini_realtime_rs_b200.build [--force]
 
 Objects are cached under csrc/build/ by source mtime; the shared library lands next to this
-file so that it travels with the repo snapshot to the GPU box (it is git-ignored).
+file, so the package imports from the source tree (both are git-ignored).
 """
 from __future__ import annotations
 
@@ -19,8 +19,8 @@ LIB = os.path.join(HERE, "libvoxtral_b200.so")
 
 CU_SOURCES = ["kernels.cu", "matvec_tc.cu", "decode_attn.cu", "decode_mega.cu", "enc_attn_tc.cu", "gemm_tc5.cu", "model.cu", "stream.cu", "capi.cu"]
 CXX_SOURCES = ["gguf.cpp", "audio_host.cpp", "tokenizer.cpp"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
-              "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=default"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=default"]
 CXX_FLAGS = ["-O2", "-std=c++17", "-fPIC", "-Wall"]
 # extra nvcc flags for instrumented builds (e.g. VOX_NVCC_EXTRA="-DVOX_MEGA_WARP_TRACE"); rebuild with force=True
 NVCC_FLAGS += os.environ.get("VOX_NVCC_EXTRA", "").split()
@@ -66,8 +66,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     with ThreadPoolExecutor(max_workers=min(len(names), os.cpu_count() or 4)) as ex:
         objs = list(ex.map(lambda n: _compile(n, force), names))
     if force or _stale(LIB, objs):
-        cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a",
-                                                        "-lcudart_static", "-ldl", "-lrt", "-lpthread"]
+        cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ARCH + ["-lcudart_static", "-ldl", "-lrt", "-lpthread"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed: {' '.join(cmd)}\n{r.stdout}\n{r.stderr}")

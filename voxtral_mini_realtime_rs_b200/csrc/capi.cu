@@ -60,9 +60,9 @@ struct vox_q4 {
     float *x = nullptr, *y = nullptr, *bias = nullptr;  // scratch for the host-buffer call
     size_t x_cap = 0, y_cap = 0;
     TcWork wk;  // split-K scratch of the tensor-core matvec (allocated with the tensor)
-    void *xt = nullptr;  // split tiles for the tcgen05 GEMM (M > 8)
+    void *xt = nullptr;  // split tiles for the wgmma GEMM (M > 8)
     size_t xt_elems = 0;
-    GemmWork gw;  // split-K scratch of the tcgen05 GEMM (allocated on first use)
+    GemmWork gw;  // split-K scratch of the wgmma GEMM (allocated on first use)
 };
 struct vox_model { Model *m; };
 struct vox_session { Session *s; };
@@ -339,7 +339,7 @@ static void q4_matmul_dispatch(const Q4Weight &w, const float *x, float *y, int 
             h->xt_elems = need;
         }
         if (!h->gw.partial) {
-            h->gw.partial_floats = (size_t)148 * 128 * 128;
+            h->gw.partial_floats = (size_t)VOX_NUM_SMS * 128 * 128;
             h->gw.partial = h->arena.alloc_n<float>(h->gw.partial_floats);
             h->gw.n_counters = 128;
             h->gw.counters = h->arena.alloc_n<int>(h->gw.n_counters);

@@ -2,9 +2,8 @@
 // (reference src/gguf/model.rs:938-960 generate_step: embed(prev token) + audio[pos], 26 decoder
 // layers forward_with_cache (model.rs:125-197, 250-255, 665-677), tied lm_head (680-691), argmax).
 //
-// Why: as separate launches the step is 134 dependent kernels of ~11 us each whose weight streams
-// last 1-5 us (profiles/README.md, r01b): launch gaps, per-kernel activation staging and CTA-wide
-// barriers dominate.  Here one CTA per SM lives for the whole step:
+// Why: as separate launches the step is 134 dependent kernels whose weight streams each last only a
+// few microseconds: launch gaps, per-kernel activation staging and CTA-wide barriers dominate.  Here one CTA per SM lives for the whole step:
 //
 //   * 20 warps in three roles: 16 consumer warps (the weight stream's arithmetic, attention, embedding), and one
 //     warpgroup of helpers: the producer warp and 3 epilogue warps.  The launch gives every thread 96 registers;
@@ -405,8 +404,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
     // Register split (the launch gives every thread 96: 640 threads x 96 = 61440 of the SM's 65536).  The kernel keeps the
     // operand fragments of the weight loop, the epilogue's prefetched operands and the op parameters live at once; at 96
     // registers that spills, and with 227 KB of the SM's 256 KB configured as shared memory there is next to no L1 left to
-    // catch local-memory traffic: every spill reload is an L2 round trip (a build with a 256-byte frame ran the step in
-    // 3.08 ms instead of 2.27).  The producer needs few registers, the three filler warps none.
+    // catch local-memory traffic: every spill reload is an L2 round trip.  The producer needs few registers, the three filler warps none.
     // =========================== producer: the step's whole weight schedule ===========================
     if (warp >= MG_CWARPS) {
         asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(MG_REGS_PRODUCER));
@@ -780,7 +778,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                     const int np = min(Ps, n_pairs - pb);
                     // The fragments land in up to 4 K chunks (whole ring stages of 16 pairs), each with its own barrier: the
                     // first tile group starts on chunk 0 while the rest of the copy is still in flight (the copy is L2-bandwidth
-                    // bound: all 148 CTAs fetch the same 70-104 KB).
+                    // bound: all 132 CTAs fetch the same 70-104 KB).
                     const int CP = 16 * ((((np + 15) >> 4) + 3) >> 2);  // pairs per chunk
                     cbar();  // every warp is done with the previous contents of scratch (and has seen all its chunks)
                     if (tid == 0) {
@@ -802,7 +800,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                     stg_phase ^= 1u;
                     // row statistics of the fused RMSNorm (first used by the epilogue).  The partial sums live as
                     // [part][8 tokens]: warps 1..4 read them with coalesced loads (lane % 8 = token).  (One warp per token reading
-                    // its column cost 2048 sector requests per CTA for the same 6 KB, by all 148 CTAs at once: the normed phases'
+                    // its column cost 2048 sector requests per CTA for the same 6 KB, by all 132 CTAs at once: the normed phases'
                     // staging was ~1 us longer than the others'.)
                     if (s == 0 && has_norm && warp >= 1 && warp <= 4) {
                         const int total = op.ssq_in_parts * 8;
@@ -921,8 +919,8 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
             }
         } else if (kind == MG_ATTN) {
             // unit = (stream, kv head, key chunk): the 4 query heads of a GQA group share one pass over their
-            // chunk of K and V; the chunks' softmax states are combined by the last chunk's CTA (tagged words, below).  (One CTA
-            // per (stream, kv head) walked all keys in ~17 us -- issue-bound -- while 140 SMs waited.)
+            // chunk of K and V; the chunks' softmax states are combined by the last chunk's CTA (tagged words, below).  (With
+            // one CTA per (stream, kv head), a few CTAs walk all keys -- issue-bound -- while the other SMs wait.)
             float *qs = reinterpret_cast<float *>(scratch);       // [G][HD]
             float *kvs = qs + G * HD;                              // [2][HD]
             float *red_m = kvs + 2 * HD;                           // [MG_CWARPS][G]

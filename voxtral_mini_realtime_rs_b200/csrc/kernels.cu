@@ -1,4 +1,4 @@
-// kernels.cu -- sm_100a kernels for the Voxtral Q4_0 hot path (f32 arithmetic throughout, like the
+// kernels.cu -- sm_90a kernels for the Voxtral Q4_0 hot path (f32 arithmetic throughout, like the
 // reference's WGSL/Burn path).  Reference semantics cited per kernel; none of this is derived from
 // the reference's shaders beyond the arithmetic they define.
 #include "kernels.h"
@@ -213,7 +213,7 @@ static void matvec_launch_t(const Q4Weight &w, const float *x, float *y, int ldy
     smem_attr_check(ensure_dyn_smem(q4_matvec_kernel<M, EPI>, 100 * 1024, attr), "q4_matvec");
     const int n_rg = (w.N + MV_ROWS - 1) / MV_ROWS;
     int grid = n_rg;
-    if (n_chunks == 1 && grid > 148 * 8) grid = 148 * 8;
+    if (n_chunks == 1 && grid > VOX_NUM_SMS * 8) grid = VOX_NUM_SMS * 8;
     q4_matvec_kernel<M, EPI><<<grid, MV_THREADS, smem, st>>>(w.qs, w.d, w.N, w.K, x, y, ldy, bias, res, kcb, n_chunks);
     post_launch("q4_matvec");
 }

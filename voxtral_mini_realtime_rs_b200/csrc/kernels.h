@@ -1,4 +1,4 @@
-// kernels.h -- host-callable launchers for the sm_100a kernels (all asynchronous on `st`).
+// kernels.h -- host-callable launchers for the sm_90a kernels (all asynchronous on `st`).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -8,6 +8,9 @@
 #include <cstdint>
 
 namespace vox {
+
+// SMs of the target GPU (H100 SXM): sizes grids and the split-K scratch of the GEMMs
+constexpr int VOX_NUM_SMS = 132;
 
 // Opt-in to more than 48 KB of dynamic shared memory.  The attribute is per (function, DEVICE), and the C ABI takes a
 // device index, so one process can drive several GPUs: remember what was set per device (not per process), with
@@ -106,10 +109,10 @@ void launch_dec_attn_fused(float *qkv, int B, int ld, int H, int Hkv, int hd, co
 // y[M,N] = A[M,K] . W^T for any M (encoder / prefill): tiled SIMT GEMM, in-tile dequant.
 void launch_q4_gemm(const Q4Weight &w, const float *a, int M, float *y, int ldy, const float *bias,
                     const float *res, int epi, cudaStream_t st);
-// tcgen05 path (gemm_tc5.cu): X is first split into three bf16 pieces laid out as UMMA operand tiles
+// wgmma path (gemm_tc5.cu): X is first split into two f16 pieces laid out as wgmma operand tiles
 // (optionally through RMSNorm), then Y = X . W^T with f32-grade accuracy on the tensor cores.
 bool gemm_tc5_supported(const Q4Weight &w, int M);
-size_t gemm_tc5_split_elems(int M, int K);  // bf16 elements needed for the split buffer
+size_t gemm_tc5_split_elems(int M, int K);  // f16 elements needed for the split buffer
 void launch_split_tiles(const float *x, int M, int K, const float *gamma, const float *ada, float eps, void *xt,
                         cudaStream_t st);
 // Caller-owned scratch for the GEMM's deterministic split-K (used when N/128 x M/128 tiles cannot fill the GPU)

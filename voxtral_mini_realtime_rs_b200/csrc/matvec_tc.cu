@@ -3,11 +3,12 @@
 // (+ ADA scale) of its input, weights streamed by TMA bulk copies, deterministic split-K.
 //
 // Why: the SIMT kernel (kernels.cu K2) needs ~4 issue slots per weight (SHF, LOP3, I2FP, FFMA);
-// B200 streams 11.7 T weights/s from HBM (6.58 TB/s / 0.5625 B) but issues only ~36 T lane-instr/s,
-// so a SIMT single-token decode can not be HBM-bound (profiles/README.md).  Here a Q4 nibble n
-// reaches the MMA as the f16 *subnormal* n * 2^-24 (nibble in bits 0-3 of a 16-bit lane) or
-// 16 n * 2^-24 (bits 4-7): one LOP3 isolates two weights, no int->float conversion, no multiply
-// (scripts/mma_denorm_test.cu verifies on hardware that HMMA treats these inputs exactly).
+// by the data sheet an H100 SXM streams ~6 T weights/s from HBM (3.35 TB/s / 0.5625 B) and issues ~33 T
+// lane-instr/s (132 SMs x 128 lanes x 1.98 GHz), so a SIMT single-token decode is issue-bound, not HBM-bound,
+// as soon as anything else shares the issue slots.  Here a Q4 nibble n reaches the MMA as the f16 *subnormal*
+// n * 2^-24 (nibble in bits 0-3 of a 16-bit lane) or 16 n * 2^-24 (bits 4-7): one LOP3 isolates two weights,
+// no int->float conversion, no multiply (scripts/mma_denorm_test.cu verifies on hardware that HMMA treats these
+// inputs exactly).
 // Same arithmetic as the reference (src/gguf/shader.wgsl:96-127), re-associated:
 //
 //   y[m,n] = sum_b d[n,b] * ( sum_{k in b} q[n,k] x[m,k]  -  8 sum_{k in b} x[m,k] )
@@ -467,10 +468,10 @@ void tc_launch_t(TcArgs a, const TcWork *wk, cudaStream_t st) {
     // give each CTA enough tiles to amortise it while keeping ~4 CTAs per SM in flight
     if (M > 2) {
         const int ctas = env_ctas > 0 ? env_ctas : 4;
-        const int tg_occ = (int)(((size_t)a.n_tiles * S + 148 * ctas - 1) / (148 * ctas));
+        const int tg_occ = (int)(((size_t)a.n_tiles * S + VOX_NUM_SMS * ctas - 1) / (VOX_NUM_SMS * ctas));
         if (tg_occ > TG) TG = tg_occ > 16 ? 16 : tg_occ;
     }
-    while (TG > 1 && (size_t)((a.n_tiles + TG - 1) / TG) * S < 2 * 148) --TG;
+    while (TG > 1 && (size_t)((a.n_tiles + TG - 1) / TG) * S < 2 * VOX_NUM_SMS) --TG;
     const int nbuf = TG > 1 ? 2 : 1;
     const size_t misc = (12 + TC_WARPS * M + TC_WARPS * 16 * M + 2 * 16 * M) * sizeof(float);
     const size_t act = misc + (size_t)Ps * 2 * M * sizeof(float2) + (size_t)Ps * 2 * 2 * 2 * M * 4 * sizeof(uint2);

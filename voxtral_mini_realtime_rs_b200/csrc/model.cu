@@ -448,7 +448,7 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames) {
         s->d_tok = s->arena.alloc_n<int>(B);
         s->d_ids = s->arena.alloc_n<int>(drows);
         s->d_out = s->arena.alloc_n<int>(B * s->out_ld);
-        {   // split-tile buffer of the tcgen05 GEMM: largest (rows, K) pair it is used with
+        {   // split-tile buffer of the wgmma GEMM: largest (rows, K) pair it is used with
             const int rows_e = max_batch * s->S_max, rows_d = max_batch * s->M_max;
             size_t e = 0;
             for (int K : {c.enc_dim, c.enc_heads * c.enc_head_dim, c.enc_ffn}) e = std::max(e, gemm_tc5_split_elems(rows_e, K / 64 * 64));
@@ -456,8 +456,8 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames) {
             for (int K : {c.dec_dim, c.dec_heads * c.dec_head_dim, c.dec_ffn}) e = std::max(e, gemm_tc5_split_elems(std::max(rows_d, max_batch * std::max(s->S4_max, 1)), K / 64 * 64));
             s->xt_elems = e;
             s->xt_buf = s->arena.alloc(e * 2);
-            // split-K scratch of the tcgen05 GEMM: at most 148 (slice, tile) partial tiles in flight
-            s->gemm_work.partial_floats = (size_t)148 * 128 * 128;
+            // split-K scratch of the wgmma GEMM: at most one (slice, tile) partial tile per SM in flight
+            s->gemm_work.partial_floats = (size_t)VOX_NUM_SMS * 128 * 128;
             s->gemm_work.partial = s->arena.alloc_n<float>(s->gemm_work.partial_floats);
             s->gemm_work.n_counters = 128;
             s->gemm_work.counters = s->arena.alloc_n<int>(s->gemm_work.n_counters);
@@ -846,8 +846,8 @@ bool Session::mega_prepare(int B) {
 void Session::decode_step(int B, bool add_audio) {
     const vox_model_info &c = m->info;
     // More than 8 rows: the rows are independent streams, so the step runs as consecutive launches of the persistent
-    // kernel over groups of 8 rows (each group streams the weights once: ~2.3 ms per 8 rows, against ~12 ms for one
-    // pass of the per-op tcgen05 GEMMs at 16-32 rows -- profiles/README.md).  The scratch activations are reused by the
+    // kernel over groups of 8 rows (each group streams the weights once; the per-op GEMMs would pad 16-32 rows to a
+    // 128-token tile).  The scratch activations are reused by the
     // groups; the per-row state (token, positions, page table, audio row, output row, logits) is addressed from the
     // group's first row.
     const int rows_per_launch = B > 8 ? 8 : B;
@@ -897,7 +897,7 @@ void Session::decode_step_mega(int b0, int B, bool add_audio) {
         p.attn_out = attn_dec;
         // key chunks per (stream, kv head): spread the KV walk over idle SMs, but no more than 4 -- the merging CTA waits
         // for the other chunks' states one after the other (an L2 round trip each), and a CTA walks 64 keys per round
-        // trip anyway: 16 chunks made a single stream's attention phase slower than 4 (12.1 vs ~9 us at 16 s contexts)
+        // trip anyway, so more chunks add merge latency without shortening the walk
         p.attn_chunks = std::max(1, std::min(4, std::min(mega_grid, mega_att_units - 8 * c.dec_kv_heads) / (B * c.dec_kv_heads)));
         {
             static const int env_nc = getenv("VOX_MEGA_NC") ? atoi(getenv("VOX_MEGA_NC")) : 0;

@@ -136,7 +136,7 @@ struct Session {
     // persistent decode-step kernel (decode_mega.cu): op table per batch size, grid barrier words,
     // per-CTA argmax candidates.  VOX_MEGA=0 (or debug "mega_off") selects the per-op launches.
     bool use_mega = true;
-    int mega_min_B = 1;  // (round 1: a single stream was slightly faster through the per-op launches; no longer -- profiles/README.md)
+    int mega_min_B = 1;  // smallest batch that uses the persistent kernel (every batch size does)
     int mega_B = 0, mega_grid = 0, mega_n_ops = 0, mega_ops_cap = 0;
     MegaPlan mega_plan;
     std::vector<MegaOp> mega_ops_host;
@@ -158,12 +158,12 @@ struct Session {
     bool mega_prepare(int B);
     bool fused_decode(int rows) const;
     void decode_step_mega(int b0, int B, bool add_audio);
-    void *xt_buf = nullptr;   // bf16 split tiles feeding the tcgen05 GEMM
+    void *xt_buf = nullptr;   // f16 split tiles feeding the wgmma GEMM
     size_t xt_elems = 0;
-    GemmWork gemm_work;       // split-K scratch of the tcgen05 GEMM
+    GemmWork gemm_work;       // split-K scratch of the wgmma GEMM
     bool use_enc_attn_tc = true;  // tensor-core encoder attention (VOX_ENC_ATTN=simt disables)
-    bool use_gemm_tc = true;  // tcgen05 GEMM for M > 8 (VOX_GEMM=simt disables)
-    // y = epi(norm(x) . W^T): RMSNorm fused into the operand split when the tcgen05 path applies,
+    bool use_gemm_tc = true;  // wgmma GEMM for M > 8 (VOX_GEMM=simt disables)
+    // y = epi(norm(x) . W^T): RMSNorm fused into the operand split when the wgmma path applies,
     // else rmsnorm into `tmp` + linear()
     void linear_n(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias, const float *res, int epi,
                   const float *gamma, const float *ada, float *tmp);
