@@ -44,7 +44,7 @@ def rope_tables(head_dim: int, max_seq: int, theta: float = 1e6):
 
 
 def apply_rope(x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, offset: int) -> torch.Tensor:
-    """rope.rs:103-141.  x [S, H, hd] interleaved pairs."""
+    """rope.rs:103-141.  x [S, H, hd] interleaved pairs; cos/sin in x's dtype."""
     s, h, hd = x.shape
     xp = x.reshape(s, h, hd // 2, 2)
     xr, xi = xp[..., 0], xp[..., 1]
@@ -61,23 +61,36 @@ def rms_norm(x: torch.Tensor, gamma: torch.Tensor, eps: float) -> torch.Tensor:
 
 
 class OracleModel:
-    def __init__(self, gguf, threads: int = 0, exact_order_max_m: int = 8):
+    """`dtype=torch.float64` runs the decoder side (forward_streaming from given audio embeddings: embed_tokens,
+    ada_scales, every linear, RMSNorm, RoPE, attention and softmax, lm_head) in float64 -- a high-precision reference
+    for the f32 GPU path.  The Q4 weights dequantise exactly to f32 and are cast per call (the f32 dequantisations
+    are cached, never f64 copies); the RoPE tables are the f32 tables cast, as the product uses f32 tables too.  The
+    default float32 mode is unchanged."""
+
+    def __init__(self, gguf, threads: int = 0, exact_order_max_m: int = 8, dtype: torch.dtype = torch.float32):
         self.g = gguf if isinstance(gguf, GgufFile) else GgufFile(gguf)
         self.cfg: VoxtralConfig = self.g.config()
         self.threads = threads
         self.exact_order_max_m = exact_order_max_m
+        assert dtype in (torch.float32, torch.float64), dtype
+        self.dtype = dtype
         c = self.cfg
         self.enc_cos, self.enc_sin = rope_tables(c.enc_head_dim, 4096, c.rope_theta)
         self.dec_cos, self.dec_sin = rope_tables(c.dec_head_dim, 16384, c.rope_theta)
+        self.dec_cos, self.dec_sin = self.dec_cos.to(dtype), self.dec_sin.to(dtype)
         self._f32 = {}
         self._deq = {}
-        self.cache_dequant = False
+        self.cache_dequant = dtype == torch.float64
 
     # ---- primitives -------------------------------------------------------
     def f32(self, name) -> torch.Tensor:
         if name not in self._f32:
             self._f32[name] = torch.from_numpy(self.g.f32(name))
         return self._f32[name]
+
+    def param(self, name) -> torch.Tensor:
+        """f32 tensor `name` in the model's dtype."""
+        return self.f32(name).to(self.dtype)
 
     def has(self, name) -> bool:
         return self.g.info(name) is not None
@@ -90,7 +103,7 @@ class OracleModel:
         x2 = x.reshape(-1, k).contiguous()
         m = x2.shape[0]
         raw = self.g.raw(wname)
-        if m <= self.exact_order_max_m:
+        if m <= self.exact_order_max_m and self.dtype == torch.float32:
             y = torch.from_numpy(q4.q4_matmul_c(x2.numpy(), raw, n, k, threads=self.threads))
         else:
             if wname in self._deq:
@@ -99,9 +112,9 @@ class OracleModel:
                 w = torch.from_numpy(q4.dequantize_c(raw)).reshape(n, k)
                 if self.cache_dequant:
                     self._deq[wname] = w
-            y = x2 @ w.t()
+            y = x2.to(self.dtype) @ w.to(self.dtype).t()
         if bname is not None and self.has(bname):
-            y = y + self.f32(bname)
+            y = y + self.param(bname)
         return y.reshape(*lead, n)
 
     # ---- encoder ----------------------------------------------------------
@@ -125,7 +138,7 @@ class OracleModel:
         scores = torch.matmul(qh, kh.transpose(1, 2)) * scale    # [H,Sq,Skv]
         i = torch.arange(sq)[:, None] + q_offset
         j = torch.arange(skv)[None, :]
-        mask = torch.zeros(sq, skv)
+        mask = torch.zeros(sq, skv, dtype=scores.dtype)
         if causal:
             mask = mask.masked_fill(j > i, float("-inf"))
         if window is not None:
@@ -259,7 +272,7 @@ class OracleModel:
     # ---- decoder ----------------------------------------------------------
     def ada_scales(self, t_embed: np.ndarray):
         """Q4AdaRmsNorm (model.rs:250-255): 1 + w2(gelu(w0(t))) per layer (t constant)."""
-        t = torch.from_numpy(np.ascontiguousarray(t_embed, np.float32)).reshape(1, -1)
+        t = torch.from_numpy(np.ascontiguousarray(t_embed, np.float32)).reshape(1, -1).to(self.dtype)
         out = []
         for j in range(self.cfg.dec_layers):
             s = self.linear(t, f"layers.{j}.ada_rms_norm_t_cond.0.weight")
@@ -272,7 +285,7 @@ class OracleModel:
         dt, (v, d), _ = self.g.info(TOK_EMB)
         raw = self.g.raw(TOK_EMB).reshape(v, d // 32 * 18)
         rows = [torch.from_numpy(q4.dequantize_q4_0(raw[int(i)])) for i in ids]
-        return torch.stack(rows)
+        return torch.stack(rows).to(self.dtype)
 
     def new_cache(self):
         return [dict(k=None, v=None) for _ in range(self.cfg.dec_layers)]
@@ -285,7 +298,7 @@ class OracleModel:
         for j in range(c.dec_layers):
             p = f"layers.{j}"
             off = 0 if cache[j]["k"] is None else cache[j]["k"].shape[0]
-            h = rms_norm(x, self.f32(f"{p}.attention_norm.weight"), c.norm_eps)
+            h = rms_norm(x, self.param(f"{p}.attention_norm.weight"), c.norm_eps)
             q = self.linear(h, f"{p}.attention.wq.weight").reshape(m, c.dec_heads, c.dec_head_dim)
             k = self.linear(h, f"{p}.attention.wk.weight").reshape(m, c.dec_kv_heads, c.dec_head_dim)
             v = self.linear(h, f"{p}.attention.wv.weight").reshape(m, c.dec_kv_heads, c.dec_head_dim)
@@ -298,14 +311,14 @@ class OracleModel:
                 cache[j]["v"] = torch.cat([cache[j]["v"], v])
             a = self._attention(q, cache[j]["k"], cache[j]["v"], scale, off, c.dec_window)
             x = self.linear(a, f"{p}.attention.wo.weight") + x
-            h = rms_norm(x, self.f32(f"{p}.ffn_norm.weight"), c.norm_eps)
+            h = rms_norm(x, self.param(f"{p}.ffn_norm.weight"), c.norm_eps)
             h = h * ada[j]
             gate = F.silu(self.linear(h, f"{p}.feed_forward.w1.weight"))
             up = self.linear(h, f"{p}.feed_forward.w3.weight")
             x = self.linear(gate * up, f"{p}.feed_forward.w2.weight") + x
             if capture is not None:
                 capture[f"dec{j}"] = x.clone()
-        return rms_norm(x, self.f32(FINAL_NORM), c.norm_eps)
+        return rms_norm(x, self.param(FINAL_NORM), c.norm_eps)
 
     def decoder_forward_batched(self, x: torch.Tensor, ada, caches, rows_per_stream: int = 1) -> torch.Tensor:
         """forward_hidden_with_cache (model.rs:665-677) for B independent streams in ONE weight sweep: x
@@ -319,7 +332,7 @@ class OracleModel:
         scale = float(np.float32(c.dec_head_dim) ** np.float32(-0.5))
         for j in range(c.dec_layers):
             p = f"layers.{j}"
-            h = rms_norm(x, self.f32(f"{p}.attention_norm.weight"), c.norm_eps)
+            h = rms_norm(x, self.param(f"{p}.attention_norm.weight"), c.norm_eps)
             q = self.linear(h, f"{p}.attention.wq.weight")
             k = self.linear(h, f"{p}.attention.wk.weight")
             v = self.linear(h, f"{p}.attention.wv.weight")
@@ -335,11 +348,11 @@ class OracleModel:
                 cache[j]["v"] = vb if off == 0 else torch.cat([cache[j]["v"], vb])
                 outs.append(self._attention(qb, cache[j]["k"], cache[j]["v"], scale, off, c.dec_window))
             x = self.linear(torch.cat(outs), f"{p}.attention.wo.weight") + x
-            h = rms_norm(x, self.f32(f"{p}.ffn_norm.weight"), c.norm_eps) * ada[j]
+            h = rms_norm(x, self.param(f"{p}.ffn_norm.weight"), c.norm_eps) * ada[j]
             gate = F.silu(self.linear(h, f"{p}.feed_forward.w1.weight"))
             up = self.linear(h, f"{p}.feed_forward.w3.weight")
             x = self.linear(gate * up, f"{p}.feed_forward.w2.weight") + x
-        return rms_norm(x, self.f32(FINAL_NORM), c.norm_eps)
+        return rms_norm(x, self.param(FINAL_NORM), c.norm_eps)
 
     def lm_head(self, h: torch.Tensor) -> torch.Tensor:
         """model.rs:680-691 (tied embeddings)."""
@@ -353,7 +366,7 @@ class OracleModel:
         audio = self.encode_audio(mel) if audio_embeds is None else audio_embeds
         ids = list(token_ids)
         assert len(ids) == audio.shape[0]
-        x = audio + self.embed_tokens(ids)
+        x = torch.as_tensor(audio).to(self.dtype) + self.embed_tokens(ids)
         hidden = self.decoder_forward_with_cache(x, self.ada_scales(t_embed), self.new_cache())
         logits = self.lm_head(hidden)
         return (logits, hidden) if return_hidden else logits

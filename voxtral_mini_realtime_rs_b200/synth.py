@@ -262,6 +262,16 @@ def refshape_config() -> VoxtralConfig:
     return VoxtralConfig(enc_ffn=512, dec_ffn=512, vocab=4096)
 
 
+def decoder_geometry_config(dec_window: int = 8192) -> VoxtralConfig:
+    """The production decoder layer (3072, 32:8 x 128 heads, FFN 9216) at 2 layers, a 32768-token vocabulary and the
+    tiny encoder: every decoder matvec, attention shape and persistent-kernel plan (K slices, 2048 lm_head tiles) is the
+    full model's, at a size a CPU reference can follow step by step.  `dec_window` makes the decoder's sliding window
+    small enough to bite within a few seconds of audio."""
+    t = VoxtralConfig.tiny()
+    return VoxtralConfig(enc_dim=t.enc_dim, enc_layers=t.enc_layers, enc_heads=t.enc_heads, enc_head_dim=t.enc_head_dim,
+                         enc_ffn=t.enc_ffn, enc_window=t.enc_window, dec_layers=2, dec_window=dec_window, vocab=32768)
+
+
 def build_aliased_gguf_bytes(cfg: VoxtralConfig, seed: int, unique: int = 2) -> bytes:
     """In-memory GGUF whose layers i >= `unique` alias the bytes of layer i % unique (several names, one offset
     in the tensor index -- legal GGUF), so a full-depth model costs `unique` layers of bytes and of generation
