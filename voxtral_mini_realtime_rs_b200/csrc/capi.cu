@@ -287,15 +287,8 @@ int32_t vox_q4_tensor_create(const uint8_t *bytes, size_t nbytes, int64_t n, int
     q->device = device;
     q->arena.device = device;
     q->w = upload_q4(q->arena, {bytes}, {(int)n}, (int)k, false, true);
-    {   // split-K scratch: up to ceil(K/64/16) slices x 8 rows x padded N, and one ticket per row tile
-        const int n_tiles = (int)((n + 15) / 16), n_pairs = (int)((k / 32 + 1) / 2);
-        const size_t S = (size_t)(n_pairs + 15) / 16;
-        q->wk.partial_floats = S * 8 * (size_t)n_tiles * 16;
-        q->wk.partial = q->arena.alloc_n<float>(q->wk.partial_floats);
-        q->wk.n_counters = n_tiles;
-        q->wk.counters = q->arena.alloc_n<int>(n_tiles);
-        CUDA_OK(cudaMemset(q->wk.counters, 0, sizeof(int) * n_tiles));
-    }
+    q->wk = q4_matvec_tc_work_size(q->w.N, q->w.K);
+    alloc_split_k(q->arena, q->wk);
     *out = q.release();
     VOX_API_END
 }
@@ -327,37 +320,28 @@ int32_t vox_q4_tensor_dequantize(const vox_q4 *w, float *out) {
     }
     VOX_API_END
 }
-// 0 = tensor-core-assisted matvec for M <= 8 (default), 1 = SIMT warp-reduce matvec
-static int g_matvec_mode = (getenv("VOX_MATVEC") && std::string(getenv("VOX_MATVEC")) == "simt") ? 1 : 0;
-static void q4_matmul_dispatch(const Q4Weight &w, const float *x, float *y, int rows, const float *bias, cudaStream_t st,
-                               const TcWork *wk = nullptr, vox_q4 *h = nullptr) {
-    const bool simt = (g_matvec_mode & 1) != 0;
-    if (rows > 8 && h && !(g_matvec_mode & 2) && gemm_tc5_supported(w, rows)) {
-        const size_t need = gemm_tc5_split_elems(rows, w.K);
+// kernel choice of the Q4 operator, process-wide and separate from the sessions' (vox_q4_set_matvec_mode)
+static Q4Path g_q4_path = {!(getenv("VOX_MATVEC") && std::string(getenv("VOX_MATVEC")) == "simt"), true};
+// the handle's scratch for a call over `rows` rows, the wgmma split buffer grown first to what they need
+static Q4Scratch q4_scratch(vox_q4 *h, int rows) {
+    if (rows > 8) {  // only M > 8 can take the wgmma GEMM
+        const size_t need = gemm_tc5_split_elems(rows, h->w.K);
         if (need > h->xt_elems) {
             h->xt = h->arena.alloc(need * 2);
             h->xt_elems = need;
         }
         if (!h->gw.partial) {
-            h->gw.partial_floats = (size_t)VOX_NUM_SMS * 128 * 128;
-            h->gw.partial = h->arena.alloc_n<float>(h->gw.partial_floats);
-            h->gw.n_counters = 128;
-            h->gw.counters = h->arena.alloc_n<int>(h->gw.n_counters);
-            CUDA_OK(cudaMemset(h->gw.counters, 0, sizeof(int) * h->gw.n_counters));
+            h->gw = gemm_tc5_work_size();
+            alloc_split_k(h->arena, h->gw);
         }
-        launch_split_tiles(x, rows, w.K, nullptr, nullptr, 0.0f, h->xt, st);
-        launch_q4_gemm_tc5(w, h->xt, rows, y, w.N, bias, nullptr, EPI_NONE, &h->gw, st);
-        return;
     }
-    if (rows <= 8 && w.qs_tc && !simt)
-        launch_q4_matvec_tc_ex(w, x, rows, y, w.N, bias, nullptr, EPI_NONE, nullptr, nullptr, 0.0f, wk, st);
-    else if (rows <= 8) launch_q4_matvec(w, x, rows, y, w.N, bias, nullptr, EPI_NONE, st);
-    else launch_q4_gemm(w, x, rows, y, w.N, bias, nullptr, EPI_NONE, st);
+    return Q4Scratch{h->xt, h->xt_elems, &h->gw, &h->wk};
 }
 int32_t vox_q4_set_matvec_mode(int32_t mode) {
     VOX_API_BEGIN
     VOX_CHECK(mode >= 0 && mode <= 3, VOX_EINVAL, "mode bits: 1 = SIMT matvec (M<=8), 2 = SIMT GEMM (M>8)");
-    g_matvec_mode = mode;
+    g_q4_path.matvec_tc = (mode & 1) == 0;
+    g_q4_path.gemm_tc = (mode & 2) == 0;
     VOX_API_END
 }
 int32_t vox_q4_matmul(const vox_q4 *w, const float *x_dev, float *y_dev, int32_t b, int32_t m, const float *bias_dev,
@@ -366,7 +350,8 @@ int32_t vox_q4_matmul(const vox_q4 *w, const float *x_dev, float *y_dev, int32_t
     REQUIRE(w); REQUIRE(x_dev); REQUIRE(y_dev);
     VOX_CHECK(b > 0 && m > 0, VOX_EINVAL, "q4_matmul: B and M must be positive");
     CUDA_OK(cudaSetDevice(w->device));
-    q4_matmul_dispatch(w->w, x_dev, y_dev, b * m, bias_dev, (cudaStream_t)stream, &w->wk, const_cast<vox_q4 *>(w));
+    launch_q4_linear(w->w, x_dev, b * m, y_dev, w->w.N, bias_dev, nullptr, EPI_NONE, nullptr, nullptr, 0.0f, nullptr,
+                     q4_scratch(const_cast<vox_q4 *>(w), b * m), g_q4_path, (cudaStream_t)stream);
     VOX_API_END
 }
 int32_t vox_q4_matmul_host(const vox_q4 *wc, const float *x, float *y, int32_t b, int32_t m, const float *bias) {
@@ -381,7 +366,8 @@ int32_t vox_q4_matmul_host(const vox_q4 *wc, const float *x, float *y, int32_t b
     if (bias && !w->bias) w->bias = w->arena.alloc_n<float>(w->w.N);
     CUDA_OK(cudaMemcpyAsync(w->x, x, sizeof(float) * xn, cudaMemcpyHostToDevice, 0));
     if (bias) CUDA_OK(cudaMemcpyAsync(w->bias, bias, sizeof(float) * w->w.N, cudaMemcpyHostToDevice, 0));
-    q4_matmul_dispatch(w->w, w->x, w->y, (int)rows, bias ? w->bias : nullptr, 0, &w->wk, w);
+    launch_q4_linear(w->w, w->x, (int)rows, w->y, w->w.N, bias ? w->bias : nullptr, nullptr, EPI_NONE, nullptr, nullptr,
+                     0.0f, nullptr, q4_scratch(w, (int)rows), g_q4_path, 0);
     CUDA_OK(cudaMemcpyAsync(y, w->y, sizeof(float) * yn, cudaMemcpyDeviceToHost, 0));
     CUDA_OK(cudaStreamSynchronize(0));
     VOX_API_END
@@ -464,10 +450,15 @@ int32_t vox_q4_matmul_bench(const vox_q4 *const *ws, int32_t n_w, int32_t m, int
     cudaEvent_t e0, e1;
     CUDA_OK(cudaEventCreate(&e0));
     CUDA_OK(cudaEventCreate(&e1));
-    for (int i = 0; i < warmup; ++i) q4_matmul_dispatch(ws[i % n_w]->w, x, y, m, nullptr, st);
+    // no scratch: no split-K, and M > 8 takes the SIMT GEMM
+    auto run = [&](int i) {
+        launch_q4_linear(ws[i % n_w]->w, x, m, y, ws[i % n_w]->w.N, nullptr, nullptr, EPI_NONE, nullptr, nullptr, 0.0f, nullptr,
+                         Q4Scratch{}, g_q4_path, st);
+    };
+    for (int i = 0; i < warmup; ++i) run(i);
     CUDA_OK(cudaStreamSynchronize(st));
     CUDA_OK(cudaEventRecord(e0, st));
-    for (int i = 0; i < iters; ++i) q4_matmul_dispatch(ws[i % n_w]->w, x, y, m, nullptr, st);
+    for (int i = 0; i < iters; ++i) run(i);
     CUDA_OK(cudaEventRecord(e1, st));
     CUDA_OK(cudaStreamSynchronize(st));
     float ms = 0;
@@ -793,7 +784,7 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
         if (n_floats) *n_floats = 0;
         return VOX_OK;
     } else if (w == "gemm_simt" || w == "gemm_tc") {
-        s->use_gemm_tc = (w == "gemm_tc");
+        s->path.gemm_tc = (w == "gemm_tc");
         if (n_floats) *n_floats = 0;
         return VOX_OK;
     } else if (w == "mega_off" || w == "mega_on" || w == "mega_auto") {
@@ -806,7 +797,7 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
         if (n_floats) *n_floats = 0;
         return VOX_OK;
     } else if (w == "tc_off" || w == "tc_on") {
-        s->use_tc = (w == "tc_on");
+        s->path.matvec_tc = (w == "tc_on");
         if (s->step_graph) { cudaGraphExecDestroy(s->step_graph); s->step_graph = nullptr; }
         if (n_floats) *n_floats = 0;
         return VOX_OK;

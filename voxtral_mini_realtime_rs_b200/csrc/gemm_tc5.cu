@@ -414,6 +414,14 @@ size_t gemm_tc5_split_elems(int M, int K) {
     const size_t TT = (size_t)(M + G5_BN - 1) / G5_BN;
     return g5_tiles_elems(M, K) + 2 * TT * G5_BN + 16;
 }
+// launch_q4_gemm_tc5 splits K only for fewer than VOX_NUM_SMS * 2 / 3 output tiles (one ticket each) and keeps
+// slices x tiles <= VOX_NUM_SMS: at most one partial tile per SM in flight
+GemmWork gemm_tc5_work_size() {
+    GemmWork w;
+    w.partial_floats = (size_t)VOX_NUM_SMS * G5_BM * G5_BN;
+    w.n_counters = 128;
+    return w;
+}
 static float *g5_oscale_ptr(void *xt, int M, int K) {
     size_t off = g5_tiles_elems(M, K) * 2;          // bytes
     off = (off + 15) & ~(size_t)15;

@@ -471,6 +471,28 @@ void launch_rmsnorm(const float *x, const float *gamma, const float *scale, floa
 }
 
 // =====================================================================================
+// Q4 linear layer: which of the four Q4 kernels runs it (kernels.h launch_q4_linear).
+// =====================================================================================
+void launch_q4_linear(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias, const float *res,
+                      int epi, const float *gamma, const float *ada, float eps, float *tmp, const Q4Scratch &sc,
+                      const Q4Path &path, cudaStream_t st) {
+    if (M > 8 && path.gemm_tc && gemm_tc5_supported(w, M) && gemm_tc5_split_elems(M, w.K) <= sc.xt_elems) {
+        launch_split_tiles(x, M, w.K, gamma, ada, gamma ? eps : 0.0f, sc.xt, st);
+        launch_q4_gemm_tc5(w, sc.xt, M, y, ldy, bias, res, epi, sc.gw, st);
+        return;
+    }
+    const bool tc = M <= 8 && path.matvec_tc && w.qs_tc;
+    if (gamma && !(tc && sc.tc && sc.tc->ssq_in)) {
+        launch_rmsnorm(x, gamma, ada, tmp, M, w.K, eps, st);
+        x = tmp;
+        gamma = ada = nullptr;
+    }
+    if (tc) launch_q4_matvec_tc_ex(w, x, M, y, ldy, bias, res, epi, gamma, ada, gamma ? eps : 0.0f, sc.tc, st);
+    else if (M <= 8) launch_q4_matvec(w, x, M, y, ldy, bias, res, epi, st);
+    else launch_q4_gemm(w, x, M, y, ldy, bias, res, epi, st);
+}
+
+// =====================================================================================
 // RoPE, interleaved pairs (reference rope.rs:103-141), tables built on the host as in rope.rs:35-64.
 // =====================================================================================
 __global__ void rope_inplace_kernel(float *buf, int ld, int q_off, int n_q, int k_off, int n_k, int hd,
@@ -939,16 +961,6 @@ __global__ void mul_vec_kernel(const float *__restrict__ a, const float *__restr
 void launch_mul_vec(const float *a, const float *b, float *out, size_t n, cudaStream_t st) {
     mul_vec_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a, b, out, n);
     post_launch("mul_vec");
-}
-
-__global__ void gelu_kernel(float *x, size_t n) {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) x[i] = gelu_erf(x[i]);
-}
-void launch_gelu(float *x, size_t n, cudaStream_t st) {
-    if (!n) return;
-    gelu_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(x, n);
-    post_launch("gelu");
 }
 
 // =====================================================================================

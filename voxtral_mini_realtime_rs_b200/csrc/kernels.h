@@ -59,11 +59,7 @@ enum Epi : int {
 // y[M,N] = x[M,K] . W^T, M <= 8 (decode / batched decode): warp-per-row-pair, shuffle reduce.
 void launch_q4_matvec(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias,
                       const float *res, int epi, cudaStream_t st);
-// same contract, dequant arithmetic on the tensor cores (mma.sync, f16 subnormal nibbles); needs the
-// TC layout (w.qs_tc).  matvec_tc.cu
-void launch_q4_matvec_tc(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias,
-                         const float *res, int epi, cudaStream_t st);
-// Session-owned scratch for the tensor-core matvec: split-K partial sums + tickets, and the per-tile
+// Caller-owned scratch for the tensor-core matvec: split-K partial sums + tickets, and the per-tile
 // sums of squares that residual epilogues leave behind for the next kernel's fused RMSNorm.
 struct TcWork {
     float *partial = nullptr;      // [S][M][n_tiles*16]
@@ -74,14 +70,15 @@ struct TcWork {
     int ssq_in_parts = 0;
     float *ssq_out = nullptr;      // [N/16][M], written by EPI_RESIDUAL epilogues
 };
+// same contract as launch_q4_matvec, dequant arithmetic on the tensor cores (mma.sync, f16 subnormal nibbles); needs
+// the TC layout (w.qs_tc).  matvec_tc.cu.  gamma (+ optional ada): RMSNorm of the input fused into the staging pass,
+// x := ((x / sqrt(mean(x^2)+eps)) * gamma) * ada.  wk (optional): split-K over K slices, fused-norm sums of squares.
 void launch_q4_matvec_tc_ex(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias,
                             const float *res, int epi, const float *gamma, const float *ada, float eps,
                             const TcWork *wk, cudaStream_t st);
-// ... with the RMSNorm (+ optional ADA scale) of the input fused into the staging pass:
-// x := ((x / sqrt(mean(x^2)+eps)) * gamma) * ada
-void launch_q4_matvec_tc_norm(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias,
-                              const float *res, int epi, const float *gamma, const float *ada, float eps,
-                              cudaStream_t st);
+// Split-K scratch sizes launch_q4_matvec_tc_ex needs for an N x K weight at up to 8 rows: partial_floats and n_counters
+// are set, the pointers are left to the caller (counters zeroed).
+TcWork q4_matvec_tc_work_size(int N, int K);
 // Decoder KV cache of ONE layer as the attention kernels see it: PAGED (KVCache semantics of kv_cache.rs:52-142 --
 // append at the stream's position, read keys 0..pos -- over fixed-size pages so that sessions of different ages
 // share one pool).  Batch row b owns logical pages page_table[b][0..max_pages); logical position j lives at
@@ -124,6 +121,29 @@ struct GemmWork {
 };
 void launch_q4_gemm_tc5(const Q4Weight &w, const void *xt, int M, float *y, int ldy, const float *bias, const float *res,
                         int epi, const GemmWork *gw, cudaStream_t st);
+// GemmWork sizes that let launch_q4_gemm_tc5 split K as far as it ever does, for any shape; pointers left to the caller
+GemmWork gemm_tc5_work_size();
+
+// Which Q4 kernels a caller lets launch_q4_linear choose: the tensor-core matvec for M <= 8 (else the SIMT matvec) and
+// the wgmma GEMM for M > 8 (else the SIMT GEMM).
+struct Q4Path {
+    bool matvec_tc = true;
+    bool gemm_tc = true;
+};
+// Caller-owned scratch of launch_q4_linear.
+struct Q4Scratch {
+    void *xt = nullptr;             // split tiles of the wgmma GEMM
+    size_t xt_elems = 0;            // capacity of xt; M > 8 rows needing more (gemm_tc5_split_elems) take the SIMT GEMM
+    const GemmWork *gw = nullptr;   // split-K of the wgmma GEMM (null: none)
+    const TcWork *tc = nullptr;     // split-K and fused-norm sums of squares of the tensor-core matvec (null: neither)
+};
+// y = epi(norm(x) . W^T + bias) (+res) for any M: the one place that picks the Q4 kernel of a linear layer.
+// gamma (optional) selects the RMSNorm (+ ADA scale `ada`) of the input.  It is fused into the wgmma GEMM's operand
+// split, or into the tensor-core matvec when sc.tc carries ssq_in; otherwise it runs as launch_rmsnorm into `tmp`
+// ([M][K]) ahead of the matvec / SIMT GEMM.
+void launch_q4_linear(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias, const float *res,
+                      int epi, const float *gamma, const float *ada, float eps, float *tmp, const Q4Scratch &sc,
+                      const Q4Path &path, cudaStream_t st);
 // conv1 / conv2 as implicit GEMM: in [B][T_in][C_in] time-major, W [C_out][3*C_in] (k = tap*C_in + c),
 // stride 2, pad 1, + bias, GELU -> out [B][T_out][C_out].
 // t_off (B == 1 only): compute conv outputs t_off .. t_off+T_out-1 into out[0..T_out) -- the incremental form used by
@@ -179,8 +199,6 @@ void launch_reshape_rows(const float *src, float *dst, int B, int S, int S_out, 
                          cudaStream_t st);
 // out[i] = a[i] * b[i]
 void launch_mul_vec(const float *a, const float *b, float *out, size_t n, cudaStream_t st);
-// GELU in place
-void launch_gelu(float *x, size_t n, cudaStream_t st);
 
 // mel: samples [B][n] device -> log-mel; layout 0 [B][frames][128], 1 [B][128][frames]
 void launch_mel(const float *samples, int B, size_t n, size_t sample_stride, const float *window,

@@ -445,16 +445,21 @@ __global__ void __launch_bounds__(TC_THREADS) q4_matvec_tc_kernel(const TcArgs a
 // programmatic dependent launch between consecutive decode kernels (VOX_PDL=0 disables)
 bool g_tc_pdl = !(getenv("VOX_PDL") && getenv("VOX_PDL")[0] == '0');
 
+// K slices of a split-K launch over n_pairs block pairs at M rows: at most 64 (M <= 2), 32 (M <= 4) or 16 pairs per
+// slice.  Tuning knob (environment, read once): VOX_TC_PS = K pairs per slice for M > 4.
+int tc_slices(int M, int n_pairs) {
+    static const int env_ps = getenv("VOX_TC_PS") ? atoi(getenv("VOX_TC_PS")) : 0;
+    const int ps_max = M <= 2 ? 64 : (M <= 4 ? 32 : (env_ps > 0 ? env_ps : 16));
+    return (n_pairs + ps_max - 1) / ps_max;
+}
+
 template <int M, int EPI>
 void tc_launch_t(TcArgs a, const TcWork *wk, cudaStream_t st) {
     // ---- work decomposition
-    // tuning knobs (environment, read once): VOX_TC_PS = K pairs per slice for M > 4,
-    // VOX_TC_CTAS = target resident CTAs per SM when several tokens share the staging
-    static const int env_ps = getenv("VOX_TC_PS") ? atoi(getenv("VOX_TC_PS")) : 0;
+    // tuning knob (environment, read once): VOX_TC_CTAS = target resident CTAs per SM when several tokens share the staging
     static const int env_ctas = getenv("VOX_TC_CTAS") ? atoi(getenv("VOX_TC_CTAS")) : 0;
-    const int ps_max = M <= 2 ? 64 : (M <= 4 ? 32 : (env_ps > 0 ? env_ps : 16));
     int S = 1;
-    if (wk && wk->partial && wk->counters) S = (a.n_pairs + ps_max - 1) / ps_max;
+    if (wk && wk->partial && wk->counters) S = tc_slices(M, a.n_pairs);
     int Ps = (a.n_pairs + S - 1) / S;
     S = (a.n_pairs + Ps - 1) / Ps;
     if (S > 1) {
@@ -551,15 +556,15 @@ void launch_q4_matvec_tc_ex(const Q4Weight &w, const float *x, int M, float *y, 
     }
 }
 
-void launch_q4_matvec_tc_norm(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias,
-                              const float *res, int epi, const float *gamma, const float *ada, float eps,
-                              cudaStream_t st) {
-    launch_q4_matvec_tc_ex(w, x, M, y, ldy, bias, res, epi, gamma, ada, eps, nullptr, st);
-}
-
-void launch_q4_matvec_tc(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias,
-                         const float *res, int epi, cudaStream_t st) {
-    launch_q4_matvec_tc_ex(w, x, M, y, ldy, bias, res, epi, nullptr, nullptr, 0.0f, nullptr, st);
+TcWork q4_matvec_tc_work_size(int N, int K) {
+    const int n_tiles = (N + 15) / 16, n_pairs = (K / 32 + 1) / 2;
+    TcWork w;
+    for (int M = 1; M <= 8; ++M) {
+        const size_t floats = (size_t)tc_slices(M, n_pairs) * M * n_tiles * 16;
+        if (floats > w.partial_floats) w.partial_floats = floats;
+    }
+    w.n_counters = n_tiles;
+    return w;
 }
 
 }  // namespace vox

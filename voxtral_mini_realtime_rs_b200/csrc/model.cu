@@ -456,39 +456,24 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames) {
             for (int K : {c.dec_dim, c.dec_heads * c.dec_head_dim, c.dec_ffn}) e = std::max(e, gemm_tc5_split_elems(std::max(rows_d, max_batch * std::max(s->S4_max, 1)), K / 64 * 64));
             s->xt_elems = e;
             s->xt_buf = s->arena.alloc(e * 2);
-            // split-K scratch of the wgmma GEMM: at most one (slice, tile) partial tile per SM in flight
-            s->gemm_work.partial_floats = (size_t)VOX_NUM_SMS * 128 * 128;
-            s->gemm_work.partial = s->arena.alloc_n<float>(s->gemm_work.partial_floats);
-            s->gemm_work.n_counters = 128;
-            s->gemm_work.counters = s->arena.alloc_n<int>(s->gemm_work.n_counters);
-            CUDA_OK(cudaMemset(s->gemm_work.counters, 0, sizeof(int) * s->gemm_work.n_counters));
+            s->gemm_work = gemm_tc5_work_size();
+            alloc_split_k(s->arena, s->gemm_work);
             const char *gv = getenv("VOX_GEMM");
-            s->use_gemm_tc = !(gv && std::string(gv) == "simt");
+            s->path.gemm_tc = !(gv && std::string(gv) == "simt");
             const char *tv = getenv("VOX_MATVEC");
-            s->use_tc = !(tv && std::string(tv) == "simt");
+            s->path.matvec_tc = !(tv && std::string(tv) == "simt");
             const char *av = getenv("VOX_ENC_ATTN");
             s->use_enc_attn_tc = !(av && std::string(av) == "simt");
         }
-        {   // fused-decode scratch (see TcWork): sized for the largest split-K matvec at max_batch rows
-            const int mb = std::min(8, max_batch * 1);
-            size_t need = 0;
-            auto acc_need = [&](int N, int K) {
-                const int n_pairs = (K / 32 + 1) / 2;
-                const int S = (n_pairs + 15) / 16;  // worst case: 16 pairs per slice (M > 4)
-                need = std::max(need, (size_t)S * 8 * (size_t)((N + 15) / 16) * 16);
-            };
-            const int qkvd2 = (c.dec_heads + 2 * c.dec_kv_heads) * c.dec_head_dim;
-            acc_need(qkvd2, c.dec_dim);
-            acc_need(c.dec_dim, c.dec_heads * c.dec_head_dim);
-            acc_need(2 * c.dec_ffn, c.dec_dim);
-            acc_need(c.dec_dim, c.dec_ffn);
-            acc_need(c.vocab, c.dec_dim);
-            (void)mb;
-            s->tc_partial_floats = need;
-            s->tc_partial = s->arena.alloc_n<float>(need);
-            s->tc_n_counters = std::max((c.vocab + 15) / 16, (2 * c.dec_ffn + 15) / 16) + 16;
-            s->tc_counters = s->arena.alloc_n<int>(s->tc_n_counters);
-            CUDA_OK(cudaMemset(s->tc_counters, 0, sizeof(int) * s->tc_n_counters));
+        {   // fused-decode scratch (see TcWork): split-K of the largest decoder / lm_head matvec
+            std::vector<const Q4Weight *> ws{&m->tok_emb};
+            for (const DecLayerW &l : m->dec) ws.insert(ws.end(), {&l.wqkv, &l.wo, &l.w13, &l.w2});
+            for (const Q4Weight *w : ws) {
+                const TcWork need = q4_matvec_tc_work_size(w->N, w->K);
+                s->tc_split.partial_floats = std::max(s->tc_split.partial_floats, need.partial_floats);
+                s->tc_split.n_counters = std::max(s->tc_split.n_counters, need.n_counters);
+            }
+            alloc_split_k(s->arena, s->tc_split);
             s->ssq_x = s->arena.alloc_n<float>((size_t)((c.dec_dim + 15) / 16) * 8);
             s->am_vals = s->arena.alloc_n<float>((size_t)max_batch * ARGMAX_PARTS);
             s->am_idx = s->arena.alloc_n<int>((size_t)max_batch * ARGMAX_PARTS);
@@ -557,30 +542,10 @@ Session::~Session() {
     if (st) cudaStreamDestroy(st);
 }
 
-void Session::linear_n(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias, const float *res,
-                       int epi, const float *gamma, const float *ada, float *tmp) {
-    if (M > 8 && use_gemm_tc && gemm_tc5_supported(w, M) && gemm_tc5_split_elems(M, w.K) <= xt_elems) {
-        launch_split_tiles(x, M, w.K, gamma, ada, m->norm_eps, xt_buf, st);
-        launch_q4_gemm_tc5(w, xt_buf, M, y, ldy, bias, res, epi, &gemm_work, st);
-        return;
-    }
-    if (gamma) {
-        launch_rmsnorm(x, gamma, ada, tmp, M, w.K, m->norm_eps, st);
-        x = tmp;
-    }
-    linear(w, x, M, y, ldy, bias, res, epi);
-}
-
-void Session::linear(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias,
-                     const float *res, int epi) {
-    if (M > 8 && use_gemm_tc && gemm_tc5_supported(w, M) && gemm_tc5_split_elems(M, w.K) <= xt_elems) {
-        launch_split_tiles(x, M, w.K, nullptr, nullptr, 0.0f, xt_buf, st);
-        launch_q4_gemm_tc5(w, xt_buf, M, y, ldy, bias, res, epi, &gemm_work, st);
-        return;
-    }
-    if (M <= 8 && w.qs_tc && use_tc) launch_q4_matvec_tc(w, x, M, y, ldy, bias, res, epi, st);
-    else if (M <= 8) launch_q4_matvec(w, x, M, y, ldy, bias, res, epi, st);
-    else launch_q4_gemm(w, x, M, y, ldy, bias, res, epi, st);
+void Session::linear(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias, const float *res,
+                     int epi, const float *gamma, const float *ada, float *tmp, const TcWork *tc) {
+    launch_q4_linear(w, x, M, y, ldy, bias, res, epi, gamma, ada, m->norm_eps, tmp, Q4Scratch{xt_buf, xt_elems, &gemm_work, tc},
+                     path, st);
 }
 
 // TimeEmbedding::embed (time_embedding.rs:41-71) + the per-layer ADA scale
@@ -620,7 +585,7 @@ void Session::encode(int B, int T) {
     const float scale = powf((float)c.enc_head_dim, -0.5f);
     for (int i = 0; i < c.enc_layers; ++i) {
         const EncLayerW &l = m->enc[i];
-        linear_n(l.wqkv, x_enc, rows, qkv_enc, 3 * hdq, l.bqkv, nullptr, EPI_NONE, l.attn_norm, nullptr, h_enc);
+        linear(l.wqkv, x_enc, rows, qkv_enc, 3 * hdq, l.bqkv, nullptr, EPI_NONE, l.attn_norm, nullptr, h_enc);
         launch_rope_inplace(qkv_enc, rows, 3 * hdq, 0, c.enc_heads, hdq, c.enc_heads, c.enc_head_dim, S, 0,
                             m->enc_cos, m->enc_sin, st);
         if (use_enc_attn_tc && enc_attention_tc_supported(c.enc_head_dim, 3 * hdq, 0, hdq, 2 * hdq))
@@ -630,7 +595,7 @@ void Session::encode(int B, int T) {
             launch_enc_attention(qkv_enc, attn_enc, B, S, c.enc_heads, c.enc_head_dim, 3 * hdq, 0, hdq, 2 * hdq,
                                  c.enc_window, scale, st);
         linear(l.wo, attn_enc, rows, x_enc, d, l.bo, x_enc, EPI_RESIDUAL);
-        linear_n(l.w13, x_enc, rows, act_enc, c.enc_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, nullptr, h_enc);
+        linear(l.w13, x_enc, rows, act_enc, c.enc_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, nullptr, h_enc);
         linear(l.w2, act_enc, rows, x_enc, d, l.b2, x_enc, EPI_RESIDUAL);
         if (debug_capture && dbg_layers)
             CUDA_OK(cudaMemcpyAsync(dbg_layers + (size_t)i * rows * d, x_enc, sizeof(float) * rows * d,
@@ -650,14 +615,10 @@ void Session::encode(int B, int T) {
 // Q4LanguageModel::forward_hidden_with_cache (model.rs:665-677) over x_dec [B*M][D]; positions
 // *d_pos + i.  Leaves the final-normed hidden states in h_dec -- or, on the fused decode path, returns
 // true and leaves the un-normed stream in x_dec for lm_head_rows().  Does not advance *d_pos.
-bool Session::fused_decode(int rows) const { return use_tc && rows <= 8 && m->tok_emb.qs_tc != nullptr; }
+bool Session::fused_decode(int rows) const { return path.matvec_tc && rows <= 8 && m->tok_emb.qs_tc != nullptr; }
 
 TcWork Session::tc_work(bool norm_in, bool ssq_out_) const {
-    TcWork w;
-    w.partial = tc_partial;
-    w.partial_floats = tc_partial_floats;
-    w.counters = tc_counters;
-    w.n_counters = tc_n_counters;
+    TcWork w = tc_split;
     if (norm_in) {
         w.ssq_in = ssq_x;
         w.ssq_in_parts = (m->info.dec_dim + 15) / 16;
@@ -685,36 +646,22 @@ bool Session::decoder_forward(int B, int M) {
     // attention kernel => 5 launches per layer instead of 8
     const bool fused = fused_decode(rows);
     const TcWork wk_norm = tc_work(true, false), wk_res = tc_work(false, true);
+    const TcWork *tc_norm = fused ? &wk_norm : nullptr, *tc_res = fused ? &wk_res : nullptr;
     const bool fattn = fused && M == 1 && dec_attn_fused_supported(H, Hkv, hd);
     for (int j = 0; j < c.dec_layers; ++j) {
         const DecLayerW &l = m->dec[j];
         const KvView kvl = kv_view(j);
-        if (fused) {
-            launch_q4_matvec_tc_ex(l.wqkv, x_dec, rows, qkv_dec, qkvd, nullptr, nullptr, EPI_NONE, l.attn_norm, nullptr,
-                                   m->norm_eps, &wk_norm, st);
-        } else {
-            linear_n(l.wqkv, x_dec, rows, qkv_dec, qkvd, nullptr, nullptr, EPI_NONE, l.attn_norm, nullptr, h_dec);
-        }
+        linear(l.wqkv, x_dec, rows, qkv_dec, qkvd, nullptr, nullptr, EPI_NONE, l.attn_norm, nullptr, h_dec, tc_norm);
         if (fattn) {
             launch_dec_attn_fused(qkv_dec, B, qkvd, H, Hkv, hd, kvl, c.dec_window, scale, m->dec_cos, m->dec_sin, attn_dec, st);
         } else {
             launch_dec_rope_append(qkv_dec, B, M, qkvd, H, Hkv, hd, kvl, m->dec_cos, m->dec_sin, st);
             launch_dec_attention(qkv_dec, B, M, qkvd, H, Hkv, hd, kvl, c.dec_window, scale, attn_dec, st);
         }
-        if (fused)
-            launch_q4_matvec_tc_ex(l.wo, attn_dec, rows, x_dec, D, nullptr, x_dec, EPI_RESIDUAL, nullptr, nullptr, 0.f, &wk_res, st);
-        else
-            linear(l.wo, attn_dec, rows, x_dec, D, nullptr, x_dec, EPI_RESIDUAL);
-        if (fused) {
-            launch_q4_matvec_tc_ex(l.w13, x_dec, rows, act_dec, c.dec_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm,
-                                   ada + (size_t)j * D, m->norm_eps, &wk_norm, st);
-        } else {
-            linear_n(l.w13, x_dec, rows, act_dec, c.dec_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, ada + (size_t)j * D, h_dec);
-        }
-        if (fused)
-            launch_q4_matvec_tc_ex(l.w2, act_dec, rows, x_dec, D, nullptr, x_dec, EPI_RESIDUAL, nullptr, nullptr, 0.f, &wk_res, st);
-        else
-            linear(l.w2, act_dec, rows, x_dec, D, nullptr, x_dec, EPI_RESIDUAL);
+        linear(l.wo, attn_dec, rows, x_dec, D, nullptr, x_dec, EPI_RESIDUAL, nullptr, nullptr, nullptr, tc_res);
+        linear(l.w13, x_dec, rows, act_dec, c.dec_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, ada + (size_t)j * D, h_dec,
+               tc_norm);
+        linear(l.w2, act_dec, rows, x_dec, D, nullptr, x_dec, EPI_RESIDUAL, nullptr, nullptr, nullptr, tc_res);
     }
     if (!fused) launch_rmsnorm(x_dec, m->dec_norm, nullptr, h_dec, rows, D, m->norm_eps, st);
     return fused;
@@ -723,21 +670,16 @@ bool Session::decoder_forward(int B, int M) {
 // lm_head over `rows` decoder rows (model.rs:680-691); `norm_pending`: x_dec still needs the final
 // RMSNorm (fused into the matvec), else h_dec already holds the normed hidden states.
 void Session::lm_head_rows(int rows, bool norm_pending, float *dst) {
-    const vox_model_info &c = m->info;
-    if (norm_pending) {
-        const TcWork wk = tc_work(true, false);
-        launch_q4_matvec_tc_ex(m->tok_emb, x_dec, rows, dst, c.vocab, nullptr, nullptr, EPI_NONE, m->dec_norm, nullptr,
-                               m->norm_eps, &wk, st);
-    }
-    else
-        linear(m->tok_emb, h_dec, rows, dst, c.vocab, nullptr, nullptr, EPI_NONE);
+    const TcWork wk = tc_work(true, false);
+    linear(m->tok_emb, norm_pending ? x_dec : h_dec, rows, dst, m->info.vocab, nullptr, nullptr, EPI_NONE,
+           norm_pending ? m->dec_norm : nullptr, nullptr, nullptr, norm_pending ? &wk : nullptr);
 }
 
 // Builds (once per batch size) the op table of the persistent decode-step kernel.  Returns false when
 // the shapes are outside what decode_mega.cu is instantiated for; the caller then uses per-op launches.
 bool Session::mega_prepare(int B) {
     const vox_model_info &c = m->info;
-    if (!use_mega || !use_tc || !fused_decode(B) || B < mega_min_B) return false;
+    if (!use_mega || !path.matvec_tc || !fused_decode(B) || B < mega_min_B) return false;
     if (!decode_mega_supported(B, c.dec_heads, c.dec_kv_heads, c.dec_head_dim)) return false;
     if (mega_B == B) return mega_n_ops > 0;
     mega_B = B;

@@ -35,6 +35,14 @@ struct DeviceArena {
     ~DeviceArena() { release(); }
 };
 
+// Allocates the buffers of a split-K scratch (TcWork, GemmWork) whose sizes are set; the tickets start at zero.
+template <typename Work>
+void alloc_split_k(DeviceArena &arena, Work &w) {
+    w.partial = arena.alloc_n<float>(w.partial_floats);
+    w.counters = arena.alloc_n<int>(w.n_counters);
+    CUDA_OK(cudaMemset(w.counters, 0, sizeof(int) * w.n_counters));
+}
+
 // Mel constants on device (window + sparse filterbank).
 struct MelTables {
     float *window = nullptr;
@@ -125,10 +133,7 @@ struct Session {
     bool use_graph = true;
     // scratch of the fused decode path: split-K partials + tickets, per-tile sums of squares of the
     // residual stream (consumed by the next kernel's fused RMSNorm), multi-CTA argmax scratch
-    float *tc_partial = nullptr;
-    size_t tc_partial_floats = 0;
-    int *tc_counters = nullptr;
-    int tc_n_counters = 0;
+    TcWork tc_split;  // split-K only; tc_work() adds the sums of squares
     float *ssq_x = nullptr;
     float *am_vals = nullptr;
     int *am_idx = nullptr, *am_cnt = nullptr;
@@ -162,12 +167,8 @@ struct Session {
     size_t xt_elems = 0;
     GemmWork gemm_work;       // split-K scratch of the wgmma GEMM
     bool use_enc_attn_tc = true;  // tensor-core encoder attention (VOX_ENC_ATTN=simt disables)
-    bool use_gemm_tc = true;  // wgmma GEMM for M > 8 (VOX_GEMM=simt disables)
-    // y = epi(norm(x) . W^T): RMSNorm fused into the operand split when the wgmma path applies,
-    // else rmsnorm into `tmp` + linear()
-    void linear_n(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias, const float *res, int epi,
-                  const float *gamma, const float *ada, float *tmp);
-    bool use_tc = true;  // tensor-core-assisted matvec for M <= 8 (VOX_MATVEC=simt disables)
+    // tensor-core matvec for M <= 8 (VOX_MATVEC=simt disables), wgmma GEMM for M > 8 (VOX_GEMM=simt disables)
+    Q4Path path;
     std::vector<float> enc_debug;  // per-layer captures when debugging is enabled
     bool debug_capture = false;
     float *dbg_layers = nullptr;   // [enc_layers][B*S][enc_dim]
@@ -178,8 +179,10 @@ struct Session {
     void set_delay(float delay);
     // mel already on device, time-major, in s->mel_tm
     void encode(int B, int T);
+    // launch_q4_linear with the session's GEMM scratch and path choice; `gamma`, `ada`, `tmp` and `tc` as there
     void linear(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias, const float *res,
-                int epi);
+                int epi, const float *gamma = nullptr, const float *ada = nullptr, float *tmp = nullptr,
+                const TcWork *tc = nullptr);
     bool decoder_forward(int B, int M);
     void lm_head_rows(int rows, bool norm_pending, float *dst);
     void decode_step(int B, bool add_audio = true);

@@ -243,14 +243,14 @@ void StreamPool::encoder_rows(int R) {
     const size_t ring_stride = (size_t)max_sessions * ring * HQ;
     for (int i = 0; i < c.enc_layers; ++i) {
         const EncLayerW &l = m->enc[i];
-        s->linear_n(l.wqkv, s->x_enc, R, s->qkv_enc, 3 * HQ, l.bqkv, nullptr, EPI_NONE, l.attn_norm, nullptr, s->h_enc);
+        s->linear(l.wqkv, s->x_enc, R, s->qkv_enc, 3 * HQ, l.bqkv, nullptr, EPI_NONE, l.attn_norm, nullptr, s->h_enc);
         stream_rope_append_kernel<<<R, 256, 0, s->st>>>(s->qkv_enc, 3 * HQ, c.enc_heads, c.enc_head_dim, d_row_slot, d_row_pos,
                                                         ek + i * ring_stride, ev + i * ring_stride, ring, m->enc_cos, m->enc_sin);
         cuda_check(cudaGetLastError(), "stream_rope_append launch");
         launch_stream_attn(s->qkv_enc, R, 3 * HQ, c.enc_heads, c.enc_head_dim, d_row_slot, d_row_pos, ek + i * ring_stride,
                            ev + i * ring_stride, ring, c.enc_window, scale, s->attn_enc, s->st);
         s->linear(l.wo, s->attn_enc, R, s->x_enc, d, l.bo, s->x_enc, EPI_RESIDUAL);
-        s->linear_n(l.w13, s->x_enc, R, s->act_enc, c.enc_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, nullptr, s->h_enc);
+        s->linear(l.w13, s->x_enc, R, s->act_enc, c.enc_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, nullptr, s->h_enc);
         s->linear(l.w2, s->act_enc, R, s->x_enc, d, l.b2, s->x_enc, EPI_RESIDUAL);
     }
     launch_rmsnorm(s->x_enc, m->enc_norm, nullptr, s->h_enc, R, d, m->norm_eps, s->st);
