@@ -234,6 +234,12 @@ typedef struct {
     int32_t live_sessions;   /* open and not yet drained after the tick               */
     int32_t mel_frames, encoder_rows, prefills, decode_steps, decode_rows;
 } vox_stream_stats;
+/* max_seconds in [1, 60]: sessions of up to that much audio, their whole history resident on the device.
+ * max_seconds = 0: sessions of ANY length.  Both attentions are sliding-window, so a session keeps only what it can
+ * still read -- decoder KV as a per-session ring of pages covering the decoder window, the encoder K/V rings, RoPE rows
+ * computed for the positions in flight, and 30 s of padded audio in its PCM / mel / conv / audio-embedding buffers --
+ * fixed when the pool is created.  push_pcm then fails with VOX_ECAPACITY while the audio not yet consumed by a tick
+ * would exceed those 30 s; encode_chunk is not available.  Absolute positions stay int32: ~248 days of audio. */
 int32_t vox_stream_pool_create(vox_model *m, int32_t max_sessions, float max_seconds, vox_stream_pool **out);
 int32_t vox_stream_open(vox_stream_pool *p, int32_t *session);
 int32_t vox_stream_push_pcm(vox_stream_pool *p, int32_t session, const float *samples, size_t n);
@@ -241,8 +247,23 @@ int32_t vox_stream_finish(vox_stream_pool *p, int32_t session);        /* end of
 int32_t vox_stream_tick(vox_stream_pool *p, vox_stream_stats *stats /* nullable */);
 /* ids emitted since the last poll; *done != 0 once the finished session has emitted everything */
 int32_t vox_stream_poll_ids(vox_stream_pool *p, int32_t session, int32_t *ids, size_t cap, size_t *n, int32_t *done);
-/* parity/debug: audio embeddings produced so far, [n][dec_dim] host */
+/* parity/debug: audio embeddings produced so far, [n][dec_dim] host.  Fails (VOX_ECAPACITY) once an unbounded session
+ * has evicted its first rows: use vox_stream_audio_embeds_range. */
 int32_t vox_stream_audio_embeds(vox_stream_pool *p, int32_t session, float *out, size_t cap_floats, int32_t *n);
+/* audio embeddings [first, first + n) (absolute indices), [n][dec_dim] host.  VOX_ECAPACITY when `first` is no longer
+ * resident (see vox_stream_session_info.first_audio_embed), VOX_EINVAL past the embeddings produced so far. */
+int32_t vox_stream_audio_embeds_range(vox_stream_pool *p, int32_t session, int64_t first, int64_t n, float *out,
+                                      size_t cap_floats);
+/* a struct tag (not a typedef): the function below has the same name */
+struct vox_stream_session_info {
+    int64_t samples;            /* padded signal samples known (left padding included; vox_stream_progress) */
+    int64_t mel_frames, encoder_frames, audio_embeds;  /* final frames / embeddings produced */
+    int64_t first_audio_embed;  /* first embedding still resident on the device */
+    int64_t decoder_positions;  /* decoder positions cached (0 until the 38-position prefill has run) */
+    int64_t ids_emitted;
+    int32_t kv_pages;           /* decoder KV pages the session holds */
+};
+int32_t vox_stream_session_info(vox_stream_pool *p, int32_t session, struct vox_stream_session_info *out);
 /* encode_audio_with_cache (model.rs:790-799) with upstream's semantics: one mel chunk [128][t_frames] (host) through the
  * conv stem on its own, the encoder layers over the session's K/V caches (RoPE / mask offsets = cached length), x4 stack
  * and adapter -> the chunk's S/4 embeddings [n][dec_dim] (host).  Chunk-wise alternative to push_pcm/tick; do not mix. */

@@ -26,6 +26,11 @@ pub struct vox_stream_stats {
     pub gpu_ms: f32, pub live_sessions: i32, pub mel_frames: i32, pub encoder_rows: i32,
     pub prefills: i32, pub decode_steps: i32, pub decode_rows: i32,
 }
+#[repr(C)] #[derive(Clone, Copy, Default)]
+pub struct vox_stream_session_info {
+    pub samples: i64, pub mel_frames: i64, pub encoder_frames: i64, pub audio_embeds: i64,
+    pub first_audio_embed: i64, pub decoder_positions: i64, pub ids_emitted: i64, pub kv_pages: i32,
+}
 #[repr(C)] #[derive(Clone, Copy)]
 pub struct vox_pad_config { pub sample_rate: u32, pub n_left_pad_tokens: u32, pub frame_rate: f32,
                             pub extra_right_pad_tokens: u32 }
@@ -88,6 +93,10 @@ extern "C" {
     pub fn vox_stream_finish(p: *mut vox_stream_pool, session: i32) -> i32;
     pub fn vox_stream_tick(p: *mut vox_stream_pool, stats: *mut vox_stream_stats) -> i32;
     pub fn vox_stream_poll_ids(p: *mut vox_stream_pool, session: i32, ids: *mut i32, cap: usize, n: *mut usize, done: *mut i32) -> i32;
+    // max_seconds = 0: sessions of any length (include/voxtral.h)
+    pub fn vox_stream_audio_embeds_range(p: *mut vox_stream_pool, session: i32, first: i64, n: i64, out: *mut f32,
+                                         cap: usize) -> i32;
+    pub fn vox_stream_session_info(p: *mut vox_stream_pool, session: i32, out: *mut vox_stream_session_info) -> i32;
     pub fn vox_stream_encode_chunk(p: *mut vox_stream_pool, session: i32, mel: *const f32, t_frames: i32, audio_embeds: *mut f32,
                                    cap: usize, n: *mut i32) -> i32;
     pub fn vox_stream_close(p: *mut vox_stream_pool, session: i32) -> i32;

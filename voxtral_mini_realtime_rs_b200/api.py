@@ -142,6 +142,8 @@ _SIGS = {
     "vox_stream_tick": (C.c_int32, [_P, _P]),
     "vox_stream_poll_ids": (C.c_int32, [_P, C.c_int32, _P, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_int32)]),
     "vox_stream_audio_embeds": (C.c_int32, [_P, C.c_int32, _P, C.c_size_t, C.POINTER(C.c_int32)]),
+    "vox_stream_audio_embeds_range": (C.c_int32, [_P, C.c_int32, C.c_int64, C.c_int64, _P, C.c_size_t]),
+    "vox_stream_session_info": (C.c_int32, [_P, C.c_int32, _P]),
     "vox_stream_encode_chunk": (C.c_int32, [_P, C.c_int32, _P, C.c_int32, _P, C.c_size_t, C.POINTER(C.c_int32)]),
     "vox_stream_close": (C.c_int32, [_P, C.c_int32]),
     "vox_stream_pool_free": (None, [_P]),
@@ -673,14 +675,22 @@ class _StreamStats(C.Structure):
                 ("prefills", C.c_int32), ("decode_steps", C.c_int32), ("decode_rows", C.c_int32)]
 
 
+class _StreamSessionInfo(C.Structure):
+    _fields_ = [("samples", C.c_int64), ("mel_frames", C.c_int64), ("encoder_frames", C.c_int64), ("audio_embeds", C.c_int64),
+                ("first_audio_embed", C.c_int64), ("decoder_positions", C.c_int64), ("ids_emitted", C.c_int64),
+                ("kv_pages", C.c_int32)]
+
+
 class StreamingPool:
     """Live streaming sessions on one GPU worker (vox_stream_*; SURVEY 8(f)-1).  `model` stays owned by the caller
-    and must outlive the pool."""
+    and must outlive the pool.  max_seconds=None: sessions of any length, with fixed device state (30 s of padded audio
+    resident per session; see include/voxtral.h)."""
 
-    def __init__(self, model: "Q4VoxtralModel", max_sessions: int = 8, max_seconds: float = 30.0):
+    def __init__(self, model: "Q4VoxtralModel", max_sessions: int = 8, max_seconds: float | None = 30.0):
         self._model = model
         self._p = _P()
-        _check(lib().vox_stream_pool_create(model._m, max_sessions, max_seconds, C.byref(self._p)))
+        _check(lib().vox_stream_pool_create(model._m, max_sessions, 0.0 if max_seconds is None else max_seconds,
+                                            C.byref(self._p)))
         self.dec_dim = model.info["dec_dim"]
 
     def open(self) -> int:
@@ -706,7 +716,21 @@ class StreamingPool:
         _check(lib().vox_stream_poll_ids(self._p, session, _ptr(ids), cap, C.byref(n), C.byref(done)))
         return ids[:n.value].tolist(), bool(done.value)
 
-    def audio_embeds(self, session: int) -> np.ndarray:
+    def session_info(self, session: int) -> dict:
+        info = _StreamSessionInfo()
+        _check(lib().vox_stream_session_info(self._p, session, C.byref(info)))
+        return {f[0]: getattr(info, f[0]) for f in _StreamSessionInfo._fields_}
+
+    def audio_embeds(self, session: int, first: int | None = None, n: int | None = None) -> np.ndarray:
+        """All embeddings so far; or, with `first` and/or `n`, the resident rows [first, first + n) (default: from the
+        first resident row to the last one produced)."""
+        if first is not None or n is not None:
+            info = self.session_info(session)
+            first = info["first_audio_embed"] if first is None else first
+            n = info["audio_embeds"] - first if n is None else n
+            out = np.empty((n, self.dec_dim), np.float32)
+            _check(lib().vox_stream_audio_embeds_range(self._p, session, first, n, _ptr(out), out.size))
+            return out
         n = C.c_int32()
         _check(lib().vox_stream_audio_embeds(self._p, session, None, 0, C.byref(n)))
         out = np.empty((n.value, self.dec_dim), np.float32)

@@ -945,6 +945,33 @@ int32_t vox_stream_audio_embeds(vox_stream_pool *p, int32_t session, float *out,
     }
     VOX_API_END
 }
+// the device check comes first, as in every compute entry point: without a device no pool can exist
+static void require_any_device() {
+    int n = 0;
+    cudaError_t e = cudaGetDeviceCount(&n);
+    VOX_CHECK(e == cudaSuccess && n > 0, VOX_ECUDA, "no CUDA device available (%s); this library has no CPU fallback",
+              cudaGetErrorString(e));
+}
+int32_t vox_stream_audio_embeds_range(vox_stream_pool *p, int32_t session, int64_t first, int64_t n, float *out, size_t cap) {
+    VOX_API_BEGIN
+    require_any_device();
+    REQUIRE(p);
+    const float *src = p->p->audio_embeds_range(session, first, n);
+    const size_t need = (size_t)n * p->p->m->info.dec_dim;
+    if (need) REQUIRE(out);
+    VOX_CHECK(cap >= need, VOX_ECAPACITY, "audio_embeds capacity %zu < %zu", cap, need);
+    CUDA_OK(cudaSetDevice(p->p->m->device));
+    CUDA_OK(cudaStreamSynchronize(p->p->s->st));
+    if (need) CUDA_OK(cudaMemcpy(out, src, sizeof(float) * need, cudaMemcpyDeviceToHost));
+    VOX_API_END
+}
+int32_t vox_stream_session_info(vox_stream_pool *p, int32_t session, struct vox_stream_session_info *out) {
+    VOX_API_BEGIN
+    require_any_device();
+    REQUIRE(p); REQUIRE(out);
+    p->p->session_info(session, out);
+    VOX_API_END
+}
 int32_t vox_stream_encode_chunk(vox_stream_pool *p, int32_t session, const float *mel, int32_t t, float *out, size_t cap, int32_t *n) {
     VOX_API_BEGIN
     REQUIRE(p); REQUIRE(mel); REQUIRE(out); REQUIRE(n);

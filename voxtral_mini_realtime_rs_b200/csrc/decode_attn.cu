@@ -18,23 +18,22 @@ namespace {
 constexpr int DA_WARPS = 8;
 constexpr int DA_THREADS = DA_WARPS * 32;
 
-template <int G, int DPL>
+template <int G, int DPL, bool RING>
 __global__ void __launch_bounds__(DA_THREADS)
 dec_attn_fused_kernel(const float *__restrict__ qkv, const int ld, const int H, const int Hkv, const KvView kv, const int window,
-                      const float scale, const float *__restrict__ cos_t, const float *__restrict__ sin_t,
-                      float *__restrict__ out) {
+                      const float scale, const RopeView rope, float *__restrict__ out) {
     constexpr int HD = DPL * 32;
     __shared__ float qs[G][HD];
     __shared__ float kvs[2][HD];
     __shared__ float red_m[DA_WARPS][G], red_l[DA_WARPS][G];
     __shared__ float red_acc[DA_WARPS][G][HD];
-    __shared__ int pts[64];  // this row's page table (first 64 logical pages = 1024 positions; beyond: global)
+    __shared__ int pts[64];  // this row's page table (first 64 slots = 1024 positions; beyond: global)
     // let the next kernel (the wo matvec) start prefetching its weights while we run
     asm volatile("griddepcontrol.launch_dependents;\n" ::: "memory");
     const int kvh = blockIdx.x, b = blockIdx.y;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int pos = kv.pos[b];
-    if (pos >= kv.max_seq()) return;
+    if (!RING && pos >= kv.max_seq()) return;
     for (int i = threadIdx.x; i < 64 && i < kv.max_pages; i += DA_THREADS) pts[i] = kv.page_table[(size_t)b * kv.max_pages + i];
     const float *row = qkv + (size_t)b * ld;  // M = 1: one row per stream
     // ---- load q (G heads), k, v of this group; RoPE q and k; append k, v at `pos`
@@ -48,14 +47,15 @@ dec_attn_fused_kernel(const float *__restrict__ qkv, const int ld, const int H, 
     for (int i = threadIdx.x; i < (G + 1) * half; i += DA_THREADS) {
         const int h = i / half, p = i - h * half;
         float *v = (h < G) ? &qs[h][2 * p] : &kvs[0][2 * p];
-        const float c = cos_t[(size_t)pos * half + p], s = sin_t[(size_t)pos * half + p];
+        const size_t rr = (size_t)(RING ? pos % rope.rows : pos) * half + p;
+        const float c = rope.cos_t[rr], s = rope.sin_t[rr];
         const float xr = v[0], xi = v[1];
         v[0] = xr * c - xi * s;
         v[1] = xr * s + xi * c;
     }
     __syncthreads();
     {
-        const size_t at = kv_index(kv, b, Hkv, kvh, pos, HD);
+        const size_t at = kv_index<RING>(kv, b, Hkv, kvh, pos, HD);
         for (int i = threadIdx.x; i < HD; i += DA_THREADS) {
             kv.k[at + i] = kvs[0][i];
             kv.v[at + i] = kvs[1][i];
@@ -79,7 +79,7 @@ dec_attn_fused_kernel(const float *__restrict__ qkv, const int ld, const int H, 
     const int j_lo = pos - window > 0 ? pos - window : 0;
     for (int j = j_lo + warp; j <= pos; j += DA_WARPS) {
         float kk[DPL], vv[DPL];
-        const int pg = j / KV_PAGE;
+        const int pg = RING ? (j / KV_PAGE) % kv.max_pages : j / KV_PAGE;
         const int phys = pg < 64 ? pts[pg] : kv.page_table[(size_t)b * kv.max_pages + pg];
         const size_t at = (((size_t)phys * Hkv + kvh) * KV_PAGE + (j % KV_PAGE)) * HD + lane * DPL;
         const float *kr = kv.k + at;
@@ -140,13 +140,13 @@ dec_attn_fused_kernel(const float *__restrict__ qkv, const int ld, const int H, 
     }
 }
 
-template <int G>
+template <int G, bool RING>
 void launch_g(int dpl, dim3 grid, cudaStream_t st, const float *qkv, int ld, int H, int Hkv, const KvView &kv, int window,
-              float scale, const float *cos_t, const float *sin_t, float *out) {
+              float scale, const RopeView &rope, float *out) {
     switch (dpl) {
-        case 1: dec_attn_fused_kernel<G, 1><<<grid, DA_THREADS, 0, st>>>(qkv, ld, H, Hkv, kv, window, scale, cos_t, sin_t, out); break;
-        case 2: dec_attn_fused_kernel<G, 2><<<grid, DA_THREADS, 0, st>>>(qkv, ld, H, Hkv, kv, window, scale, cos_t, sin_t, out); break;
-        case 4: dec_attn_fused_kernel<G, 4><<<grid, DA_THREADS, 0, st>>>(qkv, ld, H, Hkv, kv, window, scale, cos_t, sin_t, out); break;
+        case 1: dec_attn_fused_kernel<G, 1, RING><<<grid, DA_THREADS, 0, st>>>(qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        case 2: dec_attn_fused_kernel<G, 2, RING><<<grid, DA_THREADS, 0, st>>>(qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        case 4: dec_attn_fused_kernel<G, 4, RING><<<grid, DA_THREADS, 0, st>>>(qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
         default: fail(VOX_EINVAL, "dec_attn_fused: unsupported head_dim");
     }
 }
@@ -159,14 +159,17 @@ bool dec_attn_fused_supported(int H, int Hkv, int hd) {
 }
 
 void launch_dec_attn_fused(float *qkv, int B, int ld, int H, int Hkv, int hd, const KvView &kv, int window, float scale,
-                           const float *cos_t, const float *sin_t, float *out, cudaStream_t st) {
+                           const RopeView &rope, float *out, cudaStream_t st) {
     VOX_CHECK(dec_attn_fused_supported(H, Hkv, hd), VOX_EINVAL, "dec_attn_fused: unsupported shape");
     const int G = H / Hkv, dpl = hd / 32;
     dim3 grid(Hkv, B);
-    switch (G) {
-        case 1: launch_g<1>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, cos_t, sin_t, out); break;
-        case 2: launch_g<2>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, cos_t, sin_t, out); break;
-        default: launch_g<4>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, cos_t, sin_t, out); break;
+    switch (G * 2 + (kv.ring ? 1 : 0)) {
+        case 2: launch_g<1, false>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        case 3: launch_g<1, true>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        case 4: launch_g<2, false>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        case 5: launch_g<2, true>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        case 8: launch_g<4, false>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        default: launch_g<4, true>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
     }
     tc_count_launch("dec_attn_fused");
 }

@@ -364,7 +364,9 @@ __device__ __forceinline__ void mg_pair(const unsigned char *__restrict__ sb, co
     }
 }
 
-template <int MT, int G, int DPL>
+// RING: the rows are sessions of an unbounded stream pool -- KV page-table rows are rings (kernels.h KvView) and RoPE
+// rows come from p.cos_t / p.sin_t at pos % p.rope_rows; positions have no cap.  RING = false is the plain walk.
+template <int MT, int G, int DPL, bool RING>
 __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaParams p) {
     constexpr int CG = (MT + 3) / 4;
     constexpr int HD = DPL * 32;
@@ -507,13 +509,13 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                                 const int ch = unit % NC, bk = unit / NC;
                                 const int b = bk / p.Hkv, kvh = bk - b * p.Hkv;
                                 const int pos = p.d_pos[b];
-                                if (pos >= p.max_seq) continue;
+                                if (!RING && pos >= p.max_seq) continue;
                                 const int j_lo = pos - p.window > 0 ? pos - p.window : 0;
                                 const int per = (pos - j_lo + NC) / NC;
                                 const int j0 = j_lo + ch * per, j1 = min(pos, j0 + per);  // row `pos` is not written yet
                                 for (int pg = j0 / KV_PAGE; pg * KV_PAGE < j1; ++pg) {     // pages are the contiguous unit
                                     const int ka = max(j0, pg * KV_PAGE), ke = min(j1, (pg + 1) * KV_PAGE);
-                                    const size_t off = (((size_t)p.page_table[(size_t)b * p.max_pages + pg] * p.Hkv + kvh) * KV_PAGE + (ka - pg * KV_PAGE)) * HD;
+                                    const size_t off = (((size_t)p.page_table[(size_t)b * p.max_pages + (RING ? pg % p.max_pages : pg)] * p.Hkv + kvh) * KV_PAGE + (ka - pg * KV_PAGE)) * HD;
                                     bulk_prefetch_l2(nx.kc + off, (uint32_t)(ke - ka) * HD * 4u);
                                     bulk_prefetch_l2(nx.vc + off, (uint32_t)(ke - ka) * HD * 4u);
                                 }
@@ -936,7 +938,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                 const int ch = unit % NC, bk = unit / NC;
                 const int b = bk / Hkv, kvh = bk - b * Hkv;
                 const int pos = p.d_pos[b];              // per row: sessions of different ages share the step
-                if (pos >= max_seq) continue;
+                if (!RING && pos >= max_seq) continue;
                 const int j_lo = pos - p.window > 0 ? pos - p.window : 0;
                 const int per = (pos - j_lo + NC) / NC;  // ceil((pos - j_lo + 1) / NC) keys per chunk
                 const int j0 = j_lo + ch * per, j1 = min(pos + 1, j0 + per);  // keys [j0, j1)
@@ -949,7 +951,8 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                     const int h = i / half, pi = i - h * half;
                     const float *src = (h < G) ? row + (size_t)(kvh * G + h) * HD + 2 * pi : row + (size_t)H * HD + kvh * HD + 2 * pi;
                     const float2 xv = __ldcg(reinterpret_cast<const float2 *>(src));
-                    const float c = p.cos_t[(size_t)pos * half + pi], sn = p.sin_t[(size_t)pos * half + pi];
+                    const size_t rr = (size_t)(RING ? pos % p.rope_rows : pos) * half + pi;
+                    const float c = p.cos_t[rr], sn = p.sin_t[rr];
                     float *dst = (h < G) ? &qs[h * HD + 2 * pi] : &kvs[2 * pi];
                     dst[0] = xv.x * c - xv.y * sn;
                     dst[1] = xv.x * sn + xv.y * c;
@@ -959,7 +962,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                 if (tracing) p.trace[oi * 6 + 1] = (unsigned long long)clock64();
                 if (tr_all) ta[3] = (unsigned long long)clock64();
                 if (has_new) {
-                    const size_t at = kv_index(kvw, b, Hkv, kvh, pos, HD);
+                    const size_t at = kv_index<RING>(kvw, b, Hkv, kvh, pos, HD);
                     for (int i = tid; i < HD; i += MG_CTHREADS) {
                         kvw.k[at + i] = kvs[i];
                         kvw.v[at + i] = kvs[HD + i];
@@ -985,7 +988,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                     for (int u = 0; u < KU; ++u) {
                         const int j = jb + u * MG_CWARPS;
                         if (j < j1 && j != pos) {
-                            const size_t at = kv_index(kvw, b, Hkv, kvh, j, HD) + lane * DPL;
+                            const size_t at = kv_index<RING>(kvw, b, Hkv, kvh, j, HD) + lane * DPL;
                             const float *kr = kvw.k + at;
                             const float *vr = kvw.v + at;
                             if constexpr (DPL == 4) {
@@ -1257,10 +1260,10 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
     }
 }
 
-template <int MT, int G, int DPL>
+template <int MT, int G, int DPL, bool RING>
 void launch_t(const MegaParams &p, const MegaPlan &plan, int grid, cudaStream_t st) {
     static SmemAttr smem_attr;
-    cuda_check_mg(ensure_dyn_smem(decode_mega_kernel<MT, G, DPL>, MG_SMEM_MAX, smem_attr), "cudaFuncSetAttribute(decode_mega)");
+    cuda_check_mg(ensure_dyn_smem(decode_mega_kernel<MT, G, DPL, RING>, MG_SMEM_MAX, smem_attr), "cudaFuncSetAttribute(decode_mega)");
     // cooperative launch: the runtime refuses the launch (instead of the grid barrier hanging) if the
     // `grid` CTAs cannot all be resident at once
     cudaLaunchConfig_t cfg{};
@@ -1273,15 +1276,15 @@ void launch_t(const MegaParams &p, const MegaPlan &plan, int grid, cudaStream_t 
     attr[0].val.cooperative = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    cuda_check_mg(cudaLaunchKernelEx(&cfg, decode_mega_kernel<MT, G, DPL>, p), "decode_mega launch");
+    cuda_check_mg(cudaLaunchKernelEx(&cfg, decode_mega_kernel<MT, G, DPL, RING>, p), "decode_mega launch");
     tc_count_launch("decode_mega");
 }
 
 template <int MT>
 void launch_m(const MegaParams &p, const MegaPlan &plan, int grid, cudaStream_t st) {
     const int G = p.H / p.Hkv;
-    if (G == 4 && p.hd == 128) launch_t<MT, 4, 4>(p, plan, grid, st);
-    else if (G == 2 && p.hd == 32) launch_t<MT, 2, 1>(p, plan, grid, st);
+    if (G == 4 && p.hd == 128) (p.ring ? launch_t<MT, 4, 4, true> : launch_t<MT, 4, 4, false>)(p, plan, grid, st);
+    else if (G == 2 && p.hd == 32) (p.ring ? launch_t<MT, 2, 1, true> : launch_t<MT, 2, 1, false>)(p, plan, grid, st);
     else fail(VOX_EINVAL, "decode_mega: unsupported attention shape");
 }
 

@@ -102,6 +102,10 @@ struct MegaParams {
     // released after the arithmetic (instead of right after the warp's loads of the stage)
     int flags = 0;
     float *logits_out = nullptr;  // != nullptr: where the lm_head op writes its rows (row groups of a larger batch)
+    // sessions of an unbounded stream pool: page_table rows are rings of max_pages slots, positions are uncapped and
+    // RoPE row of position pos is pos % rope_rows of cos_t / sin_t (kernels.h KvView, RopeView)
+    int ring = 0;
+    int rope_rows = 0;
 };
 
 struct MegaPlan {

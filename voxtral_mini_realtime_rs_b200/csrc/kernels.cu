@@ -267,6 +267,7 @@ struct GemmArgs {
     const float *res;
     int T_in, T_out, C_in;
     int t_off;  // implicit im2col: output row t of the launch is conv output t + t_off (streaming: only the new frames)
+    int in0;    // absolute input row of a[0] (B == 1: a streaming buffer that has slid past the signal start)
 };
 
 template <int BMODE, int AMODE, int EPI>
@@ -299,7 +300,7 @@ __global__ void __launch_bounds__(GB_THREADS) gemm_kernel(const GemmArgs p) {
                     const int tap = k0 / p.C_in, c0 = k0 - tap * p.C_in;
                     const int tin = 2 * (t + p.t_off) - 1 + tap;
                     if (tin >= 0 && tin < p.T_in)
-                        v = *reinterpret_cast<const float4 *>(p.a + ((size_t)b * p.T_in + tin) * p.C_in + c0 + kq * 4);
+                        v = *reinterpret_cast<const float4 *>(p.a + ((size_t)b * p.T_in + (tin - p.in0)) * p.C_in + c0 + kq * 4);
                 }
             }
             As[kq * 4 + 0][row] = v.x;
@@ -405,14 +406,15 @@ void launch_q4_gemm(const Q4Weight &w, const float *a, int M, float *y, int ldy,
 }
 
 void launch_conv2_gemm(const float *in, const float *w, const float *bias, float *out, int B, int T_in,
-                       int T_out, int C_in, int C_out, cudaStream_t st, int t_off) {
+                       int T_out, int C_in, int C_out, cudaStream_t st, int t_off, int in0) {
     VOX_CHECK(C_in % 32 == 0, VOX_EINVAL, "conv2: C_in=%d not a multiple of 32", C_in);
-    VOX_CHECK(t_off == 0 || B == 1, VOX_EINVAL, "conv2: a frame offset needs B == 1");
+    VOX_CHECK((t_off == 0 && in0 == 0) || B == 1, VOX_EINVAL, "conv2: a frame offset needs B == 1");
+    VOX_CHECK(in0 <= 2 * t_off - 1 || in0 == 0, VOX_EINVAL, "conv2: input row %d is no longer resident", 2 * t_off - 1);
     if (B * T_out <= 0) return;
     GemmArgs p{};
     p.a = in; p.M = B * T_out; p.N = C_out; p.K = 3 * C_in; p.lda = 0;
     p.wf = w; p.y = out; p.ldy = C_out; p.bias = bias; p.res = nullptr;
-    p.T_in = T_in; p.T_out = T_out; p.C_in = C_in; p.t_off = t_off;
+    p.T_in = T_in; p.T_out = T_out; p.C_in = C_in; p.t_off = t_off; p.in0 = in0;
     gemm_launch<1, 1>(p, EPI_GELU, st);
 }
 
@@ -651,14 +653,15 @@ void launch_enc_attention(const float *qkv, float *out, int B, int S, int H, int
 // cache without materialising the repeated K/V (model.rs:125-197).  Positions come from a device
 // counter so the same CUDA graph can be replayed for every step.
 // =====================================================================================
-__global__ void dec_rope_append_kernel(float *qkv, int M, int ld, int H, int Hkv, int hd, const KvView kv,
-                                       const float *__restrict__ cos_t, const float *__restrict__ sin_t) {
+template <bool RING>
+__global__ void dec_rope_append_kernel(float *qkv, int M, int ld, int H, int Hkv, int hd, const KvView kv, const RopeView rope) {
     const int i = blockIdx.x, b = blockIdx.y;
     const int pos = kv.pos[b] + i;
-    if (pos >= kv.max_seq()) return;
+    if (!RING && pos >= kv.max_seq()) return;
     const int half = hd >> 1;
     float *row = qkv + ((size_t)b * M + i) * ld;
-    const float *cr = cos_t + (size_t)pos * half, *sr = sin_t + (size_t)pos * half;
+    const size_t rr = (size_t)(RING ? pos % rope.rows : pos) * half;
+    const float *cr = rope.cos_t + rr, *sr = rope.sin_t + rr;
     for (int t = threadIdx.x; t < H * half; t += blockDim.x) {
         const int h = t / half, p = t - h * half;
         float *v = row + h * hd + 2 * p;
@@ -671,24 +674,26 @@ __global__ void dec_rope_append_kernel(float *qkv, int M, int ld, int H, int Hkv
     for (int t = threadIdx.x; t < Hkv * half; t += blockDim.x) {
         const int h = t / half, p = t - h * half;
         const float xr = krow[h * hd + 2 * p], xi = krow[h * hd + 2 * p + 1];
-        float *dst = kv.k + kv_index(kv, b, Hkv, h, pos, hd) + 2 * p;
+        float *dst = kv.k + kv_index<RING>(kv, b, Hkv, h, pos, hd) + 2 * p;
         dst[0] = xr * cr[p] - xi * sr[p];
         dst[1] = xr * sr[p] + xi * cr[p];
     }
     for (int t = threadIdx.x; t < Hkv * hd; t += blockDim.x) {
         const int h = t / hd, d = t - h * hd;
-        kv.v[kv_index(kv, b, Hkv, h, pos, hd) + d] = vrow[t];
+        kv.v[kv_index<RING>(kv, b, Hkv, h, pos, hd) + d] = vrow[t];
     }
 }
 
 void launch_dec_rope_append(float *qkv, int B, int M, int ld, int H, int Hkv, int hd, const KvView &kv,
-                            const float *cos_t, const float *sin_t, cudaStream_t st) {
+                            const RopeView &rope, cudaStream_t st) {
     dim3 grid(M, B);
-    dec_rope_append_kernel<<<grid, 256, 0, st>>>(qkv, M, ld, H, Hkv, hd, kv, cos_t, sin_t);
+    if (kv.ring) dec_rope_append_kernel<true><<<grid, 256, 0, st>>>(qkv, M, ld, H, Hkv, hd, kv, rope);
+    else dec_rope_append_kernel<false><<<grid, 256, 0, st>>>(qkv, M, ld, H, Hkv, hd, kv, rope);
     post_launch("dec_rope_append");
 }
 
 // grid (Hkv, M, B); block = 32 * (H/Hkv): one warp per query head of the group.
+template <bool RING>
 __global__ void dec_attention_kernel(const float *__restrict__ qkv, int M, int ld, int H, int Hkv, int hd, const KvView kv,
                                      int window, float scale, float *__restrict__ out) {
     extern __shared__ float sm[];
@@ -697,17 +702,18 @@ __global__ void dec_attention_kernel(const float *__restrict__ qkv, int M, int l
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int pos = kv.pos[b] + i;
     const int max_seq = kv.max_seq();
-    if (pos >= max_seq) return;
+    if (!RING && pos >= max_seq) return;
     float *qsm = sm + warp * hd;                        // [G][hd]
-    float *sc = sm + G * hd + (size_t)warp * max_seq;   // [G][max_seq]
+    float *sc = sm + G * hd + (size_t)warp * max_seq;   // [G][max_seq]: key j at sc[j - base] (a ring's keys go past max_seq)
     const int h = kvh * G + warp;
     const float *qrow = qkv + ((size_t)b * M + i) * ld + h * hd;
     for (int d = lane; d < hd; d += 32) qsm[d] = qrow[d];
     __syncwarp();
     const int j_lo = pos - window > 0 ? pos - window : 0;
+    const int base = RING ? j_lo : 0;
     float mx = -INFINITY;
     for (int j = j_lo + lane; j <= pos; j += 32) {
-        const float4 *kr = reinterpret_cast<const float4 *>(kv.k + kv_index(kv, b, Hkv, kvh, j, hd));
+        const float4 *kr = reinterpret_cast<const float4 *>(kv.k + kv_index<RING>(kv, b, Hkv, kvh, j, hd));
         const float4 *q4 = reinterpret_cast<const float4 *>(qsm);
         float acc = 0.0f;
         for (int d = 0; d < (hd >> 2); ++d) {
@@ -719,14 +725,14 @@ __global__ void dec_attention_kernel(const float *__restrict__ qkv, int M, int l
             acc = fmaf(qv.w, kk.w, acc);
         }
         acc *= scale;
-        sc[j] = acc;
+        sc[j - base] = acc;
         mx = fmaxf(mx, acc);
     }
     mx = warp_max(mx);
     float sum = 0.0f;
     for (int j = j_lo + lane; j <= pos; j += 32) {
-        const float pv = expf(sc[j] - mx);
-        sc[j] = pv;
+        const float pv = expf(sc[j - base] - mx);
+        sc[j - base] = pv;
         sum += pv;
     }
     sum = warp_sum(sum);
@@ -735,7 +741,7 @@ __global__ void dec_attention_kernel(const float *__restrict__ qkv, int M, int l
     float *orow = out + ((size_t)b * M + i) * (H * hd) + h * hd;
     for (int d = lane; d < hd; d += 32) {
         float acc = 0.0f;
-        for (int j = j_lo; j <= pos; ++j) acc = fmaf(sc[j], kv.v[kv_index(kv, b, Hkv, kvh, j, hd) + d], acc);
+        for (int j = j_lo; j <= pos; ++j) acc = fmaf(sc[j - base], kv.v[kv_index<RING>(kv, b, Hkv, kvh, j, hd) + d], acc);
         orow[d] = acc * inv;
     }
 }
@@ -746,9 +752,15 @@ void launch_dec_attention(const float *qkv, int B, int M, int ld, int H, int Hkv
     dim3 grid(Hkv, M, B);
     const size_t smem = (size_t)G * (hd + kv.max_seq()) * sizeof(float);
     VOX_CHECK(smem <= 200 * 1024, VOX_EINVAL, "dec_attention: max_seq %d too large for the v1 kernel", kv.max_seq());
-    static SmemAttr attr;
-    if (smem > 48 * 1024) smem_attr_check(ensure_dyn_smem(dec_attention_kernel, smem, attr), "dec_attention");
-    dec_attention_kernel<<<grid, 32 * G, smem, st>>>(qkv, M, ld, H, Hkv, hd, kv, window, scale, out);
+    static SmemAttr attr, attr_ring;
+    if (kv.ring) {
+        VOX_CHECK(window < kv.max_seq(), VOX_EINVAL, "dec_attention: window %d does not fit the KV ring", window);
+        if (smem > 48 * 1024) smem_attr_check(ensure_dyn_smem(dec_attention_kernel<true>, smem, attr_ring), "dec_attention");
+        dec_attention_kernel<true><<<grid, 32 * G, smem, st>>>(qkv, M, ld, H, Hkv, hd, kv, window, scale, out);
+    } else {
+        if (smem > 48 * 1024) smem_attr_check(ensure_dyn_smem(dec_attention_kernel<false>, smem, attr), "dec_attention");
+        dec_attention_kernel<false><<<grid, 32 * G, smem, st>>>(qkv, M, ld, H, Hkv, hd, kv, window, scale, out);
+    }
     post_launch("dec_attention");
 }
 
@@ -974,14 +986,14 @@ constexpr int MEL_FR = 8, MEL_THREADS = 256, MEL_NFFT = 400, MEL_HOP = 160, MEL_
 __global__ void __launch_bounds__(MEL_THREADS)
 mel_kernel(const float *__restrict__ samples, size_t n, size_t sample_stride, const float *__restrict__ window,
            const float *__restrict__ fb_vals, const int *__restrict__ fb_start, const int *__restrict__ fb_len,
-           int fb_stride, float *__restrict__ out, int frames, int layout, int frame0) {
+           int fb_stride, float *__restrict__ out, int frames, int layout, int frame0, long long sample0, int out0) {
     __shared__ float ws[MEL_FR][MEL_NFFT];
     __shared__ __align__(16) float sp[(MEL_FR - 1) * MEL_HOP + MEL_NFFT];
     __shared__ float ct[MEL_NFFT], stt[MEL_NFFT];
     __shared__ float pw[MEL_FR][MEL_NFREQ + 3];
     const int b = blockIdx.y;
     const int f0 = frame0 + blockIdx.x * MEL_FR;   // frames [frame0, frames) of the signal (streaming: only the new ones)
-    const float *sig = samples + (size_t)b * sample_stride;
+    const float *sig = samples + (size_t)b * sample_stride;   // sig[i - sample0]: absolute sample i
     const long long nn = (long long)n;
     for (int i = threadIdx.x; i < MEL_NFFT; i += MEL_THREADS) {
         float s, c;
@@ -996,16 +1008,17 @@ mel_kernel(const float *__restrict__ samples, size_t n, size_t sample_stride, co
         const long long span0 = (long long)f0 * MEL_HOP - MEL_NFFT / 2;
         constexpr int SPAN = (MEL_FR - 1) * MEL_HOP + MEL_NFFT;   // 1520
         static_assert(SPAN % 4 == 0, "span is float4-sized");
-        const bool interior = span0 >= 0 && span0 + SPAN <= nn && ((reinterpret_cast<uintptr_t>(sig + span0) & 15) == 0);
+        const bool interior = span0 >= 0 && span0 + SPAN <= nn && ((reinterpret_cast<uintptr_t>(sig + (span0 - sample0)) & 15) == 0);
         if (interior) {
-            const float4 *src4 = reinterpret_cast<const float4 *>(sig + span0);
+            const float4 *src4 = reinterpret_cast<const float4 *>(sig + (span0 - sample0));
             for (int i = threadIdx.x; i < SPAN / 4; i += MEL_THREADS) reinterpret_cast<float4 *>(sp)[i] = src4[i];
         } else {
             for (int i = threadIdx.x; i < SPAN; i += MEL_THREADS) {
                 long long src = span0 + i;
                 if (src < 0) { src = -src; if (src > nn - 1) src = nn > 0 ? nn - 1 : 0; }
                 else if (src >= nn) { src = 2 * nn - 2 - src; if (src < 0) src = 0; }
-                sp[i] = nn > 0 ? sig[src] : 0.0f;
+                if (src < sample0) src = sample0;   // only frames >= `frames` (discarded) of a sliding buffer reach here
+                sp[i] = nn > 0 ? sig[src - sample0] : 0.0f;
             }
         }
     }
@@ -1047,18 +1060,21 @@ mel_kernel(const float *__restrict__ samples, size_t n, size_t sample_stride, co
         float v = log10f(fmaxf(acc, 1e-10f));
         v = fmaxf(v, min_val);
         v = (v + 4.0f) / 4.0f;
-        if (layout == 0) out[((size_t)b * frames + f0 + f) * MEL_NMEL + m] = v;
-        else out[((size_t)b * MEL_NMEL + m) * frames + f0 + f] = v;
+        if (layout == 0) out[((size_t)b * frames + f0 + f - out0) * MEL_NMEL + m] = v;
+        else out[((size_t)b * MEL_NMEL + m) * frames + f0 + f - out0] = v;
     }
 }
 
 void launch_mel(const float *samples, int B, size_t n, size_t sample_stride, const float *window,
                 const float *fb_vals, const int *fb_start, const int *fb_len, int fb_stride, float *out,
-                int frames, int layout, cudaStream_t st, int frame0) {
+                int frames, int layout, cudaStream_t st, int frame0, size_t sample0, int out0) {
     if (frames - frame0 <= 0 || B <= 0) return;
+    VOX_CHECK((sample0 == 0 && out0 == 0) || (B == 1 && layout == 0 && sample0 % 4 == 0 && out0 <= frame0 &&
+                                               (long long)sample0 <= (long long)frame0 * MEL_HOP - MEL_NFFT / 2),
+              VOX_EINVAL, "mel: sliding buffer offsets (%zu, %d) do not cover frame %d", sample0, out0, frame0);
     dim3 grid((frames - frame0 + MEL_FR - 1) / MEL_FR, B);
     mel_kernel<<<grid, MEL_THREADS, 0, st>>>(samples, n, sample_stride, window, fb_vals, fb_start, fb_len,
-                                             fb_stride, out, frames, layout, frame0);
+                                             fb_stride, out, frames, layout, frame0, (long long)sample0, out0);
     post_launch("mel");
 }
 

@@ -85,24 +85,36 @@ TcWork q4_matvec_tc_work_size(int N, int K);
 //   pool + ((phys(b, j / KV_PAGE) * Hkv + kv_head) * KV_PAGE + j % KV_PAGE) * hd.
 // Positions are per row (pos[b] = number of cached positions of row b = position of its next token): whole-utterance
 // batches keep them equal, streaming sessions do not.
+// ring: the page table row is a RING -- logical page lp lives in slot lp % max_pages and positions are unbounded (the
+// sessions of an unbounded stream pool, stream.cu; safe while max_pages * KV_PAGE > window + the rows a prefill writes
+// before reading).  The kernels take it as a template flag, so the non-ring code is the plain table walk.
 constexpr int KV_PAGE = 16;
 struct KvView {
     float *k = nullptr, *v = nullptr;  // [n_pages][Hkv][KV_PAGE][hd]
     const int *page_table = nullptr;   // [B][max_pages] physical page ids
-    int max_pages = 0;                 // logical pages per row; capacity = max_pages * KV_PAGE positions
+    int max_pages = 0;                 // logical pages per row; capacity = max_pages * KV_PAGE positions (ring: slots)
+    bool ring = false;
     const int *pos = nullptr;          // [B]
     __host__ __device__ int max_seq() const { return max_pages * KV_PAGE; }
 };
 #ifdef __CUDACC__
+template <bool RING = false>
 __device__ __forceinline__ size_t kv_index(const KvView &kv, const int b, const int Hkv, const int kvh, const int j, const int hd) {
-    const int phys = kv.page_table[(size_t)b * kv.max_pages + (j / KV_PAGE)];
+    const int lp = j / KV_PAGE;
+    const int phys = kv.page_table[(size_t)b * kv.max_pages + (RING ? lp % kv.max_pages : lp)];
     return (((size_t)phys * Hkv + kvh) * KV_PAGE + (j % KV_PAGE)) * hd;
 }
 #endif
+// Decoder RoPE tables as the kernels read them: cos / sin [rows][hd/2], position p at row p -- or, for a ring KvView, at
+// row p % rows of an unbounded pool's small ring tables, whose rows the host fills for the positions of each launch.
+struct RopeView {
+    const float *cos_t = nullptr, *sin_t = nullptr;
+    int rows = 0;
+};
 // single-token decoder attention fused with RoPE + KV append (decode_attn.cu); qkv rows [B][ld]
 bool dec_attn_fused_supported(int H, int Hkv, int hd);
 void launch_dec_attn_fused(float *qkv, int B, int ld, int H, int Hkv, int hd, const KvView &kv, int window, float scale,
-                           const float *cos_t, const float *sin_t, float *out, cudaStream_t st);
+                           const RopeView &rope, float *out, cudaStream_t st);
 // y[M,N] = A[M,K] . W^T for any M (encoder / prefill): tiled SIMT GEMM, in-tile dequant.
 void launch_q4_gemm(const Q4Weight &w, const float *a, int M, float *y, int ldy, const float *bias,
                     const float *res, int epi, cudaStream_t st);
@@ -147,9 +159,10 @@ void launch_q4_linear(const Q4Weight &w, const float *x, int M, float *y, int ld
 // conv1 / conv2 as implicit GEMM: in [B][T_in][C_in] time-major, W [C_out][3*C_in] (k = tap*C_in + c),
 // stride 2, pad 1, + bias, GELU -> out [B][T_out][C_out].
 // t_off (B == 1 only): compute conv outputs t_off .. t_off+T_out-1 into out[0..T_out) -- the incremental form used by
-// the streaming session; input rows outside [0, T_in) are the zero padding.
+// the streaming session; input rows outside [0, T_in) are the zero padding.  in0 (B == 1 only): absolute input row of
+// in[0] (a streaming buffer that has slid past the start of the signal); T_in stays the absolute input length.
 void launch_conv2_gemm(const float *in, const float *w, const float *bias, float *out, int B, int T_in,
-                       int T_out, int C_in, int C_out, cudaStream_t st, int t_off = 0);
+                       int T_out, int C_in, int C_out, cudaStream_t st, int t_off = 0, int in0 = 0);
 // [B][C][T] -> [B][T][C]
 void launch_transpose_mel(const float *in, float *out, int B, int C, int T, cudaStream_t st);
 // y = x / sqrt(mean(x^2)+eps) * gamma (* scale, optional ADA vector)
@@ -170,7 +183,7 @@ void launch_enc_attention_tc(const float *qkv, float *out, int B, int S, int H, 
 // decoder: RoPE q in place, RoPE k -> Kcache, v -> Vcache at positions kv.pos[b] + i.
 // qkv rows [B*M][ld].
 void launch_dec_rope_append(float *qkv, int B, int M, int ld, int H, int Hkv, int hd, const KvView &kv,
-                            const float *cos_t, const float *sin_t, cudaStream_t st);
+                            const RopeView &rope, cudaStream_t st);
 // decoder GQA attention over the cache (keys 0..kv.pos[b]+i, window), out [B*M][H*hd].
 void launch_dec_attention(const float *qkv, int B, int M, int ld, int H, int Hkv, int hd, const KvView &kv, int window,
                           float scale, float *out, cudaStream_t st);
@@ -201,9 +214,11 @@ void launch_reshape_rows(const float *src, float *dst, int B, int S, int S_out, 
 void launch_mul_vec(const float *a, const float *b, float *out, size_t n, cudaStream_t st);
 
 // mel: samples [B][n] device -> log-mel; layout 0 [B][frames][128], 1 [B][128][frames]
+// frames [frame0, frames) are computed.  B == 1 streaming buffers that slide: samples[0] is absolute sample sample0 (a
+// multiple of 4 keeps the aligned interior path) and out row 0 is absolute frame out0; n stays the absolute length.
 void launch_mel(const float *samples, int B, size_t n, size_t sample_stride, const float *window,
                 const float *fb_vals, const int *fb_start, const int *fb_len, int fb_stride, float *out,
-                int frames, int layout, cudaStream_t st, int frame0 = 0);  // frames [frame0, frames) are computed
+                int frames, int layout, cudaStream_t st, int frame0 = 0, size_t sample0 = 0, int out0 = 0);
 // peak normalisation on device: per stream max|x| then scale (target/max), skip if max < 1e-10;
 // writes into a padded buffer at offset left (rest pre-zeroed by caller)
 void launch_peak_normalize_pad(const float *in, int B, size_t n, float target, int do_norm, float *out,

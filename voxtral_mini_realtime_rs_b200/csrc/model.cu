@@ -216,21 +216,26 @@ struct Loader {
 };
 
 void build_rope(DeviceArena &arena, int hd, int max_seq, float theta, float **cos_d, float **sin_d) {
-    // RoPEConfig::init (rope.rs:35-64), f32 throughout
     const int half = hd / 2;
-    std::vector<float> inv(half), c((size_t)max_seq * half), s((size_t)max_seq * half);
-    for (int i = 0; i < half; ++i) inv[i] = 1.0f / powf(theta, (float)(2 * i) / (float)hd);
-    for (int p = 0; p < max_seq; ++p)
-        for (int i = 0; i < half; ++i) {
-            const float f = (float)p * inv[i];
-            c[(size_t)p * half + i] = cosf(f);
-            s[(size_t)p * half + i] = sinf(f);
-        }
+    std::vector<float> c((size_t)max_seq * half), s((size_t)max_seq * half);
+    rope_rows(hd, theta, 0, max_seq, c.data(), s.data());
     *cos_d = arena.upload(c.data(), c.size());
     *sin_d = arena.upload(s.data(), s.size());
 }
 
 }  // namespace
+
+void rope_rows(int hd, float theta, int64_t p0, int n, float *cos_out, float *sin_out) {
+    const int half = hd / 2;
+    std::vector<float> inv(half);
+    for (int i = 0; i < half; ++i) inv[i] = 1.0f / powf(theta, (float)(2 * i) / (float)hd);
+    for (int r = 0; r < n; ++r)
+        for (int i = 0; i < half; ++i) {
+            const float f = (float)(p0 + r) * inv[i];
+            cos_out[(size_t)r * half + i] = cosf(f);
+            sin_out[(size_t)r * half + i] = sinf(f);
+        }
+}
 
 Model *Model::load(const Gguf &g, int device) {
     int ndev = 0;
@@ -384,7 +389,7 @@ Model *Model::load(const Gguf &g, int device) {
 // ======================================================================================
 static int conv_out(int t) { return (t + 2 - 3) / 2 + 1; }  // conv.rs:47-48
 
-Session *Session::create(Model *m, int max_batch, int max_mel_frames) {
+Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ring) {
     VOX_CHECK(max_batch >= 1 && max_batch <= 64, VOX_EINVAL, "max_batch %d out of range [1,64]", max_batch);
     VOX_CHECK(max_mel_frames >= 16, VOX_EINVAL, "max_mel_frames %d too small", max_mel_frames);
     CUDA_OK(cudaSetDevice(m->device));
@@ -420,9 +425,11 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames) {
         s->audio = s->arena.alloc_n<float>(rows4 * c.dec_dim);
         // decoder
         const int kv_cap = std::max(s->S4_max, s->M_max) + s->M_max;  // room for the incremental API
-        s->kv_max_pages = (kv_cap + KV_PAGE - 1) / KV_PAGE;
+        s->kv_max_pages = kv_ring ? (c.dec_window + s->M_max) / KV_PAGE + 1 : (kv_cap + KV_PAGE - 1) / KV_PAGE;
         s->kv_n_pages = max_batch * s->kv_max_pages;
         s->out_ld = s->kv_max_pages * KV_PAGE;
+        s->kv_ring = kv_ring;
+        s->dec_rope = m->dec_rope();
         const size_t kv_elems = (size_t)c.dec_layers * s->kv_n_pages * c.dec_kv_heads * KV_PAGE * c.dec_head_dim;
         s->kc = s->arena.alloc_n<float>(kv_elems);
         s->vc = s->arena.alloc_n<float>(kv_elems);
@@ -633,6 +640,7 @@ KvView Session::kv_view(int layer) const {
     v.v = vc + (size_t)layer * kv_layer_stride();
     v.page_table = d_page_table;
     v.max_pages = kv_max_pages;
+    v.ring = kv_ring;
     v.pos = d_pos;
     return v;
 }
@@ -653,9 +661,9 @@ bool Session::decoder_forward(int B, int M) {
         const KvView kvl = kv_view(j);
         linear(l.wqkv, x_dec, rows, qkv_dec, qkvd, nullptr, nullptr, EPI_NONE, l.attn_norm, nullptr, h_dec, tc_norm);
         if (fattn) {
-            launch_dec_attn_fused(qkv_dec, B, qkvd, H, Hkv, hd, kvl, c.dec_window, scale, m->dec_cos, m->dec_sin, attn_dec, st);
+            launch_dec_attn_fused(qkv_dec, B, qkvd, H, Hkv, hd, kvl, c.dec_window, scale, dec_rope, attn_dec, st);
         } else {
-            launch_dec_rope_append(qkv_dec, B, M, qkvd, H, Hkv, hd, kvl, m->dec_cos, m->dec_sin, st);
+            launch_dec_rope_append(qkv_dec, B, M, qkvd, H, Hkv, hd, kvl, dec_rope, st);
             launch_dec_attention(qkv_dec, B, M, qkvd, H, Hkv, hd, kvl, c.dec_window, scale, attn_dec, st);
         }
         linear(l.wo, attn_dec, rows, x_dec, D, nullptr, x_dec, EPI_RESIDUAL, nullptr, nullptr, nullptr, tc_res);
@@ -834,8 +842,10 @@ void Session::decode_step_mega(int b0, int B, bool add_audio) {
         p.max_pages = kv_max_pages;
         p.window = c.dec_window;
         p.scale = powf((float)c.dec_head_dim, -0.5f);
-        p.cos_t = m->dec_cos;
-        p.sin_t = m->dec_sin;
+        p.cos_t = dec_rope.cos_t;
+        p.sin_t = dec_rope.sin_t;
+        p.rope_rows = dec_rope.rows;
+        p.ring = kv_ring ? 1 : 0;
         p.attn_out = attn_dec;
         // key chunks per (stream, kv head): spread the KV walk over idle SMs, but no more than 4 -- the merging CTA waits
         // for the other chunks' states one after the other (an L2 round trip each), and a CTA walks 64 keys per round
@@ -909,6 +919,10 @@ void Session::reset() {
     CUDA_OK(cudaMemsetAsync(d_pos, 0, sizeof(int) * max_batch, st));
     CUDA_OK(cudaMemsetAsync(d_outpos, 0, sizeof(int) * max_batch, st));
     cache_len = 0;
+    rebase_epoch();
+}
+
+void Session::rebase_epoch() {
     // the persistent kernel's attention-chunk states carry the tag epoch * 64 + layer + 1 (int): re-base the device
     // epoch long before that can overflow (2^24 steps ~ 10 hours of continuous decoding) -- and wipe the tagged words, so
     // that no stale state can match a tag of the new numbering

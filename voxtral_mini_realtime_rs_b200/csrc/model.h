@@ -78,9 +78,14 @@ struct Model {
     float *enc_cos = nullptr, *enc_sin = nullptr, *dec_cos = nullptr, *dec_sin = nullptr;
     int enc_rope_len = 4096, dec_rope_len = 16384;  // loader.rs:196, 284
     MelTables mel;
+    RopeView dec_rope() const { return RopeView{dec_cos, dec_sin, dec_rope_len}; }
 
     static Model *load(const Gguf &g, int device);
 };
+
+// RoPE rows [p0, p0 + n) of head dim hd (RoPEConfig::init, rope.rs:35-64, f32 throughout: cos/sin((float)p * inv_freq)):
+// the model's tables and the ring tables of unbounded stream pools are both filled by this one function.
+void rope_rows(int hd, float theta, int64_t p0, int n, float *cos_out, float *sin_out);
 
 // Repack raw GGUF Q4_0 blocks of one or more [N_i, K] matrices into the device layout.
 // interleave=true: two parts with equal N, rows (2i, 2i+1) = (a_i, b_i).
@@ -111,7 +116,9 @@ struct Session {
     int *d_page_table = nullptr;          // [max_batch][kv_max_pages]
     std::vector<int> page_table_host;
     size_t kv_layer_stride() const { return (size_t)kv_n_pages * m->info.dec_kv_heads * KV_PAGE * m->info.dec_head_dim; }
+    bool kv_ring = false;                 // KvView::ring (Session::create)
     KvView kv_view(int layer) const;
+    RopeView dec_rope;                    // the model's tables, or an unbounded stream pool's ring
     float *x_dec = nullptr, *h_dec = nullptr, *qkv_dec = nullptr, *attn_dec = nullptr, *act_dec = nullptr;
     float *last_h = nullptr, *logits = nullptr;
     float *logits_all = nullptr;
@@ -174,7 +181,10 @@ struct Session {
     float *dbg_layers = nullptr;   // [enc_layers][B*S][enc_dim]
     float *dbg_conv = nullptr;
 
-    static Session *create(Model *m, int max_batch, int max_mel_frames);
+    // kv_ring: each row's decoder KV is a ring of pages just long enough for the decoder window plus the rows one launch
+    // appends before reading (16 L > dec_window + M_max), and positions are unbounded (stream pools with no length
+    // limit; the pool owner points dec_rope at its RoPE ring)
+    static Session *create(Model *m, int max_batch, int max_mel_frames, bool kv_ring = false);
     ~Session();
     void set_delay(float delay);
     // mel already on device, time-major, in s->mel_tm
@@ -192,6 +202,8 @@ struct Session {
     // runs prefill + loop; returns tokens per stream
     int transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids, vox_timings *tm, bool timed_pre);
     void reset();
+    // re-bases the persistent kernel's step epoch once it has advanced far (see reset)
+    void rebase_epoch();
 };
 
 }  // namespace vox

@@ -8,8 +8,10 @@
 //   samples (the padded signal so far) -> log-mel frames (final once samples < 160 i + 200 are known) -> conv1 / conv2
 //   frames (k3 s2 p1: output t needs input 2t+1) -> 32 encoder layers over a per-layer K/V RING of window + slack
 //   positions (absolute positions for RoPE and the causal / sliding-window masks; keys older than the window are simply
-//   overwritten: bounded memory for sessions of any length) -> x4 frame stack + adapter -> one decoder position per
-//   160 ms of audio, greedy ids.
+//   overwritten) -> x4 frame stack + adapter -> one decoder position per 160 ms of audio, greedy ids.
+// Unbounded pools (max_seconds = 0) keep every stage's state fixed: the audio-side buffers are windows that slide
+// forward (slide() below), the decoder KV of a session is a ring of pages covering the decoder window (kernels.h KvView),
+// and RoPE rows come from small ring tables the host fills for the positions in flight.
 // Continuous batching: one pool = one GPU worker.  A tick gathers the new encoder frames of ALL live sessions into one
 // row batch (the linears do not care which session a row belongs to; RoPE / ring append / attention take a per-row
 // (session, absolute position)), and all sessions that can take a decoder step share ONE decode step -- rows at
@@ -27,17 +29,22 @@ namespace vox {
 namespace {
 
 constexpr int SA_WARPS = 4, SA_THREADS = SA_WARPS * 32;
+// rows of an unbounded pool's decoder RoPE ring: rows of one decoder launch must not meet in it (tick() defers a row
+// whose position collides with another row's), which is rare with a ring this long
+constexpr int kDecRopeRing = 4096;
 
 // RoPE(q) in place, RoPE(k) and v into the row's session ring at slot (pos % ring).  qkv rows [R][3*HQ].
 __global__ void stream_rope_append_kernel(float *__restrict__ qkv, const int ld, const int H, const int hd,
                                           const int *__restrict__ row_slot, const int *__restrict__ row_pos, float *__restrict__ kr,
                                           float *__restrict__ vr, const int ring, const float *__restrict__ cos_t,
-                                          const float *__restrict__ sin_t) {
+                                          const float *__restrict__ sin_t, const bool rope_ring) {
     const int r = blockIdx.x;
     const int slot = row_slot[r], pos = row_pos[r];
     const int half = hd >> 1, HQ = H * hd;
     float *row = qkv + (size_t)r * ld;
-    const float *cr = cos_t + (size_t)pos * half, *sr = sin_t + (size_t)pos * half;
+    // RoPE row: the model's table at `pos`, or (rope_ring) the session's ring row, which sits where its K/V row does
+    const size_t rr = rope_ring ? ((size_t)slot * ring + (pos % ring)) * half : (size_t)pos * half;
+    const float *cr = cos_t + rr, *sr = sin_t + rr;
     float *kdst = kr + ((size_t)slot * ring + (pos % ring)) * HQ;
     float *vdst = vr + ((size_t)slot * ring + (pos % ring)) * HQ;
     for (int i = threadIdx.x; i < H * half; i += blockDim.x) {
@@ -135,13 +142,41 @@ void launch_stream_attn(const float *qkv, int R, int ld, int H, int hd, const in
 
 int conv_out(int t) { return t > 0 ? (t + 2 - 3) / 2 + 1 : 0; }
 
+// Slides a session buffer of `cap` rows of `row` floats whose row 0 is absolute row `base` so that rows up to `end`
+// fit: rows [keep, valid) move to the front and `base` becomes `keep`.  Nothing moves while `end` already fits (always,
+// in a bounded pool).  Overlapping moves bounce through `tmp` (as large as any session buffer): two copies at most.
+// zero_tail: the rows after the moved ones are cleared (the PCM buffer's right padding is read as zeros).
+template <typename I>
+void slide(float *buf, size_t row, int64_t cap, I &base, int64_t keep, int64_t valid, int64_t end, bool zero_tail, float *tmp,
+           cudaStream_t st) {
+    if (end - (int64_t)base <= cap) return;
+    VOX_CHECK(keep >= (int64_t)base && keep <= valid && end - keep <= cap, VOX_ECAPACITY,
+              "stream buffer of %lld rows cannot hold rows %lld..%lld", (long long)cap, (long long)keep, (long long)end);
+    const int64_t shift = keep - (int64_t)base, n = valid - keep;
+    const size_t bytes = sizeof(float) * (size_t)n * row;
+    if (n > 0 && n <= shift) {
+        CUDA_OK(cudaMemcpyAsync(buf, buf + (size_t)shift * row, bytes, cudaMemcpyDeviceToDevice, st));
+    } else if (n > 0) {
+        CUDA_OK(cudaMemcpyAsync(tmp, buf + (size_t)shift * row, bytes, cudaMemcpyDeviceToDevice, st));
+        CUDA_OK(cudaMemcpyAsync(buf, tmp, bytes, cudaMemcpyDeviceToDevice, st));
+    }
+    if (zero_tail) CUDA_OK(cudaMemsetAsync(buf + (size_t)n * row, 0, sizeof(float) * (size_t)(cap - n) * row, st));
+    base = (I)keep;
+}
+
+// first sample the next mel frame reads (its window starts 200 samples left of 160 t), down to a multiple of 4: the
+// mel kernel's aligned interior path needs the buffer start aligned like the signal
+size_t pcm_keep(int n_mel) { return (size_t)std::max<int64_t>(0, (int64_t)n_mel * 160 - 200) & ~(size_t)3; }
+
 }  // namespace
 
 // ======================================================================================================
 StreamPool *StreamPool::create(Model *m, int max_sessions, float max_seconds) {
     VOX_CHECK(max_sessions >= 1 && max_sessions <= 64, VOX_EINVAL, "max_sessions %d out of range [1,64]", max_sessions);
-    VOX_CHECK(max_seconds >= 1.0f && max_seconds <= 60.0f, VOX_EINVAL, "max_seconds %.1f out of range [1,60] (encoder RoPE table: %d frames)",
-              max_seconds, m->enc_rope_len);
+    const bool unbounded = max_seconds == 0.0f;
+    VOX_CHECK(unbounded || (max_seconds >= 1.0f && max_seconds <= 60.0f), VOX_EINVAL,
+              "max_seconds %.1f out of range [1,60] (encoder RoPE table: %d frames), or 0 for sessions of any length", max_seconds,
+              m->enc_rope_len);
     const vox_model_info &c = m->info;
     vox_pad_config pc;
     pad_config_default(&pc);
@@ -150,9 +185,11 @@ StreamPool *StreamPool::create(Model *m, int max_sessions, float max_seconds) {
         p->m = m;
         p->pad = pc;
         p->max_sessions = max_sessions;
-        p->cap_samples = pad_audio_len((size_t)std::ceil(max_seconds * 16000.0f), pc);
+        p->unbounded = unbounded;
+        p->cap_samples = pad_audio_len((size_t)std::ceil((unbounded ? kResidentSeconds : max_seconds) * 16000.0f), pc);
         const int cap_mel = (int)mel_num_frames(p->cap_samples);
-        p->s = Session::create(m, max_sessions, cap_mel);
+        // unbounded: the frame buffers get a few frames beyond the resident audio for the rows their consumers still read
+        p->s = Session::create(m, max_sessions, unbounded ? cap_mel + 16 : cap_mel, unbounded);
         Session *s = p->s;
         VOX_CHECK(s->S_max <= m->enc_rope_len, VOX_EINVAL, "max_seconds exceeds the encoder RoPE table");
         p->max_new = 256;
@@ -168,6 +205,17 @@ StreamPool *StreamPool::create(Model *m, int max_sessions, float max_seconds) {
         p->d_row_slot = s->arena.alloc_n<int>(max_rows);
         p->d_row_pos = s->arena.alloc_n<int>(max_rows);
         p->d_audio_rows = (const float **)s->arena.alloc(sizeof(float *) * B);
+        if (unbounded) {
+            const size_t enc_rows = B * p->ring * (c.enc_head_dim / 2), dec_rows = (size_t)kDecRopeRing * (c.dec_head_dim / 2);
+            p->enc_rope_cos = s->arena.alloc_n<float>(enc_rows);
+            p->enc_rope_sin = s->arena.alloc_n<float>(enc_rows);
+            p->dec_rope_cos = s->arena.alloc_n<float>(dec_rows);
+            p->dec_rope_sin = s->arena.alloc_n<float>(dec_rows);
+            s->dec_rope = RopeView{p->dec_rope_cos, p->dec_rope_sin, kDecRopeRing};
+            const size_t most = std::max({p->cap_samples, (size_t)s->max_mel_frames * c.n_mels, (size_t)s->T1_max * c.enc_dim,
+                                          (size_t)s->S_max * c.enc_dim, (size_t)s->S4_max * c.dec_dim});
+            p->slide_tmp = s->arena.alloc_n<float>(most);
+        }
         p->slots.resize(max_sessions);
         // decoder KV pages: the session's identity tables are replaced by a free list
         for (int i = s->kv_n_pages - 1; i >= 0; --i) p->free_pages.push_back(i);
@@ -204,10 +252,17 @@ StreamPool::Slot &StreamPool::slot(int id) {
 void StreamPool::push(int id, const float *samples, size_t n) {
     Slot &sl = slot(id);
     VOX_CHECK(!sl.ended, VOX_EINVAL, "stream session %d already finished", id);
-    const size_t worst = sl.n_samples + n + pad_right(pad, sl.n_samples + n);
-    VOX_CHECK(worst <= cap_samples, VOX_ECAPACITY, "stream session %d: %zu samples exceed the pool's max_seconds", id, sl.n_audio + n);
+    const size_t worst = sl.n_samples + n + pad_right(pad, sl.n_samples + n);  // right padding included, should finish() follow
+    if (unbounded)
+        VOX_CHECK(worst - pcm_keep(sl.n_mel) <= cap_samples, VOX_ECAPACITY,
+                  "stream session %d: %zu samples not yet consumed exceed the resident %.0f s; call vox_stream_tick first", id,
+                  sl.n_samples + n - pcm_keep(sl.n_mel), kResidentSeconds);
+    else
+        VOX_CHECK(worst <= cap_samples, VOX_ECAPACITY, "stream session %d: %zu samples exceed the pool's max_seconds", id, sl.n_audio + n);
     CUDA_OK(cudaSetDevice(m->device));
-    if (n) CUDA_OK(cudaMemcpyAsync(pcm + (size_t)id * cap_samples + sl.n_samples, samples, sizeof(float) * n, cudaMemcpyHostToDevice, s->st));
+    float *buf = pcm + (size_t)id * cap_samples;
+    slide(buf, 1, (int64_t)cap_samples, sl.pcm0, (int64_t)pcm_keep(sl.n_mel), (int64_t)sl.n_samples, (int64_t)worst, true, slide_tmp, s->st);
+    if (n) CUDA_OK(cudaMemcpyAsync(buf + (sl.n_samples - sl.pcm0), samples, sizeof(float) * n, cudaMemcpyHostToDevice, s->st));
     CUDA_OK(cudaStreamSynchronize(s->st));  // `samples` is caller memory
     sl.n_samples += n;
     sl.n_audio += n;
@@ -228,10 +283,10 @@ void StreamPool::close(int id) {
 
 size_t StreamPool::poll(int id, int32_t *ids, size_t cap, bool *done) {
     Slot &sl = slot(id);
-    const size_t n = std::min(cap, sl.ids.size() - sl.polled);
-    if (n) memcpy(ids, sl.ids.data() + sl.polled, sizeof(int32_t) * n);
-    sl.polled += n;
-    if (done) *done = sl.ended && sl.drained && sl.polled == sl.ids.size();
+    const size_t n = std::min(cap, sl.ids.size());
+    if (n) memcpy(ids, sl.ids.data(), sizeof(int32_t) * n);
+    sl.ids.erase(sl.ids.begin(), sl.ids.begin() + n);  // polled ids are dropped: host memory stays bounded
+    if (done) *done = sl.ended && sl.drained && sl.ids.empty();
     return n;
 }
 
@@ -245,7 +300,9 @@ void StreamPool::encoder_rows(int R) {
         const EncLayerW &l = m->enc[i];
         s->linear(l.wqkv, s->x_enc, R, s->qkv_enc, 3 * HQ, l.bqkv, nullptr, EPI_NONE, l.attn_norm, nullptr, s->h_enc);
         stream_rope_append_kernel<<<R, 256, 0, s->st>>>(s->qkv_enc, 3 * HQ, c.enc_heads, c.enc_head_dim, d_row_slot, d_row_pos,
-                                                        ek + i * ring_stride, ev + i * ring_stride, ring, m->enc_cos, m->enc_sin);
+                                                        ek + i * ring_stride, ev + i * ring_stride, ring,
+                                                        unbounded ? enc_rope_cos : m->enc_cos, unbounded ? enc_rope_sin : m->enc_sin,
+                                                        unbounded);
         cuda_check(cudaGetLastError(), "stream_rope_append launch");
         launch_stream_attn(s->qkv_enc, R, 3 * HQ, c.enc_heads, c.enc_head_dim, d_row_slot, d_row_pos, ek + i * ring_stride,
                            ev + i * ring_stride, ring, c.enc_window, scale, s->attn_enc, s->st);
@@ -257,7 +314,8 @@ void StreamPool::encoder_rows(int R) {
 }
 
 void StreamPool::ensure_pages(Slot &sl, int positions) {
-    const int need = (positions + KV_PAGE - 1) / KV_PAGE;
+    int need = (positions + KV_PAGE - 1) / KV_PAGE;
+    if (unbounded) need = std::min(need, s->kv_max_pages);  // a full ring: logical page lp reuses slot lp % kv_max_pages
     VOX_CHECK(need <= s->kv_max_pages, VOX_ECAPACITY, "stream session needs %d decoder positions > capacity %d", positions, s->out_ld);
     while ((int)sl.pages.size() < need) {
         VOX_CHECK(!free_pages.empty(), VOX_ECAPACITY, "decoder KV page pool exhausted (%d pages)", s->kv_n_pages);
@@ -277,7 +335,7 @@ void StreamPool::upload_rows(const std::vector<int> &rows, bool with_tokens) {
         for (size_t k = 0; k < sl.pages.size(); ++k) pt[(size_t)i * mp + k] = sl.pages[k];
         pos[i] = sl.pos;
         tok[i] = sl.last_tok;
-        ar[i] = s->audio + ((size_t)rows[i] * s->S4_max + sl.pos) * c.dec_dim;
+        ar[i] = s->audio + ((size_t)rows[i] * s->S4_max + (sl.pos - sl.emb0)) * c.dec_dim;
     }
     CUDA_OK(cudaMemcpyAsync(s->d_page_table, pt.data(), sizeof(int) * pt.size(), cudaMemcpyHostToDevice, s->st));
     CUDA_OK(cudaMemcpyAsync(s->d_pos, pos.data(), sizeof(int) * nb, cudaMemcpyHostToDevice, s->st));
@@ -292,6 +350,7 @@ void StreamPool::tick(vox_stream_stats *st_out) {
     CUDA_OK(cudaSetDevice(m->device));
     const int d = c.enc_dim, D = c.dec_dim, rf = c.reshape_factor, P = c.prefix_len;
     vox_stream_stats stats{};
+    s->rebase_epoch();  // between ticks: no decode step is in flight
     cudaEvent_t e0 = s->ev[0], e1 = s->ev[1];
     CUDA_OK(cudaEventRecord(e0, s->st));
     bool more = true;
@@ -314,21 +373,28 @@ void StreamPool::tick(vox_stream_stats *st_out) {
             }
             float *mel_s = s->mel_tm + (size_t)id * s->max_mel_frames * c.n_mels;
             float *c1_s = s->h1 + (size_t)id * s->T1_max * d;
+            // each buffer keeps from the first row its consumer still reads: conv1 output t reads mel 2t-1..2t+1, conv2
+            // output t reads conv1 2t-1..2t+1
             if (mel_t > sl.n_mel) {
+                slide(mel_s, c.n_mels, s->max_mel_frames, sl.mel0, std::max(0, 2 * sl.n_c1 - 1), sl.n_mel, mel_t, false, slide_tmp, s->st);
                 launch_mel(pcm + (size_t)id * cap_samples, 1, sl.n_samples, cap_samples, m->mel.window, m->mel.fb_vals, m->mel.fb_start,
-                           m->mel.fb_len, m->mel.fb_stride, mel_s, mel_t, 0, s->st, sl.n_mel);
+                           m->mel.fb_len, m->mel.fb_stride, mel_s, mel_t, 0, s->st, sl.n_mel, sl.pcm0, sl.mel0);
                 stats.mel_frames += mel_t - sl.n_mel;
                 sl.n_mel = mel_t;
             }
             if (c1_t > sl.n_c1) {
-                launch_conv2_gemm(mel_s, m->conv1_w, m->conv1_b, c1_s + (size_t)sl.n_c1 * d, 1, sl.n_mel, c1_t - sl.n_c1, c.n_mels, d, s->st,
-                                  sl.n_c1);
+                slide(c1_s, d, s->T1_max, sl.c10, std::max(0, 2 * sl.n_enc - 1), sl.n_c1, c1_t, false, slide_tmp, s->st);
+                launch_conv2_gemm(mel_s, m->conv1_w, m->conv1_b, c1_s + (size_t)(sl.n_c1 - sl.c10) * d, 1, sl.n_mel, c1_t - sl.n_c1, c.n_mels,
+                                  d, s->st, sl.n_c1, sl.mel0);
                 sl.n_c1 = c1_t;
             }
             const int n_new = enc_t - sl.n_enc;
             if (n_new > 0) {
                 const int r0 = (int)row_slot.size();
-                launch_conv2_gemm(c1_s, m->conv2_w, m->conv2_b, s->x_enc + (size_t)r0 * d, 1, sl.n_c1, n_new, d, d, s->st, sl.n_enc);
+                launch_conv2_gemm(c1_s, m->conv2_w, m->conv2_b, s->x_enc + (size_t)r0 * d, 1, sl.n_c1, n_new, d, d, s->st, sl.n_enc,
+                                  sl.c10);
+                if (unbounded)
+                    fill_rope(enc_rope_cos, enc_rope_sin, c.enc_head_dim, ring, (size_t)id * ring, sl.n_enc, n_new);
                 for (int i = 0; i < n_new; ++i) {
                     row_slot.push_back(id);
                     row_pos.push_back(sl.n_enc + i);
@@ -346,7 +412,9 @@ void StreamPool::tick(vox_stream_stats *st_out) {
             stats.encoder_rows += R;
             for (const Span &sp : spans) {
                 Slot &sl = slots[sp.slot];
-                CUDA_OK(cudaMemcpyAsync(enc_out + ((size_t)sp.slot * s->S_max + sl.n_enc) * d, s->h_enc + (size_t)sp.r0 * d,
+                float *eo = enc_out + (size_t)sp.slot * s->S_max * d;
+                slide(eo, d, s->S_max, sl.enc0, (int64_t)sl.n_emb * rf, sl.n_enc, sl.n_enc + sp.n, false, slide_tmp, s->st);
+                CUDA_OK(cudaMemcpyAsync(eo + (size_t)(sl.n_enc - sl.enc0) * d, s->h_enc + (size_t)sp.r0 * d,
                                         sizeof(float) * (size_t)sp.n * d, cudaMemcpyDeviceToDevice, s->st));
                 sl.n_enc += sp.n;
             }
@@ -357,8 +425,12 @@ void StreamPool::tick(vox_stream_stats *st_out) {
             if (!sl.open || sl.drained) continue;
             const int emb_t = sl.n_enc / rf, n_new = emb_t - sl.n_emb;
             if (n_new <= 0) continue;
-            const float *src = enc_out + ((size_t)id * s->S_max + (size_t)sl.n_emb * rf) * d;
-            float *dst = s->audio + ((size_t)id * s->S4_max + sl.n_emb) * D;
+            const float *src = enc_out + ((size_t)id * s->S_max + ((size_t)sl.n_emb * rf - sl.enc0)) * d;
+            // embeddings stay resident for audio_embeds_range as long as they can: when the buffer is full, the older
+            // half goes -- never one the decoder has still to read (position pos reads embedding pos)
+            float *emb = s->audio + (size_t)id * s->S4_max * D;
+            slide(emb, D, s->S4_max, sl.emb0, std::min<int64_t>(sl.pos, emb_t - s->S4_max / 2), sl.n_emb, emb_t, false, slide_tmp, s->st);
+            float *dst = emb + (size_t)(sl.n_emb - sl.emb0) * D;
             s->linear(m->adapter0, src, n_new, s->adapter_h, D, nullptr, nullptr, EPI_GELU);
             s->linear(m->adapter2, s->adapter_h, n_new, dst, D, nullptr, nullptr, EPI_NONE);
             sl.n_emb = emb_t;
@@ -367,7 +439,9 @@ void StreamPool::tick(vox_stream_stats *st_out) {
         for (int id = 0; id < max_sessions; ++id) {
             Slot &sl = slots[id];
             if (!sl.open || sl.drained || sl.pos != 0 || sl.n_emb < P) continue;
+            VOX_CHECK(sl.emb0 == 0, VOX_ECAPACITY, "stream session %d: prefill embeddings were evicted", id);
             ensure_pages(sl, P + 1);
+            if (unbounded) fill_rope(dec_rope_cos, dec_rope_sin, c.dec_head_dim, kDecRopeRing, 0, 0, P);
             upload_rows({id}, false);
             std::vector<int> prefix((size_t)P, 32);
             prefix[0] = 1;
@@ -380,6 +454,7 @@ void StreamPool::tick(vox_stream_stats *st_out) {
             CUDA_OK(cudaStreamSynchronize(s->st));
             sl.last_tok = tok;
             sl.ids.push_back(tok);
+            sl.n_ids += 1;
             sl.pos = P;  // cached positions; the next step is position P and consumes audio[P]
             stats.prefills += 1;
         }
@@ -392,15 +467,23 @@ void StreamPool::tick(vox_stream_stats *st_out) {
                 // position p = sl.pos consumes audio[p]; the offline loop stops before the last embedding (model.rs:938)
                 // (sl.pos = cached positions = index of the next position's audio embedding)
                 const int last = sl.ended ? std::min(sl.n_emb - 1, final_enc(sl) / rf - 2) : sl.n_emb - 1;
-                if (sl.pos <= last) rows.push_back(id);
+                if (sl.pos > last) continue;
+                // a RoPE ring row serves one position per launch: a row whose position meets another's waits for the
+                // next step of this loop
+                bool clash = false;
+                for (int o : rows) clash |= unbounded && slots[o].pos != sl.pos && slots[o].pos % kDecRopeRing == sl.pos % kDecRopeRing;
+                if (!clash) rows.push_back(id);
             }
             if (rows.empty()) break;
-            for (int id : rows) ensure_pages(slots[id], slots[id].pos + 1);
+            for (int id : rows) {
+                ensure_pages(slots[id], slots[id].pos + 1);
+                if (unbounded) fill_rope(dec_rope_cos, dec_rope_sin, c.dec_head_dim, kDecRopeRing, 0, slots[id].pos, 1);
+            }
             upload_rows(rows, true);
             s->audio_rows_dev = d_audio_rows;
             s->decode_step((int)rows.size(), true);
             s->audio_rows_dev = nullptr;
-            s->mega_steps_host += 1;
+            s->mega_steps_host += ((unsigned)rows.size() + 7) / 8;  // one persistent-kernel launch per group of 8 rows
             std::vector<int> toks(rows.size());
             CUDA_OK(cudaMemcpyAsync(toks.data(), s->d_tok, sizeof(int) * rows.size(), cudaMemcpyDeviceToHost, s->st));
             CUDA_OK(cudaStreamSynchronize(s->st));
@@ -408,6 +491,7 @@ void StreamPool::tick(vox_stream_stats *st_out) {
                 Slot &sl = slots[rows[i]];
                 sl.last_tok = toks[i];
                 sl.ids.push_back(toks[i]);
+                sl.n_ids += 1;
                 sl.pos += 1;
             }
             stats.decode_steps += 1;
@@ -418,7 +502,7 @@ void StreamPool::tick(vox_stream_stats *st_out) {
             if (!sl.open || sl.drained || !sl.ended) continue;
             int64_t tg[5];
             stream_progress(sl.n_samples, true, rf, P, tg);
-            if (sl.n_enc == (int)tg[2] && sl.n_emb == (int)tg[3] && (int64_t)sl.ids.size() == tg[4]) sl.drained = true;
+            if (sl.n_enc == (int)tg[2] && sl.n_emb == (int)tg[3] && sl.n_ids == tg[4]) sl.drained = true;
         }
     }
     CUDA_OK(cudaEventRecord(e1, s->st));
@@ -436,6 +520,7 @@ void StreamPool::tick(vox_stream_stats *st_out) {
 int StreamPool::encode_chunk(int id, const float *mel, int T, float *out, size_t cap) {
     const vox_model_info &c = m->info;
     Slot &sl = slot(id);
+    VOX_CHECK(!unbounded, VOX_EINVAL, "encode_chunk needs a pool with max_seconds > 0 (its output region is linear)");
     VOX_CHECK(sl.n_samples == pad_left(pad) && sl.n_audio == 0, VOX_EINVAL, "stream session %d is fed by push(): do not mix with encode_chunk", id);
     VOX_CHECK(T >= 1 && T <= s->max_mel_frames, VOX_EINVAL, "mel chunk of %d frames exceeds the pool's capacity %d", T, s->max_mel_frames);
     CUDA_OK(cudaSetDevice(m->device));
@@ -479,8 +564,47 @@ int StreamPool::final_enc(const Slot &sl) const {
 
 const float *StreamPool::audio_embeds(int id, int *n) {
     Slot &sl = slot(id);
+    VOX_CHECK(sl.emb0 == 0, VOX_ECAPACITY, "stream session %d: audio embeddings before %d were evicted; use vox_stream_audio_embeds_range",
+              id, sl.emb0);
     *n = sl.n_emb;
     return s->audio + (size_t)id * s->S4_max * m->info.dec_dim;
+}
+
+const float *StreamPool::audio_embeds_range(int id, int64_t first, int64_t n) {
+    Slot &sl = slot(id);
+    VOX_CHECK(first >= 0 && n >= 0 && first + n <= sl.n_emb, VOX_EINVAL, "stream session %d: audio embeddings [%lld, %lld) not produced yet (%d so far)",
+              id, (long long)first, (long long)(first + n), sl.n_emb);
+    VOX_CHECK(first >= sl.emb0, VOX_ECAPACITY, "stream session %d: audio embedding %lld is no longer resident (first resident: %d)", id,
+              (long long)first, sl.emb0);
+    return s->audio + ((size_t)id * s->S4_max + (size_t)(first - sl.emb0)) * m->info.dec_dim;
+}
+
+void StreamPool::session_info(int id, struct vox_stream_session_info *out) {
+    const Slot &sl = slot(id);
+    *out = {};
+    out->samples = (int64_t)sl.n_samples;
+    out->mel_frames = sl.n_mel;
+    out->encoder_frames = sl.n_enc;
+    out->audio_embeds = sl.n_emb;
+    out->first_audio_embed = sl.emb0;
+    out->decoder_positions = sl.pos;
+    out->ids_emitted = sl.n_ids;
+    out->kv_pages = (int32_t)sl.pages.size();
+}
+
+// RoPE rows of positions [p0, p0 + n) into a ring table of `rows` rows starting at row `row0`: position p at row p % rows
+void StreamPool::fill_rope(float *cos_d, float *sin_d, int hd, int rows, size_t row0, int64_t p0, int n) {
+    const int half = hd / 2;
+    std::vector<float> cv((size_t)n * half), sv((size_t)n * half);
+    rope_rows(hd, m->rope_theta, p0, n, cv.data(), sv.data());
+    for (int i = 0; i < n;) {
+        const int r = (int)((p0 + i) % rows), len = std::min(n - i, rows - r);
+        const size_t at = (row0 + r) * half;
+        CUDA_OK(cudaMemcpyAsync(cos_d + at, cv.data() + (size_t)i * half, sizeof(float) * len * half, cudaMemcpyHostToDevice, s->st));
+        CUDA_OK(cudaMemcpyAsync(sin_d + at, sv.data() + (size_t)i * half, sizeof(float) * len * half, cudaMemcpyHostToDevice, s->st));
+        i += len;
+    }
+    // (an asynchronous copy from pageable memory has consumed its source when it returns)
 }
 
 }  // namespace vox

@@ -7,30 +7,45 @@
 
 namespace vox {
 
+// Padded audio an unbounded session keeps resident on the device: its PCM, mel, conv1, encoder-output and audio-embedding
+// buffers hold this much and slide forward as the session advances.
+constexpr float kResidentSeconds = 30.0f;
+
 struct StreamPool {
+    // Counters are absolute (since the session opened).  Every audio-side buffer of a session holds a window of rows
+    // starting at absolute row *0 (pcm0, mel0, ...): always 0 in a bounded pool, whose buffers hold the whole stream.
     struct Slot {
         bool open = false, ended = false, drained = false;
         size_t n_samples = 0, n_audio = 0;        // padded samples known so far / audio samples pushed
         int n_mel = 0, n_c1 = 0, n_enc = 0, n_emb = 0;  // final frames produced per stage
         int pos = 0;                              // decoder positions cached (0: prefill pending)
         int last_tok = 0;
-        std::vector<int32_t> ids;                 // emitted ids (positions >= 38)
-        size_t polled = 0;
-        std::vector<int> pages;                   // decoder KV pages owned (logical order)
+        std::vector<int32_t> ids;                 // emitted ids not yet polled
+        int64_t n_ids = 0;                        // ids emitted (positions >= 38)
+        std::vector<int> pages;                   // decoder KV pages owned (page-table slot order)
+        size_t pcm0 = 0;                          // absolute sample / frame / row of each buffer's row 0
+        int mel0 = 0, c10 = 0, enc0 = 0, emb0 = 0;
     };
     Model *m = nullptr;
     Session *s = nullptr;       // private session: weights view, decoder state, workspaces, stream
     vox_pad_config pad{};
     int max_sessions = 0, max_new = 0, ring = 0;
+    bool unbounded = false;     // created with max_seconds = 0: no length limit, fixed device state
     size_t cap_samples = 0;
     float *pcm = nullptr;       // [slot][cap_samples] padded signal
     float *enc_out = nullptr;   // [slot][S_max][enc_dim] encoder output frames (after the final norm)
     float *ek = nullptr, *ev = nullptr;  // encoder K/V rings [layer][slot][ring][H*hd], absolute position p at p % ring
+    // unbounded pools: encoder RoPE rows [slot][ring][hd/2] (position p at p % ring, like the K/V rings) and the
+    // decoder's RoPE ring (kernels.h RopeView), filled by the host for the positions each launch computes
+    float *enc_rope_cos = nullptr, *enc_rope_sin = nullptr;
+    float *dec_rope_cos = nullptr, *dec_rope_sin = nullptr;
+    float *slide_tmp = nullptr;  // unbounded pools: bounce buffer of slide() (stream.cu), the size of the largest session buffer
     int *d_row_slot = nullptr, *d_row_pos = nullptr;
     const float **d_audio_rows = nullptr;
     std::vector<Slot> slots;
     std::vector<int> free_pages;
 
+    // max_seconds in [1, 60]: sessions up to that long, all their state resident.  0: sessions of any length.
     static StreamPool *create(Model *m, int max_sessions, float max_seconds);
     ~StreamPool();
     int open();
@@ -39,7 +54,10 @@ struct StreamPool {
     void close(int id);
     void tick(vox_stream_stats *stats);
     size_t poll(int id, int32_t *ids, size_t cap, bool *done);
-    const float *audio_embeds(int id, int *n);   // device pointer [n][dec_dim]
+    const float *audio_embeds(int id, int *n);   // device pointer [n][dec_dim]; fails once rows were evicted
+    // device pointer to resident audio embeddings [first, first + n)
+    const float *audio_embeds_range(int id, int64_t first, int64_t n);
+    void session_info(int id, struct vox_stream_session_info *out);
     // encode_audio_with_cache (model.rs:790-799): one mel chunk [128][T] (host) through the conv stem ON ITS OWN (zero
     // padding at the chunk edges, as upstream) and the encoder layers over the session's K/V rings; returns the
     // chunk's S/4 audio embeddings (host, [n][dec_dim]).  For sessions driven chunk-wise instead of push()/tick().
@@ -51,6 +69,7 @@ struct StreamPool {
     void ensure_pages(Slot &sl, int positions);
     void upload_rows(const std::vector<int> &rows, bool with_tokens);
     int final_enc(const Slot &sl) const;
+    void fill_rope(float *cos_d, float *sin_d, int hd, int rows, size_t row0, int64_t p0, int n);
 };
 
 }  // namespace vox

@@ -18,7 +18,7 @@ import math
 import os
 import struct
 import zlib
-from dataclasses import dataclass
+from dataclasses import dataclass, replace
 
 import numpy as np
 
@@ -270,6 +270,12 @@ def decoder_geometry_config(dec_window: int = 8192) -> VoxtralConfig:
     t = VoxtralConfig.tiny()
     return VoxtralConfig(enc_dim=t.enc_dim, enc_layers=t.enc_layers, enc_heads=t.enc_heads, enc_head_dim=t.enc_head_dim,
                          enc_ffn=t.enc_ffn, enc_window=t.enc_window, dec_layers=2, dec_window=dec_window, vocab=32768)
+
+
+def tiny_window_config(dec_window: int = 48) -> VoxtralConfig:
+    """The tiny model with a decoder window short enough that a reference started part-way into a long stream (empty
+    caches, absolute positions) equals the whole stream's after dec_layers x dec_window positions."""
+    return replace(VoxtralConfig.tiny(), dec_window=dec_window)
 
 
 def build_aliased_gguf_bytes(cfg: VoxtralConfig, seed: int, unique: int = 2) -> bytes:
