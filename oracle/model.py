@@ -61,11 +61,13 @@ def rms_norm(x: torch.Tensor, gamma: torch.Tensor, eps: float) -> torch.Tensor:
 
 
 class OracleModel:
-    """`dtype=torch.float64` runs the decoder side (forward_streaming from given audio embeddings: embed_tokens,
-    ada_scales, every linear, RMSNorm, RoPE, attention and softmax, lm_head) in float64 -- a high-precision reference
-    for the f32 GPU path.  The Q4 weights dequantise exactly to f32 and are cast per call (the f32 dequantisations
-    are cached, never f64 copies); the RoPE tables are the f32 tables cast, as the product uses f32 tables too.  The
-    default float32 mode is unchanged."""
+    """`dtype=torch.float64` runs the whole model in float64 -- a high-precision reference for the f32 GPU path.  The
+    encoder side: the conv stem on the f32 mel cast, with erf-GELU; every RMSNorm, Q4 linear, RoPE, attention and
+    softmax of the layers (with and without KV caches); the final norm, the x4 reshape and the adapter.  The decoder
+    side: embed_tokens, ada_scales, every linear, RMSNorm, RoPE, attention and softmax, lm_head.  The Q4 weights
+    dequantise exactly to f32 and are cast per call (the f32 dequantisations are cached, never f64 copies); the f32
+    conv weights, biases and norm gammas are cast; the RoPE tables are the f32 tables cast, as the product uses f32
+    tables too.  The default float32 mode is unchanged."""
 
     def __init__(self, gguf, threads: int = 0, exact_order_max_m: int = 8, dtype: torch.dtype = torch.float32):
         self.g = gguf if isinstance(gguf, GgufFile) else GgufFile(gguf)
@@ -76,6 +78,7 @@ class OracleModel:
         self.dtype = dtype
         c = self.cfg
         self.enc_cos, self.enc_sin = rope_tables(c.enc_head_dim, 4096, c.rope_theta)
+        self.enc_cos, self.enc_sin = self.enc_cos.to(dtype), self.enc_sin.to(dtype)
         self.dec_cos, self.dec_sin = rope_tables(c.dec_head_dim, 16384, c.rope_theta)
         self.dec_cos, self.dec_sin = self.dec_cos.to(dtype), self.dec_sin.to(dtype)
         self._f32 = {}
@@ -118,14 +121,32 @@ class OracleModel:
         return y.reshape(*lead, n)
 
     # ---- encoder ----------------------------------------------------------
-    def conv_downsample(self, mel: torch.Tensor) -> torch.Tensor:
-        """conv.rs:78-83; mel [1,128,T] -> [1, d, T/4]."""
-        x = F.conv1d(mel, self.f32(f"{ENC}.conv_layers.0.conv.weight"),
-                     self.f32(f"{ENC}.conv_layers.0.conv.bias"), stride=2, padding=1)
+    def conv_downsample(self, mel) -> torch.Tensor:
+        """conv.rs:78-83; mel [1,128,T] (f32, numpy or torch) -> [1, d, T/4] in the model's dtype."""
+        mel = torch.as_tensor(np.ascontiguousarray(mel, np.float32)).to(self.dtype)
+        x = F.conv1d(mel, self.param(f"{ENC}.conv_layers.0.conv.weight"),
+                     self.param(f"{ENC}.conv_layers.0.conv.bias"), stride=2, padding=1)
         x = F.gelu(x)
-        x = F.conv1d(x, self.f32(f"{ENC}.conv_layers.1.conv.weight"),
-                     self.f32(f"{ENC}.conv_layers.1.conv.bias"), stride=2, padding=1)
+        x = F.conv1d(x, self.param(f"{ENC}.conv_layers.1.conv.weight"),
+                     self.param(f"{ENC}.conv_layers.1.conv.bias"), stride=2, padding=1)
         return F.gelu(x)
+
+    def conv_stem(self, mel) -> torch.Tensor:
+        """The encoder's input frames: mel [1,128,T] -> [S, d]."""
+        return self.conv_downsample(mel)[0].transpose(0, 1).contiguous()
+
+    def encoder_norm(self, x: torch.Tensor) -> torch.Tensor:
+        """The encoder's final RMSNorm."""
+        return rms_norm(x, self.param(f"{ENC}.transformer.norm.weight"), self.cfg.norm_eps)
+
+    def adapter(self, enc_out: torch.Tensor) -> torch.Tensor:
+        """Reshape x4 (adapter.rs:108-122; a trailing partial group is dropped) + Q4Adapter (model.rs:745-749):
+        enc_out [S, d] -> audio_embeds [S/4, dec_dim]."""
+        rf = self.cfg.reshape_factor
+        s4 = enc_out.shape[0] // rf
+        x = enc_out[: s4 * rf].reshape(s4, self.cfg.enc_dim * rf)
+        x = F.gelu(self.linear(x, f"{ADAPTER}.0.weight"))
+        return self.linear(x, f"{ADAPTER}.2.weight")
 
     def _attention(self, q, k, v, scale, q_offset, window, causal=True):
         """q [Sq,H,hd], k/v [Skv,Hkv,hd] -> [Sq, H*hd]; masks per masking.rs:9-107."""
@@ -172,7 +193,7 @@ class OracleModel:
         c = self.cfg
         p = f"{ENC}.transformer.layers.{i}"
         s = x.shape[0]
-        h = rms_norm(x, self.f32(f"{p}.attention_norm.weight"), c.norm_eps)
+        h = rms_norm(x, self.param(f"{p}.attention_norm.weight"), c.norm_eps)
         q = self.linear(h, f"{p}.attention.wq.weight", f"{p}.attention.wq.bias")
         k = self.linear(h, f"{p}.attention.wk.weight")
         v = self.linear(h, f"{p}.attention.wv.weight", f"{p}.attention.wv.bias")
@@ -183,34 +204,28 @@ class OracleModel:
         k = apply_rope(k, self.enc_cos, self.enc_sin, 0)
         a = self._attention(q, k, v, float(np.float32(c.enc_head_dim) ** np.float32(-0.5)), 0, c.enc_window)
         x = self.linear(a, f"{p}.attention.wo.weight", f"{p}.attention.wo.bias") + x
-        h = rms_norm(x, self.f32(f"{p}.ffn_norm.weight"), c.norm_eps)
+        h = rms_norm(x, self.param(f"{p}.ffn_norm.weight"), c.norm_eps)
         gate = F.silu(self.linear(h, f"{p}.feed_forward.w1.weight"))
         up = self.linear(h, f"{p}.feed_forward.w3.weight")
         return self.linear(gate * up, f"{p}.feed_forward.w2.weight", f"{p}.feed_forward.w2.bias") + x
 
     def encoder_forward(self, mel: np.ndarray, capture: dict | None = None) -> torch.Tensor:
         """Q4AudioEncoder::forward (model.rs:425-434): mel [1,128,T] -> [S, enc_dim]."""
-        x = self.conv_downsample(torch.from_numpy(np.ascontiguousarray(mel, np.float32)))
-        x = x[0].transpose(0, 1).contiguous()
+        x = self.conv_stem(mel)
         if capture is not None:
             capture["conv"] = x.clone()
         for i in range(self.cfg.enc_layers):
             x = self.encoder_layer(x, i)
             if capture is not None:
                 capture[f"enc{i}"] = x.clone()
-        return rms_norm(x, self.f32(f"{ENC}.transformer.norm.weight"), self.cfg.norm_eps)
+        return self.encoder_norm(x)
 
     def encode_audio(self, mel: np.ndarray, capture: dict | None = None) -> torch.Tensor:
         """model.rs:783-788 -> audio_embeds [S/4, dec_dim]."""
         x = self.encoder_forward(mel, capture)
         if capture is not None:
             capture["enc_out"] = x.clone()
-        rf = self.cfg.reshape_factor
-        s4 = x.shape[0] // rf
-        x = x[: s4 * rf].reshape(s4, self.cfg.enc_dim * rf)      # adapter.rs:108-122
-        x = self.linear(x, f"{ADAPTER}.0.weight")
-        x = F.gelu(x)
-        return self.linear(x, f"{ADAPTER}.2.weight")
+        return self.adapter(x)
 
     # ---- encoder with KV cache (incremental API; SURVEY 8(f)-1: not yet behind the C ABI) -------------
     def new_encoder_cache(self, evict: bool = False):
@@ -235,7 +250,7 @@ class OracleModel:
                 cache["k"], cache["v"] = cache["k"][drop:], cache["v"][drop:]
                 base += drop
                 cache["base"] = base
-        h = rms_norm(x, self.f32(f"{p}.attention_norm.weight"), c.norm_eps)
+        h = rms_norm(x, self.param(f"{p}.attention_norm.weight"), c.norm_eps)
         q = self.linear(h, f"{p}.attention.wq.weight", f"{p}.attention.wq.bias").reshape(s, c.enc_heads, c.enc_head_dim)
         k = self.linear(h, f"{p}.attention.wk.weight").reshape(s, c.enc_heads, c.enc_head_dim)
         v = self.linear(h, f"{p}.attention.wv.weight", f"{p}.attention.wv.bias").reshape(s, c.enc_heads, c.enc_head_dim)
@@ -246,7 +261,7 @@ class OracleModel:
         a = self._attention(q, cache["k"], cache["v"], float(np.float32(c.enc_head_dim) ** np.float32(-0.5)),
                             offset - base, c.enc_window)   # masks only depend on position differences
         x = self.linear(a, f"{p}.attention.wo.weight", f"{p}.attention.wo.bias") + x
-        h = rms_norm(x, self.f32(f"{p}.ffn_norm.weight"), c.norm_eps)
+        h = rms_norm(x, self.param(f"{p}.ffn_norm.weight"), c.norm_eps)
         gate = F.silu(self.linear(h, f"{p}.feed_forward.w1.weight"))
         up = self.linear(h, f"{p}.feed_forward.w3.weight")
         return self.linear(gate * up, f"{p}.feed_forward.w2.weight", f"{p}.feed_forward.w2.bias") + x
@@ -254,20 +269,14 @@ class OracleModel:
     def encoder_forward_with_cache(self, mel: np.ndarray, enc_cache: list) -> torch.Tensor:
         """Q4AudioEncoder::forward_with_cache (model.rs:437-452): the conv stem runs on the chunk alone
         (zero padding at the chunk edges, no carried state -- as upstream), the layers extend the caches."""
-        x = self.conv_downsample(torch.from_numpy(np.ascontiguousarray(mel, np.float32)))
-        x = x[0].transpose(0, 1).contiguous()
+        x = self.conv_stem(mel)
         for i in range(self.cfg.enc_layers):
             x = self.encoder_layer_with_cache(x, i, enc_cache[i])
-        return rms_norm(x, self.f32(f"{ENC}.transformer.norm.weight"), self.cfg.norm_eps)
+        return self.encoder_norm(x)
 
     def encode_audio_with_cache(self, mel: np.ndarray, enc_cache: list) -> torch.Tensor:
         """Q4VoxtralModel::encode_audio_with_cache (model.rs:790-799)."""
-        x = self.encoder_forward_with_cache(mel, enc_cache)
-        rf = self.cfg.reshape_factor
-        s4 = x.shape[0] // rf
-        x = x[: s4 * rf].reshape(s4, self.cfg.enc_dim * rf)
-        x = F.gelu(self.linear(x, f"{ADAPTER}.0.weight"))
-        return self.linear(x, f"{ADAPTER}.2.weight")
+        return self.adapter(self.encoder_forward_with_cache(mel, enc_cache))
 
     # ---- decoder ----------------------------------------------------------
     def ada_scales(self, t_embed: np.ndarray):

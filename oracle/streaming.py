@@ -111,13 +111,13 @@ class StreamingOracle:
         return (t + 2 - 3) // 2 + 1 if t > 0 else 0
 
     def _conv_at(self, frames: list, t: int, total_in: int, w, b) -> torch.Tensor:
-        """k3 s2 p1 convolution output t from input frames 2t-1 .. 2t+1 (zeros outside [0, total_in))."""
+        """k3 s2 p1 convolution output t from input frames 2t-1 .. 2t+1 (zeros outside [0, total_in)), in w's dtype."""
         cols = []
         for idx in (2 * t - 1, 2 * t, 2 * t + 1):
             if 0 <= idx < total_in:
-                cols.append(torch.as_tensor(frames[idx]))
+                cols.append(torch.as_tensor(frames[idx]).to(w.dtype))
             else:
-                cols.append(torch.zeros(w.shape[1]))
+                cols.append(torch.zeros(w.shape[1], dtype=w.dtype))
         x = torch.stack(cols, 1)[None]                       # [1, C_in, 3]
         return F.gelu(F.conv1d(x, w, b))[0, :, 0]            # [C_out]
 

@@ -8,16 +8,16 @@ the suffix is missing can reach its outputs.  This is how a CPU reference follow
 tables: the tables are rebuilt longer with oracle.model.rope_tables' own formula (rows inside the model's tables are
 bitwise the same) and shifted so that relative cache offsets land on absolute rows.
 
-Used by tests; oracle/ stays untouched.
+Everything after the (f32) mel runs in the model's dtype: with OracleModel(dtype=torch.float64) this is a float64
+reference for a suffix of an unbounded session.  Used by tests.
 """
 from __future__ import annotations
 
 import numpy as np
 import torch
-import torch.nn.functional as F
 
 from oracle import mel as omel
-from oracle.model import ADAPTER, ENC, PREFIX_LEN, rope_tables, rms_norm
+from oracle.model import ENC, PREFIX_LEN, rope_tables
 from oracle.streaming import StreamingOracle
 
 SAMPLES_PER_POS = 2560
@@ -66,9 +66,9 @@ def suffix_reference(model, t_embed: np.ndarray, padded: np.ndarray, s0: int, id
     f0 = s0 // omel.HOP
     n = padded.size
     f1 = (n - omel.N_FFT // 2) // omel.HOP + 1                      # frame i final once samples < 160 i + 200 known
-    mel = _mel(np.asarray(padded[s0:], omel.F32), s0, f0, f1)
-    w1, b1 = model.f32(f"{ENC}.conv_layers.0.conv.weight"), model.f32(f"{ENC}.conv_layers.0.conv.bias")
-    w2, b2 = model.f32(f"{ENC}.conv_layers.1.conv.weight"), model.f32(f"{ENC}.conv_layers.1.conv.bias")
+    mel = _mel(np.asarray(padded[s0:], omel.F32), s0, f0, f1)                       # f32, as the product computes it
+    w1, b1 = model.param(f"{ENC}.conv_layers.0.conv.weight"), model.param(f"{ENC}.conv_layers.0.conv.bias")
+    w2, b2 = model.param(f"{ENC}.conv_layers.1.conv.weight"), model.param(f"{ENC}.conv_layers.1.conv.bias")
     big = 1 << 60
     t0, t1 = f0 // 2, (f1 - 2) // 2 + 1                              # conv1 output t needs mel 2t+1
     mv = _Frames(mel, f0, c.n_mels)
@@ -78,15 +78,12 @@ def suffix_reference(model, t_embed: np.ndarray, padded: np.ndarray, s0: int, id
     x = torch.stack([StreamingOracle._conv_at(None, cv, t, big, w2, b2) for t in range(e0, e1)])
     saved = (model.enc_cos, model.enc_sin, model.dec_cos, model.dec_sin)
     try:
-        model.enc_cos, model.enc_sin = extended_rope(c.enc_head_dim, e1 + 1, c.rope_theta)
+        model.enc_cos, model.enc_sin = (t.to(model.dtype) for t in extended_rope(c.enc_head_dim, e1 + 1, c.rope_theta))
         cache = [{"k": None, "v": None, "base": e0, "evict": True} for _ in range(c.enc_layers)]
         for i in range(c.enc_layers):
             x = model.encoder_layer_with_cache(x, i, cache[i])
-        x = rms_norm(x, model.f32(f"{ENC}.transformer.norm.weight"), c.norm_eps)
-        rf = c.reshape_factor
-        n_emb = x.shape[0] // rf
-        a = F.gelu(model.linear(x[:n_emb * rf].reshape(n_emb, c.enc_dim * rf), f"{ADAPTER}.0.weight"))
-        emb = model.linear(a, f"{ADAPTER}.2.weight")                  # audio embeddings p0 .. p0 + n_emb - 1
+        emb = model.adapter(model.encoder_norm(x))                    # audio embeddings p0 .. p0 + n_emb - 1
+        n_emb = emb.shape[0]
         # decoder: positions p0 .. (teacher-forced), RoPE rows shifted so that cache offset 0 is position p0
         last = min(p0 + n_emb - 1, PREFIX_LEN + len(ids) - 2)
         if n_pos is not None:

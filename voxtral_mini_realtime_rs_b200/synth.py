@@ -272,6 +272,15 @@ def decoder_geometry_config(dec_window: int = 8192) -> VoxtralConfig:
                          enc_ffn=t.enc_ffn, enc_window=t.enc_window, dec_layers=2, dec_window=dec_window, vocab=32768)
 
 
+def encoder_geometry_config(enc_window: int = 750) -> VoxtralConfig:
+    """The production encoder layer (1280, 32 x 64 heads, FFN 5120) at 2 layers, the production adapter (5120 -> 3072 ->
+    3072) and decoder_geometry_config's decoder (3072, 32:8 x 128 heads, FFN 9216, 2 layers, vocabulary 32768): every
+    encoder GEMM, matvec, attention shape and K/V ring of the full model at a size a CPU reference can follow layer by
+    layer.  `enc_window` (production 750) sets where the encoder's sliding window bites."""
+    return replace(decoder_geometry_config(), enc_dim=1280, enc_layers=2, enc_heads=32, enc_head_dim=64, enc_ffn=5120,
+                   enc_window=enc_window)
+
+
 def tiny_window_config(dec_window: int = 48) -> VoxtralConfig:
     """The tiny model with a decoder window short enough that a reference started part-way into a long stream (empty
     caches, absolute positions) equals the whole stream's after dec_layers x dec_window positions."""
