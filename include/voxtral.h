@@ -169,8 +169,16 @@ typedef struct {
 } vox_timings;
 /* max_batch concurrent streams, up to max_mel_frames mel frames per stream */
 int32_t vox_session_create(vox_model *m, int32_t max_batch, int32_t max_mel_frames, vox_session **out);
-/* TimeEmbedding::embed(delay) + the 26 ADA scale vectors (model.rs:250-255), once per session */
+/* TimeEmbedding::embed(delay) + the 26 ADA scale vectors (model.rs:250-255), once per session: every stream at
+ * delay_tokens (80 ms each; 6.0 when the session is created) */
 int32_t vox_session_set_delay(vox_session *s, float delay_tokens);
+/* stream i of every later call (encode/prefill/decode/transcribe/generate_step/forward_streaming) is conditioned on
+ * delays[i], i < b; streams >= b keep theirs.  vox_session_set_delay(d) sets every stream to d.
+ * 1 <= b <= max_batch and every delay finite and >= 0, else VOX_EINVAL; VOX_ECUDA without a device.  Each stream keeps
+ * its own ADA vectors (2 x layers x dec_dim floats, 639 KB at production geometry).  A call whose rows all have one
+ * delay runs the shared-vector kernels; rows at different delays still share one weight sweep per decode step (the
+ * kernels read each row's own ADA vectors). */
+int32_t vox_session_set_delays(vox_session *s, const float *delays, int32_t b);
 /* encode_audio (model.rs:783-788): mel [B,128,T] host -> audio_embeds [B,S,dec_dim] host (nullable);
  * seq_len = S.  The embeddings also stay resident in the session for vox_prefill/decode. */
 int32_t vox_encode_audio(vox_session *s, const float *mel, int32_t b, int32_t t_frames,
@@ -242,6 +250,11 @@ typedef struct {
  * would exceed those 30 s; encode_chunk is not available.  Absolute positions stay int32: ~248 days of audio. */
 int32_t vox_stream_pool_create(vox_model *m, int32_t max_sessions, float max_seconds, vox_stream_pool **out);
 int32_t vox_stream_open(vox_stream_pool *p, int32_t *session);
+/* the session's transcription delay in tokens (80 ms each); default 6.0 on vox_stream_open.  Only before the session's
+ * 38-position prefill has run (vox_stream_session_info.decoder_positions == 0), else VOX_EINVAL; also VOX_EINVAL for an
+ * unknown session or a delay that is not finite and >= 0.  VOX_ECUDA without a device, before the arguments are checked.
+ * Sessions at different delays share one decode step. */
+int32_t vox_stream_set_delay(vox_stream_pool *p, int32_t session, float delay_tokens);
 int32_t vox_stream_push_pcm(vox_stream_pool *p, int32_t session, const float *samples, size_t n);
 int32_t vox_stream_finish(vox_stream_pool *p, int32_t session);        /* end of utterance: right padding, pad.rs:89-103 */
 int32_t vox_stream_tick(vox_stream_pool *p, vox_stream_stats *stats /* nullable */);

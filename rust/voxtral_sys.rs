@@ -49,6 +49,7 @@ extern "C" {
     pub fn vox_session_create(m: *mut vox_model, max_batch: i32, max_mel_frames: i32,
                               out: *mut *mut vox_session) -> i32;
     pub fn vox_session_set_delay(s: *mut vox_session, delay_tokens: f32) -> i32;
+    pub fn vox_session_set_delays(s: *mut vox_session, delays: *const f32, b: i32) -> i32;
     pub fn vox_encode_audio(s: *mut vox_session, mel: *const f32, b: i32, t: i32,
                             audio_embeds: *mut f32, cap: usize, seq_len: *mut i32) -> i32;
     pub fn vox_transcribe_streaming(s: *mut vox_session, mel: *const f32, b: i32, t: i32,
@@ -89,6 +90,7 @@ extern "C" {
     // streaming sessions: Q4AudioEncoder::forward_with_cache (model.rs:437-452), encode_audio_with_cache (790-799)
     pub fn vox_stream_pool_create(m: *mut vox_model, max_sessions: i32, max_seconds: f32, out: *mut *mut vox_stream_pool) -> i32;
     pub fn vox_stream_open(p: *mut vox_stream_pool, session: *mut i32) -> i32;
+    pub fn vox_stream_set_delay(p: *mut vox_stream_pool, session: i32, delay_tokens: f32) -> i32;
     pub fn vox_stream_push_pcm(p: *mut vox_stream_pool, session: i32, samples: *const f32, n: usize) -> i32;
     pub fn vox_stream_finish(p: *mut vox_stream_pool, session: i32) -> i32;
     pub fn vox_stream_tick(p: *mut vox_stream_pool, stats: *mut vox_stream_stats) -> i32;

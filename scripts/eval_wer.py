@@ -89,7 +89,7 @@ def main():
         a = vx.peak_normalize(read_wav(u["audio"]))
         audio_s += a.size / 16000.0
         if args.streaming:
-            sid = pool.open()
+            sid = pool.open(delay=args.delay)   # a pool session has its own delay (default 6), not the model's
             ids = []
             for p in range(0, a.size, 1280):
                 pool.push(sid, a[p:p + 1280]); pool.tick(); ids += pool.poll(sid)[0]

@@ -119,6 +119,7 @@ _SIGS = {
     "vox_model_free": (None, [_P]),
     "vox_session_create": (C.c_int32, [_P, C.c_int32, C.c_int32, C.POINTER(_P)]),
     "vox_session_set_delay": (C.c_int32, [_P, C.c_float]),
+    "vox_session_set_delays": (C.c_int32, [_P, _P, C.c_int32]),
     "vox_encode_audio": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, _P, C.c_size_t, C.POINTER(C.c_int32)]),
     "vox_transcribe_streaming": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, _P, C.c_size_t, C.POINTER(C.c_int32),
                                              C.POINTER(_Timings)]),
@@ -137,6 +138,7 @@ _SIGS = {
     "vox_session_free": (None, [_P]),
     "vox_stream_pool_create": (C.c_int32, [_P, C.c_int32, C.c_float, C.POINTER(_P)]),
     "vox_stream_open": (C.c_int32, [_P, C.POINTER(C.c_int32)]),
+    "vox_stream_set_delay": (C.c_int32, [_P, C.c_int32, C.c_float]),
     "vox_stream_push_pcm": (C.c_int32, [_P, C.c_int32, _P, C.c_size_t]),
     "vox_stream_finish": (C.c_int32, [_P, C.c_int32]),
     "vox_stream_tick": (C.c_int32, [_P, _P]),
@@ -521,6 +523,12 @@ class Q4VoxtralModel:
     def set_delay(self, delay_tokens: float):
         _check(lib().vox_session_set_delay(self._s, delay_tokens))
 
+    def set_delays(self, delays):
+        """Stream i of later calls is conditioned on delays[i] (tokens of 80 ms); streams beyond len(delays) keep
+        theirs.  Rows at different delays share one decode step."""
+        d = _f32(delays).reshape(-1)
+        _check(lib().vox_session_set_delays(self._s, _ptr(d), d.size))
+
     def _mel3(self, mel):
         mel = _f32(mel)
         if mel.ndim == 2:
@@ -693,10 +701,21 @@ class StreamingPool:
                                             C.byref(self._p)))
         self.dec_dim = model.info["dec_dim"]
 
-    def open(self) -> int:
+    def open(self, delay: float | None = None) -> int:
+        """A new session, at transcription delay `delay` (tokens of 80 ms; None: the default 6.0)."""
         v = C.c_int32()
         _check(lib().vox_stream_open(self._p, C.byref(v)))
+        if delay is not None:
+            try:
+                self.set_delay(v.value, delay)
+            except VoxtralError:
+                self.close_session(v.value)
+                raise
         return v.value
+
+    def set_delay(self, session: int, delay: float):
+        """The session's transcription delay; only before its prefill (session_info()["decoder_positions"] == 0)."""
+        _check(lib().vox_stream_set_delay(self._p, session, delay))
 
     def push(self, session: int, samples):
         s = _f32(samples).reshape(-1)

@@ -513,6 +513,14 @@ int32_t vox_session_set_delay(vox_session *s, float delay) {
     s->s->set_delay(delay);
     VOX_API_END
 }
+static void require_any_device();
+int32_t vox_session_set_delays(vox_session *s, const float *delays, int32_t b) {
+    VOX_API_BEGIN
+    require_any_device();
+    REQUIRE(s); REQUIRE(delays);
+    s->s->set_delays(delays, b);
+    VOX_API_END
+}
 
 static void upload_mel(Session *s, const float *mel, int b, int t) {
     const vox_model_info &c = s->m->info;
@@ -963,6 +971,13 @@ int32_t vox_stream_audio_embeds_range(vox_stream_pool *p, int32_t session, int64
     CUDA_OK(cudaSetDevice(p->p->m->device));
     CUDA_OK(cudaStreamSynchronize(p->p->s->st));
     if (need) CUDA_OK(cudaMemcpy(out, src, sizeof(float) * need, cudaMemcpyDeviceToHost));
+    VOX_API_END
+}
+int32_t vox_stream_set_delay(vox_stream_pool *p, int32_t session, float delay_tokens) {
+    VOX_API_BEGIN
+    require_any_device();
+    REQUIRE(p);
+    p->p->set_delay(session, delay_tokens);
     VOX_API_END
 }
 int32_t vox_stream_session_info(vox_stream_pool *p, int32_t session, struct vox_stream_session_info *out) {

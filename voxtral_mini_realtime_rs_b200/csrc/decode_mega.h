@@ -44,6 +44,9 @@ struct MegaOp {
     // MG_ATTN
     float *kc = nullptr, *vc = nullptr;  // this layer's KV page pools [n_pages][Hkv][KV_PAGE][hd] (kernels.h KvView)
     int layer = 0;
+    // MG_MATVEC whose fout_gamma is layer j's ffn_norm x ADA scale (wo): j, else -1.  With per-row ADA sets
+    // (MegaParams::ffn_ada_rows) token b's fragments are scaled by ffn_ada_rows[b] + j * D instead.
+    int fout_ada_layer = -1;
 };
 
 struct MegaParams {
@@ -106,6 +109,9 @@ struct MegaParams {
     // RoPE row of position pos is pos % rope_rows of cos_t / sin_t (kernels.h KvView, RopeView)
     int ring = 0;
     int rope_rows = 0;
+    // optional [B]: each row's [L][D] ffn_norm x ADA set (streams at different transcription delays; the launch takes
+    // the per-row instantiation).  nullptr: every row uses the op table's shared fout_gamma.
+    const float *const *ffn_ada_rows = nullptr;
 };
 
 struct MegaPlan {

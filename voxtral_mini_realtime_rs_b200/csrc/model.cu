@@ -3,6 +3,7 @@
 // src/gguf/model.rs (cited per function); nothing here is a translation of its Burn code.
 #include "model.h"
 
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 
@@ -448,6 +449,10 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ri
         s->logits = s->arena.alloc_n<float>(B * c.vocab);
         s->ada = s->arena.alloc_n<float>((size_t)c.dec_layers * c.dec_dim);
         s->ffn_gamma_ada = s->arena.alloc_n<float>((size_t)c.dec_layers * c.dec_dim);
+        s->ada_sets = s->arena.alloc_n<float>(B * s->ada_set_floats());
+        s->delays.assign(B, 0.0f);
+        s->d_ada_rows = (const float **)s->arena.alloc(sizeof(float *) * B);
+        s->d_fga_rows = (const float **)s->arena.alloc(sizeof(float *) * B);
         s->t_embed = s->arena.alloc_n<float>(c.dec_dim);
         s->ada_tmp = s->arena.alloc_n<float>(c.t_cond_dim);
         s->d_pos = s->arena.alloc_n<int>(B);      // per row (kernels.h KvView::pos)
@@ -534,7 +539,7 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ri
         }
         CUDA_OK(cudaMemset(s->d_pos, 0, sizeof(int) * B));
         CUDA_OK(cudaMemset(s->d_outpos, 0, sizeof(int) * B));
-        s->set_delay(6.0f);  // CLI default --delay 6 (transcribe.rs:49-51)
+        s->set_delay(kDefaultDelay);
     } catch (...) {
         delete s;
         throw;
@@ -550,31 +555,105 @@ Session::~Session() {
 }
 
 void Session::linear(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias, const float *res,
-                     int epi, const float *gamma, const float *ada, float *tmp, const TcWork *tc) {
+                     int epi, const float *gamma, const float *ada, float *tmp, const TcWork *tc, const AdaRows &ada_rows) {
     launch_q4_linear(w, x, M, y, ldy, bias, res, epi, gamma, ada, m->norm_eps, tmp, Q4Scratch{xt_buf, xt_elems, &gemm_work, tc},
-                     path, st);
+                     path, st, ada_rows);
 }
 
 // TimeEmbedding::embed (time_embedding.rs:41-71) + the per-layer ADA scale
-// 1 + w2(gelu(w0(t)))  (model.rs:250-255), computed once: t is constant for a session.
-void Session::set_delay(float delay) {
+// 1 + w2(gelu(w0(t)))  (model.rs:250-255) into ada_dst [L][D], and ffn_norm x that scale into fga_dst [L][D].
+static void compute_ada(Session &s, float delay, float *ada_dst, float *fga_dst) {
+    const Model *m = s.m;
     const vox_model_info &c = m->info;
-    CUDA_OK(cudaSetDevice(m->device));
     std::vector<float> t(c.dec_dim);
     time_embedding(delay, c.dec_dim, t.data());
-    CUDA_OK(cudaMemcpyAsync(t_embed, t.data(), sizeof(float) * c.dec_dim, cudaMemcpyHostToDevice, st));
-    CUDA_OK(cudaStreamSynchronize(st));
+    CUDA_OK(cudaMemcpyAsync(s.t_embed, t.data(), sizeof(float) * c.dec_dim, cudaMemcpyHostToDevice, s.st));
+    CUDA_OK(cudaStreamSynchronize(s.st));
     std::vector<float> ones(c.dec_dim, 1.0f);
     for (int j = 0; j < c.dec_layers; ++j) {
-        float *dst = ada + (size_t)j * c.dec_dim;
-        CUDA_OK(cudaMemcpyAsync(dst, ones.data(), sizeof(float) * c.dec_dim, cudaMemcpyHostToDevice, st));
-        launch_q4_matvec(m->dec[j].ada0, t_embed, 1, ada_tmp, c.t_cond_dim, nullptr, nullptr, EPI_GELU, st);
+        float *dst = ada_dst + (size_t)j * c.dec_dim;
+        CUDA_OK(cudaMemcpyAsync(dst, ones.data(), sizeof(float) * c.dec_dim, cudaMemcpyHostToDevice, s.st));
+        launch_q4_matvec(m->dec[j].ada0, s.t_embed, 1, s.ada_tmp, c.t_cond_dim, nullptr, nullptr, EPI_GELU, s.st);
         // dst = 1 + w2 . gelu(...)   (residual epilogue onto the vector of ones)
-        launch_q4_matvec(m->dec[j].ada2, ada_tmp, 1, dst, c.dec_dim, nullptr, dst, EPI_RESIDUAL, st);
-        launch_mul_vec(m->dec[j].ffn_norm, dst, ffn_gamma_ada + (size_t)j * c.dec_dim, c.dec_dim, st);
+        launch_q4_matvec(m->dec[j].ada2, s.ada_tmp, 1, dst, c.dec_dim, nullptr, dst, EPI_RESIDUAL, s.st);
+        launch_mul_vec(m->dec[j].ffn_norm, dst, fga_dst + (size_t)j * c.dec_dim, c.dec_dim, s.st);
+    }
+    CUDA_OK(cudaStreamSynchronize(s.st));
+}
+
+// t is constant for a transcription: the vectors are computed once per delay, into the shared path's buffers, and
+// copied to every stream's set.
+void Session::set_delay(float delay) {
+    CUDA_OK(cudaSetDevice(m->device));
+    const size_t LD = ada_set_floats() / 2;
+    compute_ada(*this, delay, ada, ffn_gamma_ada);
+    shared_delay = delay;
+    for (int i = 0; i < max_batch; ++i) {
+        CUDA_OK(cudaMemcpyAsync(ada_sets + i * 2 * LD, ada, sizeof(float) * LD, cudaMemcpyDeviceToDevice, st));
+        CUDA_OK(cudaMemcpyAsync(ada_sets + i * 2 * LD + LD, ffn_gamma_ada, sizeof(float) * LD, cudaMemcpyDeviceToDevice, st));
+        delays[i] = delay;
     }
     CUDA_OK(cudaStreamSynchronize(st));
-    delay_set = true;
+}
+
+// delays are compared as values; set_delay accepts any float, so two NaNs count as one delay
+static bool same_delay(float a, float b) { return a == b || (std::isnan(a) && std::isnan(b)); }
+
+void Session::set_delays(const float *d, int b) {
+    VOX_CHECK(b >= 1 && b <= max_batch, VOX_EINVAL, "set_delays: %d streams out of range [1,%d]", b, max_batch);
+    for (int i = 0; i < b; ++i)
+        VOX_CHECK(std::isfinite(d[i]) && d[i] >= 0.0f, VOX_EINVAL, "delay %g of stream %d must be finite and >= 0", d[i], i);
+    CUDA_OK(cudaSetDevice(m->device));
+    for (int i = 0; i < b; ++i) set_stream_delay(i, d[i]);
+}
+
+void Session::set_stream_delay(int i, float d) {
+    if (same_delay(delays[i], d)) return;
+    const size_t n = ada_set_floats();
+    float *set = ada_sets + (size_t)i * n;
+    int same = -1;   // another stream at this delay: copy its vectors (computed by the same launches: bitwise equal)
+    for (int j = 0; j < max_batch && same < 0; ++j)
+        if (j != i && same_delay(delays[j], d)) same = j;
+    if (same >= 0) {
+        CUDA_OK(cudaMemcpyAsync(set, ada_sets + (size_t)same * n, sizeof(float) * n, cudaMemcpyDeviceToDevice, st));
+        CUDA_OK(cudaStreamSynchronize(st));
+    } else {
+        compute_ada(*this, d, set, set + n / 2);
+    }
+    delays[i] = d;
+}
+
+void Session::bind_delays(const int *streams, int n) {
+    bool uniform = true;
+    for (int i = 1; i < n; ++i) uniform &= same_delay(delays[streams[i]], delays[streams[0]]);
+    if (uniform) {
+        ada_per_row = false;
+        if (!same_delay(delays[streams[0]], shared_delay)) {
+            const size_t LD = ada_set_floats() / 2;
+            const float *set = ada_sets + (size_t)streams[0] * 2 * LD;
+            CUDA_OK(cudaMemcpyAsync(ada, set, sizeof(float) * LD, cudaMemcpyDeviceToDevice, st));
+            CUDA_OK(cudaMemcpyAsync(ffn_gamma_ada, set + LD, sizeof(float) * LD, cudaMemcpyDeviceToDevice, st));
+            shared_delay = delays[streams[0]];
+        }
+        return;
+    }
+    ada_per_row = true;
+    if (ada_row_streams.size() >= (size_t)n && std::equal(streams, streams + n, ada_row_streams.begin())) return;
+    std::vector<const float *> a(n), f(n);
+    for (int i = 0; i < n; ++i) {
+        a[i] = ada_sets + (size_t)streams[i] * ada_set_floats();
+        f[i] = a[i] + ada_set_floats() / 2;
+    }
+    CUDA_OK(cudaMemcpyAsync(d_ada_rows, a.data(), sizeof(float *) * n, cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(d_fga_rows, f.data(), sizeof(float *) * n, cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaStreamSynchronize(st));   // the staging vectors die with this frame
+    ada_row_streams.assign(streams, streams + n);
+}
+
+void Session::bind_delays_identity(int B) {
+    std::vector<int> id(B);
+    for (int b = 0; b < B; ++b) id[b] = b;
+    bind_delays(id.data(), B);
 }
 
 // Q4VoxtralModel::encode_audio (model.rs:783-788): conv -> 32 layers -> norm -> reshape x4 -> adapter
@@ -650,6 +729,7 @@ bool Session::decoder_forward(int B, int M) {
     const int D = c.dec_dim, H = c.dec_heads, Hkv = c.dec_kv_heads, hd = c.dec_head_dim;
     const int qkvd = (H + 2 * Hkv) * hd, rows = B * M;
     const float scale = powf((float)hd, -0.5f);
+    if (!stream_mode) bind_delays_identity(B);   // (a stream pool binds its rows' sessions itself)
     // decode-sized problems: RMSNorm fused into the consuming matvec, RoPE + KV append fused into the
     // attention kernel => 5 launches per layer instead of 8
     const bool fused = fused_decode(rows);
@@ -667,8 +747,12 @@ bool Session::decoder_forward(int B, int M) {
             launch_dec_attention(qkv_dec, B, M, qkvd, H, Hkv, hd, kvl, c.dec_window, scale, attn_dec, st);
         }
         linear(l.wo, attn_dec, rows, x_dec, D, nullptr, x_dec, EPI_RESIDUAL, nullptr, nullptr, nullptr, tc_res);
-        linear(l.w13, x_dec, rows, act_dec, c.dec_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, ada + (size_t)j * D, h_dec,
-               tc_norm);
+        if (ada_per_row)
+            linear(l.w13, x_dec, rows, act_dec, c.dec_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, nullptr, h_dec, tc_norm,
+                   AdaRows{d_ada_rows, M, (size_t)j * D});
+        else
+            linear(l.w13, x_dec, rows, act_dec, c.dec_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, ada + (size_t)j * D, h_dec,
+                   tc_norm);
         linear(l.w2, act_dec, rows, x_dec, D, nullptr, x_dec, EPI_RESIDUAL, nullptr, nullptr, nullptr, tc_res);
     }
     if (!fused) launch_rmsnorm(x_dec, m->dec_norm, nullptr, h_dec, rows, D, m->norm_eps, st);
@@ -761,6 +845,7 @@ bool Session::mega_prepare(int B) {
         ops.push_back(a);
         // wo: h += attn . Wo^T; leaves fragments of h x (ffn_norm x ADA) for w13
         matvec(l.wo, AF, x_dec, D, x_dec, EPI_RESIDUAL, nullptr, true, false, 2, XF, ffn_gamma_ada + (size_t)j * D);
+        ops.back().fout_ada_layer = j;   // per-row mode: each row's own ffn_norm x ADA vector of layer j
         // w13: SwiGLU of the normed stream; leaves fragments of the activation for w2 (no plain copy)
         matvec(l.w13, XF, nullptr, c.dec_ffn, nullptr, EPI_SILU_MUL, l.ffn_norm, false, false, 4, CF, nullptr);
         // w2: h += act . W2^T; leaves fragments of h x (next attention norm | final norm)
@@ -800,6 +885,7 @@ void Session::decode_step(int B, bool add_audio) {
     // 128-token tile).  The scratch activations are reused by the
     // groups; the per-row state (token, positions, page table, audio row, output row, logits) is addressed from the
     // group's first row.
+    if (!stream_mode) bind_delays_identity(B);
     const int rows_per_launch = B > 8 ? 8 : B;
     if (mega_prepare(rows_per_launch)) {
         for (int b0 = 0; b0 < B; b0 += 8) decode_step_mega(b0, std::min(8, B - b0), add_audio);
@@ -865,6 +951,7 @@ void Session::decode_step_mega(int b0, int B, bool add_audio) {
         p.audio = add_audio && audio ? audio + (size_t)b0 * cur_S4 * c.dec_dim : nullptr;
         p.audio_rows = add_audio && audio_rows_dev ? audio_rows_dev + b0 : nullptr;
         p.audio_seq = cur_S4;
+        p.ffn_ada_rows = ada_per_row ? d_fga_rows + b0 : nullptr;
         p.x_dec = x_dec;
         p.ssq_x = ssq_x;
         p.emb_fbf = mega_xf_bf;
@@ -960,7 +1047,8 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
         if (steps > 0) {
             int done = 0;
             if (use_graph) {
-                if (!step_graph || step_graph_B != B || step_graph_S4 != S4) {
+                // (prefill() has bound the rows' delays: a captured step of the other ADA mode launches other kernels)
+                if (!step_graph || step_graph_B != B || step_graph_S4 != S4 || step_graph_per_row != ada_per_row) {
                     // first step eagerly (also performs any one-time kernel attribute setup),
                     // then capture one step and replay it
                     decode_step(B);
@@ -985,6 +1073,7 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
                         cuda_check(e, "cudaGraphInstantiate");
                         step_graph_B = B;
                         step_graph_S4 = S4;
+                        step_graph_per_row = ada_per_row;
                     }
                 }
                 for (; done < steps; ++done) {

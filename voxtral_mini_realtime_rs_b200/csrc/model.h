@@ -92,6 +92,10 @@ void rope_rows(int hd, float theta, int64_t p0, int n, float *cos_out, float *si
 Q4Weight upload_q4(DeviceArena &arena, const std::vector<const uint8_t *> &raw, const std::vector<int> &n_rows,
                    int K, bool interleave, bool tc_layout = false);
 
+// transcription delay of a new session or stream session, in tokens of 80 ms: the CLI default --delay 6
+// (transcribe.rs:49-51)
+constexpr float kDefaultDelay = 6.0f;
+
 struct Session {
     Model *m = nullptr;
     int max_batch = 0, max_mel_frames = 0;
@@ -123,9 +127,21 @@ struct Session {
     float *last_h = nullptr, *logits = nullptr;
     float *logits_all = nullptr;
     size_t logits_all_cap = 0;
+    // ADA scale of the shared path (every row of a call at one delay): [L][D], and ffn_norm weight x ADA scale [L][D]
+    // (persistent decode kernel).  They hold the vectors of `shared_delay`.
     float *ada = nullptr, *t_embed = nullptr, *ada_tmp = nullptr;
-    float *ffn_gamma_ada = nullptr;  // [L][D] ffn_norm weight x ADA scale (persistent decode kernel)
-    bool delay_set = false;
+    float *ffn_gamma_ada = nullptr;
+    float shared_delay = -1.0f;  // -1: not loaded
+    // per-stream transcription delay (vox_session_set_delays): stream i's ADA set at ada_sets + i * ada_set_floats(),
+    // {ADA scale [L][D], ffn_norm x ADA scale [L][D]}
+    std::vector<float> delays;
+    float *ada_sets = nullptr;
+    size_t ada_set_floats() const { return (size_t)2 * m->info.dec_layers * m->info.dec_dim; }
+    // per-row mode (the rows of a call at different delays): row i uses stream ada_row_streams[i]'s set through the
+    // pointer tables [max_batch] (kernels.h AdaRows, MegaParams::ffn_ada_rows)
+    bool ada_per_row = false;
+    const float **d_ada_rows = nullptr, **d_fga_rows = nullptr;
+    std::vector<int> ada_row_streams;
     int *d_pos = nullptr, *d_outpos = nullptr, *d_tok = nullptr, *d_ids = nullptr, *d_out = nullptr;
     int out_ld = 0;
     int cache_len = 0;  // host mirror of d_pos[] (all rows equal) for the incremental API
@@ -136,6 +152,7 @@ struct Session {
     const float *audio_base = nullptr;
     cudaGraphExec_t step_graph = nullptr;
     int step_graph_B = 0, step_graph_S4 = 0;
+    bool step_graph_per_row = false;  // the captured step's ADA mode (its kernels and arguments differ)
     uint64_t step_graph_nodes = 0;
     bool use_graph = true;
     // scratch of the fused decode path: split-K partials + tickets, per-tile sums of squares of the
@@ -186,13 +203,22 @@ struct Session {
     // limit; the pool owner points dec_rope at its RoPE ring)
     static Session *create(Model *m, int max_batch, int max_mel_frames, bool kv_ring = false);
     ~Session();
+    // every stream at `delay` (tokens of 80 ms)
     void set_delay(float delay);
+    // stream i at delays[i] for i < b; streams >= b keep theirs
+    void set_delays(const float *delays, int b);
+    void set_stream_delay(int stream, float delay);
+    // the ADA mode of the next launches, whose row i belongs to stream streams[i]: the shared path when every row has
+    // the same delay (loading that delay's vectors into ada / ffn_gamma_ada), else per-row tables.  Launch-free and
+    // copy-free when nothing changed (so it may run inside a stream capture).
+    void bind_delays(const int *streams, int n);
+    void bind_delays_identity(int B);  // row b = stream b (every call but the stream pool's)
     // mel already on device, time-major, in s->mel_tm
     void encode(int B, int T);
     // launch_q4_linear with the session's GEMM scratch and path choice; `gamma`, `ada`, `tmp` and `tc` as there
     void linear(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias, const float *res,
                 int epi, const float *gamma = nullptr, const float *ada = nullptr, float *tmp = nullptr,
-                const TcWork *tc = nullptr);
+                const TcWork *tc = nullptr, const AdaRows &ada_rows = AdaRows{});
     bool decoder_forward(int B, int M);
     void lm_head_rows(int rows, bool norm_pending, float *dst);
     void decode_step(int B, bool add_audio = true);

@@ -239,9 +239,18 @@ int StreamPool::open() {
             sl.n_samples = pad_left(pad);
             CUDA_OK(cudaSetDevice(m->device));
             CUDA_OK(cudaMemsetAsync(pcm + (size_t)i * cap_samples, 0, sizeof(float) * cap_samples, s->st));
+            s->set_stream_delay(i, kDefaultDelay);   // a reused slot does not inherit the previous session's delay
             return i;
         }
     fail(VOX_ECAPACITY, fmt("all %d stream sessions are in use", max_sessions));
+}
+
+void StreamPool::set_delay(int id, float delay) {
+    const Slot &sl = slot(id);
+    VOX_CHECK(sl.pos == 0, VOX_EINVAL, "stream session %d: the delay can only change before its prefill has run", id);
+    VOX_CHECK(std::isfinite(delay) && delay >= 0.0f, VOX_EINVAL, "delay %g must be finite and >= 0", delay);
+    CUDA_OK(cudaSetDevice(m->device));
+    s->set_stream_delay(id, delay);
 }
 
 StreamPool::Slot &StreamPool::slot(int id) {
@@ -324,8 +333,10 @@ void StreamPool::ensure_pages(Slot &sl, int positions) {
     }
 }
 
-// rows[i] = slot id of batch row i: page tables, positions, fed-back tokens, audio pointers of this step
+// rows[i] = slot id of batch row i: page tables, positions, fed-back tokens, audio pointers of this step, and the rows'
+// delays (the shared ADA path when they are equal, else the per-row tables of the sessions' ADA sets)
 void StreamPool::upload_rows(const std::vector<int> &rows, bool with_tokens) {
+    s->bind_delays(rows.data(), (int)rows.size());
     const vox_model_info &c = m->info;
     const int nb = (int)rows.size(), mp = s->kv_max_pages;
     std::vector<int> pt((size_t)nb * mp, 0), pos(nb), tok(nb), zero(nb, 0);

@@ -48,7 +48,9 @@ struct StreamPool {
     // max_seconds in [1, 60]: sessions up to that long, all their state resident.  0: sessions of any length.
     static StreamPool *create(Model *m, int max_sessions, float max_seconds);
     ~StreamPool();
-    int open();
+    int open();   // the new session runs at kDefaultDelay
+    // the session's transcription delay (its own ADA set); only before its prefill has run
+    void set_delay(int id, float delay);
     void push(int id, const float *samples, size_t n);
     void finish(int id);
     void close(int id);
