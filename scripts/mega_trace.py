@@ -53,7 +53,7 @@ def main():
         a[5] += t3 - t2            # grid barrier
         a[6] += t3 - t0
     step = (tm.decode_ms - tm.prefill_ms) / max(1, tm.decode_tokens - 1)
-    print(f"B={B}: step (graph) {step:.3f} ms; traced kernel span {tr[n - 1][2] - tr[0][0]:.1f} us; flags {os.environ.get('VOX_MEGA_FLAGS', '0')}")
+    print(f"B={B}: step (graph) {step:.3f} ms; traced kernel span {tr[n - 1][2] - tr[0][0]:.1f} us")
     print(f"{'op':8s} {'n':>3s} {'stage':>7s} {'w-wait':>7s} {'loop':>7s} {'tail':>7s} {'barrier':>7s} | {'sum':>7s}  (mean us)  total us")
     for nm, (c, s, w, l, t, g, tot) in agg.items():
         print(f"{nm:8s} {c:3d} {s / c:7.2f} {w / c:7.2f} {l / c:7.2f} {t / c:7.2f} {g / c:7.2f} | {tot / c:7.2f}   {tot:9.1f}")

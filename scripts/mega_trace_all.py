@@ -43,7 +43,7 @@ def main():
     per_layer = ["qkv", "attn", "wo", "w13", "w2"]
     names = ["embed"] + per_layer * ((n - 3) // len(per_layer)) + ["lm_head", "argmax"]
     step = (tm.decode_ms - tm.prefill_ms) / max(1, tm.decode_tokens - 1)
-    print(f"B={B}: step (graph) {step:.3f} ms; flags {os.environ.get('VOX_MEGA_FLAGS', '0')}")
+    print(f"B={B}: step (graph) {step:.3f} ms")
     # SM clocks are not mutually synchronised (and drift): every CTA is measured against ITS OWN exit from the previous
     # grid barrier -- all CTAs leave a barrier within one L2 round trip of each other, so these offsets are comparable.
     agg = {}
@@ -73,15 +73,6 @@ def main():
         print(f"{nm:8s} {c:3d} {a['ready'] / c:7.2f} {a['p10'] / c:7.2f} {a['p50'] / c:7.2f} {a['p90'] / c:7.2f} {a['mx'] / c:7.2f} {a['phase'] / c:7.2f} "
               f"{(a['phase'] - a['mx']) / c:7.2f} | {a['phase']:8.1f}")
     print(f"sum of phases {tot:.1f} us")
-    tw = model.debug("mega_trace_w")
-    if tw is not None:
-        tw = tw.reshape(16, 6, 8)
-        print("warp-level trace, CTA 0, op " + os.environ.get("VOX_MEGA_TRACE_W_OP", "lm_head") + " (SM cycles since the first stamp): per group = start, "
-              "stage1, stage2, stage3 ready, body done, group barrier passed, epilogue done, (reducers) partials summed")
-        for gidx in range(6):
-            print(f" group {gidx}")
-            for w in range(16):
-                print("   w%02d " % w + " ".join(f"{int(v):7d}" for v in tw[w, gidx, :8]))
 
 
 if __name__ == "__main__":

@@ -1,7 +1,7 @@
 // mg_pair_bench.cu -- the M = 8 weight-loop body of decode_mega.cu (mg_pair<8,2,2>: 2 tiles x 2 blocks, 16 chained
 // m16n8k16 + unpack + scale FMAs) timed in isolation: operands resident in shared memory, no TMA ring, no mbarriers,
 // 1 CTA per SM.  Cycles per call and warp for 4/8/16 resident warps and with parts of the body removed -- which pipe (or
-// which latency) sets the ~1300 cycles per ring stage seen in the kernel's warp trace?
+// which latency) sets the ~1300 cycles per ring stage that the kernel's weight loop was measured to take?
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o mg_pair_bench mg_pair_bench.cu
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>

@@ -22,8 +22,6 @@ CXX_SOURCES = ["gguf.cpp", "audio_host.cpp", "tokenizer.cpp"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=default"]
 CXX_FLAGS = ["-O2", "-std=c++17", "-fPIC", "-Wall"]
-# extra nvcc flags for instrumented builds (e.g. VOX_NVCC_EXTRA="-DVOX_MEGA_WARP_TRACE"); rebuild with force=True
-NVCC_FLAGS += os.environ.get("VOX_NVCC_EXTRA", "").split()
 
 
 def _nvcc() -> str:

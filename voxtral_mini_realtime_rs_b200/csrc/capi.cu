@@ -23,7 +23,6 @@ void set_last_error(const std::string &m) { g_last_error = m; }
 }  // namespace vox
 
 using namespace vox;
-namespace vox { void set_tc_pdl(bool on); }
 
 #define VOX_API_BEGIN try {
 #define VOX_API_END                                \
@@ -782,11 +781,6 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
         s->use_graph = false;
         if (n_floats) *n_floats = 0;
         return VOX_OK;
-    } else if (w == "pdl_off" || w == "pdl_on") {
-        set_tc_pdl(w == "pdl_on");
-        if (s->step_graph) { cudaGraphExecDestroy(s->step_graph); s->step_graph = nullptr; }
-        if (n_floats) *n_floats = 0;
-        return VOX_OK;
     } else if (w == "enc_attn_simt" || w == "enc_attn_tc") {
         s->use_enc_attn_tc = (w == "enc_attn_tc");
         if (n_floats) *n_floats = 0;
@@ -799,7 +793,6 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
         // mega_on / mega_auto: persistent decode kernel for every batch size (the default policy since round 2: it is no
         // slower than the per-op launches even for a single stream); mega_off: per-op launches
         s->use_mega = (w != "mega_off");
-        s->mega_min_B = 1;
         s->mega_B = 0;
         if (s->step_graph) { cudaGraphExecDestroy(s->step_graph); s->step_graph = nullptr; }
         if (n_floats) *n_floats = 0;
@@ -826,21 +819,6 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
             int khz = 0;
             CUDA_OK(cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, s->m->device));
             for (size_t i = 0; i < cnt; ++i) out[i] = (float)((double)(t[i] - t[0]) / ((double)khz * 1e-3));
-        }
-        return VOX_OK;
-    } else if (w == "mega_trace_w") {
-        // [16 warps][6 groups][8] SM cycles relative to the earliest stamp (CTA 0, lm_head phase)
-        VOX_CHECK(s->mega_trace_w != nullptr, VOX_ENOTFOUND, "warp trace not enabled (VOX_MEGA_TRACE_ALL=1 at session creation)");
-        const size_t cnt = 16 * 6 * 8;
-        if (n_floats) *n_floats = cnt;
-        if (out) {
-            VOX_CHECK(cap >= cnt, VOX_ECAPACITY, "debug_read capacity %zu < %zu", cap, cnt);
-            CUDA_OK(cudaStreamSynchronize(s->st));
-            std::vector<unsigned long long> t(cnt);
-            CUDA_OK(cudaMemcpy(t.data(), s->mega_trace_w, sizeof(unsigned long long) * cnt, cudaMemcpyDeviceToHost));
-            unsigned long long t0 = ~0ull;
-            for (auto v : t) if (v != 0 && v < t0) t0 = v;
-            for (size_t i = 0; i < cnt; ++i) out[i] = t[i] ? (float)(t[i] - t0) : -1.0f;
         }
         return VOX_OK;
     } else if (w == "mega_trace_all") {

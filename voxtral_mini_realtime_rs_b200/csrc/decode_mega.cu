@@ -289,10 +289,8 @@ __device__ __forceinline__ void mg_pair(const unsigned char *__restrict__ sb, co
     }
     // the warp's share of the stage is in registers: hand the stage back to the producer BEFORE the arithmetic (the ring
     // is only a few stages deep at 8 tokens -- the refill latency, not the MMAs, then sets the pace)
-    if (release != nullptr) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(release);
-    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(release);
 #pragma unroll
     for (int bb = 0; bb < 2; ++bb) {
         if constexpr (MT == 8) {
@@ -419,7 +417,6 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
             // weights are read once per step: evict-first keeps the KV cache, the activations and the norm
             // vectors resident in L2 under the 1.9 GB/step weight stream
             const uint64_t pol = policy_evict_first();
-            const int flags = p.flags;
             for (int oi = 0; oi < p.n_ops; ++oi) {
                 const MegaOp &op = p.ops[oi];
                 // pull what the consumers touch first in the NEXT phase into L2 now
@@ -429,14 +426,14 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                         // one row's vector per CTA, from the CTA that pulls a shared vector on: a producer that walked
                         // the whole pointer table would hold back its own weight stream and make its CTA the straggler
                         const int who = (cta - oi % nctas + nctas) % nctas;
-                        if (nx.kind == MG_MATVEC && !(flags & 4)) {
+                        if (nx.kind == MG_MATVEC) {
                             if (nx.fout_ada_layer >= 0) {
                                 if (who < B) bulk_prefetch_l2(p.ffn_ada_rows[who] + (size_t)nx.fout_ada_layer * p.D, (uint32_t)nx.N * 4u);
                             } else if (who == 0 && nx.fout_gamma) {
                                 bulk_prefetch_l2(nx.fout_gamma, (uint32_t)nx.N * 4u);
                             }
                         }
-                    } else if (nx.kind == MG_MATVEC && (oi % nctas) == cta && !(flags & 4)) {
+                    } else if (nx.kind == MG_MATVEC && (oi % nctas) == cta) {
                         if (nx.fout_gamma) bulk_prefetch_l2(nx.fout_gamma, (uint32_t)nx.N * 4u);
                     }
                 }
@@ -457,13 +454,8 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                             mbar_expect_tx(&full[stage], (uint32_t)(nt * nb) * 576u);
                             for (int u = 0; u < nt; ++u) {
                                 const size_t pair0 = (size_t)mg_tile_of(it + u, UT, cta, nctas) * n_pairs + pb + c0;
-                                if (flags & 1) {
-                                    bulk_g2s(dst + (size_t)u * MG_SLOT_BYTES, qs + pair0 * 32, (uint32_t)nb * 512u, &full[stage]);
-                                    bulk_g2s(dst + (size_t)u * MG_SLOT_BYTES + MG_SLOT_Q, ds + pair0 * 8, (uint32_t)nb * 64u, &full[stage]);
-                                } else {
-                                    bulk_g2s_hint(dst + (size_t)u * MG_SLOT_BYTES, qs + pair0 * 32, (uint32_t)nb * 512u, &full[stage], pol);
-                                    bulk_g2s_hint(dst + (size_t)u * MG_SLOT_BYTES + MG_SLOT_Q, ds + pair0 * 8, (uint32_t)nb * 64u, &full[stage], pol);
-                                }
+                                bulk_g2s_hint(dst + (size_t)u * MG_SLOT_BYTES, qs + pair0 * 32, (uint32_t)nb * 512u, &full[stage], pol);
+                                bulk_g2s_hint(dst + (size_t)u * MG_SLOT_BYTES + MG_SLOT_Q, ds + pair0 * 8, (uint32_t)nb * 64u, &full[stage], pol);
                             }
                             if (++stage == nstage) {
                                 stage = 0;
@@ -512,7 +504,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                     // (run by the last epilogue thread, which has nothing to do until the first tile group arrives: on the
                     // consumers' thread 0 the dependent loads of positions and page table delayed the fragment copies of the
                     // qkv phase by ~1.3 us)
-                    if (e == MG_ETHREADS - 1 && oi + 1 < p.n_ops && !(p.flags & 2)) {
+                    if (e == MG_ETHREADS - 1 && oi + 1 < p.n_ops) {
                         // the next phase is this layer's attention: pull this CTA's chunk of the KV cache into L2 now, so the
                         // walk does not wait on DRAM behind the weight stream
                         const MegaOp &nx = p.ops[oi + 1];
@@ -757,10 +749,9 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
 
     // =========================== consumers ===========================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(MG_REGS_CONSUMER));
-    const int epoch = *p.d_epoch;  // decode steps run by this session so far (attention chunk flags)
+    const int epoch = *p.d_epoch;  // decode steps run by this session so far (tags of the attention chunk states)
     int stage = 0;
     uint32_t phase = 0, stg_phase = 0;
-    const bool early_release = !(p.flags & 32);  // flag 32: experiment -- release a stage after the arithmetic
     int par = 0, group_ctr = 0;
     unsigned bar_target = 0;
 
@@ -844,15 +835,6 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                     // share one read of the activation fragments
                     for (int it = 0; it < ntl; it += NT) {
                         const int nt = min(NT, ntl - it);
-#ifdef VOX_MEGA_WARP_TRACE
-                        // warp-level trace of the lm_head phase's first groups (CTA 0; debug "mega_trace_w")
-                        unsigned long long *tw = nullptr;
-                        if (p.trace_w != nullptr && cta == 0 && lane == 0 && oi == p.n_ops - 2 && s == 0 && it / NT < 6)
-                            tw = p.trace_w + ((size_t)warp * 6 + it / NT) * 8;
-                        if (tw) tw[0] = (unsigned long long)clock64();
-#else
-                        constexpr unsigned long long *tw = nullptr;   // compile with -DVOX_MEGA_WARP_TRACE to record
-#endif
                         float acc[NT][2 * CG];
 #pragma unroll
                         for (int u = 0; u < NT; ++u)
@@ -874,21 +856,16 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                                 mbar_wait(&full[stage], phase, wd_flag, 0x200u + (unsigned)oi);
                                 if (tracing && s == 0 && it == 0 && c0 == 0) p.trace[oi * 6 + 4] = (unsigned long long)clock64();
                                 if (tr_all && s == 0 && it == 0 && c0 == 0) ta[3] = (unsigned long long)clock64();
-                                if (tw && c0 / MG_CHUNK < 3) tw[1 + c0 / MG_CHUNK] = (unsigned long long)clock64();
                                 const int pp = c0 + warp;  // pair index inside the slice
-                                if (pp < np && !(p.flags & 16)) {   // flag 16: experiment -- consume the ring without the arithmetic
+                                if (pp < np) {
                                     const unsigned char *sb = ring + (size_t)stage * (NT * MG_SLOT_BYTES);
                                     const uint2 *bfp = bf + (size_t)pp * (2 * 16 * MT);
                                     const float2 *ofp = off2 + (size_t)pp * (2 * MT);
-                                    uint64_t *rel = early_release ? &empty[stage] : nullptr;
+                                    uint64_t *const rel = &empty[stage];   // released by mg_pair once the warp's loads are done
                                     if (nt == NT) mg_pair<MT, NT, NT>(sb, slot_q, slot_d, bfp, ofp, g, t, lane, acc, rel);
                                     else if (NT > 1 && nt == 1) mg_pair<MT, NT, 1>(sb, slot_q, slot_d, bfp, ofp, g, t, lane, acc, rel);
                                     else if (NT > 2 && nt == 2) mg_pair<MT, NT, 2>(sb, slot_q, slot_d, bfp, ofp, g, t, lane, acc, rel);
                                     else if (NT > 3 && nt == 3) mg_pair<MT, NT, 3>(sb, slot_q, slot_d, bfp, ofp, g, t, lane, acc, rel);
-                                    if (!early_release) {
-                                        __syncwarp();
-                                        if (lane == 0) mbar_arrive(&empty[stage]);
-                                    }
                                 } else {
                                     __syncwarp();
                                     if (lane == 0) mbar_arrive(&empty[stage]);
@@ -900,7 +877,6 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                             }
                         }
                         if (tracing && s + 1 == S && it + NT >= ntl) p.trace[oi * 6 + 5] = (unsigned long long)clock64();
-                        if (tw) tw[4] = (unsigned long long)clock64();
                         // ---- the 16 warps' partial sums of these tiles meet in shared memory: red[par] is handed to the epilogue
                         // warps (they read it, run the epilogue, and give it back two groups later); this warp goes straight on
                         // to the next group's weight stream
@@ -927,9 +903,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                             }
                         }
                         hbar_arrive(MG_BAR_FULL + par, true);
-                        if (tw) tw[5] = (unsigned long long)clock64();
                         ++group_ctr;
-                        if (tw) tw[6] = (unsigned long long)clock64();
                         par ^= 1;
                     }
                 }

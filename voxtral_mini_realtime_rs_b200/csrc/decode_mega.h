@@ -66,7 +66,6 @@ struct MegaParams {
     // chunk states as 8-byte words {value, tag}, tag = epoch * 64 + layer + 1 (unique per decode step and layer, never 0):
     float *att_acc = nullptr;     // [B*Hkv*chunks][G][hd][2] unnormalised weighted V per chunk
     float *att_ml = nullptr;      // [B*Hkv*chunks][G][2][2]  running max, sum of exp
-    int *att_flags = nullptr;     // (unused since the chunk states carry their tag in-word; kept for ABI stability of the struct)
     int *d_epoch = nullptr;       // decode steps executed by this session (never reset)
     // embedding (row-major planes of the tied table)
     const uint4 *emb_qs = nullptr;
@@ -97,13 +96,6 @@ struct MegaParams {
     // optional all-CTA trace [grid][n_ops][4]: op start, body done, barrier passed, first weights ready / KV walk
     // start (SM clocks; the host aligns the CTAs on their exit from the first grid barrier)
     unsigned long long *trace_all = nullptr;
-    // optional warp-level trace of CTA 0's first 6 tile groups of the lm_head phase: [16 warps][6 groups][8 stamps]
-    unsigned long long *trace_w = nullptr;
-    int trace_w_op = -1;   // op index the warp trace records (-1: the lm_head phase)
-    // experiment switches (VOX_MEGA_FLAGS): 1 no evict-first hint on the weight stream, 2 no KV-cache L2 prefetch, 4 no norm-weight
-    // prefetch, 16 weight loop without the arithmetic (garbage results: measures the memory pipeline alone), 32 ring stages
-    // released after the arithmetic (instead of right after the warp's loads of the stage)
-    int flags = 0;
     float *logits_out = nullptr;  // != nullptr: where the lm_head op writes its rows (row groups of a larger batch)
     // sessions of an unbounded stream pool: page_table rows are rings of max_pages slots, positions are uncapped and
     // RoPE row of position pos is pos % rope_rows of cos_t / sin_t (kernels.h KvView, RopeView)

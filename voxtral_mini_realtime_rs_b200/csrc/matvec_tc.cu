@@ -38,15 +38,12 @@
 //   kcol 2t -> 4t, 2t+1 -> 4t+2, 2t+8 -> 4t+1, 2t+9 -> 4t+3   (B fragments are staged to match).
 #include <cuda_fp16.h>
 
-#include <cstdlib>
-
 #include "common.h"
 #include "kernels.h"
 
 namespace vox {
 
 void tc_count_launch(const char *name);
-void set_tc_pdl(bool on);
 
 namespace {
 
@@ -451,22 +448,16 @@ __global__ void __launch_bounds__(TC_THREADS) q4_matvec_tc_kernel(const Args a) 
     }
 }
 
-// programmatic dependent launch between consecutive decode kernels (VOX_PDL=0 disables)
-bool g_tc_pdl = !(getenv("VOX_PDL") && getenv("VOX_PDL")[0] == '0');
-
 // K slices of a split-K launch over n_pairs block pairs at M rows: at most 64 (M <= 2), 32 (M <= 4) or 16 pairs per
-// slice.  Tuning knob (environment, read once): VOX_TC_PS = K pairs per slice for M > 4.
+// slice.
 int tc_slices(int M, int n_pairs) {
-    static const int env_ps = getenv("VOX_TC_PS") ? atoi(getenv("VOX_TC_PS")) : 0;
-    const int ps_max = M <= 2 ? 64 : (M <= 4 ? 32 : (env_ps > 0 ? env_ps : 16));
+    const int ps_max = M <= 2 ? 64 : (M <= 4 ? 32 : 16);
     return (n_pairs + ps_max - 1) / ps_max;
 }
 
 template <int M, int EPI, typename Args = TcArgs>
 void tc_launch_t(Args a, const TcWork *wk, cudaStream_t st) {
     // ---- work decomposition
-    // tuning knob (environment, read once): VOX_TC_CTAS = target resident CTAs per SM when several tokens share the staging
-    static const int env_ctas = getenv("VOX_TC_CTAS") ? atoi(getenv("VOX_TC_CTAS")) : 0;
     int S = 1;
     if (wk && wk->partial && wk->counters) S = tc_slices(M, a.n_pairs);
     int Ps = (a.n_pairs + S - 1) / S;
@@ -481,7 +472,7 @@ void tc_launch_t(Args a, const TcWork *wk, cudaStream_t st) {
     // the activation staging is per CTA: with several tokens it is a sizeable share of the work, so
     // give each CTA enough tiles to amortise it while keeping ~4 CTAs per SM in flight
     if (M > 2) {
-        const int ctas = env_ctas > 0 ? env_ctas : 4;
+        constexpr int ctas = 4;
         const int tg_occ = (int)(((size_t)a.n_tiles * S + VOX_NUM_SMS * ctas - 1) / (VOX_NUM_SMS * ctas));
         if (tg_occ > TG) TG = tg_occ > 16 ? 16 : tg_occ;
     }
@@ -505,11 +496,12 @@ void tc_launch_t(Args a, const TcWork *wk, cudaStream_t st) {
     cfg.blockDim = dim3(TC_THREADS);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
+    // programmatic dependent launch: the kernel's prologue overlaps the tail of the previous decode kernel
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = g_tc_pdl ? 1 : 0;
+    cfg.numAttrs = 1;
     cuda_check_tc(cudaLaunchKernelEx(&cfg, q4_matvec_tc_kernel<M, EPI, Args>, a), "cudaLaunchKernelEx(q4_matvec_tc)");
     tc_count_launch("q4_matvec_tc");
 }
@@ -536,8 +528,6 @@ void tc_launch_m(const TcArgs &a, const TcWork *wk, int epi, cudaStream_t st, co
 }
 
 }  // namespace
-
-void set_tc_pdl(bool on) { g_tc_pdl = on; }
 
 void launch_q4_matvec_tc_ex(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias,
                             const float *res, int epi, const float *gamma, const float *ada, float eps,

@@ -495,7 +495,6 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ri
         {   // persistent decode-step kernel
             const char *mv = getenv("VOX_MEGA");
             s->use_mega = !(mv && mv[0] == '0');
-            if (const char *mb = getenv("VOX_MEGA_MIN_B")) s->mega_min_B = atoi(mb);
             s->mega_grid = decode_mega_grid(m->device);
             s->mega_ops_cap = 6 * c.dec_layers + 4;
             s->mega_ops = s->arena.alloc_n<MegaOp>(s->mega_ops_cap);
@@ -506,9 +505,7 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ri
             s->mega_att_units = std::max(s->mega_grid, 8 * c.dec_kv_heads) + 8 * c.dec_kv_heads;
             s->mega_att_acc = s->arena.alloc_n<float>((size_t)2 * s->mega_att_units * (c.dec_heads / c.dec_kv_heads) * c.dec_head_dim);  // {value, tag}
             s->mega_att_ml = s->arena.alloc_n<float>((size_t)2 * s->mega_att_units * (c.dec_heads / c.dec_kv_heads) * 2);  // {value, tag}
-            s->mega_att_flags = s->arena.alloc_n<int>(s->mega_att_units);
             s->mega_epoch = s->arena.alloc_n<int>(1);
-            CUDA_OK(cudaMemset(s->mega_att_flags, 0, sizeof(int) * s->mega_att_units));
             // chunk states carry their own validity tag (decode step, layer): never 0
             CUDA_OK(cudaMemset(s->mega_att_acc, 0, sizeof(float) * 2 * s->mega_att_units * (c.dec_heads / c.dec_kv_heads) * c.dec_head_dim));
             CUDA_OK(cudaMemset(s->mega_att_ml, 0, sizeof(float) * 2 * s->mega_att_units * (c.dec_heads / c.dec_kv_heads) * 2));
@@ -532,8 +529,6 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ri
                     const size_t n = (size_t)s->mega_grid * s->mega_ops_cap * 4;
                     s->mega_trace_all = s->arena.alloc_n<unsigned long long>(n);
                     CUDA_OK(cudaMemset(s->mega_trace_all, 0, sizeof(unsigned long long) * n));
-                    s->mega_trace_w = s->arena.alloc_n<unsigned long long>(16 * 6 * 8);
-                    CUDA_OK(cudaMemset(s->mega_trace_w, 0, sizeof(unsigned long long) * 16 * 6 * 8));
                 }
             }
         }
@@ -771,7 +766,7 @@ void Session::lm_head_rows(int rows, bool norm_pending, float *dst) {
 // the shapes are outside what decode_mega.cu is instantiated for; the caller then uses per-op launches.
 bool Session::mega_prepare(int B) {
     const vox_model_info &c = m->info;
-    if (!use_mega || !path.matvec_tc || !fused_decode(B) || B < mega_min_B) return false;
+    if (!use_mega || !path.matvec_tc || !fused_decode(B)) return false;
     if (!decode_mega_supported(B, c.dec_heads, c.dec_kv_heads, c.dec_head_dim)) return false;
     if (mega_B == B) return mega_n_ops > 0;
     mega_B = B;
@@ -863,17 +858,21 @@ bool Session::mega_prepare(int B) {
     if ((D + 15) / 16 != parts || D % 32 != 0) ok = false;
     if (!ok || (int)ops.size() > mega_ops_cap) return false;
     // padding tokens (capacity MT > B) and padding blocks must read as zero fragments
+    mega_clear_fragments();
+    mega_ops_host = ops;
+    CUDA_OK(cudaMemcpyAsync(mega_ops, mega_ops_host.data(), sizeof(MegaOp) * ops.size(), cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    mega_n_ops = (int)ops.size();
+    return true;
+}
+
+void Session::mega_clear_fragments() {
     CUDA_OK(cudaMemsetAsync(mega_xf_bf, 0, sizeof(uint2) * mega_xf_blocks * 16 * 8, st));
     CUDA_OK(cudaMemsetAsync(mega_af_bf, 0, sizeof(uint2) * mega_af_blocks * 16 * 8, st));
     CUDA_OK(cudaMemsetAsync(mega_cf_bf, 0, sizeof(uint2) * mega_cf_blocks * 16 * 8, st));
     CUDA_OK(cudaMemsetAsync(mega_xf_off, 0, sizeof(float2) * mega_xf_blocks * 8, st));
     CUDA_OK(cudaMemsetAsync(mega_af_off, 0, sizeof(float2) * mega_af_blocks * 8, st));
     CUDA_OK(cudaMemsetAsync(mega_cf_off, 0, sizeof(float2) * mega_cf_blocks * 8, st));
-    mega_ops_host = ops;
-    CUDA_OK(cudaMemcpyAsync(mega_ops, mega_ops_host.data(), sizeof(MegaOp) * ops.size(), cudaMemcpyHostToDevice, st));
-    CUDA_OK(cudaStreamSynchronize(st));
-    mega_n_ops = (int)ops.size();
-    return true;
 }
 
 // One autoregressive step for B streams (model.rs:938-960): embed(prev token) + audio[pos-1],
@@ -906,12 +905,7 @@ void Session::decode_step_mega(int b0, int B, bool add_audio) {
         if (B < mega_B) {
             // a ragged last group on the 8-token instantiation: its padding tokens must read as zero fragments, not as
             // the previous group's rows
-            CUDA_OK(cudaMemsetAsync(mega_xf_bf, 0, sizeof(uint2) * mega_xf_blocks * 16 * 8, st));
-            CUDA_OK(cudaMemsetAsync(mega_af_bf, 0, sizeof(uint2) * mega_af_blocks * 16 * 8, st));
-            CUDA_OK(cudaMemsetAsync(mega_cf_bf, 0, sizeof(uint2) * mega_cf_blocks * 16 * 8, st));
-            CUDA_OK(cudaMemsetAsync(mega_xf_off, 0, sizeof(float2) * mega_xf_blocks * 8, st));
-            CUDA_OK(cudaMemsetAsync(mega_af_off, 0, sizeof(float2) * mega_af_blocks * 8, st));
-            CUDA_OK(cudaMemsetAsync(mega_cf_off, 0, sizeof(float2) * mega_cf_blocks * 8, st));
+            mega_clear_fragments();
         }
         MegaParams p;
         p.ops = mega_ops;
@@ -937,13 +931,8 @@ void Session::decode_step_mega(int b0, int B, bool add_audio) {
         // for the other chunks' states one after the other (an L2 round trip each), and a CTA walks 64 keys per round
         // trip anyway, so more chunks add merge latency without shortening the walk
         p.attn_chunks = std::max(1, std::min(4, std::min(mega_grid, mega_att_units - 8 * c.dec_kv_heads) / (B * c.dec_kv_heads)));
-        {
-            static const int env_nc = getenv("VOX_MEGA_NC") ? atoi(getenv("VOX_MEGA_NC")) : 0;
-            if (env_nc > 0 && env_nc <= p.attn_chunks) p.attn_chunks = env_nc;
-        }
         p.att_acc = mega_att_acc;
         p.att_ml = mega_att_ml;
-        p.att_flags = mega_att_flags;
         p.d_epoch = mega_epoch;
         p.emb_qs = m->tok_emb.qs;
         p.emb_d = m->tok_emb.d;
@@ -972,15 +961,6 @@ void Session::decode_step_mega(int b0, int B, bool add_audio) {
         p.scratch_bytes = mega_plan.scratch_bytes;
         p.trace = mega_trace;
         p.trace_all = mega_trace_all;
-        p.trace_w = mega_trace_w;
-        {
-            static const int env_two = getenv("VOX_MEGA_TRACE_W_OP") ? atoi(getenv("VOX_MEGA_TRACE_W_OP")) : -1;
-            p.trace_w_op = env_two;
-        }
-        {
-            static const int env_flags = getenv("VOX_MEGA_FLAGS") ? atoi(getenv("VOX_MEGA_FLAGS")) : 0;
-            p.flags = env_flags;
-        }
         launch_decode_mega(p, mega_plan, mega_grid, st);
     }
 }
@@ -1016,7 +996,6 @@ void Session::rebase_epoch() {
     if (mega_steps_host > (1u << 24)) {
         const vox_model_info &ci = m->info;
         const size_t gq = (size_t)(ci.dec_heads / ci.dec_kv_heads);
-        CUDA_OK(cudaMemsetAsync(mega_att_flags, 0, sizeof(int) * mega_att_units, st));
         CUDA_OK(cudaMemsetAsync(mega_att_acc, 0, sizeof(float) * 2 * mega_att_units * gq * ci.dec_head_dim, st));
         CUDA_OK(cudaMemsetAsync(mega_att_ml, 0, sizeof(float) * 2 * mega_att_units * gq * 2, st));
         CUDA_OK(cudaMemsetAsync(mega_epoch, 0, sizeof(int), st));

@@ -165,7 +165,6 @@ struct Session {
     // persistent decode-step kernel (decode_mega.cu): op table per batch size, grid barrier words,
     // per-CTA argmax candidates.  VOX_MEGA=0 (or debug "mega_off") selects the per-op launches.
     bool use_mega = true;
-    int mega_min_B = 1;  // smallest batch that uses the persistent kernel (every batch size does)
     int mega_B = 0, mega_grid = 0, mega_n_ops = 0, mega_ops_cap = 0;
     MegaPlan mega_plan;
     std::vector<MegaOp> mega_ops_host;
@@ -175,13 +174,13 @@ struct Session {
     int *mega_am_idx = nullptr;
     float *mega_att_acc = nullptr, *mega_att_ml = nullptr;  // key-chunk softmax states (MG_ATTN -> MG_ATTN_MERGE)
     int mega_att_units = 0;
-    int *mega_att_flags = nullptr, *mega_epoch = nullptr;
+    int *mega_epoch = nullptr;
     unsigned mega_steps_host = 0;  // decode steps since the device epoch was last re-based (Session::reset)
     // activation fragments (decode_mega.cu frag_build): residual stream x norm weight, attention output, SwiGLU output
     uint2 *mega_xf_bf = nullptr, *mega_af_bf = nullptr, *mega_cf_bf = nullptr;
     float2 *mega_xf_off = nullptr, *mega_af_off = nullptr, *mega_cf_off = nullptr;
     size_t mega_xf_blocks = 0, mega_af_blocks = 0, mega_cf_blocks = 0;
-    unsigned long long *mega_trace_w = nullptr;    // [16][6][8] (debug "mega_trace_w", VOX_MEGA_TRACE_ALL=1)
+    void mega_clear_fragments();   // zero all three (padding tokens and blocks must read as zero), on st
     unsigned long long *mega_trace_all = nullptr;  // [grid][mega_ops_cap][4] (debug "mega_trace_all", VOX_MEGA_TRACE_ALL=1)
     unsigned long long *mega_trace = nullptr;  // [mega_ops_cap][6] SM-clock stamps of CTA 0 (debug "mega_trace")
     bool mega_prepare(int B);
