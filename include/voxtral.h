@@ -214,6 +214,20 @@ int32_t vox_forward_streaming(vox_session *s, const float *mel, int32_t b, int32
 int32_t vox_prefill(vox_session *s, const int32_t *ids, int32_t b, int32_t m, int32_t add_audio, int32_t *next_tok);
 int32_t vox_decode_step(vox_session *s, const int32_t *tok /* nullable */, int32_t b, int32_t add_audio,
                         int32_t *next_tok /* nullable */);
+/* Token confidences.  k = 0 (the default) turns them off; 1 <= k <= VOX_MAX_TOP_K turns them on for every later
+ * vox_transcribe_streaming, vox_transcribe_pcm, vox_transcribe_pcm_dev, vox_prefill and vox_decode_step; any other k is
+ * VOX_EINVAL.  For each emitted token the device keeps the k most likely ids (descending logit, the lower id first on
+ * equal logits, so top_ids[0] is the emitted greedy id) and their log-probabilities logit - logsumexp(logits) (f32,
+ * temperature 1).  The ids do not change.  Costs one extra kernel launch per prefill and decode step, and
+ * 2 x max_batch x (KV capacity) x 8 x 4 bytes of device memory from the first k > 0. */
+#define VOX_MAX_TOP_K 8
+int32_t vox_session_set_top_k(vox_session *s, int32_t k);
+/* The scores of the last transcribe call ([b][n][k], n = its n_out) or of the last vox_prefill / vox_decode_step
+ * ([b][1][k], the position that call emitted), row-major in top_ids / top_logprobs (cap elements each).  Synchronises the
+ * session's stream.  Both buffers NULL: only *b, *n, *k are set.  VOX_EINVAL if that call ran with k = 0, VOX_ECAPACITY
+ * if cap < b * n * k. */
+int32_t vox_session_token_scores(vox_session *s, int32_t *top_ids, float *top_logprobs, size_t cap, int32_t *b,
+                                 int32_t *n, int32_t *k);
 int32_t vox_session_cache_len(const vox_session *s, int32_t *len);             /* LayerCaches::seq_len */
 int32_t vox_session_reset(vox_session *s);                                       /* LayerCaches::reset  */
 /* debugging / parity: copy an internal activation by name ("enc_out","audio_embeds","conv","enc<i>",
@@ -260,6 +274,13 @@ int32_t vox_stream_finish(vox_stream_pool *p, int32_t session);        /* end of
 int32_t vox_stream_tick(vox_stream_pool *p, vox_stream_stats *stats /* nullable */);
 /* ids emitted since the last poll; *done != 0 once the finished session has emitted everything */
 int32_t vox_stream_poll_ids(vox_stream_pool *p, int32_t session, int32_t *ids, size_t cap, size_t *n, int32_t *done);
+/* token confidences (see vox_session_set_top_k) for every session of the pool: one batched step serves them all, so k is
+ * pool-wide and can change only while no session is open (else VOX_EINVAL); VOX_EINVAL for k outside [0, VOX_MAX_TOP_K]. */
+int32_t vox_stream_pool_set_top_k(vox_stream_pool *p, int32_t k);
+/* vox_stream_poll_ids plus the scores of the same n <= cap tokens, [n][k] in top_ids / top_logprobs (cap * k elements
+ * each).  VOX_EINVAL while the pool's k is 0.  Both poll functions drop the tokens they return, with their scores. */
+int32_t vox_stream_poll_scored(vox_stream_pool *p, int32_t session, int32_t *ids, int32_t *top_ids, float *top_logprobs,
+                               size_t cap, size_t *n, int32_t *done);
 /* parity/debug: audio embeddings produced so far, [n][dec_dim] host.  Fails (VOX_ECAPACITY) once an unbounded session
  * has evicted its first rows: use vox_stream_audio_embeds_range. */
 int32_t vox_stream_audio_embeds(vox_stream_pool *p, int32_t session, float *out, size_t cap_floats, int32_t *n);

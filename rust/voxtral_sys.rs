@@ -67,6 +67,10 @@ extern "C" {
     pub fn vox_prefill(s: *mut vox_session, ids: *const i32, b: i32, m: i32, add_audio: i32, next_tok: *mut i32) -> i32;
     pub fn vox_decode_step(s: *mut vox_session, tok: *const i32, b: i32, add_audio: i32, next_tok: *mut i32) -> i32;
     pub fn vox_session_reset(s: *mut vox_session) -> i32;
+    // token confidences: top-k ids and log-probabilities of every emitted token (k <= VOX_MAX_TOP_K = 8; 0 = off)
+    pub fn vox_session_set_top_k(s: *mut vox_session, k: i32) -> i32;
+    pub fn vox_session_token_scores(s: *mut vox_session, top_ids: *mut i32, top_logprobs: *mut f32, cap: usize,
+                                    b: *mut i32, n: *mut i32, k: *mut i32) -> i32;
     pub fn vox_session_free(s: *mut vox_session);
     // src/gguf/{tensor,linear,op}.rs
     pub fn vox_q4_tensor_create(bytes: *const u8, nbytes: usize, n: i64, k: i64, device: i32,
@@ -95,6 +99,9 @@ extern "C" {
     pub fn vox_stream_finish(p: *mut vox_stream_pool, session: i32) -> i32;
     pub fn vox_stream_tick(p: *mut vox_stream_pool, stats: *mut vox_stream_stats) -> i32;
     pub fn vox_stream_poll_ids(p: *mut vox_stream_pool, session: i32, ids: *mut i32, cap: usize, n: *mut usize, done: *mut i32) -> i32;
+    pub fn vox_stream_pool_set_top_k(p: *mut vox_stream_pool, k: i32) -> i32;
+    pub fn vox_stream_poll_scored(p: *mut vox_stream_pool, session: i32, ids: *mut i32, top_ids: *mut i32, top_logprobs: *mut f32,
+                                  cap: usize, n: *mut usize, done: *mut i32) -> i32;
     // max_seconds = 0: sessions of any length (include/voxtral.h)
     pub fn vox_stream_audio_embeds_range(p: *mut vox_stream_pool, session: i32, first: i64, n: i64, out: *mut f32,
                                          cap: usize) -> i32;

@@ -10,7 +10,9 @@ cannot be downloaded in the build environment, so the loader is a manifest, not 
 and tokenizer (absent offline: SURVEY F3); `--streaming` feeds every utterance through vox_stream_* in 80 ms pieces
 instead of vox_transcribe_pcm and must give the same hypotheses.
 Word error rate = word-level Levenshtein distance / reference words after the same normalisation for both sides
-(lower-case, punctuation stripped) -- what jiwer computes for the reference's report.
+(lower-case, punctuation stripped) -- what jiwer computes for the reference's report.  Next to each utterance's WER
+the report gives its mean log-probability over the emitted text tokens (ids >= 1000; vox_session_set_top_k): the
+utterances the model was least sure of are the ones to review first.
 """
 from __future__ import annotations
 
@@ -75,6 +77,7 @@ def main():
     max_mel = int(args.max_seconds * 100) + 1200
     model = vx.Q4ModelLoader.from_file(args.gguf).load(args.device, max_batch=args.batch, max_mel_frames=max_mel)
     model.set_delay(args.delay)
+    model.set_top_k(1)   # each emitted token's log-probability
     errs = words = 0
     audio_s = 0.0
     t0 = time.time()
@@ -83,26 +86,38 @@ def main():
     def decode(ids):
         return tok.decode([int(t) for t in ids if t >= 1000])       # control tokens filtered as transcribe.rs:309-318
 
+    def mean_logprob(ids, lp):   # over the emitted text tokens: the utterance's confidence
+        text = np.asarray(ids) >= 1000
+        return float(np.mean(lp[text])) if text.any() else None
+
     if args.streaming:
         pool = vx.StreamingPool(model, max_sessions=args.batch, max_seconds=args.max_seconds)
+        pool.set_top_k(1)
     for u in utts:
         a = vx.peak_normalize(read_wav(u["audio"]))
         audio_s += a.size / 16000.0
         if args.streaming:
             sid = pool.open(delay=args.delay)   # a pool session has its own delay (default 6), not the model's
-            ids = []
+            ids, lps = [], []
+
+            def poll():
+                got, _, _, lp = pool.poll(sid, scores=True)
+                ids.extend(got)
+                lps.append(lp[:, 0])
             for p in range(0, a.size, 1280):
-                pool.push(sid, a[p:p + 1280]); pool.tick(); ids += pool.poll(sid)[0]
-            pool.finish(sid); pool.tick(); ids += pool.poll(sid)[0]
+                pool.push(sid, a[p:p + 1280]); pool.tick(); poll()
+            pool.finish(sid); pool.tick(); poll()
             pool.close_session(sid)
+            lp = np.concatenate(lps)
         else:
             ids = model.transcribe_pcm(a, peak_normalize=False)[0]
+            lp = model.token_scores()[1][0, :, 0]
         hyp = decode(ids)
         r, h = normalise(u["text"]), normalise(hyp)
         e = edit_distance(r, h)
         errs += e
         words += len(r)
-        out.append({"id": u.get("id"), "wer": e / max(1, len(r)), "hypothesis": hyp})
+        out.append({"id": u.get("id"), "wer": e / max(1, len(r)), "mean_logprob": mean_logprob(ids, lp), "hypothesis": hyp})
     wall = time.time() - t0
     print(json.dumps({"utterances": len(utts), "wer": errs / max(1, words), "audio_seconds": audio_s, "wall_seconds": wall,
                       "rtf": wall / max(audio_s, 1e-9), "delay_tokens": args.delay, "results": out}, indent=1))

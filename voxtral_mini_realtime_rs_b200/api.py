@@ -131,6 +131,9 @@ _SIGS = {
     "vox_forward_streaming": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, _P, C.c_int32, _P, C.c_size_t]),
     "vox_prefill": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, C.c_int32, _P]),
     "vox_decode_step": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, _P]),
+    "vox_session_set_top_k": (C.c_int32, [_P, C.c_int32]),
+    "vox_session_token_scores": (C.c_int32, [_P, _P, _P, C.c_size_t, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                             C.POINTER(C.c_int32)]),
     "vox_session_cache_len": (C.c_int32, [_P, C.POINTER(C.c_int32)]),
     "vox_session_reset": (C.c_int32, [_P]),
     "vox_session_debug_read": (C.c_int32, [_P, C.c_char_p, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
@@ -143,6 +146,9 @@ _SIGS = {
     "vox_stream_finish": (C.c_int32, [_P, C.c_int32]),
     "vox_stream_tick": (C.c_int32, [_P, _P]),
     "vox_stream_poll_ids": (C.c_int32, [_P, C.c_int32, _P, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_int32)]),
+    "vox_stream_pool_set_top_k": (C.c_int32, [_P, C.c_int32]),
+    "vox_stream_poll_scored": (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_size_t, C.POINTER(C.c_size_t),
+                                           C.POINTER(C.c_int32)]),
     "vox_stream_audio_embeds": (C.c_int32, [_P, C.c_int32, _P, C.c_size_t, C.POINTER(C.c_int32)]),
     "vox_stream_audio_embeds_range": (C.c_int32, [_P, C.c_int32, C.c_int64, C.c_int64, _P, C.c_size_t]),
     "vox_stream_session_info": (C.c_int32, [_P, C.c_int32, _P]),
@@ -641,6 +647,21 @@ class Q4VoxtralModel:
                                      _ptr(nxt) if read else None))
         return nxt
 
+    def set_top_k(self, k: int):
+        """Token confidences for later transcribe / prefill / decode_step calls: the k (<= 8) most likely ids of every
+        emitted token and their log-probabilities; 0 turns them off.  The ids do not change."""
+        _check(lib().vox_session_set_top_k(self._s, k))
+
+    def token_scores(self):
+        """(top_ids [B,n,k] int32, top_logprobs [B,n,k] f32) of the last transcribe call (n = its tokens per stream) or
+        of the last prefill / decode_step (n = 1).  top_ids[..., 0] is the emitted id."""
+        b, n, k = C.c_int32(), C.c_int32(), C.c_int32()
+        _check(lib().vox_session_token_scores(self._s, None, None, 0, C.byref(b), C.byref(n), C.byref(k)))
+        ids = np.empty((b.value, n.value, k.value), np.int32)
+        lp = np.empty((b.value, n.value, k.value), np.float32)
+        _check(lib().vox_session_token_scores(self._s, _ptr(ids), _ptr(lp), ids.size, C.byref(b), C.byref(n), C.byref(k)))
+        return ids, lp
+
     def cache_len(self) -> int:
         v = C.c_int32()
         _check(lib().vox_session_cache_len(self._s, C.byref(v)))
@@ -700,6 +721,12 @@ class StreamingPool:
         _check(lib().vox_stream_pool_create(model._m, max_sessions, 0.0 if max_seconds is None else max_seconds,
                                             C.byref(self._p)))
         self.dec_dim = model.info["dec_dim"]
+        self.top_k = 0
+
+    def set_top_k(self, k: int):
+        """Token confidences (Q4VoxtralModel.set_top_k) for every session of the pool; only while no session is open."""
+        _check(lib().vox_stream_pool_set_top_k(self._p, k))
+        self.top_k = k
 
     def open(self, delay: float | None = None) -> int:
         """A new session, at transcription delay `delay` (tokens of 80 ms; None: the default 6.0)."""
@@ -729,11 +756,20 @@ class StreamingPool:
         _check(lib().vox_stream_tick(self._p, C.byref(st)))
         return {f[0]: getattr(st, f[0]) for f in _StreamStats._fields_}
 
-    def poll(self, session: int, cap: int = 4096):
+    def poll(self, session: int, cap: int = 4096, scores: bool = False):
+        """(ids, done) of the tokens emitted since the last poll; with scores=True (after set_top_k(k > 0))
+        (ids, done, top_ids [n,k] int32, top_logprobs [n,k] f32)."""
         ids = np.empty(cap, np.int32)
         n, done = C.c_size_t(), C.c_int32()
-        _check(lib().vox_stream_poll_ids(self._p, session, _ptr(ids), cap, C.byref(n), C.byref(done)))
-        return ids[:n.value].tolist(), bool(done.value)
+        if not scores:
+            _check(lib().vox_stream_poll_ids(self._p, session, _ptr(ids), cap, C.byref(n), C.byref(done)))
+            return ids[:n.value].tolist(), bool(done.value)
+        k = max(self.top_k, 1)
+        top = np.empty((cap, k), np.int32)
+        lp = np.empty((cap, k), np.float32)
+        _check(lib().vox_stream_poll_scored(self._p, session, _ptr(ids), _ptr(top), _ptr(lp), cap, C.byref(n),
+                                            C.byref(done)))
+        return ids[:n.value].tolist(), bool(done.value), top[:n.value].copy(), lp[:n.value].copy()
 
     def session_info(self, session: int) -> dict:
         info = _StreamSessionInfo()

@@ -697,6 +697,15 @@ int32_t vox_forward_streaming(vox_session *sh, const float *mel, int32_t b, int3
     VOX_API_END
 }
 
+// what vox_session_token_scores returns after an incremental call over rows [0, b): each row's position just emitted
+static void record_step_scores(Session *s, int b) {
+    s->scores_k = s->top_k;
+    s->scores_b = b;
+    s->scores_n = 1;
+    s->scores_pos.assign(s->out_rows.begin(), s->out_rows.begin() + b);
+    for (int &p : s->scores_pos) p -= 1;
+}
+
 // Device-side incremental decode (SURVEY 8(b); model.rs:857-867 without the logits round trip): the argmax stays on
 // the device and feeds the next step; only b int32 ids cross the bus, and only when the caller asks for them.
 int32_t vox_prefill(vox_session *sh, const int32_t *ids, int32_t b, int32_t m, int32_t add_audio, int32_t *next_tok) {
@@ -715,6 +724,7 @@ int32_t vox_prefill(vox_session *sh, const int32_t *ids, int32_t b, int32_t m, i
     CUDA_OK(cudaSetDevice(s->m->device));
     s->prefill(b, m, ids, add_audio != 0);
     s->cache_len += m;
+    record_step_scores(s, b);
     if (next_tok) CUDA_OK(cudaMemcpyAsync(next_tok, s->d_tok, sizeof(int) * b, cudaMemcpyDeviceToHost, s->st));
     CUDA_OK(cudaStreamSynchronize(s->st));   // `ids` is caller memory
     VOX_API_END
@@ -737,8 +747,43 @@ int32_t vox_decode_step(vox_session *sh, const int32_t *tok, int32_t b, int32_t 
     s->decode_step(b, add_audio != 0);
     s->mega_steps_host += 1;
     s->cache_len += 1;
+    record_step_scores(s, b);
     if (next_tok) CUDA_OK(cudaMemcpyAsync(next_tok, s->d_tok, sizeof(int) * b, cudaMemcpyDeviceToHost, s->st));
     if (next_tok || tok) CUDA_OK(cudaStreamSynchronize(s->st));
+    VOX_API_END
+}
+static_assert(VOX_MAX_TOP_K == TOPK_MAX, "the score buffers hold VOX_MAX_TOP_K entries per position");
+int32_t vox_session_set_top_k(vox_session *s, int32_t k) {
+    VOX_API_BEGIN
+    REQUIRE(s);
+    s->s->set_top_k(k);
+    VOX_API_END
+}
+int32_t vox_session_token_scores(vox_session *sh, int32_t *top_ids, float *top_logprobs, size_t cap, int32_t *b, int32_t *n,
+                                 int32_t *k) {
+    VOX_API_BEGIN
+    REQUIRE(sh);
+    Session *s = sh->s;
+    const int B = s->scores_b, N = s->scores_n, K = s->scores_k;
+    VOX_CHECK(K > 0, VOX_EINVAL, "no token scores: the last transcribe, prefill or decode step ran with top_k 0 (vox_session_set_top_k)");
+    if (b) *b = B;
+    if (n) *n = N;
+    if (k) *k = K;
+    if (!top_ids && !top_logprobs) return VOX_OK;
+    REQUIRE(top_ids); REQUIRE(top_logprobs);
+    VOX_CHECK(cap >= (size_t)B * N * K, VOX_ECAPACITY, "token scores capacity %zu < %d x %d x %d", cap, B, N, K);
+    CUDA_OK(cudaSetDevice(s->m->device));
+    CUDA_OK(cudaStreamSynchronize(s->st));
+    // row r's entries [p0, p0 + N) of the device's [row][out_ld][VOX_MAX_TOP_K] buffers, the first K of each
+    const size_t pitch = sizeof(int32_t) * VOX_MAX_TOP_K;
+    for (int r = 0; r < B && N > 0; ++r) {
+        const size_t at = ((size_t)r * s->out_ld + (s->scores_pos.empty() ? 0 : s->scores_pos[r])) * VOX_MAX_TOP_K;
+        const size_t dst = (size_t)r * N * K;
+        CUDA_OK(cudaMemcpy2D(top_ids + dst, sizeof(int32_t) * K, s->d_top_ids + at, pitch, sizeof(int32_t) * K, N,
+                             cudaMemcpyDeviceToHost));
+        CUDA_OK(cudaMemcpy2D(top_logprobs + dst, sizeof(float) * K, s->d_top_lp + at, pitch, sizeof(float) * K, N,
+                             cudaMemcpyDeviceToHost));
+    }
     VOX_API_END
 }
 int32_t vox_session_cache_len(const vox_session *s, int32_t *len) {
@@ -912,7 +957,25 @@ int32_t vox_stream_poll_ids(vox_stream_pool *p, int32_t session, int32_t *ids, s
     REQUIRE(p); REQUIRE(n);
     if (cap) REQUIRE(ids);
     bool d = false;
-    *n = p->p->poll(session, ids, cap, &d);
+    *n = p->p->poll(session, ids, nullptr, nullptr, cap, &d);
+    if (done) *done = d ? 1 : 0;
+    VOX_API_END
+}
+int32_t vox_stream_pool_set_top_k(vox_stream_pool *p, int32_t k) {
+    VOX_API_BEGIN
+    REQUIRE(p);
+    CUDA_OK(cudaSetDevice(p->p->m->device));
+    p->p->set_top_k(k);
+    VOX_API_END
+}
+int32_t vox_stream_poll_scored(vox_stream_pool *p, int32_t session, int32_t *ids, int32_t *top_ids, float *top_logprobs,
+                               size_t cap, size_t *n, int32_t *done) {
+    VOX_API_BEGIN
+    REQUIRE(p); REQUIRE(n);
+    VOX_CHECK(p->p->s->top_k > 0, VOX_EINVAL, "no token scores: the pool's top_k is 0 (vox_stream_pool_set_top_k)");
+    if (cap) { REQUIRE(ids); REQUIRE(top_ids); REQUIRE(top_logprobs); }
+    bool d = false;
+    *n = p->p->poll(session, ids, top_ids, top_logprobs, cap, &d);
     if (done) *done = d ? 1 : 0;
     VOX_API_END
 }

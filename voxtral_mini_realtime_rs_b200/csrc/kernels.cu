@@ -940,6 +940,163 @@ void launch_argmax_multi(const float *logits, int B, int V, int *tok, int *out_i
     post_launch("argmax_multi");
 }
 
+// =====================================================================================
+// Token confidences (kernels.h launch_token_scores): logsumexp and top-k of each logits row, after the argmax.
+// A thread keeps a running (max, sum of exp(x - max)) and a sorted top-TOPK_MAX list of its strided elements; the warp
+// extracts its best TOPK_MAX from the lanes' list heads, 8 warps merge through shared memory, and the row's last CTA
+// merges the ARGMAX_PARTS partials.  Every merge runs in a fixed order: the output is bitwise reproducible.
+// =====================================================================================
+constexpr int SCORE_THREADS = 256;
+constexpr int TOPK_NONE = 0x7fffffff;   // id of an empty list entry (value -inf): ranks after every real entry
+
+// (v, i) ranks before (bv, bx) in the greedy argmax's order: the larger logit, the lower id on equal logits.  A NaN
+// ranks before nothing, so it never enters a list.
+__device__ __forceinline__ bool rank_before(float v, int i, float bv, int bx) { return v > bv || (v == bv && i < bx); }
+
+// sorted insertion into a register list (fully unrolled, so the list stays in registers)
+__device__ __forceinline__ void topk_insert(float (&tv)[TOPK_MAX], int (&ti)[TOPK_MAX], float v, int i) {
+    if (!rank_before(v, i, tv[TOPK_MAX - 1], ti[TOPK_MAX - 1])) return;
+    tv[TOPK_MAX - 1] = v;
+    ti[TOPK_MAX - 1] = i;
+#pragma unroll
+    for (int j = TOPK_MAX - 1; j > 0; --j)
+        if (rank_before(tv[j], ti[j], tv[j - 1], ti[j - 1])) {
+            const float t = tv[j]; tv[j] = tv[j - 1]; tv[j - 1] = t;
+            const int u = ti[j]; ti[j] = ti[j - 1]; ti[j - 1] = u;
+        }
+}
+
+// the warp's best TOPK_MAX entries of the lanes' sorted lists, into every lane's (ov, oi); consumes the lists.  A real id
+// sits in one lane only, so the lane whose head won is the one whose head id equals the winner's.
+__device__ __forceinline__ void warp_topk(float (&tv)[TOPK_MAX], int (&ti)[TOPK_MAX], float (&ov)[TOPK_MAX], int (&oi)[TOPK_MAX]) {
+#pragma unroll
+    for (int r = 0; r < TOPK_MAX; ++r) {
+        float bv = tv[0];
+        int bx = ti[0];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float v = __shfl_xor_sync(0xffffffffu, bv, o);
+            const int x = __shfl_xor_sync(0xffffffffu, bx, o);
+            if (rank_before(v, x, bv, bx)) { bv = v; bx = x; }
+        }
+        ov[r] = bv;
+        oi[r] = bx;
+        if (ti[0] == bx) {
+#pragma unroll
+            for (int j = 0; j < TOPK_MAX - 1; ++j) { tv[j] = tv[j + 1]; ti[j] = ti[j + 1]; }
+            tv[TOPK_MAX - 1] = -INFINITY;
+            ti[TOPK_MAX - 1] = TOPK_NONE;
+        }
+    }
+}
+
+// (m, l) <- the pair of the union: m = max, l = sum of exp(x - m).  Commutative, so a butterfly leaves every lane equal.
+__device__ __forceinline__ void lse_merge(float &m, float &l, float om, float ol) {
+    const float nm = fmaxf(m, om);
+    if (nm == -INFINITY) return;
+    l = (m == -INFINITY ? 0.0f : l * expf(m - nm)) + (om == -INFINITY ? 0.0f : ol * expf(om - nm));
+    m = nm;
+}
+
+__device__ __forceinline__ void warp_lse(float &m, float &l) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) lse_merge(m, l, __shfl_xor_sync(0xffffffffu, m, o), __shfl_xor_sync(0xffffffffu, l, o));
+}
+
+__global__ void __launch_bounds__(SCORE_THREADS)
+token_scores_kernel(const float *__restrict__ logits, int V, int k, const int *__restrict__ out_pos_ptr, int out_ld,
+                    int *top_ids, float *top_logprobs, ScoreWork w) {
+    constexpr int NW = SCORE_THREADS / 32;
+    __shared__ float s_v[NW][TOPK_MAX], s_m[NW], s_l[NW];
+    __shared__ int s_i[NW][TOPK_MAX];
+    __shared__ int is_last;
+    const int part = blockIdx.x, b = blockIdx.y;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int per = (V + ARGMAX_PARTS - 1) / ARGMAX_PARTS;
+    const int i0 = part * per, i1 = min(V, i0 + per);
+    const float *row = logits + (size_t)b * V;
+    float m = -INFINITY, l = 0.0f;
+    float tv[TOPK_MAX], ov[TOPK_MAX];
+    int ti[TOPK_MAX], oi[TOPK_MAX];
+#pragma unroll
+    for (int j = 0; j < TOPK_MAX; ++j) { tv[j] = -INFINITY; ti[j] = TOPK_NONE; }
+    for (int i = i0 + threadIdx.x; i < i1; i += SCORE_THREADS) {
+        const float x = row[i];
+        if (x > m) {
+            l = (m == -INFINITY ? 0.0f : l * expf(m - x)) + 1.0f;
+            m = x;
+        } else if (x > -INFINITY) {
+            l += expf(x - m);
+        }
+        topk_insert(tv, ti, x, i);
+    }
+    warp_lse(m, l);
+    warp_topk(tv, ti, ov, oi);
+    if (lane == 0) {
+        s_m[warp] = m;
+        s_l[warp] = l;
+#pragma unroll
+        for (int j = 0; j < TOPK_MAX; ++j) { s_v[warp][j] = ov[j]; s_i[warp][j] = oi[j]; }
+    }
+    __syncthreads();
+    const size_t slot = (size_t)b * ARGMAX_PARTS + part;
+    if (warp == 0) {
+        m = lane < NW ? s_m[lane] : -INFINITY;
+        l = lane < NW ? s_l[lane] : 0.0f;
+#pragma unroll
+        for (int j = 0; j < TOPK_MAX; ++j) {   // each warp's list is sorted already
+            tv[j] = lane < NW ? s_v[lane][j] : -INFINITY;
+            ti[j] = lane < NW ? s_i[lane][j] : TOPK_NONE;
+        }
+        warp_lse(m, l);
+        warp_topk(tv, ti, ov, oi);
+        if (lane == 0) {
+            w.m[slot] = m;
+            w.l[slot] = l;
+#pragma unroll
+            for (int j = 0; j < TOPK_MAX; ++j) { w.vals[slot * TOPK_MAX + j] = ov[j]; w.idx[slot * TOPK_MAX + j] = oi[j]; }
+            __threadfence();
+            const int old = atomicAdd(&w.counters[b], 1);
+            is_last = (old == ARGMAX_PARTS - 1);
+            if (is_last) w.counters[b] = 0;
+        }
+    }
+    __syncthreads();
+    if (!is_last || warp != 0) return;
+    __threadfence();
+    // the row's last CTA: lane p merges parts p, p + 32, ... in that order, then the warp merges the lanes
+    m = -INFINITY;
+    l = 0.0f;
+#pragma unroll
+    for (int j = 0; j < TOPK_MAX; ++j) { tv[j] = -INFINITY; ti[j] = TOPK_NONE; }
+    for (int p = lane; p < ARGMAX_PARTS; p += 32) {
+        const size_t s = (size_t)b * ARGMAX_PARTS + p;
+        lse_merge(m, l, __ldcg(w.m + s), __ldcg(w.l + s));
+#pragma unroll
+        for (int j = 0; j < TOPK_MAX; ++j) topk_insert(tv, ti, __ldcg(w.vals + s * TOPK_MAX + j), __ldcg(w.idx + s * TOPK_MAX + j));
+    }
+    warp_lse(m, l);
+    warp_topk(tv, ti, ov, oi);
+    if (lane == 0) {
+        const float lse = m + logf(l);
+        const size_t at = ((size_t)b * out_ld + (out_pos_ptr[b] - 1)) * TOPK_MAX;
+#pragma unroll
+        for (int j = 0; j < TOPK_MAX; ++j)
+            if (j < k) {
+                const bool real = oi[j] != TOPK_NONE;   // (fewer than k finite logits in the row)
+                top_ids[at + j] = real ? oi[j] : -1;
+                top_logprobs[at + j] = real ? ov[j] - lse : -INFINITY;
+            }
+    }
+}
+
+void launch_token_scores(const float *logits, int B, int V, int k, const int *out_pos_ptr, int out_ld, int *top_ids,
+                         float *top_logprobs, const ScoreWork &w, cudaStream_t st) {
+    dim3 grid(ARGMAX_PARTS, B);
+    token_scores_kernel<<<grid, SCORE_THREADS, 0, st>>>(logits, V, k, out_pos_ptr, out_ld, top_ids, top_logprobs, w);
+    post_launch("token_scores");
+}
+
 __global__ void advance_kernel(int *a, int da, int *b, int db, int n) {
     asm volatile("griddepcontrol.launch_dependents;\n" ::: "memory");
     const int i = threadIdx.x;

@@ -214,6 +214,19 @@ constexpr int ARGMAX_PARTS = 64;
 void launch_argmax_multi(const float *logits, int B, int V, int *tok, int *out_ids, int out_ld,
                          const int *out_pos_ptr, float *scratch_vals, int *scratch_idx, int *counters,
                          cudaStream_t st);
+// Token confidences (vox_session_set_top_k): per row b, the k most likely ids of logits [B][V] (descending logit, the
+// lower id first on equal logits -- so ids[0] is the greedy argmax) and their log-probabilities logit - logsumexp(row),
+// in f32 at temperature 1.  ARGMAX_PARTS CTAs per row; the last to arrive (atomic ticket) merges the partial
+// (max, sum of exp) pairs and top-k lists in fixed order, so the result is bitwise reproducible.  Row b's result goes to
+// position out_pos[b] - 1 (the argmax and the step counters have run): ids / logprobs [B][out_ld][TOPK_MAX], entries
+// [0, k).  scratch: m/l [B][ARGMAX_PARTS], vals/idx [B][ARGMAX_PARTS][TOPK_MAX], counters [B] zero between launches.
+constexpr int TOPK_MAX = 8;   // VOX_MAX_TOP_K
+struct ScoreWork {
+    float *m = nullptr, *l = nullptr, *vals = nullptr;
+    int *idx = nullptr, *counters = nullptr;
+};
+void launch_token_scores(const float *logits, int B, int V, int k, const int *out_pos_ptr, int out_ld, int *top_ids,
+                         float *top_logprobs, const ScoreWork &w, cudaStream_t st);
 // a[i] += da; b[i] += db for i < n  (device-side per-row step counters for graph replay)
 void launch_advance(int *a, int da, int *b, int db, int n, cudaStream_t st);
 // gather rows: dst[b][:] = src[b*M + (M-1)][:]

@@ -534,6 +534,7 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ri
         }
         CUDA_OK(cudaMemset(s->d_pos, 0, sizeof(int) * B));
         CUDA_OK(cudaMemset(s->d_outpos, 0, sizeof(int) * B));
+        s->out_rows.assign(B, 0);
         s->set_delay(kDefaultDelay);
     } catch (...) {
         delete s;
@@ -886,8 +887,11 @@ void Session::decode_step(int B, bool add_audio) {
     // group's first row.
     if (!stream_mode) bind_delays_identity(B);
     const int rows_per_launch = B > 8 ? 8 : B;
+    if (!stream_mode)
+        for (int b = 0; b < B; ++b) out_rows[b] += 1;
     if (mega_prepare(rows_per_launch)) {
         for (int b0 = 0; b0 < B; b0 += 8) decode_step_mega(b0, std::min(8, B - b0), add_audio);
+        token_scores(B);   // one launch over every group's rows
         return;
     }
     launch_embed(m->tok_emb, d_tok, add_audio ? audio : nullptr, cur_S4, B, 1, d_pos, x_dec, fused_decode(B) ? ssq_x : nullptr, st,
@@ -896,6 +900,29 @@ void Session::decode_step(int B, bool add_audio) {
     lm_head_rows(B, pending, logits);
     launch_argmax_multi(logits, B, c.vocab, d_tok, stream_mode ? nullptr : d_out, out_ld, d_outpos, am_vals, am_idx, am_cnt, st);
     launch_advance(d_pos, 1, d_outpos, 1, B, st);
+    token_scores(B);
+}
+
+void Session::set_top_k(int k) {
+    VOX_CHECK(k >= 0 && k <= TOPK_MAX, VOX_EINVAL, "top_k %d out of range [0,%d]", k, TOPK_MAX);
+    if (k > 0 && !d_top_ids) {
+        CUDA_OK(cudaSetDevice(m->device));
+        const size_t n = (size_t)max_batch * out_ld * TOPK_MAX, parts = (size_t)max_batch * ARGMAX_PARTS;
+        d_top_ids = arena.alloc_n<int>(n);
+        d_top_lp = arena.alloc_n<float>(n);
+        score_work.m = arena.alloc_n<float>(parts);
+        score_work.l = arena.alloc_n<float>(parts);
+        score_work.vals = arena.alloc_n<float>(parts * TOPK_MAX);
+        score_work.idx = arena.alloc_n<int>(parts * TOPK_MAX);
+        score_work.counters = arena.alloc_n<int>(max_batch);
+        CUDA_OK(cudaMemset(score_work.counters, 0, sizeof(int) * max_batch));
+    }
+    top_k = k;
+}
+
+// after the step's argmax and counter advance: row b's scores land at its output position d_outpos[b] - 1
+void Session::token_scores(int B) {
+    if (top_k > 0) launch_token_scores(logits, B, m->info.vocab, top_k, d_outpos, out_ld, d_top_ids, d_top_lp, score_work, st);
 }
 
 // One launch of the persistent kernel for rows [b0, b0 + B) (B <= 8) of the session; mega_prepare() has built the op table.
@@ -980,11 +1007,15 @@ void Session::prefill(int B, int M, const int *ids_host, bool add_audio) {
     linear(m->tok_emb, last_h, B, logits, c.vocab, nullptr, nullptr, EPI_NONE);
     launch_argmax(logits, B, c.vocab, d_tok, stream_mode ? nullptr : d_out, out_ld, d_outpos, st);
     launch_advance(d_pos, M, d_outpos, 1, B, st);
+    token_scores(B);
+    if (!stream_mode)
+        for (int b = 0; b < B; ++b) out_rows[b] += 1;
 }
 
 void Session::reset() {
     CUDA_OK(cudaMemsetAsync(d_pos, 0, sizeof(int) * max_batch, st));
     CUDA_OK(cudaMemsetAsync(d_outpos, 0, sizeof(int) * max_batch, st));
+    std::fill(out_rows.begin(), out_rows.end(), 0);
     cache_len = 0;
     rebase_epoch();
 }
@@ -1027,7 +1058,8 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
             int done = 0;
             if (use_graph) {
                 // (prefill() has bound the rows' delays: a captured step of the other ADA mode launches other kernels)
-                if (!step_graph || step_graph_B != B || step_graph_S4 != S4 || step_graph_per_row != ada_per_row) {
+                if (!step_graph || step_graph_B != B || step_graph_S4 != S4 || step_graph_per_row != ada_per_row ||
+                    step_graph_top_k != top_k) {
                     // first step eagerly (also performs any one-time kernel attribute setup),
                     // then capture one step and replay it
                     decode_step(B);
@@ -1053,6 +1085,7 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
                         step_graph_B = B;
                         step_graph_S4 = S4;
                         step_graph_per_row = ada_per_row;
+                        step_graph_top_k = top_k;
                     }
                 }
                 for (; done < steps; ++done) {
@@ -1072,6 +1105,12 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
     for (int b = 0; b < B; ++b)
         for (int i = 0; i < n_out; ++i) out_ids[(size_t)b * n_out + i] = host[(size_t)b * out_ld + i];
     cache_len = n_out > 0 ? S4 - 1 : 0;
+    if (n_out > 0)   // (a captured step counted an output it did not produce)
+        for (int b = 0; b < B; ++b) out_rows[b] = n_out;
+    scores_k = top_k;
+    scores_b = B;
+    scores_n = n_out;
+    scores_pos.clear();
     if (tm) {
         tm->seq_len = S4;
         tm->decode_tokens = n_out;

@@ -150,8 +150,23 @@ struct Session {
     bool stream_mode = false;
     const float *const *audio_rows_dev = nullptr;
     const float *audio_base = nullptr;
+    // token confidences (vox_session_set_top_k): 0 = off (no launch, no memory).  k > 0: every prefill and decode step
+    // ends with launch_token_scores over its rows into [max_batch][out_ld][TOPK_MAX] ids / log-probabilities, allocated
+    // by the first set_top_k(k > 0)
+    int top_k = 0;
+    int *d_top_ids = nullptr;
+    float *d_top_lp = nullptr;
+    ScoreWork score_work;
+    void set_top_k(int k);
+    void token_scores(int B);   // launch over rows [0, B) of the step that just ran (no-op while top_k == 0)
+    // what vox_session_token_scores returns: the last transcribe (positions [0, n) of `b` rows) or incremental call (the
+    // position `step_pos` of each row), scored with k = scores_k (0: that call ran with scores off)
+    int scores_k = 0, scores_b = 0, scores_n = 0;
+    std::vector<int> scores_pos;    // per row, empty after a transcribe
+    // host mirror of d_outpos[] outside stream mode: outputs per row since reset (prefill / decode_step / transcribe)
+    std::vector<int> out_rows;
     cudaGraphExec_t step_graph = nullptr;
-    int step_graph_B = 0, step_graph_S4 = 0;
+    int step_graph_B = 0, step_graph_S4 = 0, step_graph_top_k = 0;
     bool step_graph_per_row = false;  // the captured step's ADA mode (its kernels and arguments differ)
     uint64_t step_graph_nodes = 0;
     bool use_graph = true;

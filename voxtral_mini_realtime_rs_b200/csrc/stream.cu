@@ -290,11 +290,21 @@ void StreamPool::close(int id) {
     sl = Slot();
 }
 
-size_t StreamPool::poll(int id, int32_t *ids, size_t cap, bool *done) {
+void StreamPool::set_top_k(int k) {
+    for (int i = 0; i < max_sessions; ++i)
+        VOX_CHECK(!slots[i].open, VOX_EINVAL, "top_k of a stream pool can only change while no session is open (session %d is)", i);
+    s->set_top_k(k);
+}
+
+size_t StreamPool::poll(int id, int32_t *ids, int32_t *top_ids, float *top_lp, size_t cap, bool *done) {
     Slot &sl = slot(id);
-    const size_t n = std::min(cap, sl.ids.size());
+    const size_t n = std::min(cap, sl.ids.size()), nk = n * (size_t)s->top_k;
     if (n) memcpy(ids, sl.ids.data(), sizeof(int32_t) * n);
+    if (nk && top_ids) memcpy(top_ids, sl.top_ids.data(), sizeof(int32_t) * nk);
+    if (nk && top_lp) memcpy(top_lp, sl.top_lp.data(), sizeof(float) * nk);
     sl.ids.erase(sl.ids.begin(), sl.ids.begin() + n);  // polled ids are dropped: host memory stays bounded
+    sl.top_ids.erase(sl.top_ids.begin(), sl.top_ids.begin() + nk);
+    sl.top_lp.erase(sl.top_lp.begin(), sl.top_lp.begin() + nk);
     if (done) *done = sl.ended && sl.drained && sl.ids.empty();
     return n;
 }
@@ -461,10 +471,14 @@ void StreamPool::tick(vox_stream_stats *st_out) {
             s->prefill(1, P, prefix.data(), true);
             s->audio_base = nullptr;
             int tok = 0;
+            std::vector<int32_t> top((size_t)s->top_k);
+            std::vector<float> lp((size_t)s->top_k);
             CUDA_OK(cudaMemcpyAsync(&tok, s->d_tok, sizeof(int), cudaMemcpyDeviceToHost, s->st));
+            fetch_scores(1, top.data(), lp.data());
             CUDA_OK(cudaStreamSynchronize(s->st));
             sl.last_tok = tok;
             sl.ids.push_back(tok);
+            append_scores(sl, top.data(), lp.data());
             sl.n_ids += 1;
             sl.pos = P;  // cached positions; the next step is position P and consumes audio[P]
             stats.prefills += 1;
@@ -496,12 +510,16 @@ void StreamPool::tick(vox_stream_stats *st_out) {
             s->audio_rows_dev = nullptr;
             s->mega_steps_host += ((unsigned)rows.size() + 7) / 8;  // one persistent-kernel launch per group of 8 rows
             std::vector<int> toks(rows.size());
+            std::vector<int32_t> top(rows.size() * s->top_k);
+            std::vector<float> lp(rows.size() * s->top_k);
             CUDA_OK(cudaMemcpyAsync(toks.data(), s->d_tok, sizeof(int) * rows.size(), cudaMemcpyDeviceToHost, s->st));
+            fetch_scores((int)rows.size(), top.data(), lp.data());
             CUDA_OK(cudaStreamSynchronize(s->st));
             for (size_t i = 0; i < rows.size(); ++i) {
                 Slot &sl = slots[rows[i]];
                 sl.last_tok = toks[i];
                 sl.ids.push_back(toks[i]);
+                append_scores(sl, top.data() + i * s->top_k, lp.data() + i * s->top_k);
                 sl.n_ids += 1;
                 sl.pos += 1;
             }
@@ -601,6 +619,22 @@ void StreamPool::session_info(int id, struct vox_stream_session_info *out) {
     out->decoder_positions = sl.pos;
     out->ids_emitted = sl.n_ids;
     out->kv_pages = (int32_t)sl.pages.size();
+}
+
+// stream mode resets every row's output position before a step, so its scores sit at position 0 of the row
+void StreamPool::fetch_scores(int n, int32_t *top_ids, float *top_lp) {
+    const int k = s->top_k;
+    if (k == 0) return;
+    const size_t row = (size_t)s->out_ld * TOPK_MAX;
+    CUDA_OK(cudaMemcpy2DAsync(top_ids, sizeof(int32_t) * k, s->d_top_ids, sizeof(int32_t) * row, sizeof(int32_t) * k, n,
+                              cudaMemcpyDeviceToHost, s->st));
+    CUDA_OK(cudaMemcpy2DAsync(top_lp, sizeof(float) * k, s->d_top_lp, sizeof(float) * row, sizeof(float) * k, n,
+                              cudaMemcpyDeviceToHost, s->st));
+}
+
+void StreamPool::append_scores(Slot &sl, const int32_t *top_ids, const float *top_lp) {
+    sl.top_ids.insert(sl.top_ids.end(), top_ids, top_ids + s->top_k);
+    sl.top_lp.insert(sl.top_lp.end(), top_lp, top_lp + s->top_k);
 }
 
 // RoPE rows of positions [p0, p0 + n) into a ring table of `rows` rows starting at row `row0`: position p at row p % rows

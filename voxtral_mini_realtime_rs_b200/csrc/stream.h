@@ -21,6 +21,8 @@ struct StreamPool {
         int pos = 0;                              // decoder positions cached (0: prefill pending)
         int last_tok = 0;
         std::vector<int32_t> ids;                 // emitted ids not yet polled
+        std::vector<int32_t> top_ids;             // their scores, [ids.size()][s->top_k] (pool top_k > 0)
+        std::vector<float> top_lp;
         int64_t n_ids = 0;                        // ids emitted (positions >= 38)
         std::vector<int> pages;                   // decoder KV pages owned (page-table slot order)
         size_t pcm0 = 0;                          // absolute sample / frame / row of each buffer's row 0
@@ -55,7 +57,10 @@ struct StreamPool {
     void finish(int id);
     void close(int id);
     void tick(vox_stream_stats *stats);
-    size_t poll(int id, int32_t *ids, size_t cap, bool *done);
+    // token confidences of every session (one batched step serves them all): only while no session is open
+    void set_top_k(int k);
+    // up to `cap` ids (and, when top_ids / top_lp are given, their [n][top_k] scores); what is returned is dropped
+    size_t poll(int id, int32_t *ids, int32_t *top_ids, float *top_lp, size_t cap, bool *done);
     const float *audio_embeds(int id, int *n);   // device pointer [n][dec_dim]; fails once rows were evicted
     // device pointer to resident audio embeddings [first, first + n)
     const float *audio_embeds_range(int id, int64_t first, int64_t n);
@@ -70,6 +75,9 @@ struct StreamPool {
     void encoder_rows(int R);
     void ensure_pages(Slot &sl, int positions);
     void upload_rows(const std::vector<int> &rows, bool with_tokens);
+    // enqueues the copy of the last step's scores of rows [0, n) (position 0 of each) into [n][top_k] host arrays
+    void fetch_scores(int n, int32_t *top_ids, float *top_lp);
+    void append_scores(Slot &sl, const int32_t *top_ids, const float *top_lp);
     int final_enc(const Slot &sl) const;
     void fill_rope(float *cos_d, float *sin_d, int hd, int rows, size_t row0, int64_t p0, int n);
 };
