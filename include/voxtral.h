@@ -228,6 +228,27 @@ int32_t vox_session_set_top_k(vox_session *s, int32_t k);
  * if cap < b * n * k. */
 int32_t vox_session_token_scores(vox_session *s, int32_t *top_ids, float *top_logprobs, size_t cap, int32_t *b,
                                  int32_t *n, int32_t *k);
+/* Beam search for vox_transcribe_streaming, vox_transcribe_pcm and vox_transcribe_pcm_dev: width W in
+ * [1, VOX_MAX_BEAM] beams per stream, else VOX_EINVAL.  W = 1 (the default) is the greedy path, unchanged.
+ *   - After the prefill the beam list holds one entry, the prefix, with score 0.  At each emitted position every live
+ *     beam j offers its W most likely tokens (the token-score order, see vox_session_set_top_k) with log-probability
+ *     lp; a candidate's score is cum[j] + (double)lp, summed in f64 on the device.  The new beam list is the W best
+ *     candidates ordered by score descending, then parent rank j ascending, then token id ascending.  That order is the
+ *     beam ranking.
+ *   - Every position emits exactly one token, so every hypothesis has n_out tokens and no length penalty applies.  The
+ *     call returns the rank-0 hypothesis in out_ids; vox_session_nbest returns all W in rank order.
+ *   - The W beams of stream s run as W rows of the batched decode step, so b * W <= max_batch, else VOX_EINVAL.  Each
+ *     stream's delay applies to all of its beams.
+ *   - With token confidences on (k > 0), vox_session_token_scores returns, for the rank-0 hypothesis, the top-k of the
+ *     distribution each of its tokens was chosen from; top_ids[0] need not be the emitted id.
+ *   - While W > 1, vox_prefill and vox_decode_step return VOX_EINVAL (no incremental beam search).  A beam call leaves
+ *     the decoder cache empty (vox_session_cache_len 0).  Streaming pools always decode greedily. */
+#define VOX_MAX_BEAM 8
+int32_t vox_session_set_beam(vox_session *s, int32_t width);
+/* The n-best list of the last transcribe call: ids [b][w][n] (n = its n_out) and summed log-probabilities scores [b][w]
+ * (descending per stream); ids needs cap >= b * w * n elements and scores b * w.  Synchronises the session's stream.  Both
+ * buffers NULL: only *b, *w, *n are set.  VOX_EINVAL if that call ran at width 1, VOX_ECAPACITY if cap is short. */
+int32_t vox_session_nbest(vox_session *s, int32_t *ids, double *scores, size_t cap, int32_t *b, int32_t *w, int32_t *n);
 int32_t vox_session_cache_len(const vox_session *s, int32_t *len);             /* LayerCaches::seq_len */
 int32_t vox_session_reset(vox_session *s);                                       /* LayerCaches::reset  */
 /* debugging / parity: copy an internal activation by name ("enc_out","audio_embeds","conv","enc<i>",

@@ -71,6 +71,10 @@ extern "C" {
     pub fn vox_session_set_top_k(s: *mut vox_session, k: i32) -> i32;
     pub fn vox_session_token_scores(s: *mut vox_session, top_ids: *mut i32, top_logprobs: *mut f32, cap: usize,
                                     b: *mut i32, n: *mut i32, k: *mut i32) -> i32;
+    // beam search of the transcribe calls (width <= VOX_MAX_BEAM = 8; 1 = greedy) and its n-best list
+    pub fn vox_session_set_beam(s: *mut vox_session, width: i32) -> i32;
+    pub fn vox_session_nbest(s: *mut vox_session, ids: *mut i32, scores: *mut f64, cap: usize, b: *mut i32, w: *mut i32,
+                             n: *mut i32) -> i32;
     pub fn vox_session_free(s: *mut vox_session);
     // src/gguf/{tensor,linear,op}.rs
     pub fn vox_q4_tensor_create(bytes: *const u8, nbytes: usize, n: i64, k: i64, device: i32,

@@ -3,7 +3,7 @@
 `voxtral-transcribe` binary; here the model is loaded once in-process and utterances are batched per GPU step).
 
     python scripts/eval_wer.py --gguf models/voxtral-q4.gguf --tokenizer models/voxtral/tekken.json \
-        --manifest utts.jsonl [--batch 8] [--delay 6] [--streaming]
+        --manifest utts.jsonl [--batch 8] [--delay 6] [--streaming | --beam W]
 
 `utts.jsonl`: one {"id", "audio": path to a 16 kHz mono WAV (PCM16/float32), "text": reference} per line -- datasets
 cannot be downloaded in the build environment, so the loader is a manifest, not HF `datasets`.  Needs the REAL weights
@@ -12,7 +12,9 @@ instead of vox_transcribe_pcm and must give the same hypotheses.
 Word error rate = word-level Levenshtein distance / reference words after the same normalisation for both sides
 (lower-case, punctuation stripped) -- what jiwer computes for the reference's report.  Next to each utterance's WER
 the report gives its mean log-probability over the emitted text tokens (ids >= 1000; vox_session_set_top_k): the
-utterances the model was least sure of are the ones to review first.
+utterances the model was least sure of are the ones to review first.  `--beam W` transcribes with beam search of width
+W (the best hypothesis, with each token's log-probability in the distribution it was chosen from).  Like the rest of
+this script it needs the real weights; the beam option has not been run on real speech.
 """
 from __future__ import annotations
 
@@ -69,15 +71,19 @@ def main():
     ap.add_argument("--max-seconds", type=float, default=30.0)
     ap.add_argument("--streaming", action="store_true")
     ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--beam", type=int, default=1, help="beam width (offline only; 1 = greedy)")
     args = ap.parse_args()
     import voxtral_mini_realtime_rs_b200 as vx
 
+    assert args.beam == 1 or not args.streaming, "streaming pools decode greedily"
     utts = [json.loads(l) for l in open(args.manifest) if l.strip()]
     tok = vx.VoxtralTokenizer.from_file(args.tokenizer)
     max_mel = int(args.max_seconds * 100) + 1200
-    model = vx.Q4ModelLoader.from_file(args.gguf).load(args.device, max_batch=args.batch, max_mel_frames=max_mel)
+    model = vx.Q4ModelLoader.from_file(args.gguf).load(args.device, max_batch=max(args.batch, args.beam),
+                                                        max_mel_frames=max_mel)
     model.set_delay(args.delay)
-    model.set_top_k(1)   # each emitted token's log-probability
+    model.set_beam(args.beam)
+    model.set_top_k(max(1, args.beam))   # each emitted token's log-probability (at W > 1: among its parent's W best)
     errs = words = 0
     audio_s = 0.0
     t0 = time.time()
@@ -111,7 +117,8 @@ def main():
             lp = np.concatenate(lps)
         else:
             ids = model.transcribe_pcm(a, peak_normalize=False)[0]
-            lp = model.token_scores()[1][0, :, 0]
+            top_ids, top_lp = (x[0] for x in model.token_scores())
+            lp = top_lp[np.arange(len(ids)), np.argmax(top_ids == np.asarray(ids)[:, None], axis=1)]
         hyp = decode(ids)
         r, h = normalise(u["text"]), normalise(hyp)
         e = edit_distance(r, h)

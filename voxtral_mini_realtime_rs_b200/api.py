@@ -134,6 +134,9 @@ _SIGS = {
     "vox_session_set_top_k": (C.c_int32, [_P, C.c_int32]),
     "vox_session_token_scores": (C.c_int32, [_P, _P, _P, C.c_size_t, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
                                              C.POINTER(C.c_int32)]),
+    "vox_session_set_beam": (C.c_int32, [_P, C.c_int32]),
+    "vox_session_nbest": (C.c_int32, [_P, _P, _P, C.c_size_t, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                      C.POINTER(C.c_int32)]),
     "vox_session_cache_len": (C.c_int32, [_P, C.POINTER(C.c_int32)]),
     "vox_session_reset": (C.c_int32, [_P]),
     "vox_session_debug_read": (C.c_int32, [_P, C.c_char_p, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
@@ -661,6 +664,21 @@ class Q4VoxtralModel:
         lp = np.empty((b.value, n.value, k.value), np.float32)
         _check(lib().vox_session_token_scores(self._s, _ptr(ids), _ptr(lp), ids.size, C.byref(b), C.byref(n), C.byref(k)))
         return ids, lp
+
+    def set_beam(self, w: int):
+        """Beam search of width w (1..8) for later transcribe calls; 1 is greedy.  B streams at width w need
+        B * w <= max_batch.  The calls return the best hypothesis; nbest() returns all w."""
+        _check(lib().vox_session_set_beam(self._s, w))
+
+    def nbest(self):
+        """(ids [B,W,n] int32, scores [B,W] float64) of the last transcribe call at beam width W > 1, in rank order;
+        scores are summed log-probabilities."""
+        b, w, n = C.c_int32(), C.c_int32(), C.c_int32()
+        _check(lib().vox_session_nbest(self._s, None, None, 0, C.byref(b), C.byref(w), C.byref(n)))
+        ids = np.empty((b.value, w.value, n.value), np.int32)
+        scores = np.empty((b.value, w.value), np.float64)
+        _check(lib().vox_session_nbest(self._s, _ptr(ids), _ptr(scores), ids.size, C.byref(b), C.byref(w), C.byref(n)))
+        return ids, scores
 
     def cache_len(self) -> int:
         v = C.c_int32()

@@ -715,6 +715,7 @@ int32_t vox_prefill(vox_session *sh, const int32_t *ids, int32_t b, int32_t m, i
     const vox_model_info &c = s->m->info;
     VOX_CHECK(b >= 1 && b <= s->max_batch, VOX_EINVAL, "batch %d exceeds session max_batch %d", b, s->max_batch);
     VOX_CHECK(m >= 1 && m <= s->M_max, VOX_EINVAL, "M=%d out of range [1,%d]", m, s->M_max);
+    VOX_CHECK(s->beam_w == 1, VOX_EINVAL, "vox_prefill runs greedy only: the session's beam width is %d", s->beam_w);
     VOX_CHECK(s->cache_len + m <= s->out_ld, VOX_EINVAL, "KV cache full (%d + %d > %d)", s->cache_len, m, s->out_ld);
     if (add_audio)
         VOX_CHECK(b == s->cur_B && s->cache_len + m <= s->cur_S4, VOX_EINVAL,
@@ -735,6 +736,7 @@ int32_t vox_decode_step(vox_session *sh, const int32_t *tok, int32_t b, int32_t 
     Session *s = sh->s;
     const vox_model_info &c = s->m->info;
     VOX_CHECK(b >= 1 && b <= s->max_batch, VOX_EINVAL, "batch %d exceeds session max_batch %d", b, s->max_batch);
+    VOX_CHECK(s->beam_w == 1, VOX_EINVAL, "vox_decode_step runs greedy only: the session's beam width is %d", s->beam_w);
     VOX_CHECK(s->cache_len + 1 <= s->out_ld, VOX_EINVAL, "KV cache full (%d + 1 > %d)", s->cache_len, s->out_ld);
     if (add_audio)
         VOX_CHECK(b == s->cur_B && s->cache_len < s->cur_S4, VOX_EINVAL,
@@ -784,6 +786,31 @@ int32_t vox_session_token_scores(vox_session *sh, int32_t *top_ids, float *top_l
         CUDA_OK(cudaMemcpy2D(top_logprobs + dst, sizeof(float) * K, s->d_top_lp + at, pitch, sizeof(float) * K, N,
                              cudaMemcpyDeviceToHost));
     }
+    VOX_API_END
+}
+static_assert(VOX_MAX_BEAM == BEAM_MAX, "the beam kernels handle up to VOX_MAX_BEAM beams per stream");
+int32_t vox_session_set_beam(vox_session *s, int32_t width) {
+    VOX_API_BEGIN
+    REQUIRE(s);
+    s->s->set_beam(width);
+    VOX_API_END
+}
+int32_t vox_session_nbest(vox_session *sh, int32_t *ids, double *scores, size_t cap, int32_t *b, int32_t *w, int32_t *n) {
+    VOX_API_BEGIN
+    REQUIRE(sh);
+    Session *s = sh->s;
+    const int B = s->nbest_b, W = s->nbest_w, N = s->nbest_n;
+    VOX_CHECK(W > 0, VOX_EINVAL, "no n-best list: the last transcribe ran at beam width 1 (vox_session_set_beam)");
+    if (b) *b = B;
+    if (w) *w = W;
+    if (n) *n = N;
+    if (!ids && !scores) return VOX_OK;
+    REQUIRE(ids); REQUIRE(scores);
+    VOX_CHECK(cap >= (size_t)B * W * N, VOX_ECAPACITY, "n-best capacity %zu < %d x %d x %d", cap, B, W, N);
+    CUDA_OK(cudaSetDevice(s->m->device));
+    CUDA_OK(cudaStreamSynchronize(s->st));
+    if (N > 0) CUDA_OK(cudaMemcpy(ids, s->d_nbest_ids, sizeof(int32_t) * B * W * N, cudaMemcpyDeviceToHost));
+    CUDA_OK(cudaMemcpy(scores, s->d_nbest_scores, sizeof(double) * B * W, cudaMemcpyDeviceToHost));
     VOX_API_END
 }
 int32_t vox_session_cache_len(const vox_session *s, int32_t *len) {

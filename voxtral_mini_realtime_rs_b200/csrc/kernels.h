@@ -227,6 +227,28 @@ struct ScoreWork {
 };
 void launch_token_scores(const float *logits, int B, int V, int k, const int *out_pos_ptr, int out_ld, int *top_ids,
                          float *top_logprobs, const ScoreWork &w, cudaStream_t st);
+// Beam search (vox_session_set_beam, beam.cu): the W beams of stream s (of b) run as rows w * b + s of the decode step.
+// After each step (token scores at k >= W have run), launch_beam_select takes, per stream, the W best of the candidates
+// (live rank j, one of its row's top-W ids) by score cum[j] + (double)logprob descending, then parent rank ascending,
+// then id ascending; writes the new ranks' rows, cum and d_tok, and each row's (token, parent row) at its output
+// position out_pos - 1.  The first child of a surviving parent keeps the parent's row; the other children take the rows
+// of the ranks without children.  launch_beam_fork then gives every row whose parent row q differs from itself q's
+// page-table entries of the full pages below its next write position and a copy of the filled part of q's current page.
+// launch_beam_traceback walks the parent rows back from the last position: ids [b][W][n] and scores [b][W] in rank
+// order; rank 0's ids into out rows [0, b); with top_ids (non-null), rank 0's token scores gathered into rows [0, b).
+constexpr int BEAM_MAX = 8;   // VOX_MAX_BEAM (the top-k list holds the W candidates of a row: BEAM_MAX <= TOPK_MAX)
+struct BeamWork {
+    int *rank_row = nullptr;                        // [b][W] row holding each rank
+    double *cum = nullptr;                          // [b][W] summed log-probability of each rank
+    int *src = nullptr;                             // [rows] parent row of each row's beam (== row: nothing to fork)
+    int *hist_tok = nullptr, *hist_par = nullptr;   // [rows][out_ld] token and parent row per output position
+};
+void launch_beam_select(const int *top_ids, const float *top_lp, const int *out_pos, int out_ld, int b, int W, int n_live,
+                        const BeamWork &w, int *tok, cudaStream_t st);
+void launch_beam_fork(float *kc, float *vc, size_t layer_stride, int layers, int *page_table, int max_pages, const int *pos,
+                      const int *src, int rows, int Hkv, int hd, cudaStream_t st);
+void launch_beam_traceback(const BeamWork &w, int b, int W, int n, int out_ld, int *ids, double *scores, int *out,
+                           int *top_ids, float *top_lp, cudaStream_t st);
 // a[i] += da; b[i] += db for i < n  (device-side per-row step counters for graph replay)
 void launch_advance(int *a, int da, int *b, int db, int n, cudaStream_t st);
 // gather rows: dst[b][:] = src[b*M + (M-1)][:]

@@ -646,9 +646,9 @@ void Session::bind_delays(const int *streams, int n) {
     ada_row_streams.assign(streams, streams + n);
 }
 
-void Session::bind_delays_identity(int B) {
+void Session::bind_row_delays(int B) {
     std::vector<int> id(B);
-    for (int b = 0; b < B; ++b) id[b] = b;
+    for (int b = 0; b < B; ++b) id[b] = beam_streams > 0 ? b % beam_streams : b;
     bind_delays(id.data(), B);
 }
 
@@ -725,7 +725,7 @@ bool Session::decoder_forward(int B, int M) {
     const int D = c.dec_dim, H = c.dec_heads, Hkv = c.dec_kv_heads, hd = c.dec_head_dim;
     const int qkvd = (H + 2 * Hkv) * hd, rows = B * M;
     const float scale = powf((float)hd, -0.5f);
-    if (!stream_mode) bind_delays_identity(B);   // (a stream pool binds its rows' sessions itself)
+    if (!stream_mode) bind_row_delays(B);   // (a stream pool binds its rows' sessions itself)
     // decode-sized problems: RMSNorm fused into the consuming matvec, RoPE + KV append fused into the
     // attention kernel => 5 launches per layer instead of 8
     const bool fused = fused_decode(rows);
@@ -885,7 +885,7 @@ void Session::decode_step(int B, bool add_audio) {
     // 128-token tile).  The scratch activations are reused by the
     // groups; the per-row state (token, positions, page table, audio row, output row, logits) is addressed from the
     // group's first row.
-    if (!stream_mode) bind_delays_identity(B);
+    if (!stream_mode) bind_row_delays(B);
     const int rows_per_launch = B > 8 ? 8 : B;
     if (!stream_mode)
         for (int b = 0; b < B; ++b) out_rows[b] += 1;
@@ -905,24 +905,74 @@ void Session::decode_step(int B, bool add_audio) {
 
 void Session::set_top_k(int k) {
     VOX_CHECK(k >= 0 && k <= TOPK_MAX, VOX_EINVAL, "top_k %d out of range [0,%d]", k, TOPK_MAX);
-    if (k > 0 && !d_top_ids) {
-        CUDA_OK(cudaSetDevice(m->device));
-        const size_t n = (size_t)max_batch * out_ld * TOPK_MAX, parts = (size_t)max_batch * ARGMAX_PARTS;
-        d_top_ids = arena.alloc_n<int>(n);
-        d_top_lp = arena.alloc_n<float>(n);
-        score_work.m = arena.alloc_n<float>(parts);
-        score_work.l = arena.alloc_n<float>(parts);
-        score_work.vals = arena.alloc_n<float>(parts * TOPK_MAX);
-        score_work.idx = arena.alloc_n<int>(parts * TOPK_MAX);
-        score_work.counters = arena.alloc_n<int>(max_batch);
-        CUDA_OK(cudaMemset(score_work.counters, 0, sizeof(int) * max_batch));
-    }
+    if (k > 0) alloc_scores();
     top_k = k;
+}
+
+void Session::alloc_scores() {
+    if (d_top_ids) return;
+    CUDA_OK(cudaSetDevice(m->device));
+    const size_t n = (size_t)max_batch * out_ld * TOPK_MAX, parts = (size_t)max_batch * ARGMAX_PARTS;
+    d_top_ids = arena.alloc_n<int>(n);
+    d_top_lp = arena.alloc_n<float>(n);
+    score_work.m = arena.alloc_n<float>(parts);
+    score_work.l = arena.alloc_n<float>(parts);
+    score_work.vals = arena.alloc_n<float>(parts * TOPK_MAX);
+    score_work.idx = arena.alloc_n<int>(parts * TOPK_MAX);
+    score_work.counters = arena.alloc_n<int>(max_batch);
+    CUDA_OK(cudaMemset(score_work.counters, 0, sizeof(int) * max_batch));
 }
 
 // after the step's argmax and counter advance: row b's scores land at its output position d_outpos[b] - 1
 void Session::token_scores(int B) {
-    if (top_k > 0) launch_token_scores(logits, B, m->info.vocab, top_k, d_outpos, out_ld, d_top_ids, d_top_lp, score_work, st);
+    const int k = std::max(top_k, beam_streams > 0 ? beam_w : 0);
+    if (k > 0) launch_token_scores(logits, B, m->info.vocab, k, d_outpos, out_ld, d_top_ids, d_top_lp, score_work, st);
+}
+
+static_assert(BEAM_MAX <= TOPK_MAX, "a beam's candidates are the first W entries of its row's top-k list");
+
+void Session::set_beam(int w) {
+    VOX_CHECK(w >= 1 && w <= BEAM_MAX, VOX_EINVAL, "beam width %d out of range [1,%d]", w, BEAM_MAX);
+    if (w > 1 && !beam.rank_row) {
+        alloc_scores();
+        const size_t rows = max_batch, hist = (size_t)max_batch * out_ld;
+        beam.rank_row = arena.alloc_n<int>(rows);
+        beam.cum = arena.alloc_n<double>(rows);
+        beam.src = arena.alloc_n<int>(rows);
+        beam.hist_tok = arena.alloc_n<int>(hist);
+        beam.hist_par = arena.alloc_n<int>(hist);
+        d_nbest_ids = arena.alloc_n<int>(hist);   // b * W <= max_batch hypotheses of n <= out_ld ids
+        d_nbest_scores = arena.alloc_n<double>(rows);
+    }
+    beam_w = w;
+}
+
+// The prefill left stream s's prefix in row s.  Beam rows w * b + s take stream s's audio embeddings and step counters;
+// the selection at position 0 has one live rank per stream (the prefix, score 0), whose top-W ids become the W beams,
+// and the fork hands the prefix's KV to the other rows.
+void Session::beam_start(int b) {
+    const int W = beam_w;
+    const size_t per = (size_t)cur_S4 * m->info.dec_dim;
+    for (int w = 1; w < W; ++w) {
+        CUDA_OK(cudaMemcpyAsync(audio + (size_t)w * b * per, audio, sizeof(float) * b * per, cudaMemcpyDeviceToDevice, st));
+        CUDA_OK(cudaMemcpyAsync(d_pos + w * b, d_pos, sizeof(int) * b, cudaMemcpyDeviceToDevice, st));
+        CUDA_OK(cudaMemcpyAsync(d_outpos + w * b, d_outpos, sizeof(int) * b, cudaMemcpyDeviceToDevice, st));
+    }
+    std::vector<int> rank_row((size_t)b * W);
+    for (int s = 0; s < b; ++s)
+        for (int w = 0; w < W; ++w) rank_row[(size_t)s * W + w] = w * b + s;
+    CUDA_OK(cudaMemcpyAsync(beam.rank_row, rank_row.data(), sizeof(int) * rank_row.size(), cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaMemsetAsync(beam.cum, 0, sizeof(double) * b * W, st));
+    CUDA_OK(cudaStreamSynchronize(st));   // rank_row dies with this frame
+    page_table_forked = true;
+    beam_step(b, 1);
+}
+
+void Session::beam_step(int b, int n_live) {
+    const vox_model_info &c = m->info;
+    launch_beam_select(d_top_ids, d_top_lp, d_outpos, out_ld, b, beam_w, n_live, beam, d_tok, st);
+    launch_beam_fork(kc, vc, kv_layer_stride(), c.dec_layers, d_page_table, kv_max_pages, d_pos, beam.src, b * beam_w,
+                     c.dec_kv_heads, c.dec_head_dim, st);
 }
 
 // One launch of the persistent kernel for rows [b0, b0 + B) (B <= 8) of the session; mega_prepare() has built the op table.
@@ -1017,6 +1067,11 @@ void Session::reset() {
     CUDA_OK(cudaMemsetAsync(d_outpos, 0, sizeof(int) * max_batch, st));
     std::fill(out_rows.begin(), out_rows.end(), 0);
     cache_len = 0;
+    if (page_table_forked) {
+        CUDA_OK(cudaMemcpyAsync(d_page_table, page_table_host.data(), sizeof(int) * page_table_host.size(),
+                                cudaMemcpyHostToDevice, st));
+        page_table_forked = false;
+    }
     rebase_epoch();
 }
 
@@ -1039,10 +1094,21 @@ void Session::rebase_epoch() {
 int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids, vox_timings *tm, bool timed_pre) {
     const vox_model_info &c = m->info;
     (void)timed_pre;
+    const int W = beam_w, R = B * W;   // decode rows: beam w of stream s in row w * B + s
+    VOX_CHECK(W == 1 || R <= max_batch, VOX_EINVAL, "beam width %d x %d streams exceeds session max_batch %d", W, B, max_batch);
+    struct BeamRows {   // the rows map to their streams for this call only, also when it throws
+        Session *s;
+        ~BeamRows() { s->beam_streams = 0; }
+    } beam_rows{this};
+    beam_streams = W > 1 ? B : 0;
     encode(B, T);
     CUDA_OK(cudaEventRecord(ev[2], st));
     const int S4 = cur_S4, P = c.prefix_len;
     int n_out = 0;
+    auto step = [&] {
+        decode_step(R);
+        if (W > 1) beam_step(B, W);
+    };
     if (S4 >= P) {
         n_out = S4 - P;
         VOX_CHECK(cap_ids >= (size_t)B * n_out, VOX_ECAPACITY, "out_ids capacity %zu < %d x %d", cap_ids, B, n_out);
@@ -1051,6 +1117,7 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
         std::vector<int> prefix((size_t)B * P, 32);
         for (int b = 0; b < B; ++b) prefix[(size_t)b * P] = 1;
         prefill(B, P, prefix.data(), true);
+        if (W > 1) beam_start(B);
         CUDA_OK(cudaEventRecord(ev[4], st));
         const int steps = S4 - P - 1;
         if (steps > 0) mega_steps_host += (unsigned)steps;  // upper bound of the device epoch's advance
@@ -1058,11 +1125,11 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
             int done = 0;
             if (use_graph) {
                 // (prefill() has bound the rows' delays: a captured step of the other ADA mode launches other kernels)
-                if (!step_graph || step_graph_B != B || step_graph_S4 != S4 || step_graph_per_row != ada_per_row ||
-                    step_graph_top_k != top_k) {
+                if (!step_graph || step_graph_B != R || step_graph_S4 != S4 || step_graph_per_row != ada_per_row ||
+                    step_graph_top_k != top_k || step_graph_beam != W) {
                     // first step eagerly (also performs any one-time kernel attribute setup),
                     // then capture one step and replay it
-                    decode_step(B);
+                    step();
                     done = 1;
                     if (step_graph) { cudaGraphExecDestroy(step_graph); step_graph = nullptr; }
                     if (steps > 1) {
@@ -1070,7 +1137,7 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
                         const uint64_t before = kernel_launch_count();
                         CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
                         try {
-                            decode_step(B);
+                            step();
                         } catch (...) {
                             cudaStreamEndCapture(st, &graph);
                             if (graph) cudaGraphDestroy(graph);
@@ -1082,10 +1149,11 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
                         cudaError_t e = cudaGraphInstantiate(&step_graph, graph, 0);
                         cudaGraphDestroy(graph);
                         cuda_check(e, "cudaGraphInstantiate");
-                        step_graph_B = B;
+                        step_graph_B = R;
                         step_graph_S4 = S4;
                         step_graph_per_row = ada_per_row;
                         step_graph_top_k = top_k;
+                        step_graph_beam = W;
                     }
                 }
                 for (; done < steps; ++done) {
@@ -1093,9 +1161,14 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
                     add_graph_launches((int64_t)step_graph_nodes);
                 }
             } else {
-                for (; done < steps; ++done) decode_step(B);
+                for (; done < steps; ++done) step();
             }
         }
+        if (W > 1)
+            launch_beam_traceback(beam, B, W, n_out, out_ld, d_nbest_ids, d_nbest_scores, d_out, top_k > 0 ? d_top_ids : nullptr,
+                                  d_top_lp, st);
+    } else if (W > 1) {
+        CUDA_OK(cudaMemsetAsync(d_nbest_scores, 0, sizeof(double) * R, st));
     }
     if (S4 < P) CUDA_OK(cudaEventRecord(ev[4], st));
     CUDA_OK(cudaEventRecord(ev[3], st));
@@ -1104,9 +1177,18 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
     CUDA_OK(cudaStreamSynchronize(st));
     for (int b = 0; b < B; ++b)
         for (int i = 0; i < n_out; ++i) out_ids[(size_t)b * n_out + i] = host[(size_t)b * out_ld + i];
-    cache_len = n_out > 0 ? S4 - 1 : 0;
-    if (n_out > 0)   // (a captured step counted an output it did not produce)
-        for (int b = 0; b < B; ++b) out_rows[b] = n_out;
+    nbest_b = B;
+    nbest_w = W > 1 ? W : 0;
+    nbest_n = n_out;
+    if (W > 1) {
+        // the cache holds W hypotheses per stream, not one: the incremental API starts over, on the identity page table
+        reset();
+        CUDA_OK(cudaStreamSynchronize(st));
+    } else {
+        cache_len = n_out > 0 ? S4 - 1 : 0;
+        if (n_out > 0)   // (a captured step counted an output it did not produce)
+            for (int b = 0; b < B; ++b) out_rows[b] = n_out;
+    }
     scores_k = top_k;
     scores_b = B;
     scores_n = n_out;

@@ -158,7 +158,22 @@ struct Session {
     float *d_top_lp = nullptr;
     ScoreWork score_work;
     void set_top_k(int k);
-    void token_scores(int B);   // launch over rows [0, B) of the step that just ran (no-op while top_k == 0)
+    void alloc_scores();        // the score buffers above (first use)
+    // launch over rows [0, B) of the step that just ran at k = max(top_k, beam width of a running beam call); no-op at 0
+    void token_scores(int B);
+    // beam search (vox_session_set_beam): beam_w beams per stream for the transcribe calls; 1 = greedy (no launch, no
+    // memory).  A call over b streams at W > 1 runs rows w * b + s (beam w of stream s; kernels.h BeamWork), allocated
+    // with the n-best results by the first set_beam(W > 1).
+    int beam_w = 1;
+    int beam_streams = 0;           // > 0 while a beam call runs: row r belongs to stream r % beam_streams
+    BeamWork beam;
+    int *d_nbest_ids = nullptr;     // [b][W][n] of the last transcribe
+    double *d_nbest_scores = nullptr;
+    int nbest_b = 0, nbest_w = 0, nbest_n = 0;   // nbest_w == 0: the last transcribe ran greedy
+    bool page_table_forked = false; // a beam call has rewritten page-table rows: reset() re-uploads the identity table
+    void set_beam(int w);
+    void beam_start(int b);         // after the prefill of rows [0, b): replicate them to every beam row, select position 0
+    void beam_step(int b, int n_live);   // selection + KV fork after a step over the b * beam_w rows
     // what vox_session_token_scores returns: the last transcribe (positions [0, n) of `b` rows) or incremental call (the
     // position `step_pos` of each row), scored with k = scores_k (0: that call ran with scores off)
     int scores_k = 0, scores_b = 0, scores_n = 0;
@@ -166,7 +181,7 @@ struct Session {
     // host mirror of d_outpos[] outside stream mode: outputs per row since reset (prefill / decode_step / transcribe)
     std::vector<int> out_rows;
     cudaGraphExec_t step_graph = nullptr;
-    int step_graph_B = 0, step_graph_S4 = 0, step_graph_top_k = 0;
+    int step_graph_B = 0, step_graph_S4 = 0, step_graph_top_k = 0, step_graph_beam = 1;
     bool step_graph_per_row = false;  // the captured step's ADA mode (its kernels and arguments differ)
     uint64_t step_graph_nodes = 0;
     bool use_graph = true;
@@ -226,7 +241,8 @@ struct Session {
     // the same delay (loading that delay's vectors into ada / ffn_gamma_ada), else per-row tables.  Launch-free and
     // copy-free when nothing changed (so it may run inside a stream capture).
     void bind_delays(const int *streams, int n);
-    void bind_delays_identity(int B);  // row b = stream b (every call but the stream pool's)
+    // row b = stream b, or stream b % beam_streams during a beam call (every call but the stream pool's)
+    void bind_row_delays(int B);
     // mel already on device, time-major, in s->mel_tm
     void encode(int B, int T);
     // launch_q4_linear with the session's GEMM scratch and path choice; `gamma`, `ada`, `tmp` and `tc` as there
