@@ -523,7 +523,7 @@ int32_t vox_session_set_delays(vox_session *s, const float *delays, int32_t b) {
 
 static void upload_mel(Session *s, const float *mel, int b, int t) {
     const vox_model_info &c = s->m->info;
-    VOX_CHECK(b >= 1 && b <= s->max_batch, VOX_EINVAL, "batch %d exceeds session max_batch %d", b, s->max_batch);
+    s->check_batch(b);
     VOX_CHECK(t >= 1 && t <= s->max_mel_frames, VOX_EINVAL, "mel frames %d exceed session max_mel_frames %d", t,
               s->max_mel_frames);
     CUDA_OK(cudaSetDevice(s->m->device));
@@ -571,15 +571,14 @@ int32_t vox_transcribe_streaming(vox_session *sh, const float *mel, int32_t b, i
     CUDA_OK(cudaEventRecord(s->ev[0], s->st));
     upload_mel(s, mel, b, t);
     CUDA_OK(cudaEventRecord(s->ev[1], s->st));
-    *n_out = s->transcribe_from_mel(b, t, out_ids, cap, tm, true);
+    *n_out = s->transcribe_from_mel(b, t, out_ids, cap, tm);
     fill_timings(s, tm);
     VOX_API_END
 }
 
 static int32_t transcribe_pcm_impl(Session *s, const float *host, const float *dev, int b, size_t n, int normalize,
                                    int32_t *out_ids, size_t cap, int32_t *n_out, vox_timings *tm) {
-    const vox_model_info &c = s->m->info;
-    VOX_CHECK(b >= 1 && b <= s->max_batch, VOX_EINVAL, "batch %d exceeds session max_batch %d", b, s->max_batch);
+    s->check_batch(b);
     VOX_CHECK(n >= 1, VOX_EINVAL, "empty audio");
     CUDA_OK(cudaSetDevice(s->m->device));
     vox_pad_config pc;
@@ -607,8 +606,7 @@ static int32_t transcribe_pcm_impl(Session *s, const float *host, const float *d
     launch_mel(s->pcm_pad, b, padded, padded, s->m->mel.window, s->m->mel.fb_vals, s->m->mel.fb_start, s->m->mel.fb_len,
                s->m->mel.fb_stride, s->mel_tm, (int)frames, 0, s->st);
     CUDA_OK(cudaEventRecord(s->ev[1], s->st));
-    (void)c;
-    *n_out = s->transcribe_from_mel(b, (int)frames, out_ids, cap, tm, true);
+    *n_out = s->transcribe_from_mel(b, (int)frames, out_ids, cap, tm);
     fill_timings(s, tm);
     return VOX_OK;
 }
@@ -633,26 +631,17 @@ int32_t vox_generate_step_with_cache(vox_session *sh, const int32_t *ids, int32_
     REQUIRE(sh); REQUIRE(ids); REQUIRE(logits);
     Session *s = sh->s;
     const vox_model_info &c = s->m->info;
-    VOX_CHECK(b >= 1 && b <= s->max_batch, VOX_EINVAL, "batch %d exceeds session max_batch %d", b, s->max_batch);
+    s->check_batch(b);
     VOX_CHECK(m >= 1 && m <= s->M_max, VOX_EINVAL, "M=%d out of range [1,%d]", m, s->M_max);
     VOX_CHECK(s->cache_len + m <= s->out_ld, VOX_EINVAL, "KV cache full (%d + %d > %d)", s->cache_len, m, s->out_ld);
-    for (int i = 0; i < b * m; ++i)
-        VOX_CHECK(ids[i] >= 0 && ids[i] < c.vocab, VOX_EINVAL, "token id %d out of range", ids[i]);
+    s->check_ids(ids, (size_t)b * m);
     const size_t n = (size_t)b * m * c.vocab;
     VOX_CHECK(cap >= n, VOX_ECAPACITY, "logits capacity %zu < %zu", cap, n);
     CUDA_OK(cudaSetDevice(s->m->device));
-    if (n > s->logits_all_cap) {
-        s->logits_all = s->arena.alloc_n<float>(n);
-        s->logits_all_cap = n;
-    }
-    CUDA_OK(cudaMemcpyAsync(s->d_ids, ids, sizeof(int) * (size_t)b * m, cudaMemcpyHostToDevice, s->st));
-    launch_embed(s->m->tok_emb, s->d_ids, nullptr, 0, b, m, nullptr, s->x_dec, s->fused_decode(b * m) ? s->ssq_x : nullptr, s->st);
-    const bool pending = s->decoder_forward(b, m);
-    s->lm_head_rows(b * m, pending, s->logits_all);
-    launch_advance(s->d_pos, m, nullptr, 0, b, s->st);
+    if (n > s->logits_all_cap) { s->logits_all = s->arena.alloc_n<float>(n); s->logits_all_cap = n; }
+    s->forward_logits(b, m, ids, false, s->logits_all);
     CUDA_OK(cudaMemcpyAsync(logits, s->logits_all, sizeof(float) * n, cudaMemcpyDeviceToHost, s->st));
     CUDA_OK(cudaStreamSynchronize(s->st));
-    s->cache_len += m;
     VOX_API_END
 }
 // forward_streaming (model.rs:801-814): teacher-forced full pass, inputs = audio_embeds + embed(ids).
@@ -667,43 +656,26 @@ int32_t vox_forward_streaming(vox_session *sh, const float *mel, int32_t b, int3
     const int S4 = s->cur_S4;
     VOX_CHECK(n_ids == S4, VOX_EINVAL, "forward_streaming needs one token id per audio position (%d), got %d", S4, n_ids);
     VOX_CHECK(S4 <= s->out_ld, VOX_EINVAL, "sequence %d exceeds the session KV capacity %d", S4, s->out_ld);
-    for (int i = 0; i < b * n_ids; ++i) VOX_CHECK(ids[i] >= 0 && ids[i] < c.vocab, VOX_EINVAL, "token id %d out of range", ids[i]);
+    s->check_ids(ids, (size_t)b * n_ids);
     const size_t n = (size_t)b * S4 * c.vocab;
     VOX_CHECK(cap >= n, VOX_ECAPACITY, "logits capacity %zu < %zu", cap, n);
     s->reset();
     const int Mc = s->M_max;
     const size_t chunk_floats = (size_t)b * Mc * c.vocab;
-    if (chunk_floats > s->logits_all_cap) {
-        s->logits_all = s->arena.alloc_n<float>(chunk_floats);
-        s->logits_all_cap = chunk_floats;
-    }
+    if (chunk_floats > s->logits_all_cap) { s->logits_all = s->arena.alloc_n<float>(chunk_floats); s->logits_all_cap = chunk_floats; }
     std::vector<int> chunk_ids;
     for (int p0 = 0; p0 < S4; p0 += Mc) {
         const int m = std::min(Mc, S4 - p0);
         chunk_ids.resize((size_t)b * m);
         for (int bb = 0; bb < b; ++bb)
             for (int i = 0; i < m; ++i) chunk_ids[(size_t)bb * m + i] = ids[(size_t)bb * S4 + p0 + i];
-        CUDA_OK(cudaMemcpyAsync(s->d_ids, chunk_ids.data(), sizeof(int) * chunk_ids.size(), cudaMemcpyHostToDevice, s->st));
-        launch_embed(s->m->tok_emb, s->d_ids, s->audio, S4, b, m, s->d_pos, s->x_dec, s->fused_decode(b * m) ? s->ssq_x : nullptr, s->st);
-        const bool pending = s->decoder_forward(b, m);
-        s->lm_head_rows(b * m, pending, s->logits_all);
-        launch_advance(s->d_pos, m, nullptr, 0, b, s->st);
+        s->forward_logits(b, m, chunk_ids.data(), true, s->logits_all);
         for (int bb = 0; bb < b; ++bb)
             CUDA_OK(cudaMemcpyAsync(logits + ((size_t)bb * S4 + p0) * c.vocab, s->logits_all + (size_t)bb * m * c.vocab,
                                     sizeof(float) * (size_t)m * c.vocab, cudaMemcpyDeviceToHost, s->st));
         CUDA_OK(cudaStreamSynchronize(s->st));  // chunk_ids is reused
     }
-    s->cache_len = S4;
     VOX_API_END
-}
-
-// what vox_session_token_scores returns after an incremental call over rows [0, b): each row's position just emitted
-static void record_step_scores(Session *s, int b) {
-    s->scores_k = s->top_k;
-    s->scores_b = b;
-    s->scores_n = 1;
-    s->scores_pos.assign(s->out_rows.begin(), s->out_rows.begin() + b);
-    for (int &p : s->scores_pos) p -= 1;
 }
 
 // Device-side incremental decode (SURVEY 8(b); model.rs:857-867 without the logits round trip): the argmax stays on
@@ -712,8 +684,7 @@ int32_t vox_prefill(vox_session *sh, const int32_t *ids, int32_t b, int32_t m, i
     VOX_API_BEGIN
     REQUIRE(sh); REQUIRE(ids);
     Session *s = sh->s;
-    const vox_model_info &c = s->m->info;
-    VOX_CHECK(b >= 1 && b <= s->max_batch, VOX_EINVAL, "batch %d exceeds session max_batch %d", b, s->max_batch);
+    s->check_batch(b);
     VOX_CHECK(m >= 1 && m <= s->M_max, VOX_EINVAL, "M=%d out of range [1,%d]", m, s->M_max);
     VOX_CHECK(s->beam_w == 1, VOX_EINVAL, "vox_prefill runs greedy only: the session's beam width is %d", s->beam_w);
     VOX_CHECK(s->cache_len + m <= s->out_ld, VOX_EINVAL, "KV cache full (%d + %d > %d)", s->cache_len, m, s->out_ld);
@@ -721,11 +692,9 @@ int32_t vox_prefill(vox_session *sh, const int32_t *ids, int32_t b, int32_t m, i
         VOX_CHECK(b == s->cur_B && s->cache_len + m <= s->cur_S4, VOX_EINVAL,
                   "add_audio: positions %d..%d need audio embeddings of %d streams (have %d positions for %d streams; call vox_encode_audio first)",
                   s->cache_len, s->cache_len + m, b, s->cur_S4, s->cur_B);
-    for (int i = 0; i < b * m; ++i) VOX_CHECK(ids[i] >= 0 && ids[i] < c.vocab, VOX_EINVAL, "token id %d out of range", ids[i]);
+    s->check_ids(ids, (size_t)b * m);
     CUDA_OK(cudaSetDevice(s->m->device));
-    s->prefill(b, m, ids, add_audio != 0);
-    s->cache_len += m;
-    record_step_scores(s, b);
+    s->step_incremental(b, m, ids, add_audio != 0);
     if (next_tok) CUDA_OK(cudaMemcpyAsync(next_tok, s->d_tok, sizeof(int) * b, cudaMemcpyDeviceToHost, s->st));
     CUDA_OK(cudaStreamSynchronize(s->st));   // `ids` is caller memory
     VOX_API_END
@@ -734,8 +703,7 @@ int32_t vox_decode_step(vox_session *sh, const int32_t *tok, int32_t b, int32_t 
     VOX_API_BEGIN
     REQUIRE(sh);
     Session *s = sh->s;
-    const vox_model_info &c = s->m->info;
-    VOX_CHECK(b >= 1 && b <= s->max_batch, VOX_EINVAL, "batch %d exceeds session max_batch %d", b, s->max_batch);
+    s->check_batch(b);
     VOX_CHECK(s->beam_w == 1, VOX_EINVAL, "vox_decode_step runs greedy only: the session's beam width is %d", s->beam_w);
     VOX_CHECK(s->cache_len + 1 <= s->out_ld, VOX_EINVAL, "KV cache full (%d + 1 > %d)", s->cache_len, s->out_ld);
     if (add_audio)
@@ -743,13 +711,10 @@ int32_t vox_decode_step(vox_session *sh, const int32_t *tok, int32_t b, int32_t 
                   "add_audio: position %d has no audio embedding (%d positions, %d streams encoded)", s->cache_len, s->cur_S4, s->cur_B);
     CUDA_OK(cudaSetDevice(s->m->device));
     if (tok) {
-        for (int i = 0; i < b; ++i) VOX_CHECK(tok[i] >= 0 && tok[i] < c.vocab, VOX_EINVAL, "token id %d out of range", tok[i]);
+        s->check_ids(tok, b);
         CUDA_OK(cudaMemcpyAsync(s->d_tok, tok, sizeof(int) * b, cudaMemcpyHostToDevice, s->st));
     }
-    s->decode_step(b, add_audio != 0);
-    s->mega_steps_host += 1;
-    s->cache_len += 1;
-    record_step_scores(s, b);
+    s->step_incremental(b, 1, nullptr, add_audio != 0);
     if (next_tok) CUDA_OK(cudaMemcpyAsync(next_tok, s->d_tok, sizeof(int) * b, cudaMemcpyDeviceToHost, s->st));
     if (next_tok || tok) CUDA_OK(cudaStreamSynchronize(s->st));
     VOX_API_END
@@ -849,8 +814,8 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
         s->debug_capture = false;
         if (n_floats) *n_floats = 0;
         return VOX_OK;
-    } else if (w == "graph_off") {
-        s->use_graph = false;
+    } else if (w == "graph_off" || w == "graph_on") {
+        s->use_graph = (w == "graph_on");
         if (n_floats) *n_floats = 0;
         return VOX_OK;
     } else if (w == "enc_attn_simt" || w == "enc_attn_tc") {
@@ -865,18 +830,23 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
         // mega_on / mega_auto: persistent decode kernel for every batch size (the default policy since round 2: it is no
         // slower than the per-op launches even for a single stream); mega_off: per-op launches
         s->use_mega = (w != "mega_off");
-        s->mega_B = 0;
-        if (s->step_graph) { cudaGraphExecDestroy(s->step_graph); s->step_graph = nullptr; }
         if (n_floats) *n_floats = 0;
         return VOX_OK;
     } else if (w == "tc_off" || w == "tc_on") {
         s->path.matvec_tc = (w == "tc_on");
-        if (s->step_graph) { cudaGraphExecDestroy(s->step_graph); s->step_graph = nullptr; }
         if (n_floats) *n_floats = 0;
         return VOX_OK;
-    } else if (w == "graph_on") {
-        s->use_graph = true;
-        if (n_floats) *n_floats = 0;
+    } else if (w == "mega_epoch") {
+        // {persistent-kernel launches counted on the host since the last re-base, the device epoch}: equal between calls
+        int epoch = 0;
+        CUDA_OK(cudaStreamSynchronize(s->st));
+        CUDA_OK(cudaMemcpy(&epoch, s->mega_epoch, sizeof(int), cudaMemcpyDeviceToHost));
+        const float v[2] = {(float)s->mega_steps_host, (float)epoch};
+        if (n_floats) *n_floats = 2;
+        if (out) {
+            VOX_CHECK(cap >= 2, VOX_ECAPACITY, "debug_read capacity %zu < 2", cap);
+            memcpy(out, v, sizeof(v));
+        }
         return VOX_OK;
     } else if (w == "mega_trace") {
         // phase trace of the last persistent decode step (CTA 0): per op {start, staged, body done,

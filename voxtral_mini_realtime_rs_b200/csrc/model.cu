@@ -544,7 +544,7 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ri
 }
 
 Session::~Session() {
-    if (step_graph) cudaGraphExecDestroy(step_graph);
+    if (step_graph.exec) cudaGraphExecDestroy(step_graph.exec);
     for (auto &e : ev)
         if (e) cudaEventDestroy(e);
     if (st) cudaStreamDestroy(st);
@@ -652,10 +652,15 @@ void Session::bind_row_delays(int B) {
     bind_delays(id.data(), B);
 }
 
+void Session::check_batch(int b) const { VOX_CHECK(b >= 1 && b <= max_batch, VOX_EINVAL, "batch %d exceeds session max_batch %d", b, max_batch); }
+void Session::check_ids(const int32_t *ids, size_t n) const {
+    for (size_t i = 0; i < n; ++i) VOX_CHECK(ids[i] >= 0 && ids[i] < m->info.vocab, VOX_EINVAL, "token id %d out of range", ids[i]);
+}
+
 // Q4VoxtralModel::encode_audio (model.rs:783-788): conv -> 32 layers -> norm -> reshape x4 -> adapter
 void Session::encode(int B, int T) {
     const vox_model_info &c = m->info;
-    VOX_CHECK(B >= 1 && B <= max_batch, VOX_EINVAL, "batch %d exceeds session max_batch %d", B, max_batch);
+    check_batch(B);
     VOX_CHECK(T >= 1 && T <= max_mel_frames, VOX_EINVAL, "mel frames %d exceed session max_mel_frames %d", T, max_mel_frames);
     const int T1 = conv_out(T), S = conv_out(T1), S4 = S / c.reshape_factor;
     const int d = c.enc_dim, hdq = c.enc_heads * c.enc_head_dim;
@@ -761,6 +766,16 @@ void Session::lm_head_rows(int rows, bool norm_pending, float *dst) {
     const TcWork wk = tc_work(true, false);
     linear(m->tok_emb, norm_pending ? x_dec : h_dec, rows, dst, m->info.vocab, nullptr, nullptr, EPI_NONE,
            norm_pending ? m->dec_norm : nullptr, nullptr, nullptr, norm_pending ? &wk : nullptr);
+}
+
+void Session::forward_logits(int b, int M, const int *ids_host, bool with_audio, float *dst) {
+    CUDA_OK(cudaMemcpyAsync(d_ids, ids_host, sizeof(int) * (size_t)b * M, cudaMemcpyHostToDevice, st));
+    launch_embed(m->tok_emb, d_ids, with_audio ? audio : nullptr, with_audio ? cur_S4 : 0, b, M, with_audio ? d_pos : nullptr,
+                 x_dec, fused_decode(b * M) ? ssq_x : nullptr, st);
+    const bool pending = decoder_forward(b, M);
+    lm_head_rows(b * M, pending, dst);
+    launch_advance(d_pos, M, nullptr, 0, b, st);
+    cache_len += M;
 }
 
 // Builds (once per batch size) the op table of the persistent decode-step kernel.  Returns false when
@@ -876,31 +891,32 @@ void Session::mega_clear_fragments() {
     CUDA_OK(cudaMemsetAsync(mega_cf_off, 0, sizeof(float2) * mega_cf_blocks * 8, st));
 }
 
+// More than 8 rows: the rows are independent streams, so the step runs as consecutive launches of the persistent
+// kernel over groups of 8 rows (each group streams the weights once; the per-op GEMMs would pad 16-32 rows to a
+// 128-token tile).  The scratch activations are reused by the groups; the per-row state (token, positions, page table,
+// audio row, output row, logits) is addressed from the group's first row.
+unsigned Session::prepare_step(int R) {
+    if (!stream_mode) bind_row_delays(R);   // (a stream pool binds its rows' sessions itself)
+    return mega_prepare(std::min(R, 8)) ? (unsigned)(R + 7) / 8 : 0u;
+}
+
 // One autoregressive step for B streams (model.rs:938-960): embed(prev token) + audio[pos-1],
 // 26 layers, lm_head, argmax, device-side feedback; all positions read from device counters.
-void Session::decode_step(int B, bool add_audio) {
-    const vox_model_info &c = m->info;
-    // More than 8 rows: the rows are independent streams, so the step runs as consecutive launches of the persistent
-    // kernel over groups of 8 rows (each group streams the weights once; the per-op GEMMs would pad 16-32 rows to a
-    // 128-token tile).  The scratch activations are reused by the
-    // groups; the per-row state (token, positions, page table, audio row, output row, logits) is addressed from the
-    // group's first row.
-    if (!stream_mode) bind_row_delays(B);
-    const int rows_per_launch = B > 8 ? 8 : B;
-    if (!stream_mode)
-        for (int b = 0; b < B; ++b) out_rows[b] += 1;
-    if (mega_prepare(rows_per_launch)) {
+unsigned Session::decode_step(int B, bool add_audio) {
+    const unsigned mega_launches = prepare_step(B);
+    if (mega_launches > 0) {
         for (int b0 = 0; b0 < B; b0 += 8) decode_step_mega(b0, std::min(8, B - b0), add_audio);
-        token_scores(B);   // one launch over every group's rows
-        return;
+    } else {
+        launch_embed(m->tok_emb, d_tok, add_audio ? audio : nullptr, cur_S4, B, 1, d_pos, x_dec, fused_decode(B) ? ssq_x : nullptr,
+                     st, add_audio ? audio_rows_dev : nullptr);
+        const bool pending = decoder_forward(B, 1);
+        lm_head_rows(B, pending, logits);
+        launch_argmax_multi(logits, B, m->info.vocab, d_tok, stream_mode ? nullptr : d_out, out_ld, d_outpos, am_vals, am_idx,
+                            am_cnt, st);
+        launch_advance(d_pos, 1, d_outpos, 1, B, st);
     }
-    launch_embed(m->tok_emb, d_tok, add_audio ? audio : nullptr, cur_S4, B, 1, d_pos, x_dec, fused_decode(B) ? ssq_x : nullptr, st,
-                 add_audio ? audio_rows_dev : nullptr);
-    const bool pending = decoder_forward(B, 1);
-    lm_head_rows(B, pending, logits);
-    launch_argmax_multi(logits, B, c.vocab, d_tok, stream_mode ? nullptr : d_out, out_ld, d_outpos, am_vals, am_idx, am_cnt, st);
-    launch_advance(d_pos, 1, d_outpos, 1, B, st);
-    token_scores(B);
+    token_scores(B);   // one launch over every row (every group of the persistent kernel's)
+    return mega_launches;
 }
 
 void Session::set_top_k(int k) {
@@ -978,68 +994,66 @@ void Session::beam_step(int b, int n_live) {
 // One launch of the persistent kernel for rows [b0, b0 + B) (B <= 8) of the session; mega_prepare() has built the op table.
 void Session::decode_step_mega(int b0, int B, bool add_audio) {
     const vox_model_info &c = m->info;
-    {
-        if (B < mega_B) {
-            // a ragged last group on the 8-token instantiation: its padding tokens must read as zero fragments, not as
-            // the previous group's rows
-            mega_clear_fragments();
-        }
-        MegaParams p;
-        p.ops = mega_ops;
-        p.n_ops = mega_n_ops;
-        p.B = B;
-        p.eps = m->norm_eps;
-        p.qkv = qkv_dec;
-        p.ld_qkv = (c.dec_heads + 2 * c.dec_kv_heads) * c.dec_head_dim;
-        p.H = c.dec_heads;
-        p.Hkv = c.dec_kv_heads;
-        p.hd = c.dec_head_dim;
-        p.max_seq = out_ld;
-        p.page_table = d_page_table + (size_t)b0 * kv_max_pages;
-        p.max_pages = kv_max_pages;
-        p.window = c.dec_window;
-        p.scale = powf((float)c.dec_head_dim, -0.5f);
-        p.cos_t = dec_rope.cos_t;
-        p.sin_t = dec_rope.sin_t;
-        p.rope_rows = dec_rope.rows;
-        p.ring = kv_ring ? 1 : 0;
-        p.attn_out = attn_dec;
-        // key chunks per (stream, kv head): spread the KV walk over idle SMs, but no more than 4 -- the merging CTA waits
-        // for the other chunks' states one after the other (an L2 round trip each), and a CTA walks 64 keys per round
-        // trip anyway, so more chunks add merge latency without shortening the walk
-        p.attn_chunks = std::max(1, std::min(4, std::min(mega_grid, mega_att_units - 8 * c.dec_kv_heads) / (B * c.dec_kv_heads)));
-        p.att_acc = mega_att_acc;
-        p.att_ml = mega_att_ml;
-        p.d_epoch = mega_epoch;
-        p.emb_qs = m->tok_emb.qs;
-        p.emb_d = m->tok_emb.d;
-        p.D = c.dec_dim;
-        p.audio = add_audio && audio ? audio + (size_t)b0 * cur_S4 * c.dec_dim : nullptr;
-        p.audio_rows = add_audio && audio_rows_dev ? audio_rows_dev + b0 : nullptr;
-        p.audio_seq = cur_S4;
-        p.ffn_ada_rows = ada_per_row ? d_fga_rows + b0 : nullptr;
-        p.x_dec = x_dec;
-        p.ssq_x = ssq_x;
-        p.emb_fbf = mega_xf_bf;
-        p.emb_foff = mega_xf_off;
-        p.emb_gamma = m->dec[0].attn_norm;
-        p.att_fbf = mega_af_bf;
-        p.att_foff = mega_af_off;
-        p.d_pos = d_pos + b0;
-        p.d_outpos = d_outpos + b0;
-        p.d_tok = d_tok + b0;
-        p.d_out = stream_mode ? nullptr : d_out + (size_t)b0 * out_ld;
-        p.out_ld = out_ld;
-        p.logits_out = logits + (size_t)b0 * c.vocab;
-        p.am_vals = mega_am_vals;
-        p.am_idx = mega_am_idx;
-        p.bar = mega_bar;
-        p.nstage = mega_plan.nstage;
-        p.scratch_bytes = mega_plan.scratch_bytes;
-        p.trace = mega_trace;
-        p.trace_all = mega_trace_all;
-        launch_decode_mega(p, mega_plan, mega_grid, st);
+    if (B < mega_B) {
+        // a ragged last group on the 8-token instantiation: its padding tokens must read as zero fragments, not as
+        // the previous group's rows
+        mega_clear_fragments();
     }
+    MegaParams p;
+    p.ops = mega_ops;
+    p.n_ops = mega_n_ops;
+    p.B = B;
+    p.eps = m->norm_eps;
+    p.qkv = qkv_dec;
+    p.ld_qkv = (c.dec_heads + 2 * c.dec_kv_heads) * c.dec_head_dim;
+    p.H = c.dec_heads;
+    p.Hkv = c.dec_kv_heads;
+    p.hd = c.dec_head_dim;
+    p.max_seq = out_ld;
+    p.page_table = d_page_table + (size_t)b0 * kv_max_pages;
+    p.max_pages = kv_max_pages;
+    p.window = c.dec_window;
+    p.scale = powf((float)c.dec_head_dim, -0.5f);
+    p.cos_t = dec_rope.cos_t;
+    p.sin_t = dec_rope.sin_t;
+    p.rope_rows = dec_rope.rows;
+    p.ring = kv_ring ? 1 : 0;
+    p.attn_out = attn_dec;
+    // key chunks per (stream, kv head): spread the KV walk over idle SMs, but no more than 4 -- the merging CTA waits
+    // for the other chunks' states one after the other (an L2 round trip each), and a CTA walks 64 keys per round
+    // trip anyway, so more chunks add merge latency without shortening the walk
+    p.attn_chunks = std::max(1, std::min(4, std::min(mega_grid, mega_att_units - 8 * c.dec_kv_heads) / (B * c.dec_kv_heads)));
+    p.att_acc = mega_att_acc;
+    p.att_ml = mega_att_ml;
+    p.d_epoch = mega_epoch;
+    p.emb_qs = m->tok_emb.qs;
+    p.emb_d = m->tok_emb.d;
+    p.D = c.dec_dim;
+    p.audio = add_audio && audio ? audio + (size_t)b0 * cur_S4 * c.dec_dim : nullptr;
+    p.audio_rows = add_audio && audio_rows_dev ? audio_rows_dev + b0 : nullptr;
+    p.audio_seq = cur_S4;
+    p.ffn_ada_rows = ada_per_row ? d_fga_rows + b0 : nullptr;
+    p.x_dec = x_dec;
+    p.ssq_x = ssq_x;
+    p.emb_fbf = mega_xf_bf;
+    p.emb_foff = mega_xf_off;
+    p.emb_gamma = m->dec[0].attn_norm;
+    p.att_fbf = mega_af_bf;
+    p.att_foff = mega_af_off;
+    p.d_pos = d_pos + b0;
+    p.d_outpos = d_outpos + b0;
+    p.d_tok = d_tok + b0;
+    p.d_out = stream_mode ? nullptr : d_out + (size_t)b0 * out_ld;
+    p.out_ld = out_ld;
+    p.logits_out = logits + (size_t)b0 * c.vocab;
+    p.am_vals = mega_am_vals;
+    p.am_idx = mega_am_idx;
+    p.bar = mega_bar;
+    p.nstage = mega_plan.nstage;
+    p.scratch_bytes = mega_plan.scratch_bytes;
+    p.trace = mega_trace;
+    p.trace_all = mega_trace_all;
+    launch_decode_mega(p, mega_plan, mega_grid, st);
 }
 
 // Prefill of M positions for B streams (model.rs:894-923 with M = 38; also the incremental vox_prefill).
@@ -1058,8 +1072,17 @@ void Session::prefill(int B, int M, const int *ids_host, bool add_audio) {
     launch_argmax(logits, B, c.vocab, d_tok, stream_mode ? nullptr : d_out, out_ld, d_outpos, st);
     launch_advance(d_pos, M, d_outpos, 1, B, st);
     token_scores(B);
-    if (!stream_mode)
-        for (int b = 0; b < B; ++b) out_rows[b] += 1;
+}
+
+void Session::step_incremental(int b, int M, const int *ids_host, bool add_audio) {
+    if (ids_host) prefill(b, M, ids_host, add_audio);
+    else mega_steps_host += decode_step(b, add_audio);
+    cache_len += M;
+    scores_k = top_k;
+    scores_b = b;
+    scores_n = 1;
+    scores_pos.resize(b);
+    for (int r = 0; r < b; ++r) scores_pos[r] = out_rows[r]++;   // each row's output just emitted
 }
 
 void Session::reset() {
@@ -1077,7 +1100,7 @@ void Session::reset() {
 
 void Session::rebase_epoch() {
     // the persistent kernel's attention-chunk states carry the tag epoch * 64 + layer + 1 (int): re-base the device
-    // epoch long before that can overflow (2^24 steps ~ 10 hours of continuous decoding) -- and wipe the tagged words, so
+    // epoch long before that can overflow (2^24 launches ~ 10 hours of continuous decoding) -- and wipe the tagged words, so
     // that no stale state can match a tag of the new numbering
     if (mega_steps_host > (1u << 24)) {
         const vox_model_info &ci = m->info;
@@ -1089,11 +1112,51 @@ void Session::rebase_epoch() {
     }
 }
 
+// A replay reads the op table and the ADA bindings the host built for the captured step's shape: prepare_step re-builds
+// them before the first replay (an incremental call in between may have built them for another row count), and every
+// other host-side choice the captured kernels depend on is in the key.  `step()` returns its persistent-kernel launches.
+template <class Step>
+void Session::run_steps(int R, int n, Step step) {
+    if (n <= 0) return;
+    prepare_step(R);
+    const StepKey key{R, cur_S4, top_k, beam_w, ada_per_row, path.matvec_tc, path.gemm_tc, use_mega};
+    if (use_graph && !(step_graph.exec && step_graph.key == key)) {
+        // first step eagerly (also performs any one-time kernel attribute setup), then capture one step and replay it
+        mega_steps_host += step();
+        --n;
+        if (step_graph.exec) { cudaGraphExecDestroy(step_graph.exec); step_graph.exec = nullptr; }
+        if (n > 0) {
+            cudaGraph_t graph = nullptr;
+            const uint64_t before = kernel_launch_count();
+            CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+            try {
+                step_graph.mega_launches = step();   // captured, not executed: not counted
+            } catch (...) {
+                cudaStreamEndCapture(st, &graph);
+                if (graph) cudaGraphDestroy(graph);
+                throw;
+            }
+            CUDA_OK(cudaStreamEndCapture(st, &graph));
+            step_graph.nodes = kernel_launch_count() - before;
+            add_graph_launches(-(int64_t)step_graph.nodes);  // captured, not executed
+            cudaError_t e = cudaGraphInstantiate(&step_graph.exec, graph, 0);
+            cudaGraphDestroy(graph);
+            cuda_check(e, "cudaGraphInstantiate");
+            step_graph.key = key;
+        }
+    }
+    for (int i = 0; i < n; ++i) {
+        if (!use_graph) { mega_steps_host += step(); continue; }
+        CUDA_OK(cudaGraphLaunch(step_graph.exec, st));
+        add_graph_launches((int64_t)step_graph.nodes);
+        mega_steps_host += step_graph.mega_launches;
+    }
+}
+
 // Q4VoxtralModel::transcribe_streaming (model.rs:873-963).  Expects the mel in s->mel; records
 // ev[1] (after encode) and ev[2] (after decode) on the stream.  Returns tokens per stream.
-int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids, vox_timings *tm, bool timed_pre) {
+int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids, vox_timings *tm) {
     const vox_model_info &c = m->info;
-    (void)timed_pre;
     const int W = beam_w, R = B * W;   // decode rows: beam w of stream s in row w * B + s
     VOX_CHECK(W == 1 || R <= max_batch, VOX_EINVAL, "beam width %d x %d streams exceeds session max_batch %d", W, B, max_batch);
     struct BeamRows {   // the rows map to their streams for this call only, also when it throws
@@ -1105,10 +1168,6 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
     CUDA_OK(cudaEventRecord(ev[2], st));
     const int S4 = cur_S4, P = c.prefix_len;
     int n_out = 0;
-    auto step = [&] {
-        decode_step(R);
-        if (W > 1) beam_step(B, W);
-    };
     if (S4 >= P) {
         n_out = S4 - P;
         VOX_CHECK(cap_ids >= (size_t)B * n_out, VOX_ECAPACITY, "out_ids capacity %zu < %d x %d", cap_ids, B, n_out);
@@ -1119,51 +1178,11 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
         prefill(B, P, prefix.data(), true);
         if (W > 1) beam_start(B);
         CUDA_OK(cudaEventRecord(ev[4], st));
-        const int steps = S4 - P - 1;
-        if (steps > 0) mega_steps_host += (unsigned)steps;  // upper bound of the device epoch's advance
-        if (steps > 0) {
-            int done = 0;
-            if (use_graph) {
-                // (prefill() has bound the rows' delays: a captured step of the other ADA mode launches other kernels)
-                if (!step_graph || step_graph_B != R || step_graph_S4 != S4 || step_graph_per_row != ada_per_row ||
-                    step_graph_top_k != top_k || step_graph_beam != W) {
-                    // first step eagerly (also performs any one-time kernel attribute setup),
-                    // then capture one step and replay it
-                    step();
-                    done = 1;
-                    if (step_graph) { cudaGraphExecDestroy(step_graph); step_graph = nullptr; }
-                    if (steps > 1) {
-                        cudaGraph_t graph = nullptr;
-                        const uint64_t before = kernel_launch_count();
-                        CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-                        try {
-                            step();
-                        } catch (...) {
-                            cudaStreamEndCapture(st, &graph);
-                            if (graph) cudaGraphDestroy(graph);
-                            throw;
-                        }
-                        CUDA_OK(cudaStreamEndCapture(st, &graph));
-                        step_graph_nodes = kernel_launch_count() - before;
-                        add_graph_launches(-(int64_t)step_graph_nodes);  // captured, not executed
-                        cudaError_t e = cudaGraphInstantiate(&step_graph, graph, 0);
-                        cudaGraphDestroy(graph);
-                        cuda_check(e, "cudaGraphInstantiate");
-                        step_graph_B = R;
-                        step_graph_S4 = S4;
-                        step_graph_per_row = ada_per_row;
-                        step_graph_top_k = top_k;
-                        step_graph_beam = W;
-                    }
-                }
-                for (; done < steps; ++done) {
-                    CUDA_OK(cudaGraphLaunch(step_graph, st));
-                    add_graph_launches((int64_t)step_graph_nodes);
-                }
-            } else {
-                for (; done < steps; ++done) step();
-            }
-        }
+        run_steps(R, S4 - P - 1, [&] {
+            const unsigned launches = decode_step(R);
+            if (W > 1) beam_step(B, W);
+            return launches;
+        });
         if (W > 1)
             launch_beam_traceback(beam, B, W, n_out, out_ld, d_nbest_ids, d_nbest_scores, d_out, top_k > 0 ? d_top_ids : nullptr,
                                   d_top_lp, st);
@@ -1186,8 +1205,8 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
         CUDA_OK(cudaStreamSynchronize(st));
     } else {
         cache_len = n_out > 0 ? S4 - 1 : 0;
-        if (n_out > 0)   // (a captured step counted an output it did not produce)
-            for (int b = 0; b < B; ++b) out_rows[b] = n_out;
+        if (S4 >= P)   // the prefill's output and one per step
+            for (int b = 0; b < B; ++b) out_rows[b] = std::max(n_out, 1);
     }
     scores_k = top_k;
     scores_b = B;

@@ -5,6 +5,7 @@
 
 #include <cstdint>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #include "audio_host.h"
@@ -96,6 +97,21 @@ Q4Weight upload_q4(DeviceArena &arena, const std::vector<const uint8_t *> &raw, 
 // (transcribe.rs:49-51)
 constexpr float kDefaultDelay = 6.0f;
 
+// Everything a captured decode step depends on that is chosen on the host: a step captured under another key launches
+// other kernels or reads another op table.
+struct StepKey {
+    int rows = 0, S4 = 0, top_k = 0, beam_w = 1;
+    bool ada_per_row = false, matvec_tc = true, gemm_tc = true, use_mega = true;
+    auto tie() const { return std::tie(rows, S4, top_k, beam_w, ada_per_row, matvec_tc, gemm_tc, use_mega); }
+    bool operator==(const StepKey &o) const { return tie() == o.tie(); }
+};
+struct StepGraph {
+    StepKey key;
+    cudaGraphExec_t exec = nullptr;
+    uint64_t nodes = 0;            // kernel launches per replay
+    unsigned mega_launches = 0;    // persistent-kernel launches per replay
+};
+
 struct Session {
     Model *m = nullptr;
     int max_batch = 0, max_mel_frames = 0;
@@ -178,12 +194,9 @@ struct Session {
     // position `step_pos` of each row), scored with k = scores_k (0: that call ran with scores off)
     int scores_k = 0, scores_b = 0, scores_n = 0;
     std::vector<int> scores_pos;    // per row, empty after a transcribe
-    // host mirror of d_outpos[] outside stream mode: outputs per row since reset (prefill / decode_step / transcribe)
+    // host mirror of d_outpos[] outside stream mode: outputs per row since reset (incremental calls / transcribe)
     std::vector<int> out_rows;
-    cudaGraphExec_t step_graph = nullptr;
-    int step_graph_B = 0, step_graph_S4 = 0, step_graph_top_k = 0, step_graph_beam = 1;
-    bool step_graph_per_row = false;  // the captured step's ADA mode (its kernels and arguments differ)
-    uint64_t step_graph_nodes = 0;
+    StepGraph step_graph;   // the offline transcription's decode step, captured once per key and replayed
     bool use_graph = true;
     // scratch of the fused decode path: split-K partials + tickets, per-tile sums of squares of the
     // residual stream (consumed by the next kernel's fused RMSNorm), multi-CTA argmax scratch
@@ -205,7 +218,9 @@ struct Session {
     float *mega_att_acc = nullptr, *mega_att_ml = nullptr;  // key-chunk softmax states (MG_ATTN -> MG_ATTN_MERGE)
     int mega_att_units = 0;
     int *mega_epoch = nullptr;
-    unsigned mega_steps_host = 0;  // decode steps since the device epoch was last re-based (Session::reset)
+    // persistent-kernel launches executed since the device epoch was last re-based (Session::reset): advanced by the
+    // code that issues or replays steps, never under stream capture
+    unsigned mega_steps_host = 0;
     // activation fragments (decode_mega.cu frag_build): residual stream x norm weight, attention output, SwiGLU output
     uint2 *mega_xf_bf = nullptr, *mega_af_bf = nullptr, *mega_cf_bf = nullptr;
     float2 *mega_xf_off = nullptr, *mega_af_off = nullptr, *mega_cf_off = nullptr;
@@ -251,12 +266,28 @@ struct Session {
                 const TcWork *tc = nullptr, const AdaRows &ada_rows = AdaRows{});
     bool decoder_forward(int B, int M);
     void lm_head_rows(int rows, bool norm_pending, float *dst);
-    void decode_step(int B, bool add_audio = true);
+    // teacher-forced pass over ids [b][M] (+ the audio embeddings at positions *d_pos.. when with_audio): logits of every
+    // row into dst [b * M][vocab], positions advanced by M
+    void forward_logits(int b, int M, const int *ids_host, bool with_audio, float *dst);
+    // host-side preparation a decode step over R rows depends on (row delays outside stream mode, the persistent
+    // kernel's op table); returns the step's persistent-kernel launches, 0 on the per-op path.  Copy- and sync-free when
+    // the last step had the same shape, so that it may run under stream capture.
+    unsigned prepare_step(int R);
+    // returns prepare_step(B); advances no host counter (it also runs under stream capture)
+    unsigned decode_step(int B, bool add_audio = true);
+    // `n` decode steps over R rows, each one `step()`: CUDA-graph replay of one captured step when use_graph, else eager
+    template <class Step> void run_steps(int R, int n, Step step);
     // generic prefill over ids [B][M] at positions *d_pos.. (+ audio rows when add_audio): KV append, lm_head of the
-    // last row, argmax -> d_tok (device feedback) and d_out; advances the counters
+    // last row, argmax -> d_tok (device feedback) and d_out; advances the device counters
     void prefill(int B, int M, const int *ids_host, bool add_audio);
+    // the incremental API after argument validation: vox_prefill over ids_host [b][M], or vox_decode_step (ids_host
+    // nullptr, M = 1) over rows [0, b); then advances cache_len, out_rows, the epoch count and the positions
+    // vox_session_token_scores reads
+    void step_incremental(int b, int M, const int *ids_host, bool add_audio);
+    void check_batch(int b) const;
+    void check_ids(const int32_t *ids, size_t n) const;
     // runs prefill + loop; returns tokens per stream
-    int transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids, vox_timings *tm, bool timed_pre);
+    int transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids, vox_timings *tm);
     void reset();
     // re-bases the persistent kernel's step epoch once it has advanced far (see reset)
     void rebase_epoch();

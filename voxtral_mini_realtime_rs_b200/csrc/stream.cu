@@ -506,9 +506,8 @@ void StreamPool::tick(vox_stream_stats *st_out) {
             }
             upload_rows(rows, true);
             s->audio_rows_dev = d_audio_rows;
-            s->decode_step((int)rows.size(), true);
+            s->mega_steps_host += s->decode_step((int)rows.size(), true);
             s->audio_rows_dev = nullptr;
-            s->mega_steps_host += ((unsigned)rows.size() + 7) / 8;  // one persistent-kernel launch per group of 8 rows
             std::vector<int> toks(rows.size());
             std::vector<int32_t> top(rows.size() * s->top_k);
             std::vector<float> lp(rows.size() * s->top_k);
