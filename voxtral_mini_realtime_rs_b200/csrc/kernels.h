@@ -135,16 +135,16 @@ bool gemm_tc5_supported(const Q4Weight &w, int M);
 size_t gemm_tc5_split_elems(int M, int K);  // f16 elements needed for the split buffer
 void launch_split_tiles(const float *x, int M, int K, const float *gamma, const float *ada, float eps, void *xt,
                         cudaStream_t st, const AdaRows &ada_rows = AdaRows{});
-// Caller-owned scratch for the GEMM's deterministic split-K (used when N/128 x M/128 tiles cannot fill the GPU)
+// Caller-owned scratch for the GEMM's stream-K schedule: partial sums of tiles split across CTAs, summed in a fixed order
 struct GemmWork {
-    float *partial = nullptr;  // [slices][tiles][128][128]
+    float *partial = nullptr;  // [2 per CTA][tokens of the tile][128 features]
     size_t partial_floats = 0;
     int *counters = nullptr;   // [n_counters] zero between launches
     int n_counters = 0;
 };
 void launch_q4_gemm_tc5(const Q4Weight &w, const void *xt, int M, float *y, int ldy, const float *bias, const float *res,
                         int epi, const GemmWork *gw, cudaStream_t st);
-// GemmWork sizes that let launch_q4_gemm_tc5 split K as far as it ever does, for any shape; pointers left to the caller
+// GemmWork sizes launch_q4_gemm_tc5 needs (it refuses less), for any shape; pointers left to the caller
 GemmWork gemm_tc5_work_size();
 
 // Which Q4 kernels a caller lets launch_q4_linear choose: the tensor-core matvec for M <= 8 (else the SIMT matvec) and
@@ -157,7 +157,7 @@ struct Q4Path {
 struct Q4Scratch {
     void *xt = nullptr;             // split tiles of the wgmma GEMM
     size_t xt_elems = 0;            // capacity of xt; M > 8 rows needing more (gemm_tc5_split_elems) take the SIMT GEMM
-    const GemmWork *gw = nullptr;   // split-K of the wgmma GEMM (null: none)
+    const GemmWork *gw = nullptr;   // split tiles of the wgmma GEMM (required when xt is given)
     const TcWork *tc = nullptr;     // split-K and fused-norm sums of squares of the tensor-core matvec (null: neither)
 };
 // y = epi(norm(x) . W^T + bias) (+res) for any M: the one place that picks the Q4 kernel of a linear layer.
