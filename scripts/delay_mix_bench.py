@@ -2,8 +2,8 @@
 """What mixing transcription delays in one batch costs, on the full-size synthetic model (seed 42, the weights bench.py
 runs).  Alternating in one run, so that both arms see the same clocks and neighbours:
 
-  * decode step, B = 8 (one persistent-kernel launch): every stream at delay 6 (the shared-vector kernels) against
-    8 distinct delays (the per-row kernels: each row reads its own ffn_norm x ADA vector);
+  * decode step, B = 8 (one persistent-kernel launch): every stream at delay 6 against 8 distinct delays (the same
+    kernels either way: each row reads its own stream's ffn_norm x ADA vector);
   * pool tick, 8 streaming sessions fed 160 ms each per tick: all at delay 6 against 8 distinct delays.
 
     python scripts/delay_mix_bench.py [--rounds 10] [--steps 120] [--out DIR]

@@ -110,16 +110,16 @@ def test_prefill_mixed_delays(mixed, gemm):
 
 
 @pytest.mark.parametrize("path", ["mega_auto", "mega_off"])
-def test_shared_mode_is_unchanged(mixed, path):
-    """set_delays([d] * B) runs the shared-vector kernels: bitwise the logits, ids and launch counts of set_delay(d)."""
+def test_one_delay_via_set_delays_equals_set_delay(mixed, path):
+    """set_delays([d] * B) after another delay: bitwise the logits, ids and launch counts of set_delay(d)."""
     m, B, d = mixed.model, 5, 12.0
     m.debug(path)
     try:
         m.set_delay(d)
         a = mixed.teacher_forced(B, steps=6)
-        m.set_delay(30.0)                    # the shared vectors now hold delay 30 ...
+        m.set_delay(30.0)                    # every stream's set now holds delay 30 ...
         mixed.teacher_forced(B, steps=1)
-        m.set_delays([d] * B)                # ... and the next call loads stream 0's set (delay 12) into them
+        m.set_delays([d] * B)                # ... and is rewritten with delay 12
         b = mixed.teacher_forced(B, steps=6)
     finally:
         m.debug("mega_auto")
@@ -130,9 +130,9 @@ def test_shared_mode_is_unchanged(mixed, path):
 
 def test_graph_replay_follows_delay_changes(mixed):
     """transcribe_streaming replays a captured decode step.  Between consecutive graph transcriptions at the same B and
-    length, set_delay -> set_delays -> set_delays (other values) -> set_delay must re-capture when the ADA mode changes
-    (the per-row step launches other kernels) and may replay when only the delays change.  Each stream's ids equal the
-    eager transcription and the B = 1 transcription at that stream's delay, both run afterwards without graphs."""
+    length, set_delay -> set_delays -> set_delays (other values) -> set_delay only rewrite the streams' ADA sets, which
+    the replayed step reads in place.  Each stream's ids equal the eager transcription and the B = 1 transcription at that
+    stream's delay, both run afterwards without graphs."""
     m, B = mixed.model, 4
     mels = mixed.mels[:B]
     o32 = OracleModel(mixed.data)

@@ -349,7 +349,7 @@ int32_t vox_q4_matmul(const vox_q4 *w, const float *x_dev, float *y_dev, int32_t
     REQUIRE(w); REQUIRE(x_dev); REQUIRE(y_dev);
     VOX_CHECK(b > 0 && m > 0, VOX_EINVAL, "q4_matmul: B and M must be positive");
     CUDA_OK(cudaSetDevice(w->device));
-    launch_q4_linear(w->w, x_dev, b * m, y_dev, w->w.N, bias_dev, nullptr, EPI_NONE, nullptr, nullptr, 0.0f, nullptr,
+    launch_q4_linear(w->w, x_dev, b * m, y_dev, w->w.N, bias_dev, nullptr, EPI_NONE, nullptr, 0.0f, nullptr,
                      q4_scratch(const_cast<vox_q4 *>(w), b * m), g_q4_path, (cudaStream_t)stream);
     VOX_API_END
 }
@@ -365,7 +365,7 @@ int32_t vox_q4_matmul_host(const vox_q4 *wc, const float *x, float *y, int32_t b
     if (bias && !w->bias) w->bias = w->arena.alloc_n<float>(w->w.N);
     CUDA_OK(cudaMemcpyAsync(w->x, x, sizeof(float) * xn, cudaMemcpyHostToDevice, 0));
     if (bias) CUDA_OK(cudaMemcpyAsync(w->bias, bias, sizeof(float) * w->w.N, cudaMemcpyHostToDevice, 0));
-    launch_q4_linear(w->w, w->x, (int)rows, w->y, w->w.N, bias ? w->bias : nullptr, nullptr, EPI_NONE, nullptr, nullptr,
+    launch_q4_linear(w->w, w->x, (int)rows, w->y, w->w.N, bias ? w->bias : nullptr, nullptr, EPI_NONE, nullptr,
                      0.0f, nullptr, q4_scratch(w, (int)rows), g_q4_path, 0);
     CUDA_OK(cudaMemcpyAsync(y, w->y, sizeof(float) * yn, cudaMemcpyDeviceToHost, 0));
     CUDA_OK(cudaStreamSynchronize(0));
@@ -451,7 +451,7 @@ int32_t vox_q4_matmul_bench(const vox_q4 *const *ws, int32_t n_w, int32_t m, int
     CUDA_OK(cudaEventCreate(&e1));
     // no scratch: no split-K, and M > 8 takes the SIMT GEMM
     auto run = [&](int i) {
-        launch_q4_linear(ws[i % n_w]->w, x, m, y, ws[i % n_w]->w.N, nullptr, nullptr, EPI_NONE, nullptr, nullptr, 0.0f, nullptr,
+        launch_q4_linear(ws[i % n_w]->w, x, m, y, ws[i % n_w]->w.N, nullptr, nullptr, EPI_NONE, nullptr, 0.0f, nullptr,
                          Q4Scratch{}, g_q4_path, st);
     };
     for (int i = 0; i < warmup; ++i) run(i);
@@ -887,7 +887,7 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
     else if (w == "mel") { src = s->mel; n = 0; /* size unknown here */ }
     else if (w == "conv") { src = s->dbg_conv; n = rows * c.enc_dim; }
     else if (w == "logits") { src = s->logits; n = (size_t)s->cur_B * c.vocab; }
-    else if (w == "ada") { src = s->ada; n = (size_t)c.dec_layers * c.dec_dim; }
+    else if (w == "ada") { src = s->ada_sets; n = (size_t)c.dec_layers * c.dec_dim; }   // stream 0's ADA scale
     else if (w.rfind("enc", 0) == 0 && w.size() > 3) {
         const int i = atoi(w.c_str() + 3);
         VOX_CHECK(i >= 0 && i < c.enc_layers && s->dbg_layers, VOX_EINVAL, "no capture for '%s'", what);

@@ -364,9 +364,9 @@ __device__ __forceinline__ void mg_pair(const unsigned char *__restrict__ sb, co
 
 // RING: the rows are sessions of an unbounded stream pool -- KV page-table rows are rings (kernels.h KvView) and RoPE
 // rows come from p.cos_t / p.sin_t at pos % p.rope_rows; positions have no cap.  RING = false is the plain walk.
-// ROWS: the rows are streams at different transcription delays -- the wo phases scale token b's w13 input fragments by
-// its own ffn_norm x ADA vector (p.ffn_ada_rows[b]); ROWS = false reads the op's shared fout_gamma.
-template <int MT, int G, int DPL, bool RING, bool ROWS>
+// Each row is a stream at its own transcription delay: the wo phases scale token b's w13 input fragments by its own
+// ffn_norm x ADA vector (p.ffn_ada_rows[b]).
+template <int MT, int G, int DPL, bool RING>
 __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaParams p) {
     constexpr int CG = (MT + 3) / 4;
     constexpr int HD = DPL * 32;
@@ -422,19 +422,15 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                 // pull what the consumers touch first in the NEXT phase into L2 now
                 if (oi + 1 < p.n_ops) {
                     const MegaOp &nx = p.ops[oi + 1];
-                    if constexpr (ROWS) {
-                        // one row's vector per CTA, from the CTA that pulls a shared vector on: a producer that walked
-                        // the whole pointer table would hold back its own weight stream and make its CTA the straggler
-                        const int who = (cta - oi % nctas + nctas) % nctas;
-                        if (nx.kind == MG_MATVEC) {
-                            if (nx.fout_ada_layer >= 0) {
-                                if (who < B) bulk_prefetch_l2(p.ffn_ada_rows[who] + (size_t)nx.fout_ada_layer * p.D, (uint32_t)nx.N * 4u);
-                            } else if (who == 0 && nx.fout_gamma) {
-                                bulk_prefetch_l2(nx.fout_gamma, (uint32_t)nx.N * 4u);
-                            }
+                    // one row's vector per CTA, from the CTA that pulls a shared vector on: a producer that walked the
+                    // whole pointer table would hold back its own weight stream and make its CTA the straggler
+                    const int who = (cta - oi % nctas + nctas) % nctas;
+                    if (nx.kind == MG_MATVEC) {
+                        if (nx.fout_ada_layer >= 0) {
+                            if (who < B) bulk_prefetch_l2(p.ffn_ada_rows[who] + (size_t)nx.fout_ada_layer * p.D, (uint32_t)nx.N * 4u);
+                        } else if (who == 0 && nx.fout_gamma) {
+                            bulk_prefetch_l2(nx.fout_gamma, (uint32_t)nx.N * 4u);
                         }
-                    } else if (nx.kind == MG_MATVEC && (oi % nctas) == cta) {
-                        if (nx.fout_gamma) bulk_prefetch_l2(nx.fout_gamma, (uint32_t)nx.N * 4u);
                     }
                 }
                 if (op.kind != MG_MATVEC) continue;
@@ -567,9 +563,8 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                             const int f_blk = cta + (f_lb >> ush) * nctas;            // unit index = block index
                             const bool bact = fout_bf != nullptr && last && bi < f_nblk && bm_ < B;
                             float4 fg_lo = make_float4(1.f, 1.f, 1.f, 1.f), fg_hi = fg_lo;
-                            if (bact && fout_gamma) {
-                                const float *fg = fout_gamma;
-                                if (ROWS && vop->fout_ada_layer >= 0) fg = p.ffn_ada_rows[bm_] + (size_t)vop->fout_ada_layer * p.D;
+                            if (bact && (fout_gamma || vop->fout_ada_layer >= 0)) {
+                                const float *fg = vop->fout_ada_layer >= 0 ? p.ffn_ada_rows[bm_] + (size_t)vop->fout_ada_layer * p.D : fout_gamma;
                                 const float4 *gq4 = reinterpret_cast<const float4 *>(fg + (size_t)f_blk * 32);
                                 fg_lo = gq4[bt];
                                 fg_hi = gq4[4 + bt];
@@ -1249,10 +1244,10 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
     }
 }
 
-template <int MT, int G, int DPL, bool RING, bool ROWS>
+template <int MT, int G, int DPL, bool RING>
 void launch_t(const MegaParams &p, const MegaPlan &plan, int grid, cudaStream_t st) {
     static SmemAttr smem_attr;
-    cuda_check_mg(ensure_dyn_smem(decode_mega_kernel<MT, G, DPL, RING, ROWS>, MG_SMEM_MAX, smem_attr), "cudaFuncSetAttribute(decode_mega)");
+    cuda_check_mg(ensure_dyn_smem(decode_mega_kernel<MT, G, DPL, RING>, MG_SMEM_MAX, smem_attr), "cudaFuncSetAttribute(decode_mega)");
     // cooperative launch: the runtime refuses the launch (instead of the grid barrier hanging) if the
     // `grid` CTAs cannot all be resident at once
     cudaLaunchConfig_t cfg{};
@@ -1265,22 +1260,13 @@ void launch_t(const MegaParams &p, const MegaPlan &plan, int grid, cudaStream_t 
     attr[0].val.cooperative = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    cuda_check_mg(cudaLaunchKernelEx(&cfg, decode_mega_kernel<MT, G, DPL, RING, ROWS>, p), "decode_mega launch");
+    cuda_check_mg(cudaLaunchKernelEx(&cfg, decode_mega_kernel<MT, G, DPL, RING>, p), "decode_mega launch");
     tc_count_launch("decode_mega");
 }
 
-// one token (MT = 1) has one delay: the per-row instantiations exist for MT >= 2 only
 template <int MT, int G, int DPL>
 void launch_g(const MegaParams &p, const MegaPlan &plan, int grid, cudaStream_t st) {
-    if constexpr (MT > 1) {
-        if (p.ffn_ada_rows) {
-            (p.ring ? launch_t<MT, G, DPL, true, true> : launch_t<MT, G, DPL, false, true>)(p, plan, grid, st);
-            return;
-        }
-    } else {
-        VOX_CHECK(p.ffn_ada_rows == nullptr, VOX_EINVAL, "decode_mega: per-row ADA vectors need two or more rows");
-    }
-    (p.ring ? launch_t<MT, G, DPL, true, false> : launch_t<MT, G, DPL, false, false>)(p, plan, grid, st);
+    (p.ring ? launch_t<MT, G, DPL, true> : launch_t<MT, G, DPL, false>)(p, plan, grid, st);
 }
 
 template <int MT>
@@ -1329,6 +1315,7 @@ int decode_mega_grid(int device) {
 
 void launch_decode_mega(const MegaParams &p, const MegaPlan &plan, int grid, cudaStream_t st) {
     VOX_CHECK(p.nstage == plan.nstage && p.scratch_bytes == plan.scratch_bytes, VOX_EINVAL, "decode_mega: plan mismatch");
+    VOX_CHECK(p.ffn_ada_rows != nullptr, VOX_EINVAL, "decode_mega: no per-row ADA table");
     switch (plan.MT) {
         case 1: launch_m<1>(p, plan, grid, st); break;
         case 2: launch_m<2>(p, plan, grid, st); break;

@@ -28,7 +28,8 @@ struct MegaOp {
     const uint2 *fin_bf = nullptr;    // [K/32 (+pad)][2][2*MT][4]
     const float2 *fin_off = nullptr;  // [K/32 (+pad)][MT]
     // fragments of this op's OUTPUT for the next matvec (nullptr: plain output only): one 32-value block per
-    // unit of `unit_tiles` consecutive tiles (2: plain rows, 4: SiLU pairs), scaled by fout_gamma if set
+    // unit of `unit_tiles` consecutive tiles (2: plain rows, 4: SiLU pairs), scaled by fout_gamma if set (or per row:
+    // fout_ada_layer)
     uint2 *fout_bf = nullptr;
     float2 *fout_off = nullptr;
     const float *fout_gamma = nullptr;
@@ -44,8 +45,8 @@ struct MegaOp {
     // MG_ATTN
     float *kc = nullptr, *vc = nullptr;  // this layer's KV page pools [n_pages][Hkv][KV_PAGE][hd] (kernels.h KvView)
     int layer = 0;
-    // MG_MATVEC whose fout_gamma is layer j's ffn_norm x ADA scale (wo): j, else -1.  With per-row ADA sets
-    // (MegaParams::ffn_ada_rows) token b's fragments are scaled by ffn_ada_rows[b] + j * D instead.
+    // MG_MATVEC whose output fragments take layer j's ffn_norm x ADA scale (wo): j, else -1.  Token b's fragments are
+    // scaled by MegaParams::ffn_ada_rows[b] + j * D (fout_gamma is unset).
     int fout_ada_layer = -1;
 };
 
@@ -101,8 +102,7 @@ struct MegaParams {
     // RoPE row of position pos is pos % rope_rows of cos_t / sin_t (kernels.h KvView, RopeView)
     int ring = 0;
     int rope_rows = 0;
-    // optional [B]: each row's [L][D] ffn_norm x ADA set (streams at different transcription delays; the launch takes
-    // the per-row instantiation).  nullptr: every row uses the op table's shared fout_gamma.
+    // [B]: each row's [L][D] ffn_norm x ADA set (the rows' streams may be at different transcription delays)
     const float *const *ffn_ada_rows = nullptr;
 };
 

@@ -429,13 +429,12 @@ __global__ void __launch_bounds__(G5_THREADS, 1) gemm_tc5_kernel(const G5Args a)
 }
 
 // X (f32, row-major [M][K]) -> two f16 pieces of X * 2^s_t in the wgmma operand tile layout, optionally through RMSNorm
-// (x / sqrt(mean(x^2)+eps) * gamma (* ada)); s_t = per-token power of two putting the row maximum in [2^7, 2^8);
-// oscale[t] = 2^-(s_t + 8) undoes it (and the weights' 2^8) in the GEMM epilogue.  CTA = 8 token rows; rows >= M are
-// written as zeros.  ROWS: each row takes its own ADA vector from ada_rows (streams at different delays), not `ada`.
-template <bool ROWS>
-__device__ __forceinline__ void split_tiles_body(const float *__restrict__ x, int M, int K, const float *__restrict__ gamma,
-                                                 const float *__restrict__ ada_shared, const AdaRows &ada_rows, float eps,
-                                                 __half *__restrict__ xt, float *__restrict__ oscale, int TT, int KC, int BN) {
+// (x / sqrt(mean(x^2)+eps) * gamma (* the row's ADA vector, ada_rows.row(row))); s_t = per-token power of two putting
+// the row maximum in [2^7, 2^8); oscale[t] = 2^-(s_t + 8) undoes it (and the weights' 2^8) in the GEMM epilogue.
+// CTA = 8 token rows; rows >= M are written as zeros.
+__global__ void __launch_bounds__(256) split_tiles_kernel(const float *__restrict__ x, int M, int K, const float *__restrict__ gamma,
+                                                          const AdaRows ada_rows, float eps, __half *__restrict__ xt,
+                                                          float *__restrict__ oscale, int TT, int KC, int BN) {
     __shared__ float ssq_part[32][8], max_part[32][8];
     __shared__ float rms_s[8], sc_s[8];
     const int r8 = threadIdx.x & 7, cth = threadIdx.x >> 3;  // cth: 0..31 strides over the 16-byte chunks
@@ -443,7 +442,7 @@ __device__ __forceinline__ void split_tiles_body(const float *__restrict__ x, in
     const int nchunk = K >> 3;
     const bool valid = row < M;
     const float *xr = x + (size_t)(valid ? row : 0) * K;
-    const float *__restrict__ ada = ROWS ? (valid ? ada_rows.row(row) : nullptr) : ada_shared;
+    const float *__restrict__ ada = valid && ada_rows.rows ? ada_rows.row(row) : nullptr;
     {   // pass 1: sum of squares (RMSNorm) and max |x * gamma * ada| (the row maximum after the norm is this / rms)
         float ssq = 0.0f, mx = 0.0f;
         if (valid)
@@ -519,18 +518,6 @@ __device__ __forceinline__ void split_tiles_body(const float *__restrict__ x, in
     }
 }
 
-__global__ void __launch_bounds__(256) split_tiles_kernel(const float *__restrict__ x, int M, int K, const float *__restrict__ gamma,
-                                                          const float *__restrict__ ada, float eps, __half *__restrict__ xt,
-                                                          float *__restrict__ oscale, int TT, int KC, int BN) {
-    split_tiles_body<false>(x, M, K, gamma, ada, AdaRows{}, eps, xt, oscale, TT, KC, BN);
-}
-
-__global__ void __launch_bounds__(256) split_tiles_rows_kernel(const float *__restrict__ x, int M, int K, const float *__restrict__ gamma,
-                                                               const AdaRows ada_rows, float eps, __half *__restrict__ xt,
-                                                               float *__restrict__ oscale, int TT, int KC, int BN) {
-    split_tiles_body<true>(x, M, K, gamma, nullptr, ada_rows, eps, xt, oscale, TT, KC, BN);
-}
-
 
 }  // namespace
 
@@ -560,16 +547,12 @@ static float *g5_oscale_ptr(void *xt, int M, int K) {
 }
 
 // x [M][K] f32 -> xt (f16 pieces, tile layout; per-token scales behind them); rows padded to whole token tiles with zeros
-void launch_split_tiles(const float *x, int M, int K, const float *gamma, const float *ada, float eps, void *xt,
-                        cudaStream_t st, const AdaRows &ada_rows) {
+void launch_split_tiles(const float *x, int M, int K, const float *gamma, float eps, void *xt, cudaStream_t st,
+                        const AdaRows &ada_rows) {
     VOX_CHECK(K % G5_BK == 0, VOX_EINVAL, "split_tiles: K=%d not a multiple of 64", K);
     const int BN = g5_bn(M), TT = (M + BN - 1) / BN, KC = K / G5_BK;
-    if (ada_rows.rows)
-        split_tiles_rows_kernel<<<TT * (BN / 8), 256, 0, st>>>(x, M, K, gamma, ada_rows, eps, (__half *)xt, g5_oscale_ptr(xt, M, K),
-                                                               TT, KC, BN);
-    else
-        split_tiles_kernel<<<TT * (BN / 8), 256, 0, st>>>(x, M, K, gamma, ada, eps, (__half *)xt, g5_oscale_ptr(xt, M, K), TT, KC,
-                                                          BN);
+    split_tiles_kernel<<<TT * (BN / 8), 256, 0, st>>>(x, M, K, gamma, ada_rows, eps, (__half *)xt, g5_oscale_ptr(xt, M, K), TT, KC,
+                                                      BN);
     tc_count_launch("split_tiles");
 }
 

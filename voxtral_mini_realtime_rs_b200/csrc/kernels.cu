@@ -441,8 +441,11 @@ void launch_transpose_mel(const float *in, float *out, int B, int C, int T, cuda
 // RMSNorm (reference rms_norm.rs:42-47, burn::nn::RmsNorm): y = x / sqrt(mean(x^2)+eps) * gamma,
 // optionally times the precomputed ADA vector (1 + w2(gelu(w0 t))), model.rs:250-255.
 // =====================================================================================
-__device__ __forceinline__ void rmsnorm_row(const float *__restrict__ xr, const float *__restrict__ gamma,
-                                            const float *__restrict__ scale, float *__restrict__ yr, int dim, float eps) {
+__global__ void rmsnorm_kernel(const float *__restrict__ x, const float *__restrict__ gamma, const AdaRows ada_rows,
+                               float *__restrict__ y, int dim, float eps) {
+    const float *__restrict__ xr = x + (size_t)blockIdx.x * dim;
+    const float *__restrict__ scale = ada_rows.rows ? ada_rows.row(blockIdx.x) : nullptr;
+    float *__restrict__ yr = y + (size_t)blockIdx.x * dim;
     __shared__ float red[32];
     float s = 0.0f;
     for (int i = threadIdx.x; i < dim; i += blockDim.x) s = fmaf(xr[i], xr[i], s);
@@ -463,22 +466,10 @@ __device__ __forceinline__ void rmsnorm_row(const float *__restrict__ xr, const 
     }
 }
 
-__global__ void rmsnorm_kernel(const float *__restrict__ x, const float *__restrict__ gamma,
-                               const float *__restrict__ scale, float *__restrict__ y, int dim, float eps) {
-    rmsnorm_row(x + (size_t)blockIdx.x * dim, gamma, scale, y + (size_t)blockIdx.x * dim, dim, eps);
-}
-
-// rows of streams at different delays: row r takes its own ADA vector
-__global__ void rmsnorm_rows_kernel(const float *__restrict__ x, const float *__restrict__ gamma, const AdaRows ada_rows,
-                                    float *__restrict__ y, int dim, float eps) {
-    rmsnorm_row(x + (size_t)blockIdx.x * dim, gamma, ada_rows.row(blockIdx.x), y + (size_t)blockIdx.x * dim, dim, eps);
-}
-
-void launch_rmsnorm(const float *x, const float *gamma, const float *scale, float *y, int rows, int dim,
-                    float eps, cudaStream_t st, const AdaRows &ada_rows) {
+void launch_rmsnorm(const float *x, const float *gamma, float *y, int rows, int dim, float eps, cudaStream_t st,
+                    const AdaRows &ada_rows) {
     if (rows <= 0) return;
-    if (ada_rows.rows) rmsnorm_rows_kernel<<<rows, 256, 0, st>>>(x, gamma, ada_rows, y, dim, eps);
-    else rmsnorm_kernel<<<rows, 256, 0, st>>>(x, gamma, scale, y, dim, eps);
+    rmsnorm_kernel<<<rows, 256, 0, st>>>(x, gamma, ada_rows, y, dim, eps);
     post_launch("rmsnorm");
 }
 
@@ -486,23 +477,23 @@ void launch_rmsnorm(const float *x, const float *gamma, const float *scale, floa
 // Q4 linear layer: which of the four Q4 kernels runs it (kernels.h launch_q4_linear).
 // =====================================================================================
 void launch_q4_linear(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias, const float *res,
-                      int epi, const float *gamma, const float *ada, float eps, float *tmp, const Q4Scratch &sc,
-                      const Q4Path &path, cudaStream_t st, const AdaRows &ada_rows) {
-    VOX_CHECK(!ada_rows.rows || (gamma && !ada), VOX_EINVAL, "q4_linear: per-row ADA vectors need a norm and no shared vector");
+                      int epi, const float *gamma, float eps, float *tmp, const Q4Scratch &sc, const Q4Path &path,
+                      cudaStream_t st, const AdaRows &ada_rows) {
+    VOX_CHECK(!ada_rows.rows || gamma, VOX_EINVAL, "q4_linear: per-row ADA vectors need a norm");
     if (M > 8 && path.gemm_tc && gemm_tc5_supported(w, M) && gemm_tc5_split_elems(M, w.K) <= sc.xt_elems) {
-        launch_split_tiles(x, M, w.K, gamma, ada, gamma ? eps : 0.0f, sc.xt, st, ada_rows);
+        launch_split_tiles(x, M, w.K, gamma, gamma ? eps : 0.0f, sc.xt, st, ada_rows);
         launch_q4_gemm_tc5(w, sc.xt, M, y, ldy, bias, res, epi, sc.gw, st);
         return;
     }
     const bool tc = M <= 8 && path.matvec_tc && w.qs_tc;
     AdaRows rows = ada_rows;
     if (gamma && !(tc && sc.tc && sc.tc->ssq_in)) {
-        launch_rmsnorm(x, gamma, ada, tmp, M, w.K, eps, st, rows);
+        launch_rmsnorm(x, gamma, tmp, M, w.K, eps, st, rows);
         x = tmp;
-        gamma = ada = nullptr;
+        gamma = nullptr;
         rows = AdaRows{};
     }
-    if (tc) launch_q4_matvec_tc_ex(w, x, M, y, ldy, bias, res, epi, gamma, ada, gamma ? eps : 0.0f, sc.tc, st, rows);
+    if (tc) launch_q4_matvec_tc_ex(w, x, M, y, ldy, bias, res, epi, gamma, gamma ? eps : 0.0f, sc.tc, st, rows);
     else if (M <= 8) launch_q4_matvec(w, x, M, y, ldy, bias, res, epi, st);
     else launch_q4_gemm(w, x, M, y, ldy, bias, res, epi, st);
 }

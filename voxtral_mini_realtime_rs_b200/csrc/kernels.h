@@ -56,9 +56,9 @@ enum Epi : int {
     EPI_GELU = 3,      // y = gelu_erf(acc + bias)
 };
 
-// Per-row ADA scale: rows of one call that belong to streams of different transcription delays.  Row r of a B x M
-// problem is scaled by rows[r / m] + off (one pointer per stream, e.g. its [L][D] ADA set, off = layer * D) instead of
-// a shared `ada` vector.  rows == nullptr selects the shared vector, i.e. the unchanged kernels.
+// Per-row ADA scale: the rows of one call belong to streams, each at its own transcription delay.  Row r of a B x M
+// problem is scaled by rows[r / m] + off (one pointer per stream, e.g. its [L][D] ADA set, off = layer * D).
+// rows == nullptr: no ADA scale.
 struct AdaRows {
     const float *const *rows = nullptr;
     int m = 1;
@@ -81,12 +81,12 @@ struct TcWork {
     float *ssq_out = nullptr;      // [N/16][M], written by EPI_RESIDUAL epilogues
 };
 // same contract as launch_q4_matvec, dequant arithmetic on the tensor cores (mma.sync, f16 subnormal nibbles); needs
-// the TC layout (w.qs_tc).  matvec_tc.cu.  gamma (+ optional ada): RMSNorm of the input fused into the staging pass,
-// x := ((x / sqrt(mean(x^2)+eps)) * gamma) * ada.  wk (optional): split-K over K slices, fused-norm sums of squares.
-// ada_rows (EPI_SILU_MUL only, the decoder's w13): the ADA vector of each row instead of `ada`.
+// the TC layout (w.qs_tc).  matvec_tc.cu.  gamma (+ optional ada_rows): RMSNorm of the input fused into the staging
+// pass, x := ((x / sqrt(mean(x^2)+eps)) * gamma) * ada_rows.row(m).  wk (optional): split-K over K slices, fused-norm
+// sums of squares.
 void launch_q4_matvec_tc_ex(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias,
-                            const float *res, int epi, const float *gamma, const float *ada, float eps,
-                            const TcWork *wk, cudaStream_t st, const AdaRows &ada_rows = AdaRows{});
+                            const float *res, int epi, const float *gamma, float eps, const TcWork *wk, cudaStream_t st,
+                            const AdaRows &ada_rows = AdaRows{});
 // Split-K scratch sizes launch_q4_matvec_tc_ex needs for an N x K weight at up to 8 rows: partial_floats and n_counters
 // are set, the pointers are left to the caller (counters zeroed).
 TcWork q4_matvec_tc_work_size(int N, int K);
@@ -133,8 +133,8 @@ void launch_q4_gemm(const Q4Weight &w, const float *a, int M, float *y, int ldy,
 // (optionally through RMSNorm), then Y = X . W^T with f32-grade accuracy on the tensor cores.
 bool gemm_tc5_supported(const Q4Weight &w, int M);
 size_t gemm_tc5_split_elems(int M, int K);  // f16 elements needed for the split buffer
-void launch_split_tiles(const float *x, int M, int K, const float *gamma, const float *ada, float eps, void *xt,
-                        cudaStream_t st, const AdaRows &ada_rows = AdaRows{});
+void launch_split_tiles(const float *x, int M, int K, const float *gamma, float eps, void *xt, cudaStream_t st,
+                        const AdaRows &ada_rows = AdaRows{});
 // Caller-owned scratch for the GEMM's stream-K schedule: partial sums of tiles split across CTAs, summed in a fixed order
 struct GemmWork {
     float *partial = nullptr;  // [2 per CTA][tokens of the tile][128 features]
@@ -161,12 +161,12 @@ struct Q4Scratch {
     const TcWork *tc = nullptr;     // split-K and fused-norm sums of squares of the tensor-core matvec (null: neither)
 };
 // y = epi(norm(x) . W^T + bias) (+res) for any M: the one place that picks the Q4 kernel of a linear layer.
-// gamma (optional) selects the RMSNorm (+ ADA scale `ada`, or per row `ada_rows`) of the input.  It is fused into the
-// wgmma GEMM's operand split, or into the tensor-core matvec when sc.tc carries ssq_in; otherwise it runs as
-// launch_rmsnorm into `tmp` ([M][K]) ahead of the matvec / SIMT GEMM.
+// gamma (optional) selects the RMSNorm (+ per-row ADA scale `ada_rows`) of the input.  It is fused into the wgmma
+// GEMM's operand split, or into the tensor-core matvec when sc.tc carries ssq_in; otherwise it runs as launch_rmsnorm
+// into `tmp` ([M][K]) ahead of the matvec / SIMT GEMM.
 void launch_q4_linear(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias, const float *res,
-                      int epi, const float *gamma, const float *ada, float eps, float *tmp, const Q4Scratch &sc,
-                      const Q4Path &path, cudaStream_t st, const AdaRows &ada_rows = AdaRows{});
+                      int epi, const float *gamma, float eps, float *tmp, const Q4Scratch &sc, const Q4Path &path,
+                      cudaStream_t st, const AdaRows &ada_rows = AdaRows{});
 // conv1 / conv2 as implicit GEMM: in [B][T_in][C_in] time-major, W [C_out][3*C_in] (k = tap*C_in + c),
 // stride 2, pad 1, + bias, GELU -> out [B][T_out][C_out].
 // t_off (B == 1 only): compute conv outputs t_off .. t_off+T_out-1 into out[0..T_out) -- the incremental form used by
@@ -176,9 +176,9 @@ void launch_conv2_gemm(const float *in, const float *w, const float *bias, float
                        int T_out, int C_in, int C_out, cudaStream_t st, int t_off = 0, int in0 = 0);
 // [B][C][T] -> [B][T][C]
 void launch_transpose_mel(const float *in, float *out, int B, int C, int T, cudaStream_t st);
-// y = x / sqrt(mean(x^2)+eps) * gamma (* scale, optional ADA vector; or per row: ada_rows)
-void launch_rmsnorm(const float *x, const float *gamma, const float *scale, float *y, int rows, int dim,
-                    float eps, cudaStream_t st, const AdaRows &ada_rows = AdaRows{});
+// y = x / sqrt(mean(x^2)+eps) * gamma (* ada_rows.row(r), the optional per-row ADA vector)
+void launch_rmsnorm(const float *x, const float *gamma, float *y, int rows, int dim, float eps, cudaStream_t st,
+                    const AdaRows &ada_rows = AdaRows{});
 // in-place interleaved-pair RoPE on q (n_q heads) and k (n_k heads) inside a fused row buffer;
 // row r has position pos0 + (r % seq).  cos/sin: [max_pos][hd/2].
 void launch_rope_inplace(float *buf, int rows, int ld, int q_off, int n_q, int k_off, int n_k, int hd,

@@ -106,8 +106,9 @@ struct TcArgs {
     float *y;
     int ldy;
     const float *bias, *res;
-    // fused RMSNorm of the input
-    const float *gamma, *ada;
+    // fused RMSNorm of the input (x the row's ADA vector if ada_rows.rows)
+    const float *gamma;
+    AdaRows ada_rows;
     float eps;
     const float *ssq_in;  // [ssq_in_parts][M] partial sums of squares of x (nullptr: computed here)
     int ssq_in_parts;
@@ -118,14 +119,6 @@ struct TcArgs {
     int ldp;
     int *counters;        // [n_tiles], zero between launches
 };
-
-// Arguments of the per-row instantiations (rows at different transcription delays): token m takes ada_rows.row(m)
-// instead of `ada`.  The shared instantiations keep plain TcArgs.
-struct TcRowsArgs : TcArgs {
-    AdaRows ada_rows;
-};
-__device__ __forceinline__ const float *row_ada(const TcArgs &a, int) { return a.ada; }
-__device__ __forceinline__ const float *row_ada(const TcRowsArgs &a, int m) { return a.ada_rows.row(m); }
 
 // Effective activation value (after the optional fused RMSNorm).
 // `rinv` = 1 / sqrt(mean(x^2)+eps): the reference divides (x / rms); multiplying by the reciprocal
@@ -147,8 +140,8 @@ __device__ __forceinline__ float4 eff4(const float4 v, const float rinv, const f
 // Column c = 2*token + split (0 = hi, 1 = mid).  One work item = (block, token, t): elements
 // 4t..4t+3 and 16+4t..16+4t+3; the four t-items of a block sit in adjacent lanes so the block sum and
 // block max are 2-step shuffles.  Two items per thread are loaded before either is processed.
-template <int M, typename Args>
-__device__ __forceinline__ void tc_stage(const Args &a, const int b0, const int nb, const float *__restrict__ rms,
+template <int M>
+__device__ __forceinline__ void tc_stage(const TcArgs &a, const int b0, const int nb, const float *__restrict__ rms,
                                          uint2 *__restrict__ bf, float2 *__restrict__ off2) {
     const int items = nb * M * 4;
     constexpr int U = 2;
@@ -177,7 +170,7 @@ __device__ __forceinline__ void tc_stage(const Args &a, const int b0, const int 
             const int kb = (b0 + bl[u]) * 32;
             float4 l = lo[u], h = hi[u];
             if (act[u] && kb < a.K) {
-                const float *ada = row_ada(a, m);
+                const float *ada = a.ada_rows.rows ? a.ada_rows.row(m) : nullptr;
                 l = eff4(l, rms[m], a.gamma, ada, kb + 4 * t);
                 h = eff4(h, rms[m], a.gamma, ada, kb + 16 + 4 * t);
             }
@@ -257,9 +250,9 @@ __device__ __forceinline__ void tc_epilogue(const TcArgs &a, const int tile, con
     }
 }
 
-// EPI semantics as in kernels.h (Epi).  grid = (tile groups, K slices).  Args = TcRowsArgs: per-row ADA vectors.
-template <int M, int EPI, typename Args = TcArgs>
-__global__ void __launch_bounds__(TC_THREADS) q4_matvec_tc_kernel(const Args a) {
+// EPI semantics as in kernels.h (Epi).  grid = (tile groups, K slices).
+template <int M, int EPI>
+__global__ void __launch_bounds__(TC_THREADS) q4_matvec_tc_kernel(const TcArgs a) {
     constexpr int CG = (M + 3) / 4;  // column groups of 8 (= 4 tokens x 2 splits)
     extern __shared__ __align__(128) unsigned char smem_raw[];
     float *rms = reinterpret_cast<float *>(smem_raw);                  // [8] reciprocal rms per token
@@ -455,8 +448,8 @@ int tc_slices(int M, int n_pairs) {
     return (n_pairs + ps_max - 1) / ps_max;
 }
 
-template <int M, int EPI, typename Args = TcArgs>
-void tc_launch_t(Args a, const TcWork *wk, cudaStream_t st) {
+template <int M, int EPI>
+void tc_launch_t(TcArgs a, const TcWork *wk, cudaStream_t st) {
     // ---- work decomposition
     int S = 1;
     if (wk && wk->partial && wk->counters) S = tc_slices(M, a.n_pairs);
@@ -483,7 +476,7 @@ void tc_launch_t(Args a, const TcWork *wk, cudaStream_t st) {
     const size_t smem = act + 128 + (size_t)nbuf * slice_bytes + 64;
     VOX_CHECK(smem <= 200 * 1024, VOX_EINVAL, "q4_matvec_tc: shared memory %zu too large (K=%d, M=%d)", smem, a.K, M);
     static SmemAttr smem_attr;
-    cuda_check_tc(ensure_dyn_smem(q4_matvec_tc_kernel<M, EPI, Args>, 208 * 1024, smem_attr), "cudaFuncSetAttribute(q4_matvec_tc)");
+    cuda_check_tc(ensure_dyn_smem(q4_matvec_tc_kernel<M, EPI>, 208 * 1024, smem_attr), "cudaFuncSetAttribute(q4_matvec_tc)");
     a.S = S;
     a.Ps = Ps;
     a.TG = TG;
@@ -502,26 +495,16 @@ void tc_launch_t(Args a, const TcWork *wk, cudaStream_t st) {
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    cuda_check_tc(cudaLaunchKernelEx(&cfg, q4_matvec_tc_kernel<M, EPI, Args>, a), "cudaLaunchKernelEx(q4_matvec_tc)");
+    cuda_check_tc(cudaLaunchKernelEx(&cfg, q4_matvec_tc_kernel<M, EPI>, a), "cudaLaunchKernelEx(q4_matvec_tc)");
     tc_count_launch("q4_matvec_tc");
 }
 
 template <int M>
-void tc_launch_m(const TcArgs &a, const TcWork *wk, int epi, cudaStream_t st, const AdaRows &ada_rows) {
-    // the ADA scale enters the decoder only at the input of w13 (SwiGLU): the per-row form is instantiated there alone
-    VOX_CHECK(!ada_rows.rows || epi == EPI_SILU_MUL, VOX_EINVAL, "q4_matvec_tc: per-row ADA vectors need the SwiGLU epilogue");
+void tc_launch_m(const TcArgs &a, const TcWork *wk, int epi, cudaStream_t st) {
     switch (epi) {
         case EPI_NONE: tc_launch_t<M, EPI_NONE>(a, wk, st); break;
         case EPI_RESIDUAL: tc_launch_t<M, EPI_RESIDUAL>(a, wk, st); break;
-        case EPI_SILU_MUL:
-            if (ada_rows.rows) {
-                TcRowsArgs r;
-                static_cast<TcArgs &>(r) = a;
-                r.ada_rows = ada_rows;
-                tc_launch_t<M, EPI_SILU_MUL, TcRowsArgs>(r, wk, st);
-            }
-            else tc_launch_t<M, EPI_SILU_MUL>(a, wk, st);
-            break;
+        case EPI_SILU_MUL: tc_launch_t<M, EPI_SILU_MUL>(a, wk, st); break;
         case EPI_GELU: tc_launch_t<M, EPI_GELU>(a, wk, st); break;
         default: fail(VOX_EINVAL, "bad epilogue");
     }
@@ -530,8 +513,8 @@ void tc_launch_m(const TcArgs &a, const TcWork *wk, int epi, cudaStream_t st, co
 }  // namespace
 
 void launch_q4_matvec_tc_ex(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias,
-                            const float *res, int epi, const float *gamma, const float *ada, float eps,
-                            const TcWork *wk, cudaStream_t st, const AdaRows &ada_rows) {
+                            const float *res, int epi, const float *gamma, float eps, const TcWork *wk, cudaStream_t st,
+                            const AdaRows &ada_rows) {
     VOX_CHECK(w.qs_tc != nullptr, VOX_EINVAL, "q4_matvec_tc: weight has no tensor-core layout");
     VOX_CHECK(!ada_rows.rows || gamma, VOX_EINVAL, "q4_matvec_tc: per-row ADA vectors without a norm");
     VOX_CHECK(M >= 1 && M <= 8, VOX_EINVAL, "q4_matvec_tc: M=%d out of range", M);
@@ -549,20 +532,20 @@ void launch_q4_matvec_tc_ex(const Q4Weight &w, const float *x, int M, float *y, 
     a.bias = bias;
     a.res = res;
     a.gamma = gamma;
-    a.ada = ada;
+    a.ada_rows = ada_rows;
     a.eps = eps;
     a.ssq_in = (gamma && wk) ? wk->ssq_in : nullptr;
     a.ssq_in_parts = wk ? wk->ssq_in_parts : 0;
     a.ssq_out = (epi == EPI_RESIDUAL && wk) ? wk->ssq_out : nullptr;
     switch (M) {
-        case 1: tc_launch_m<1>(a, wk, epi, st, ada_rows); break;
-        case 2: tc_launch_m<2>(a, wk, epi, st, ada_rows); break;
-        case 3: tc_launch_m<3>(a, wk, epi, st, ada_rows); break;
-        case 4: tc_launch_m<4>(a, wk, epi, st, ada_rows); break;
-        case 5: tc_launch_m<5>(a, wk, epi, st, ada_rows); break;
-        case 6: tc_launch_m<6>(a, wk, epi, st, ada_rows); break;
-        case 7: tc_launch_m<7>(a, wk, epi, st, ada_rows); break;
-        default: tc_launch_m<8>(a, wk, epi, st, ada_rows); break;
+        case 1: tc_launch_m<1>(a, wk, epi, st); break;
+        case 2: tc_launch_m<2>(a, wk, epi, st); break;
+        case 3: tc_launch_m<3>(a, wk, epi, st); break;
+        case 4: tc_launch_m<4>(a, wk, epi, st); break;
+        case 5: tc_launch_m<5>(a, wk, epi, st); break;
+        case 6: tc_launch_m<6>(a, wk, epi, st); break;
+        case 7: tc_launch_m<7>(a, wk, epi, st); break;
+        default: tc_launch_m<8>(a, wk, epi, st); break;
     }
 }
 

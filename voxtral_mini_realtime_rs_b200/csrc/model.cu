@@ -447,8 +447,6 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ri
         s->act_dec = s->arena.alloc_n<float>(drows * c.dec_ffn);
         s->last_h = s->arena.alloc_n<float>(B * c.dec_dim);
         s->logits = s->arena.alloc_n<float>(B * c.vocab);
-        s->ada = s->arena.alloc_n<float>((size_t)c.dec_layers * c.dec_dim);
-        s->ffn_gamma_ada = s->arena.alloc_n<float>((size_t)c.dec_layers * c.dec_dim);
         s->ada_sets = s->arena.alloc_n<float>(B * s->ada_set_floats());
         s->delays.assign(B, 0.0f);
         s->d_ada_rows = (const float **)s->arena.alloc(sizeof(float *) * B);
@@ -551,8 +549,8 @@ Session::~Session() {
 }
 
 void Session::linear(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias, const float *res,
-                     int epi, const float *gamma, const float *ada, float *tmp, const TcWork *tc, const AdaRows &ada_rows) {
-    launch_q4_linear(w, x, M, y, ldy, bias, res, epi, gamma, ada, m->norm_eps, tmp, Q4Scratch{xt_buf, xt_elems, &gemm_work, tc},
+                     int epi, const float *gamma, float *tmp, const TcWork *tc, const AdaRows &ada_rows) {
+    launch_q4_linear(w, x, M, y, ldy, bias, res, epi, gamma, m->norm_eps, tmp, Q4Scratch{xt_buf, xt_elems, &gemm_work, tc},
                      path, st, ada_rows);
 }
 
@@ -577,16 +575,15 @@ static void compute_ada(Session &s, float delay, float *ada_dst, float *fga_dst)
     CUDA_OK(cudaStreamSynchronize(s.st));
 }
 
-// t is constant for a transcription: the vectors are computed once per delay, into the shared path's buffers, and
-// copied to every stream's set.
+// t is constant for a transcription: the vectors are computed once per delay, into stream 0's set, and copied to the
+// other streams' sets.
 void Session::set_delay(float delay) {
     CUDA_OK(cudaSetDevice(m->device));
-    const size_t LD = ada_set_floats() / 2;
-    compute_ada(*this, delay, ada, ffn_gamma_ada);
-    shared_delay = delay;
-    for (int i = 0; i < max_batch; ++i) {
-        CUDA_OK(cudaMemcpyAsync(ada_sets + i * 2 * LD, ada, sizeof(float) * LD, cudaMemcpyDeviceToDevice, st));
-        CUDA_OK(cudaMemcpyAsync(ada_sets + i * 2 * LD + LD, ffn_gamma_ada, sizeof(float) * LD, cudaMemcpyDeviceToDevice, st));
+    const size_t n = ada_set_floats();
+    compute_ada(*this, delay, ada_sets, ada_sets + n / 2);
+    delays[0] = delay;
+    for (int i = 1; i < max_batch; ++i) {
+        CUDA_OK(cudaMemcpyAsync(ada_sets + i * n, ada_sets, sizeof(float) * n, cudaMemcpyDeviceToDevice, st));
         delays[i] = delay;
     }
     CUDA_OK(cudaStreamSynchronize(st));
@@ -620,20 +617,6 @@ void Session::set_stream_delay(int i, float d) {
 }
 
 void Session::bind_delays(const int *streams, int n) {
-    bool uniform = true;
-    for (int i = 1; i < n; ++i) uniform &= same_delay(delays[streams[i]], delays[streams[0]]);
-    if (uniform) {
-        ada_per_row = false;
-        if (!same_delay(delays[streams[0]], shared_delay)) {
-            const size_t LD = ada_set_floats() / 2;
-            const float *set = ada_sets + (size_t)streams[0] * 2 * LD;
-            CUDA_OK(cudaMemcpyAsync(ada, set, sizeof(float) * LD, cudaMemcpyDeviceToDevice, st));
-            CUDA_OK(cudaMemcpyAsync(ffn_gamma_ada, set + LD, sizeof(float) * LD, cudaMemcpyDeviceToDevice, st));
-            shared_delay = delays[streams[0]];
-        }
-        return;
-    }
-    ada_per_row = true;
     if (ada_row_streams.size() >= (size_t)n && std::equal(streams, streams + n, ada_row_streams.begin())) return;
     std::vector<const float *> a(n), f(n);
     for (int i = 0; i < n; ++i) {
@@ -672,7 +655,7 @@ void Session::encode(int B, int T) {
     const float scale = powf((float)c.enc_head_dim, -0.5f);
     for (int i = 0; i < c.enc_layers; ++i) {
         const EncLayerW &l = m->enc[i];
-        linear(l.wqkv, x_enc, rows, qkv_enc, 3 * hdq, l.bqkv, nullptr, EPI_NONE, l.attn_norm, nullptr, h_enc);
+        linear(l.wqkv, x_enc, rows, qkv_enc, 3 * hdq, l.bqkv, nullptr, EPI_NONE, l.attn_norm, h_enc);
         launch_rope_inplace(qkv_enc, rows, 3 * hdq, 0, c.enc_heads, hdq, c.enc_heads, c.enc_head_dim, S, 0,
                             m->enc_cos, m->enc_sin, st);
         if (use_enc_attn_tc && enc_attention_tc_supported(c.enc_head_dim, 3 * hdq, 0, hdq, 2 * hdq))
@@ -682,13 +665,13 @@ void Session::encode(int B, int T) {
             launch_enc_attention(qkv_enc, attn_enc, B, S, c.enc_heads, c.enc_head_dim, 3 * hdq, 0, hdq, 2 * hdq,
                                  c.enc_window, scale, st);
         linear(l.wo, attn_enc, rows, x_enc, d, l.bo, x_enc, EPI_RESIDUAL);
-        linear(l.w13, x_enc, rows, act_enc, c.enc_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, nullptr, h_enc);
+        linear(l.w13, x_enc, rows, act_enc, c.enc_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, h_enc);
         linear(l.w2, act_enc, rows, x_enc, d, l.b2, x_enc, EPI_RESIDUAL);
         if (debug_capture && dbg_layers)
             CUDA_OK(cudaMemcpyAsync(dbg_layers + (size_t)i * rows * d, x_enc, sizeof(float) * rows * d,
                                     cudaMemcpyDeviceToDevice, st));
     }
-    launch_rmsnorm(x_enc, m->enc_norm, nullptr, h_enc, rows, d, m->norm_eps, st);
+    launch_rmsnorm(x_enc, m->enc_norm, h_enc, rows, d, m->norm_eps, st);
     cur_B = B;
     cur_S = S;
     cur_S4 = S4;
@@ -740,23 +723,19 @@ bool Session::decoder_forward(int B, int M) {
     for (int j = 0; j < c.dec_layers; ++j) {
         const DecLayerW &l = m->dec[j];
         const KvView kvl = kv_view(j);
-        linear(l.wqkv, x_dec, rows, qkv_dec, qkvd, nullptr, nullptr, EPI_NONE, l.attn_norm, nullptr, h_dec, tc_norm);
+        linear(l.wqkv, x_dec, rows, qkv_dec, qkvd, nullptr, nullptr, EPI_NONE, l.attn_norm, h_dec, tc_norm);
         if (fattn) {
             launch_dec_attn_fused(qkv_dec, B, qkvd, H, Hkv, hd, kvl, c.dec_window, scale, dec_rope, attn_dec, st);
         } else {
             launch_dec_rope_append(qkv_dec, B, M, qkvd, H, Hkv, hd, kvl, dec_rope, st);
             launch_dec_attention(qkv_dec, B, M, qkvd, H, Hkv, hd, kvl, c.dec_window, scale, attn_dec, st);
         }
-        linear(l.wo, attn_dec, rows, x_dec, D, nullptr, x_dec, EPI_RESIDUAL, nullptr, nullptr, nullptr, tc_res);
-        if (ada_per_row)
-            linear(l.w13, x_dec, rows, act_dec, c.dec_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, nullptr, h_dec, tc_norm,
-                   AdaRows{d_ada_rows, M, (size_t)j * D});
-        else
-            linear(l.w13, x_dec, rows, act_dec, c.dec_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, ada + (size_t)j * D, h_dec,
-                   tc_norm);
-        linear(l.w2, act_dec, rows, x_dec, D, nullptr, x_dec, EPI_RESIDUAL, nullptr, nullptr, nullptr, tc_res);
+        linear(l.wo, attn_dec, rows, x_dec, D, nullptr, x_dec, EPI_RESIDUAL, nullptr, nullptr, tc_res);
+        linear(l.w13, x_dec, rows, act_dec, c.dec_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, h_dec, tc_norm,
+               AdaRows{d_ada_rows, M, (size_t)j * D});
+        linear(l.w2, act_dec, rows, x_dec, D, nullptr, x_dec, EPI_RESIDUAL, nullptr, nullptr, tc_res);
     }
-    if (!fused) launch_rmsnorm(x_dec, m->dec_norm, nullptr, h_dec, rows, D, m->norm_eps, st);
+    if (!fused) launch_rmsnorm(x_dec, m->dec_norm, h_dec, rows, D, m->norm_eps, st);
     return fused;
 }
 
@@ -765,7 +744,7 @@ bool Session::decoder_forward(int B, int M) {
 void Session::lm_head_rows(int rows, bool norm_pending, float *dst) {
     const TcWork wk = tc_work(true, false);
     linear(m->tok_emb, norm_pending ? x_dec : h_dec, rows, dst, m->info.vocab, nullptr, nullptr, EPI_NONE,
-           norm_pending ? m->dec_norm : nullptr, nullptr, nullptr, norm_pending ? &wk : nullptr);
+           norm_pending ? m->dec_norm : nullptr, nullptr, norm_pending ? &wk : nullptr);
 }
 
 void Session::forward_logits(int b, int M, const int *ids_host, bool with_audio, float *dst) {
@@ -855,8 +834,8 @@ bool Session::mega_prepare(int B) {
         a.layer = j;
         ops.push_back(a);
         // wo: h += attn . Wo^T; leaves fragments of h x (ffn_norm x ADA) for w13
-        matvec(l.wo, AF, x_dec, D, x_dec, EPI_RESIDUAL, nullptr, true, false, 2, XF, ffn_gamma_ada + (size_t)j * D);
-        ops.back().fout_ada_layer = j;   // per-row mode: each row's own ffn_norm x ADA vector of layer j
+        matvec(l.wo, AF, x_dec, D, x_dec, EPI_RESIDUAL, nullptr, true, false, 2, XF, nullptr);
+        ops.back().fout_ada_layer = j;   // each row's own ffn_norm x ADA vector of layer j
         // w13: SwiGLU of the normed stream; leaves fragments of the activation for w2 (no plain copy)
         matvec(l.w13, XF, nullptr, c.dec_ffn, nullptr, EPI_SILU_MUL, l.ffn_norm, false, false, 4, CF, nullptr);
         // w2: h += act . W2^T; leaves fragments of h x (next attention norm | final norm)
@@ -1032,7 +1011,7 @@ void Session::decode_step_mega(int b0, int B, bool add_audio) {
     p.audio = add_audio && audio ? audio + (size_t)b0 * cur_S4 * c.dec_dim : nullptr;
     p.audio_rows = add_audio && audio_rows_dev ? audio_rows_dev + b0 : nullptr;
     p.audio_seq = cur_S4;
-    p.ffn_ada_rows = ada_per_row ? d_fga_rows + b0 : nullptr;
+    p.ffn_ada_rows = d_fga_rows + b0;
     p.x_dec = x_dec;
     p.ssq_x = ssq_x;
     p.emb_fbf = mega_xf_bf;
@@ -1064,7 +1043,7 @@ void Session::prefill(int B, int M, const int *ids_host, bool add_audio) {
                  fused_decode(B * M) ? ssq_x : nullptr, st);
     const bool pending = decoder_forward(B, M);
     if (pending) {   // decode-sized prefill (B*M <= 8): final norm still pending in x_dec
-        launch_rmsnorm(x_dec, m->dec_norm, nullptr, h_dec, B * M, c.dec_dim, m->norm_eps, st);
+        launch_rmsnorm(x_dec, m->dec_norm, h_dec, B * M, c.dec_dim, m->norm_eps, st);
     }
     // lm_head on the last row only (the reference computes all M rows and keeps one)
     launch_gather_last(h_dec, last_h, B, M, c.dec_dim, st);
@@ -1119,7 +1098,7 @@ template <class Step>
 void Session::run_steps(int R, int n, Step step) {
     if (n <= 0) return;
     prepare_step(R);
-    const StepKey key{R, cur_S4, top_k, beam_w, ada_per_row, path.matvec_tc, path.gemm_tc, use_mega};
+    const StepKey key{R, cur_S4, top_k, beam_w, path.matvec_tc, path.gemm_tc, use_mega};
     if (use_graph && !(step_graph.exec && step_graph.key == key)) {
         // first step eagerly (also performs any one-time kernel attribute setup), then capture one step and replay it
         mega_steps_host += step();

@@ -101,8 +101,8 @@ constexpr float kDefaultDelay = 6.0f;
 // other kernels or reads another op table.
 struct StepKey {
     int rows = 0, S4 = 0, top_k = 0, beam_w = 1;
-    bool ada_per_row = false, matvec_tc = true, gemm_tc = true, use_mega = true;
-    auto tie() const { return std::tie(rows, S4, top_k, beam_w, ada_per_row, matvec_tc, gemm_tc, use_mega); }
+    bool matvec_tc = true, gemm_tc = true, use_mega = true;
+    auto tie() const { return std::tie(rows, S4, top_k, beam_w, matvec_tc, gemm_tc, use_mega); }
     bool operator==(const StepKey &o) const { return tie() == o.tie(); }
 };
 struct StepGraph {
@@ -143,19 +143,13 @@ struct Session {
     float *last_h = nullptr, *logits = nullptr;
     float *logits_all = nullptr;
     size_t logits_all_cap = 0;
-    // ADA scale of the shared path (every row of a call at one delay): [L][D], and ffn_norm weight x ADA scale [L][D]
-    // (persistent decode kernel).  They hold the vectors of `shared_delay`.
-    float *ada = nullptr, *t_embed = nullptr, *ada_tmp = nullptr;
-    float *ffn_gamma_ada = nullptr;
-    float shared_delay = -1.0f;  // -1: not loaded
     // per-stream transcription delay (vox_session_set_delays): stream i's ADA set at ada_sets + i * ada_set_floats(),
-    // {ADA scale [L][D], ffn_norm x ADA scale [L][D]}
+    // {ADA scale [L][D], ffn_norm x ADA scale [L][D]} (the latter for the persistent decode kernel)
     std::vector<float> delays;
-    float *ada_sets = nullptr;
+    float *ada_sets = nullptr, *t_embed = nullptr, *ada_tmp = nullptr;
     size_t ada_set_floats() const { return (size_t)2 * m->info.dec_layers * m->info.dec_dim; }
-    // per-row mode (the rows of a call at different delays): row i uses stream ada_row_streams[i]'s set through the
-    // pointer tables [max_batch] (kernels.h AdaRows, MegaParams::ffn_ada_rows)
-    bool ada_per_row = false;
+    // row i of a launch uses stream ada_row_streams[i]'s set through the pointer tables [max_batch] (kernels.h AdaRows,
+    // MegaParams::ffn_ada_rows)
     const float **d_ada_rows = nullptr, **d_fga_rows = nullptr;
     std::vector<int> ada_row_streams;
     int *d_pos = nullptr, *d_outpos = nullptr, *d_tok = nullptr, *d_ids = nullptr, *d_out = nullptr;
@@ -252,18 +246,18 @@ struct Session {
     // stream i at delays[i] for i < b; streams >= b keep theirs
     void set_delays(const float *delays, int b);
     void set_stream_delay(int stream, float delay);
-    // the ADA mode of the next launches, whose row i belongs to stream streams[i]: the shared path when every row has
-    // the same delay (loading that delay's vectors into ada / ffn_gamma_ada), else per-row tables.  Launch-free and
-    // copy-free when nothing changed (so it may run inside a stream capture).
+    // the ADA sets of the next launches, whose row i belongs to stream streams[i]: points the per-row tables at the
+    // streams' sets.  Launch-free, and copy-free when the row-to-stream mapping has not changed (so it may run inside a
+    // stream capture); a delay change rewrites the sets in place and needs no new binding.
     void bind_delays(const int *streams, int n);
     // row b = stream b, or stream b % beam_streams during a beam call (every call but the stream pool's)
     void bind_row_delays(int B);
     // mel already on device, time-major, in s->mel_tm
     void encode(int B, int T);
-    // launch_q4_linear with the session's GEMM scratch and path choice; `gamma`, `ada`, `tmp` and `tc` as there
+    // launch_q4_linear with the session's GEMM scratch and path choice; `gamma`, `tmp`, `tc` and `ada_rows` as there
     void linear(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias, const float *res,
-                int epi, const float *gamma = nullptr, const float *ada = nullptr, float *tmp = nullptr,
-                const TcWork *tc = nullptr, const AdaRows &ada_rows = AdaRows{});
+                int epi, const float *gamma = nullptr, float *tmp = nullptr, const TcWork *tc = nullptr,
+                const AdaRows &ada_rows = AdaRows{});
     bool decoder_forward(int B, int M);
     void lm_head_rows(int rows, bool norm_pending, float *dst);
     // teacher-forced pass over ids [b][M] (+ the audio embeddings at positions *d_pos.. when with_audio): logits of every

@@ -317,7 +317,7 @@ void StreamPool::encoder_rows(int R) {
     const size_t ring_stride = (size_t)max_sessions * ring * HQ;
     for (int i = 0; i < c.enc_layers; ++i) {
         const EncLayerW &l = m->enc[i];
-        s->linear(l.wqkv, s->x_enc, R, s->qkv_enc, 3 * HQ, l.bqkv, nullptr, EPI_NONE, l.attn_norm, nullptr, s->h_enc);
+        s->linear(l.wqkv, s->x_enc, R, s->qkv_enc, 3 * HQ, l.bqkv, nullptr, EPI_NONE, l.attn_norm, s->h_enc);
         stream_rope_append_kernel<<<R, 256, 0, s->st>>>(s->qkv_enc, 3 * HQ, c.enc_heads, c.enc_head_dim, d_row_slot, d_row_pos,
                                                         ek + i * ring_stride, ev + i * ring_stride, ring,
                                                         unbounded ? enc_rope_cos : m->enc_cos, unbounded ? enc_rope_sin : m->enc_sin,
@@ -326,10 +326,10 @@ void StreamPool::encoder_rows(int R) {
         launch_stream_attn(s->qkv_enc, R, 3 * HQ, c.enc_heads, c.enc_head_dim, d_row_slot, d_row_pos, ek + i * ring_stride,
                            ev + i * ring_stride, ring, c.enc_window, scale, s->attn_enc, s->st);
         s->linear(l.wo, s->attn_enc, R, s->x_enc, d, l.bo, s->x_enc, EPI_RESIDUAL);
-        s->linear(l.w13, s->x_enc, R, s->act_enc, c.enc_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, nullptr, s->h_enc);
+        s->linear(l.w13, s->x_enc, R, s->act_enc, c.enc_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, s->h_enc);
         s->linear(l.w2, s->act_enc, R, s->x_enc, d, l.b2, s->x_enc, EPI_RESIDUAL);
     }
-    launch_rmsnorm(s->x_enc, m->enc_norm, nullptr, s->h_enc, R, d, m->norm_eps, s->st);
+    launch_rmsnorm(s->x_enc, m->enc_norm, s->h_enc, R, d, m->norm_eps, s->st);
 }
 
 void StreamPool::ensure_pages(Slot &sl, int positions) {
@@ -344,7 +344,7 @@ void StreamPool::ensure_pages(Slot &sl, int positions) {
 }
 
 // rows[i] = slot id of batch row i: page tables, positions, fed-back tokens, audio pointers of this step, and the rows'
-// delays (the shared ADA path when they are equal, else the per-row tables of the sessions' ADA sets)
+// ADA sets (the sessions' delays)
 void StreamPool::upload_rows(const std::vector<int> &rows, bool with_tokens) {
     s->bind_delays(rows.data(), (int)rows.size());
     const vox_model_info &c = m->info;
