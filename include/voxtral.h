@@ -184,7 +184,8 @@ int32_t vox_session_set_delays(vox_session *s, const float *delays, int32_t b);
 int32_t vox_encode_audio(vox_session *s, const float *mel, int32_t b, int32_t t_frames,
                          float *audio_embeds /* nullable */, size_t cap_floats, int32_t *seq_len);
 /* transcribe_streaming (model.rs:873-963): mel [B,128,T] host -> out_ids [B][n_out], n_out = S-38
- * (0 when S<38).  Equal-length streams per call (the reference is batch 1). */
+ * (0 when S<38).  Equal-length streams per call (the reference is batch 1; vox_transcribe_pcm_ragged takes streams of
+ * different lengths). */
 int32_t vox_transcribe_streaming(vox_session *s, const float *mel, int32_t b, int32_t t_frames,
                                  int32_t *out_ids, size_t cap_ids, int32_t *n_out, vox_timings *tm);
 /* full pipeline from PCM (transcribe.rs:187-318 per chunk): samples [B][n] host, optional
@@ -192,6 +193,29 @@ int32_t vox_transcribe_streaming(vox_session *s, const float *mel, int32_t b, in
 int32_t vox_transcribe_pcm(vox_session *s, const float *samples, int32_t b, size_t n,
                            int32_t peak_normalize, int32_t *out_ids, size_t cap_ids, int32_t *n_out,
                            vox_timings *tm);
+/* Streams of different lengths in one call.  samples: stream s's lens[s] samples follow stream s-1's (host, 16 kHz).
+ * Each stream is handled exactly as vox_transcribe_pcm handles a single stream: optional peak_normalize(0.95) over its
+ * own samples, pad_audio, log-mel, encode, 38-position prefill, greedy (or beam) decode.
+ * out_ids: stream s's n_out[s] ids follow stream s-1's; n_out[s] = max(0, S4_s - 38), where S4_s follows from lens[s]
+ * alone (pad_audio length -> mel frames -> two stride-2 convolutions -> / reshape_factor).
+ *   - Arguments: VOX_EINVAL unless 1 <= b <= max_batch (b * W <= max_batch at beam width W > 1), every lens[s] >= 1
+ *     and every stream's mel frames <= max_mel_frames; VOX_ECAPACITY when cap_ids < sum of n_out.  All of these are
+ *     checked on the host before any device work; a refused call leaves the session as it was.
+ *   - Equal lengths: when every lens[s] is equal the call is vox_transcribe_pcm of the same [b][n] array, bit for bit
+ *     (ids, token scores, n-best).
+ *   - Work: the encoder runs over the sum of the streams' frames, not b x the longest.  The decoder's rows are the
+ *     streams sorted by decreasing n_out, and a stream's rows leave the decode step after its last token, so the step's
+ *     cost follows the streams still running.  A stream with n_out = 0 takes no decoder rows; n_out = 1 takes the
+ *     prefill only.
+ *   - Per-stream settings: vox_session_set_delays applies stream i's delay to stream i of the call.  With
+ *     vox_session_set_top_k(k), vox_session_token_scores returns stream s's n_out[s] x k entries after those of stream
+ *     s-1, with *b = b and *n = sum of n_out (for equal lengths the [b][n][k] layout).  vox_session_nbest likewise:
+ *     stream s's W hypotheses of n_out[s] ids each after stream s-1's, scores [b][W].
+ *   - Timings: seq_len and decode_tokens are the longest stream's (the positions actually run).
+ *   - Like a beam call, the call leaves the decoder cache empty (vox_session_cache_len 0). */
+int32_t vox_transcribe_pcm_ragged(vox_session *s, const float *samples, const size_t *lens, int32_t b,
+                                  int32_t peak_normalize, int32_t *out_ids, size_t cap_ids,
+                                  int32_t *n_out /* [b] */, vox_timings *tm);
 /* same, samples already resident in HBM ([B][n] device); used for the device-resident bench leg */
 int32_t vox_transcribe_pcm_dev(vox_session *s, const float *samples_dev, int32_t b, size_t n,
                                int32_t *out_ids, size_t cap_ids, int32_t *n_out, vox_timings *tm);

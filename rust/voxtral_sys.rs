@@ -58,6 +58,9 @@ extern "C" {
     pub fn vox_transcribe_pcm(s: *mut vox_session, samples: *const f32, b: i32, n: usize,
                               peak_normalize: i32, out_ids: *mut i32, cap: usize, n_out: *mut i32,
                               tm: *mut vox_timings) -> i32;
+    pub fn vox_transcribe_pcm_ragged(s: *mut vox_session, samples: *const f32, lens: *const usize, b: i32,
+                                     peak_normalize: i32, out_ids: *mut i32, cap: usize,
+                                     n_out: *mut i32, tm: *mut vox_timings) -> i32;
     pub fn vox_generate_step_with_cache(s: *mut vox_session, ids: *const i32, b: i32, m: i32,
                                         logits: *mut f32, cap: usize) -> i32;
     // forward_streaming (model.rs:801-814) and the device-side incremental decode (model.rs:857-867 without the

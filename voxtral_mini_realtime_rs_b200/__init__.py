@@ -7,6 +7,7 @@ surface for this path (TrevorS/voxtral-mini-realtime-rs, ``src/lib.rs:22-39``):
     Q4Tensor, Q4Linear, q4_matmul                    src/gguf/{tensor,linear,op}.rs
     MelSpectrogram, MelConfig, PadConfig, pad_audio  src/audio/{mel,pad}.rs
     peak_normalize, chunk_audio, needs_chunking      src/audio/{io,chunk}.rs
+    join_chunk_texts                                 src/bin/transcribe.rs (chunk join)
     TimeEmbedding                                    src/models/time_embedding.rs
     VoxtralTokenizer                                 src/tokenizer/mod.rs
 
@@ -17,12 +18,13 @@ from .api import (  # noqa: F401
     VoxtralError, lib, lib_path, device_count,
     GgufReader, Q4ModelLoader, Q4VoxtralModel, Q4Tensor, Q4Linear, q4_matmul,
     MelSpectrogram, PadConfig, pad_audio, peak_normalize, chunk_audio, needs_chunking, stream_progress,
+    stream_n_out, frames_n_out, join_chunk_texts,
     TimeEmbedding, VoxtralTokenizer, Timings, DeviceBuffer, PinnedArray, q4_matmul_bench, StreamingPool,
 )
 
 __all__ = [
     "VoxtralError", "lib", "lib_path", "device_count", "GgufReader", "Q4ModelLoader", "Q4VoxtralModel",
     "Q4Tensor", "Q4Linear", "q4_matmul", "MelSpectrogram", "PadConfig", "pad_audio", "peak_normalize",
-    "chunk_audio", "needs_chunking", "stream_progress", "TimeEmbedding", "VoxtralTokenizer", "Timings", "DeviceBuffer",
+    "chunk_audio", "needs_chunking", "stream_progress", "stream_n_out", "frames_n_out", "join_chunk_texts", "TimeEmbedding", "VoxtralTokenizer", "Timings", "DeviceBuffer",
     "q4_matmul_bench", "PinnedArray", "StreamingPool",
 ]

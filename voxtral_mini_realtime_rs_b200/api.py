@@ -125,6 +125,8 @@ _SIGS = {
                                              C.POINTER(_Timings)]),
     "vox_transcribe_pcm": (C.c_int32, [_P, _P, C.c_int32, C.c_size_t, C.c_int32, _P, C.c_size_t,
                                        C.POINTER(C.c_int32), C.POINTER(_Timings)]),
+    "vox_transcribe_pcm_ragged": (C.c_int32, [_P, _P, _P, C.c_int32, C.c_int32, _P, C.c_size_t, _P,
+                                              C.POINTER(_Timings)]),
     "vox_transcribe_pcm_dev": (C.c_int32, [_P, _P, C.c_int32, C.c_size_t, _P, C.c_size_t, C.POINTER(C.c_int32),
                                            C.POINTER(_Timings)]),
     "vox_generate_step_with_cache": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, _P, C.c_size_t]),
@@ -286,6 +288,9 @@ def peak_normalize(samples, target_peak: float = 0.95) -> np.ndarray:
     return s
 
 
+peak_normalize_samples = peak_normalize
+
+
 class PadConfig:
     """PadConfig (pad.rs:20-46)."""
 
@@ -333,6 +338,31 @@ def stream_progress(n_samples: int, ended: bool = False, reshape_factor: int = 4
 
 def needs_chunking(n_samples: int, max_mel_frames: int = 1500) -> bool:
     return n_samples > max_mel_frames * 160
+
+
+def stream_n_out(n_samples: int, reshape_factor: int = 4, prefix_len: int = 38) -> int:
+    """Token ids a transcribe call emits for one stream of n_samples: pad_audio length -> mel frames -> two
+    stride-2 convolutions (k3 p1) -> / reshape_factor -> minus the prefix (0 when shorter)."""
+    return frames_n_out(lib().vox_mel_num_frames(lib().vox_pad_audio_len(n_samples, None)), reshape_factor, prefix_len)
+
+
+def frames_n_out(mel_frames: int, reshape_factor: int = 4, prefix_len: int = 38) -> int:
+    """Token ids a transcribe call emits for mel_frames frames (see stream_n_out)."""
+    t = mel_frames
+    for _ in range(2):
+        t = (t + 2 - 3) // 2 + 1
+    return max(0, t // reshape_factor - prefix_len)
+
+
+def join_chunk_texts(tokenizer, chunk_ids) -> str:
+    """The reference CLI's join of independently transcribed chunks (transcribe.rs:256-275): per chunk keep the ids
+    >= 1000 (text tokens), decode, trim; drop empty texts; join with one space."""
+    texts = []
+    for ids in chunk_ids:
+        text = tokenizer.decode([int(i) for i in ids if int(i) >= 1000]).strip()
+        if text:
+            texts.append(text)
+    return " ".join(texts)
 
 
 class TimeEmbedding:
@@ -588,6 +618,70 @@ class Q4VoxtralModel:
         self._fill(timings, tm)
         return out[: b * no.value].reshape(b, no.value)
 
+    def transcribe_pcm_ragged(self, streams, peak_normalize: bool = True, timings: Timings | None = None):
+        """Streams of different lengths in one call (vox_transcribe_pcm_ragged): a list of 1-D f32 arrays -> a list of
+        int32 id arrays, one per stream, each what transcribe_pcm gives that stream alone.  After the call,
+        token_scores_ragged() and nbest_ragged() return the per-stream scores and n-best lists."""
+        arrs = [_f32(x).reshape(-1) for x in streams]
+        if not arrs:
+            raise VoxtralError(1, "transcribe_pcm_ragged needs at least one stream")
+        lens = np.array([a.size for a in arrs], np.uint64)
+        n_out = [stream_n_out(int(n), self.info["reshape_factor"], self.info["prefix_len"]) for n in lens]
+        samples = np.concatenate(arrs) if lens.sum() else np.zeros(1, np.float32)
+        out = np.zeros(max(sum(n_out), 1), np.int32)
+        no = np.zeros(len(arrs), np.int32)
+        tm = _Timings()
+        _check(lib().vox_transcribe_pcm_ragged(self._s, _ptr(samples), lens.ctypes.data_as(_P), len(arrs),
+                                               1 if peak_normalize else 0, _ptr(out), sum(n_out), _ptr(no), C.byref(tm)))
+        assert no.tolist() == n_out, (no.tolist(), n_out)
+        self._fill(timings, tm)
+        self._ragged_n = n_out
+        offs = np.concatenate([[0], np.cumsum(n_out)]).astype(int)
+        return [out[offs[i]:offs[i + 1]].copy() for i in range(len(arrs))]
+
+    def token_scores_ragged(self):
+        """Per stream (top_ids [n_out, k], top_logprobs [n_out, k]) of the last transcribe_pcm_ragged call."""
+        n_out = self._ragged_n
+        b, n, k = C.c_int32(), C.c_int32(), C.c_int32()
+        _check(lib().vox_session_token_scores(self._s, None, None, 0, C.byref(b), C.byref(n), C.byref(k)))
+        ids = np.empty((n.value, k.value), np.int32)
+        lp = np.empty((n.value, k.value), np.float32)
+        _check(lib().vox_session_token_scores(self._s, _ptr(ids), _ptr(lp), max(ids.size, 1), C.byref(b), C.byref(n),
+                                              C.byref(k)))
+        offs = np.concatenate([[0], np.cumsum(n_out)]).astype(int)
+        return [(ids[offs[i]:offs[i + 1]], lp[offs[i]:offs[i + 1]]) for i in range(len(n_out))]
+
+    def nbest_ragged(self):
+        """Per stream (ids [W, n_out], scores [W]) of the last transcribe_pcm_ragged call at beam width W > 1."""
+        n_out = self._ragged_n
+        b, w, n = C.c_int32(), C.c_int32(), C.c_int32()
+        _check(lib().vox_session_nbest(self._s, None, None, 0, C.byref(b), C.byref(w), C.byref(n)))
+        W = w.value
+        ids = np.empty(max(W * n.value, 1), np.int32)
+        scores = np.empty((b.value, W), np.float64)
+        _check(lib().vox_session_nbest(self._s, _ptr(ids), _ptr(scores), ids.size, C.byref(b), C.byref(w), C.byref(n)))
+        out, off = [], 0
+        for i, m in enumerate(n_out):
+            out.append((ids[off:off + W * m].reshape(W, m), scores[i]))
+            off += W * m
+        return out
+
+    def transcribe_long(self, samples, max_mel_frames: int = 1200, overlap_frames: int = 0, peak_normalize: bool = True):
+        """A recording of any length, as the reference CLI transcribes it (transcribe.rs:187-275): peak-normalise the
+        whole recording once, cut it with the chunk plan (vox_chunk_plan), transcribe every chunk on its own -- as
+        rows of vox_transcribe_pcm_ragged calls of up to max_batch // W chunks (W the beam width).  Returns
+        (per-chunk id arrays, the plan [(start, end, index, is_last)]); join_chunk_texts makes the text."""
+        s = _f32(samples).reshape(-1)
+        if peak_normalize:
+            s = peak_normalize_samples(s)
+        plan = chunk_audio(s.size, max_mel_frames, overlap_frames)
+        per_call = max(1, self.max_batch // max(1, getattr(self, "_beam", 1)))
+        ids = []
+        for c0 in range(0, len(plan), per_call):
+            group = plan[c0:c0 + per_call]
+            ids.extend(self.transcribe_pcm_ragged([s[a:b] for a, b, _, _ in group], peak_normalize=False))
+        return ids, plan
+
     def transcribe_pcm_dev(self, samples_dev: DeviceBuffer, b: int, n: int, timings: Timings | None = None) -> np.ndarray:
         cap = b * (n // 1280 + 120)
         out = np.zeros(cap, np.int32)
@@ -669,6 +763,7 @@ class Q4VoxtralModel:
         """Beam search of width w (1..8) for later transcribe calls; 1 is greedy.  B streams at width w need
         B * w <= max_batch.  The calls return the best hypothesis; nbest() returns all w."""
         _check(lib().vox_session_set_beam(self._s, w))
+        self._beam = w
 
     def nbest(self):
         """(ids [B,W,n] int32, scores [B,W] float64) of the last transcribe call at beam width W > 1, in rank order;

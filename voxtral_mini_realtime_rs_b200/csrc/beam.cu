@@ -123,17 +123,18 @@ void launch_beam_fork(float *kc, float *vc, size_t layer_stride, int layers, int
 // into the stream's own score row (position i is read from another row at position i only, before the walk moves on
 // to lower positions, so the gather runs in place).
 __global__ void __launch_bounds__(32)
-beam_traceback_kernel(BeamWork w, int W, int n, int out_ld, int *ids, double *scores, int *out, int *top_ids, float *top_lp) {
-    const int s = blockIdx.x, r = threadIdx.x;
+beam_traceback_kernel(BeamWork w, int W, int n, int out_ld, int *ids, double *scores, int *out, int *top_ids, float *top_lp,
+                      int s0, int out_stride) {
+    const int s = s0 + blockIdx.x, r = threadIdx.x;
     if (r >= W) return;
     int R = w.rank_row[s * W + r];
-    int *dst = ids + ((size_t)s * W + r) * n;
+    int *dst = ids + ((size_t)blockIdx.x * W + r) * n;
     for (int i = n - 1; i >= 0; --i) {
         const size_t at = (size_t)R * out_ld + i;
         const int tk = w.hist_tok[at], q = w.hist_par[at];
         dst[i] = tk;
         if (r == 0) {
-            const size_t o = (size_t)s * out_ld + i;
+            const size_t o = (size_t)s * out_stride * out_ld + i;
             out[o] = tk;
             if (top_ids)
                 for (int j = 0; j < TOPK_MAX; ++j) {
@@ -147,8 +148,9 @@ beam_traceback_kernel(BeamWork w, int W, int n, int out_ld, int *ids, double *sc
 }
 
 void launch_beam_traceback(const BeamWork &w, int b, int W, int n, int out_ld, int *ids, double *scores, int *out,
-                           int *top_ids, float *top_lp, cudaStream_t st) {
-    beam_traceback_kernel<<<b, 32, 0, st>>>(w, W, n, out_ld, ids, scores, out, top_ids, top_lp);
+                           int *top_ids, float *top_lp, cudaStream_t st, int s0, int out_stride) {
+    if (b <= 0) return;
+    beam_traceback_kernel<<<b, 32, 0, st>>>(w, W, n, out_ld, ids, scores, out, top_ids, top_lp, s0, out_stride);
     tc_count_launch("beam_traceback");
 }
 

@@ -618,6 +618,44 @@ int32_t vox_transcribe_pcm(vox_session *sh, const float *samples, int32_t b, siz
     return transcribe_pcm_impl(sh->s, samples, nullptr, b, n, normalize, out_ids, cap, n_out, tm);
     VOX_API_END
 }
+int32_t vox_transcribe_pcm_ragged(vox_session *sh, const float *samples, const size_t *lens, int32_t b, int32_t normalize,
+                                  int32_t *out_ids, size_t cap, int32_t *n_out, vox_timings *tm) {
+    VOX_API_BEGIN
+    REQUIRE(sh); REQUIRE(samples); REQUIRE(lens); REQUIRE(out_ids); REQUIRE(n_out);
+    Session *s = sh->s;
+    const vox_model_info &c = s->m->info;
+    // every argument on the host, before any device work
+    s->check_batch(b);
+    VOX_CHECK(s->beam_w == 1 || b * s->beam_w <= s->max_batch, VOX_EINVAL, "beam width %d x %d streams exceeds session max_batch %d",
+              s->beam_w, b, s->max_batch);
+    size_t total = 0;
+    bool equal = true;
+    for (int i = 0; i < b; ++i) {
+        VOX_CHECK(lens[i] >= 1, VOX_EINVAL, "stream %d is empty", i);
+        const StreamGeom g = stream_geometry(c, lens[i]);
+        VOX_CHECK(g.frames >= 1, VOX_EINVAL, "stream %d too short to produce mel frames", i);
+        VOX_CHECK(g.frames <= s->max_mel_frames, VOX_EINVAL,
+                  "stream %d needs %d mel frames > session max_mel_frames %d (chunk it: vox_chunk_plan)", i, g.frames,
+                  s->max_mel_frames);
+        total += (size_t)g.n_out;
+        equal = equal && lens[i] == lens[0];
+    }
+    VOX_CHECK(cap >= total, VOX_ECAPACITY, "out_ids capacity %zu < %zu", cap, total);
+    if (equal) {   // the batched [b][n] path: its layouts of ids, scores and n-best are the packed ones
+        int32_t n = 0;
+        const int32_t rc = transcribe_pcm_impl(s, samples, nullptr, b, lens[0], normalize, out_ids, cap, &n, tm);
+        for (int i = 0; i < b; ++i) n_out[i] = n;
+        s->pack_uniform_results(b, n);
+        if (s->beam_w == 1) {   // like a ragged call, leave the decoder cache empty
+            s->reset();
+            CUDA_OK(cudaStreamSynchronize(s->st));
+        }
+        return rc;
+    }
+    s->transcribe_ragged(samples, lens, b, normalize, out_ids, n_out, tm);
+    fill_timings(s, tm);
+    VOX_API_END
+}
 int32_t vox_transcribe_pcm_dev(vox_session *sh, const float *samples_dev, int32_t b, size_t n, int32_t *out_ids,
                                size_t cap, int32_t *n_out, vox_timings *tm) {
     VOX_API_BEGIN
@@ -738,9 +776,15 @@ int32_t vox_session_token_scores(vox_session *sh, int32_t *top_ids, float *top_l
     if (k) *k = K;
     if (!top_ids && !top_logprobs) return VOX_OK;
     REQUIRE(top_ids); REQUIRE(top_logprobs);
-    VOX_CHECK(cap >= (size_t)B * N * K, VOX_ECAPACITY, "token scores capacity %zu < %d x %d x %d", cap, B, N, K);
+    const size_t need = (size_t)(s->packed_results ? 1 : B) * N * K;
+    VOX_CHECK(cap >= need, VOX_ECAPACITY, "token scores capacity %zu < %zu", cap, need);
     CUDA_OK(cudaSetDevice(s->m->device));
     CUDA_OK(cudaStreamSynchronize(s->st));
+    if (s->packed_results) {   // vox_transcribe_pcm_ragged: N entries of K over all streams, already on the host
+        memcpy(top_ids, s->scores_host_ids.data(), sizeof(int32_t) * N * K);
+        memcpy(top_logprobs, s->scores_host_lp.data(), sizeof(float) * N * K);
+        return VOX_OK;
+    }
     // row r's entries [p0, p0 + N) of the device's [row][out_ld][VOX_MAX_TOP_K] buffers, the first K of each
     const size_t pitch = sizeof(int32_t) * VOX_MAX_TOP_K;
     for (int r = 0; r < B && N > 0; ++r) {
@@ -771,9 +815,15 @@ int32_t vox_session_nbest(vox_session *sh, int32_t *ids, double *scores, size_t 
     if (n) *n = N;
     if (!ids && !scores) return VOX_OK;
     REQUIRE(ids); REQUIRE(scores);
-    VOX_CHECK(cap >= (size_t)B * W * N, VOX_ECAPACITY, "n-best capacity %zu < %d x %d x %d", cap, B, W, N);
+    const size_t need = (size_t)(s->packed_results ? 1 : B) * W * N;
+    VOX_CHECK(cap >= need, VOX_ECAPACITY, "n-best capacity %zu < %zu", cap, need);
     CUDA_OK(cudaSetDevice(s->m->device));
     CUDA_OK(cudaStreamSynchronize(s->st));
+    if (s->packed_results) {   // vox_transcribe_pcm_ragged: stream s's W x n_out[s] ids after stream s-1's
+        memcpy(ids, s->nbest_host_ids.data(), sizeof(int32_t) * W * N);
+        memcpy(scores, s->nbest_host_scores.data(), sizeof(double) * B * W);
+        return VOX_OK;
+    }
     if (N > 0) CUDA_OK(cudaMemcpy(ids, s->d_nbest_ids, sizeof(int32_t) * B * W * N, cudaMemcpyDeviceToHost));
     CUDA_OK(cudaMemcpy(scores, s->d_nbest_scores, sizeof(double) * B * W, cudaMemcpyDeviceToHost));
     VOX_API_END
@@ -801,7 +851,7 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
     const std::string w = what;
     const float *src = nullptr;
     size_t n = 0;
-    const size_t rows = (size_t)s->cur_B * s->cur_S;
+    const size_t rows = (size_t)s->enc_rows;
     if (w == "capture_on") {
         if (!s->dbg_layers) {
             s->dbg_layers = s->arena.alloc_n<float>((size_t)c.enc_layers * s->max_batch * s->S_max * c.enc_dim);

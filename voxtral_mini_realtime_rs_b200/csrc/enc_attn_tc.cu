@@ -59,8 +59,9 @@ __device__ __forceinline__ void split2(const float x, const float y, uint32_t &h
 
 template <int HD>
 __global__ void __launch_bounds__(ET_THREADS)
-enc_attention_tc_kernel(const float *__restrict__ qkv, float *__restrict__ out, const int S, const int H, const int ld,
-                        const int q_off, const int k_off, const int v_off, const int window, const float scale) {
+enc_attention_tc_kernel(const float *__restrict__ qkv, float *__restrict__ out, const int S_grid, const int H, const int ld,
+                        const int q_off, const int k_off, const int v_off, const int window, const float scale,
+                        const int *__restrict__ seg) {
     constexpr int STR = HD + ET_PAD;  // halves per shared-memory row
     constexpr int KS = HD / 16;       // k-steps of Q K^T
     constexpr int ND = HD / 8;        // n-tiles of the output
@@ -68,7 +69,10 @@ enc_attention_tc_kernel(const float *__restrict__ qkv, float *__restrict__ out, 
     const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * ET_BQ;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int g = lane >> 2, t = lane & 3;
-    const float *base = qkv + (size_t)b * S * ld;
+    // stream b's rows [row0, row0 + S): the segment table's, or b * S_grid.. of a uniform batch
+    const int row0 = seg ? seg[b] : b * S_grid, S = seg ? seg[b + 1] - row0 : S_grid;
+    if (q0 >= S) return;   // the grid covers the longest segment
+    const float *base = qkv + (size_t)row0 * ld;
 
     // ---- Q fragments (A operand), hi and lo pieces: rows q0 + 16*warp + {g, g+8}
     const int qr0 = q0 + warp * 16 + g, qr1 = qr0 + 8;
@@ -219,10 +223,10 @@ enc_attention_tc_kernel(const float *__restrict__ qkv, float *__restrict__ out, 
 #pragma unroll
     for (int n = 0; n < ND; ++n) {
         if (qr0 < S)
-            *reinterpret_cast<float2 *>(out + ((size_t)b * S + qr0) * (H * HD) + h * HD + n * 8 + 2 * t) =
+            *reinterpret_cast<float2 *>(out + ((size_t)row0 + qr0) * (H * HD) + h * HD + n * 8 + 2 * t) =
                 make_float2(o[n][0] * inv0, o[n][1] * inv0);
         if (qr1 < S)
-            *reinterpret_cast<float2 *>(out + ((size_t)b * S + qr1) * (H * HD) + h * HD + n * 8 + 2 * t) =
+            *reinterpret_cast<float2 *>(out + ((size_t)row0 + qr1) * (H * HD) + h * HD + n * 8 + 2 * t) =
                 make_float2(o[n][2] * inv1, o[n][3] * inv1);
     }
 }
@@ -234,12 +238,12 @@ bool enc_attention_tc_supported(int hd, int ld, int q_off, int k_off, int v_off)
 }
 
 void launch_enc_attention_tc(const float *qkv, float *out, int B, int S, int H, int hd, int ld, int q_off, int k_off,
-                             int v_off, int window, float scale, cudaStream_t st) {
+                             int v_off, int window, float scale, cudaStream_t st, const int *seg) {
     if (S <= 0) return;
     VOX_CHECK(enc_attention_tc_supported(hd, ld, q_off, k_off, v_off), VOX_EINVAL, "enc_attention_tc: unsupported shape");
     dim3 grid((S + ET_BQ - 1) / ET_BQ, H, B);
-    if (hd == 64) enc_attention_tc_kernel<64><<<grid, ET_THREADS, 0, st>>>(qkv, out, S, H, ld, q_off, k_off, v_off, window, scale);
-    else enc_attention_tc_kernel<32><<<grid, ET_THREADS, 0, st>>>(qkv, out, S, H, ld, q_off, k_off, v_off, window, scale);
+    if (hd == 64) enc_attention_tc_kernel<64><<<grid, ET_THREADS, 0, st>>>(qkv, out, S, H, ld, q_off, k_off, v_off, window, scale, seg);
+    else enc_attention_tc_kernel<32><<<grid, ET_THREADS, 0, st>>>(qkv, out, S, H, ld, q_off, k_off, v_off, window, scale, seg);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) fail(VOX_ECUDA, fmt("CUDA error: enc_attention_tc launch: %s", cudaGetErrorString(e)));
     tc_count_launch("enc_attention_tc");

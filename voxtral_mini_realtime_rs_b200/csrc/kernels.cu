@@ -503,9 +503,19 @@ void launch_q4_linear(const Q4Weight &w, const float *x, int M, float *y, int ld
 // =====================================================================================
 __global__ void rope_inplace_kernel(float *buf, int ld, int q_off, int n_q, int k_off, int n_k, int hd,
                                     int seq, int pos0, const float *__restrict__ cos_t,
-                                    const float *__restrict__ sin_t) {
+                                    const float *__restrict__ sin_t, const int *__restrict__ seg, int n_seg) {
     const int r = blockIdx.x;
-    const int pos = pos0 + (r % seq);
+    int row0 = r - r % seq;
+    if (seg) {   // the last segment starting at or before r
+        int lo = 0, hi = n_seg - 1;
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (seg[mid] <= r) lo = mid;
+            else hi = mid - 1;
+        }
+        row0 = seg[lo];
+    }
+    const int pos = pos0 + (r - row0);
     const int half = hd >> 1;
     float *row = buf + (size_t)r * ld;
     const int total = (n_q + n_k) * half;
@@ -520,9 +530,10 @@ __global__ void rope_inplace_kernel(float *buf, int ld, int q_off, int n_q, int 
 }
 
 void launch_rope_inplace(float *buf, int rows, int ld, int q_off, int n_q, int k_off, int n_k, int hd,
-                         int seq, int pos0, const float *cos_t, const float *sin_t, cudaStream_t st) {
+                         int seq, int pos0, const float *cos_t, const float *sin_t, cudaStream_t st, const int *seg,
+                         int n_seg) {
     if (rows <= 0) return;
-    rope_inplace_kernel<<<rows, 256, 0, st>>>(buf, ld, q_off, n_q, k_off, n_k, hd, seq, pos0, cos_t, sin_t);
+    rope_inplace_kernel<<<rows, 256, 0, st>>>(buf, ld, q_off, n_q, k_off, n_k, hd, seq, pos0, cos_t, sin_t, seg, n_seg);
     post_launch("rope");
 }
 
@@ -537,8 +548,8 @@ constexpr int EA_BQ = 32, EA_BK = 64, EA_THREADS = 128;
 
 template <int HD>
 __global__ void __launch_bounds__(EA_THREADS)
-enc_attention_kernel(const float *__restrict__ qkv, float *__restrict__ out, int S, int H, int ld, int q_off,
-                     int k_off, int v_off, int window, float scale) {
+enc_attention_kernel(const float *__restrict__ qkv, float *__restrict__ out, int S_grid, int H, int ld, int q_off,
+                     int k_off, int v_off, int window, float scale, const int *__restrict__ seg) {
     extern __shared__ __align__(16) float sm[];
     float *Qs = sm;                          // [32][HD+1]  (odd strides: rows map to distinct banks)
     float *Ks = Qs + EA_BQ * (HD + 1);       // [64][HD+1]
@@ -547,7 +558,10 @@ enc_attention_kernel(const float *__restrict__ qkv, float *__restrict__ out, int
     const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * EA_BQ;
     const int tid = threadIdx.x, r = tid >> 2, c = tid & 3;
     constexpr int DQ = HD / 4;
-    const float *base = qkv + (size_t)b * S * ld;
+    // stream b's rows [row0, row0 + S): the segment table's, or b * S_grid.. of a uniform batch
+    const int row0 = seg ? seg[b] : b * S_grid, S = seg ? seg[b + 1] - row0 : S_grid;
+    if (q0 >= S) return;   // the grid covers the longest segment
+    const float *base = qkv + (size_t)row0 * ld;
     for (int i = tid; i < EA_BQ * HD; i += EA_THREADS) {
         const int rr = i / HD, d = i - rr * HD;
         const int gi = q0 + rr;
@@ -623,14 +637,14 @@ enc_attention_kernel(const float *__restrict__ qkv, float *__restrict__ out, int
     }
     if (gi < S) {
         const float inv = 1.0f / l_run;
-        float *orow = out + ((size_t)b * S + gi) * (H * HD) + h * HD + c;
+        float *orow = out + ((size_t)row0 + gi) * (H * HD) + h * HD + c;
 #pragma unroll
         for (int d = 0; d < DQ; ++d) orow[4 * d] = o[d] * inv;
     }
 }
 
 void launch_enc_attention(const float *qkv, float *out, int B, int S, int H, int hd, int ld, int q_off,
-                          int k_off, int v_off, int window, float scale, cudaStream_t st) {
+                          int k_off, int v_off, int window, float scale, cudaStream_t st, const int *seg) {
     if (S <= 0) return;
     dim3 grid((S + EA_BQ - 1) / EA_BQ, H, B);
     const size_t smem = (size_t)(EA_BQ * (hd + 1) + EA_BK * (hd + 1) + EA_BK * hd + EA_BQ * (EA_BK + 1)) * sizeof(float);
@@ -639,7 +653,7 @@ void launch_enc_attention(const float *qkv, float *out, int B, int S, int H, int
         static SmemAttr attr;                                                                               \
         smem_attr_check(ensure_dyn_smem(enc_attention_kernel<HD>, smem, attr), "enc_attention");              \
         enc_attention_kernel<HD><<<grid, EA_THREADS, smem, st>>>(qkv, out, S, H, ld, q_off, k_off, v_off,   \
-                                                                 window, scale);                            \
+                                                                 window, scale, seg);                       \
         break;                                                                                              \
     }
     switch (hd) {

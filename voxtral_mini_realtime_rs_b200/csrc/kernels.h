@@ -181,16 +181,21 @@ void launch_rmsnorm(const float *x, const float *gamma, float *y, int rows, int 
                     const AdaRows &ada_rows = AdaRows{});
 // in-place interleaved-pair RoPE on q (n_q heads) and k (n_k heads) inside a fused row buffer;
 // row r has position pos0 + (r % seq).  cos/sin: [max_pos][hd/2].
+// seg (device, optional): rows of streams of different lengths packed one after the other, stream s's rows
+// [seg[s], seg[s+1]) for s < n_seg; row r then has position pos0 + r - (start of its stream), and seq is unused.
 void launch_rope_inplace(float *buf, int rows, int ld, int q_off, int n_q, int k_off, int n_k, int hd,
-                         int seq, int pos0, const float *cos_t, const float *sin_t, cudaStream_t st);
+                         int seq, int pos0, const float *cos_t, const float *sin_t, cudaStream_t st,
+                         const int *seg = nullptr, int n_seg = 0);
 // encoder attention: causal + sliding window (|i-j| <= window), per (batch, head); qkv rows
 // [B*S][ld] with q at q_off, k at k_off, v at v_off; out [B*S][H*hd].
+// seg (device, optional): stream b's rows are [seg[b], seg[b+1]) of qkv and out instead of [b*S, (b+1)*S), and S is the
+// longest stream's length; a stream's band never reaches into another stream's rows.
 void launch_enc_attention(const float *qkv, float *out, int B, int S, int H, int hd, int ld, int q_off,
-                          int k_off, int v_off, int window, float scale, cudaStream_t st);
+                          int k_off, int v_off, int window, float scale, cudaStream_t st, const int *seg = nullptr);
 // same contract on the tensor cores (enc_attn_tc.cu): mma.sync with two-piece f16 operands, f32-grade accuracy
 bool enc_attention_tc_supported(int hd, int ld, int q_off, int k_off, int v_off);
 void launch_enc_attention_tc(const float *qkv, float *out, int B, int S, int H, int hd, int ld, int q_off,
-                             int k_off, int v_off, int window, float scale, cudaStream_t st);
+                             int k_off, int v_off, int window, float scale, cudaStream_t st, const int *seg = nullptr);
 // decoder: RoPE q in place, RoPE k -> Kcache, v -> Vcache at positions kv.pos[b] + i.
 // qkv rows [B*M][ld].
 void launch_dec_rope_append(float *qkv, int B, int M, int ld, int H, int Hkv, int hd, const KvView &kv,
@@ -236,6 +241,9 @@ void launch_token_scores(const float *logits, int B, int V, int k, const int *ou
 // page-table entries of the full pages below its next write position and a copy of the filled part of q's current page.
 // launch_beam_traceback walks the parent rows back from the last position: ids [b][W][n] and scores [b][W] in rank
 // order; rank 0's ids into out rows [0, b); with top_ids (non-null), rank 0's token scores gathered into rows [0, b).
+// s0 / out_stride: the launch walks streams s0 .. s0 + b - 1 (ids relative to stream s0, scores absolute) and writes
+// stream s's rank-0 ids and scores into row s * out_stride -- the stream's first beam row when its beams are rows
+// s * W .. s * W + W - 1 (streams of different lengths, one launch per output length).
 constexpr int BEAM_MAX = 8;   // VOX_MAX_BEAM (the top-k list holds the W candidates of a row: BEAM_MAX <= TOPK_MAX)
 struct BeamWork {
     int *rank_row = nullptr;                        // [b][W] row holding each rank
@@ -248,7 +256,7 @@ void launch_beam_select(const int *top_ids, const float *top_lp, const int *out_
 void launch_beam_fork(float *kc, float *vc, size_t layer_stride, int layers, int *page_table, int max_pages, const int *pos,
                       const int *src, int rows, int Hkv, int hd, cudaStream_t st);
 void launch_beam_traceback(const BeamWork &w, int b, int W, int n, int out_ld, int *ids, double *scores, int *out,
-                           int *top_ids, float *top_lp, cudaStream_t st);
+                           int *top_ids, float *top_lp, cudaStream_t st, int s0 = 0, int out_stride = 1);
 // a[i] += da; b[i] += db for i < n  (device-side per-row step counters for graph replay)
 void launch_advance(int *a, int da, int *b, int db, int n, cudaStream_t st);
 // gather rows: dst[b][:] = src[b*M + (M-1)][:]

@@ -390,6 +390,19 @@ Model *Model::load(const Gguf &g, int device) {
 // ======================================================================================
 static int conv_out(int t) { return (t + 2 - 3) / 2 + 1; }  // conv.rs:47-48
 
+StreamGeom stream_geometry(const vox_model_info &c, size_t n) {
+    vox_pad_config pc;
+    pad_config_default(&pc);
+    StreamGeom g;
+    g.padded = pad_audio_len(n, pc);
+    const size_t frames = mel_num_frames(g.padded);
+    g.frames = (int)std::min(frames, (size_t)1 << 30);
+    g.S = conv_out(conv_out(g.frames));
+    g.S4 = g.S / c.reshape_factor;
+    g.n_out = std::max(0, g.S4 - c.prefix_len);
+    return g;
+}
+
 Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ring) {
     VOX_CHECK(max_batch >= 1 && max_batch <= 64, VOX_EINVAL, "max_batch %d out of range [1,64]", max_batch);
     VOX_CHECK(max_mel_frames >= 16, VOX_EINVAL, "max_mel_frames %d too small", max_mel_frames);
@@ -455,6 +468,7 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ri
         s->ada_tmp = s->arena.alloc_n<float>(c.t_cond_dim);
         s->d_pos = s->arena.alloc_n<int>(B);      // per row (kernels.h KvView::pos)
         s->d_outpos = s->arena.alloc_n<int>(B);
+        s->d_seg = s->arena.alloc_n<int>(B + 1);
         s->d_tok = s->arena.alloc_n<int>(B);
         s->d_ids = s->arena.alloc_n<int>(drows);
         s->d_out = s->arena.alloc_n<int>(B * s->out_ld);
@@ -631,7 +645,7 @@ void Session::bind_delays(const int *streams, int n) {
 
 void Session::bind_row_delays(int B) {
     std::vector<int> id(B);
-    for (int b = 0; b < B; ++b) id[b] = beam_streams > 0 ? b % beam_streams : b;
+    for (int b = 0; b < B; ++b) id[b] = !row_streams.empty() ? row_streams[b] : beam_streams > 0 ? b % beam_streams : b;
     bind_delays(id.data(), B);
 }
 
@@ -675,6 +689,7 @@ void Session::encode(int B, int T) {
     cur_B = B;
     cur_S = S;
     cur_S4 = S4;
+    enc_rows = rows;
     if (S4 > 0) {
         launch_reshape_rows(h_enc, packed, B, S, S4, d, c.reshape_factor, st);
         linear(m->adapter0, packed, B * S4, adapter_h, c.dec_dim, nullptr, nullptr, EPI_GELU);
@@ -1062,6 +1077,7 @@ void Session::step_incremental(int b, int M, const int *ids_host, bool add_audio
     scores_n = 1;
     scores_pos.resize(b);
     for (int r = 0; r < b; ++r) scores_pos[r] = out_rows[r]++;   // each row's output just emitted
+    packed_results = false;
 }
 
 void Session::reset() {
@@ -1178,6 +1194,7 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
     nbest_b = B;
     nbest_w = W > 1 ? W : 0;
     nbest_n = n_out;
+    packed_results = false;
     if (W > 1) {
         // the cache holds W hypotheses per stream, not one: the incremental API starts over, on the identity page table
         reset();
@@ -1196,6 +1213,271 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
         tm->decode_tokens = n_out;
     }
     return n_out;
+}
+
+// ======================================================================================
+// Streams of different lengths in one call (vox_transcribe_pcm_ragged)
+// ======================================================================================
+
+// encode() on streams packed one after the other: the convolutions run per stream (their zero padding is at each
+// stream's own ends), the layers' linears run over all rows at once, RoPE and attention read the segment table, and
+// each stream keeps its own S / 4 embeddings.  Work follows the sum of the lengths, not b x the longest.
+void Session::encode_ragged(int b, const int *T, const std::vector<std::vector<int>> &audio_rows) {
+    const vox_model_info &c = m->info;
+    check_batch(b);
+    const int d = c.enc_dim, hdq = c.enc_heads * c.enc_head_dim, f = c.reshape_factor, D = c.dec_dim;
+    std::vector<int> T1(b), S(b), S4(b);
+    seg_host.assign(b + 1, 0);
+    int S_long = 0, sum_T = 0, sum_S4 = 0, n_rows = 0;
+    for (int i = 0; i < b; ++i) {
+        VOX_CHECK(T[i] >= 1 && T[i] <= max_mel_frames, VOX_EINVAL, "mel frames %d exceed session max_mel_frames %d", T[i],
+                  max_mel_frames);
+        T1[i] = conv_out(T[i]);
+        S[i] = conv_out(T1[i]);
+        S4[i] = S[i] / f;
+        seg_host[i + 1] = seg_host[i] + S[i];
+        S_long = std::max(S_long, S[i]);
+        sum_T += T[i];
+        sum_S4 += S4[i];
+        for (int r : audio_rows[i]) n_rows = std::max(n_rows, r + 1);
+    }
+    const int rows = seg_host[b];
+    // b <= max_batch streams of <= max_mel_frames frames: the scratch Session::create sized for max_batch uniform streams
+    // holds them packed; the adapter's output passes through x_enc on its way to the audio rows
+    if (!(sum_T <= max_batch * max_mel_frames && rows <= max_batch * S_max && n_rows <= max_batch &&
+          (size_t)sum_S4 * D <= (size_t)max_batch * S_max * d))
+        fail(VOX_EINVAL, "encode_ragged: packed streams exceed the session scratch");
+    CUDA_OK(cudaMemcpyAsync(d_seg, seg_host.data(), sizeof(int) * (b + 1), cudaMemcpyHostToDevice, st));
+    for (int i = 0, t0 = 0, t1 = 0; i < b; t0 += T[i], t1 += T1[i], ++i) {
+        launch_conv2_gemm(mel_tm + (size_t)t0 * c.n_mels, m->conv1_w, m->conv1_b, h1 + (size_t)t1 * d, 1, T[i], T1[i], c.n_mels,
+                          d, st);
+        launch_conv2_gemm(h1 + (size_t)t1 * d, m->conv2_w, m->conv2_b, x_enc + (size_t)seg_host[i] * d, 1, T1[i], S[i], d, d, st);
+    }
+    if (debug_capture && dbg_conv) CUDA_OK(cudaMemcpyAsync(dbg_conv, x_enc, sizeof(float) * rows * d, cudaMemcpyDeviceToDevice, st));
+    const float scale = powf((float)c.enc_head_dim, -0.5f);
+    for (int i = 0; i < c.enc_layers; ++i) {
+        const EncLayerW &l = m->enc[i];
+        linear(l.wqkv, x_enc, rows, qkv_enc, 3 * hdq, l.bqkv, nullptr, EPI_NONE, l.attn_norm, h_enc);
+        launch_rope_inplace(qkv_enc, rows, 3 * hdq, 0, c.enc_heads, hdq, c.enc_heads, c.enc_head_dim, S_long, 0,
+                            m->enc_cos, m->enc_sin, st, d_seg, b);
+        if (use_enc_attn_tc && enc_attention_tc_supported(c.enc_head_dim, 3 * hdq, 0, hdq, 2 * hdq))
+            launch_enc_attention_tc(qkv_enc, attn_enc, b, S_long, c.enc_heads, c.enc_head_dim, 3 * hdq, 0, hdq, 2 * hdq,
+                                    c.enc_window, scale, st, d_seg);
+        else
+            launch_enc_attention(qkv_enc, attn_enc, b, S_long, c.enc_heads, c.enc_head_dim, 3 * hdq, 0, hdq, 2 * hdq,
+                                 c.enc_window, scale, st, d_seg);
+        linear(l.wo, attn_enc, rows, x_enc, d, l.bo, x_enc, EPI_RESIDUAL);
+        linear(l.w13, x_enc, rows, act_enc, c.enc_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, h_enc);
+        linear(l.w2, act_enc, rows, x_enc, d, l.b2, x_enc, EPI_RESIDUAL);
+        if (debug_capture && dbg_layers)
+            CUDA_OK(cudaMemcpyAsync(dbg_layers + (size_t)i * rows * d, x_enc, sizeof(float) * rows * d,
+                                    cudaMemcpyDeviceToDevice, st));
+    }
+    launch_rmsnorm(x_enc, m->enc_norm, h_enc, rows, d, m->norm_eps, st);
+    enc_rows = rows;
+    cur_B = n_rows;
+    cur_S = S_max;
+    cur_S4 = S4_max;   // the decoder reads row r's embeddings at audio + r * S4_max
+    if (sum_S4 == 0) return;
+    for (int i = 0, o = 0; i < b; o += S4[i], ++i)
+        launch_reshape_rows(h_enc + (size_t)seg_host[i] * d, packed + (size_t)o * d * f, 1, S[i], S4[i], d, f, st);
+    linear(m->adapter0, packed, sum_S4, adapter_h, D, nullptr, nullptr, EPI_GELU);
+    linear(m->adapter2, adapter_h, sum_S4, x_enc, D, nullptr, nullptr, EPI_NONE);
+    for (int i = 0, o = 0; i < b; o += S4[i], ++i)
+        for (int r : audio_rows[i])
+            if (S4[i] > 0)
+                CUDA_OK(cudaMemcpyAsync(audio + (size_t)r * S4_max * D, x_enc + (size_t)o * D, sizeof(float) * S4[i] * D,
+                                        cudaMemcpyDeviceToDevice, st));
+}
+
+// Streams sorted (stably) by decreasing output count own the rows: beams w of sorted stream i run in row i * W + w, so
+// the streams that still need tokens are always the rows [0, R).  Every stream with output takes the prefill; then the
+// steps run in segments, one per distinct output count, each over the rows still live.
+void Session::transcribe_ragged(const float *samples, const size_t *lens, int b, int normalize, int32_t *out_ids,
+                                int32_t *n_out, vox_timings *tm) {
+    const vox_model_info &c = m->info;
+    const int W = beam_w, P = c.prefix_len;
+    check_batch(b);
+    VOX_CHECK(W == 1 || b * W <= max_batch, VOX_EINVAL, "beam width %d x %d streams exceeds session max_batch %d", W, b, max_batch);
+    vox_pad_config pc;
+    pad_config_default(&pc);
+    const size_t left = pad_left(pc);
+    std::vector<StreamGeom> g(b);
+    std::vector<size_t> in_off(b + 1, 0), pad_off(b + 1, 0);
+    std::vector<int> T(b);
+    for (int s = 0; s < b; ++s) {
+        g[s] = stream_geometry(c, lens[s]);
+        T[s] = g[s].frames;
+        n_out[s] = g[s].n_out;
+        in_off[s + 1] = in_off[s] + lens[s];
+        pad_off[s + 1] = pad_off[s] + (g[s].padded + 3) / 4 * 4;   // each stream's padded signal 16-byte aligned
+    }
+    CUDA_OK(cudaSetDevice(m->device));
+    if (pad_off[b] > pcm_pad_cap) {
+        pcm_pad = arena.alloc_n<float>(pad_off[b]);
+        pcm_pad_cap = pad_off[b];
+    }
+    if (in_off[b] > pcm_cap) {
+        pcm = arena.alloc_n<float>(in_off[b]);
+        pcm_cap = in_off[b];
+    }
+    std::vector<int> order(b);
+    for (int s = 0; s < b; ++s) order[s] = s;
+    std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return g[x].n_out > g[y].n_out; });
+    int live = 0;
+    while (live < b && g[order[live]].n_out > 0) ++live;
+    std::vector<std::vector<int>> rows(b);
+    struct RaggedRows {   // the rows map to their streams for this call only, also when it throws
+        Session *s;
+        ~RaggedRows() { s->row_streams.clear(); s->beam_streams = 0; }
+    } ragged_rows{this};
+    row_streams.assign((size_t)b * W, 0);
+    for (int i = 0; i < b; ++i)
+        for (int w = 0; w < W; ++w) {
+            rows[order[i]].push_back(i * W + w);
+            row_streams[(size_t)i * W + w] = order[i];
+        }
+
+    CUDA_OK(cudaEventRecord(ev[0], st));
+    CUDA_OK(cudaMemcpyAsync(pcm, samples, sizeof(float) * in_off[b], cudaMemcpyHostToDevice, st));
+    for (int s = 0, t0 = 0; s < b; t0 += T[s], ++s) {
+        launch_peak_normalize_pad(pcm + in_off[s], 1, lens[s], 0.95f, normalize, pcm_pad + pad_off[s], g[s].padded, left,
+                                  peak_scale + s, st);
+        launch_mel(pcm_pad + pad_off[s], 1, g[s].padded, g[s].padded, m->mel.window, m->mel.fb_vals, m->mel.fb_start,
+                   m->mel.fb_len, m->mel.fb_stride, mel_tm + (size_t)t0 * c.n_mels, T[s], 0, st);
+    }
+    CUDA_OK(cudaEventRecord(ev[1], st));
+    encode_ragged(b, T.data(), rows);
+    CUDA_OK(cudaEventRecord(ev[2], st));
+
+    const int n_max = live > 0 ? g[order[0]].n_out : 0;
+    reset();
+    if (live > 0) {
+        beam_streams = W > 1 ? live : 0;
+        const int R0 = live * W;
+        // prefix = [BOS] + [STREAMING_PAD]*37 (model.rs:883-892) in every row, each beam row of a stream included: the
+        // first selection then reads one parent row per stream (its rank 0) and forks it into the others
+        std::vector<int> prefix((size_t)R0 * P, 32);
+        for (int r = 0; r < R0; ++r) prefix[(size_t)r * P] = 1;
+        prefill(R0, P, prefix.data(), true);
+        if (W > 1) {
+            std::vector<int> rank_row(R0);
+            for (int r = 0; r < R0; ++r) rank_row[r] = r;
+            CUDA_OK(cudaMemcpyAsync(beam.rank_row, rank_row.data(), sizeof(int) * R0, cudaMemcpyHostToDevice, st));
+            CUDA_OK(cudaMemsetAsync(beam.cum, 0, sizeof(double) * R0, st));
+            CUDA_OK(cudaStreamSynchronize(st));   // rank_row dies with this frame
+            page_table_forked = true;
+            beam_step(live, 1);
+        }
+        CUDA_OK(cudaEventRecord(ev[4], st));
+        for (int t = 1; t < n_max;) {   // outputs [0, t) of every live stream are done
+            int L = 0;
+            while (L < live && g[order[L]].n_out > t) ++L;
+            const int t_end = g[order[L - 1]].n_out;
+            run_steps(L * W, t_end - t, [&] {
+                const unsigned launches = decode_step(L * W);
+                if (W > 1) beam_step(L, W);
+                return launches;
+            });
+            t = t_end;
+        }
+        if (W > 1)
+            for (int i0 = 0, off = 0; i0 < live;) {   // one traceback per output count
+                const int n = g[order[i0]].n_out;
+                int i1 = i0;
+                while (i1 < live && g[order[i1]].n_out == n) ++i1;
+                launch_beam_traceback(beam, i1 - i0, W, n, out_ld, d_nbest_ids + off, d_nbest_scores, d_out,
+                                      top_k > 0 ? d_top_ids : nullptr, d_top_lp, st, i0, W);
+                off += (i1 - i0) * W * n;
+                i0 = i1;
+            }
+    } else {
+        CUDA_OK(cudaEventRecord(ev[4], st));
+    }
+    CUDA_OK(cudaEventRecord(ev[3], st));
+
+    // results back in the caller's stream order: stream s's outputs are in the row of its rank 0 beam, rows[s][0]
+    std::vector<size_t> out_off(b + 1, 0);
+    for (int s = 0; s < b; ++s) out_off[s + 1] = out_off[s] + g[s].n_out;
+    const size_t total = out_off[b];
+    std::vector<int> host((size_t)live * W * out_ld);
+    if (live > 0) CUDA_OK(cudaMemcpyAsync(host.data(), d_out, sizeof(int) * host.size(), cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    for (int s = 0; s < b; ++s)
+        for (int i = 0; i < g[s].n_out; ++i) out_ids[out_off[s] + i] = host[(size_t)rows[s][0] * out_ld + i];
+    scores_host_ids.clear();
+    scores_host_lp.clear();
+    if (top_k > 0) {
+        const int K = top_k;
+        scores_host_ids.resize(total * K);
+        scores_host_lp.resize(total * K);
+        const size_t pitch = sizeof(int) * TOPK_MAX;
+        for (int s = 0; s < b; ++s) {
+            if (g[s].n_out == 0) continue;
+            const size_t at = (size_t)rows[s][0] * out_ld * TOPK_MAX, dst = out_off[s] * K;
+            CUDA_OK(cudaMemcpy2D(scores_host_ids.data() + dst, sizeof(int) * K, d_top_ids + at, pitch, sizeof(int) * K, g[s].n_out,
+                                 cudaMemcpyDeviceToHost));
+            CUDA_OK(cudaMemcpy2D(scores_host_lp.data() + dst, sizeof(float) * K, d_top_lp + at, pitch, sizeof(float) * K, g[s].n_out,
+                                 cudaMemcpyDeviceToHost));
+        }
+    }
+    nbest_host_ids.clear();
+    nbest_host_scores.clear();
+    if (W > 1) {
+        // the tracebacks packed sorted stream i's W hypotheses after those of sorted stream i - 1
+        std::vector<int> packed_ids(total * W);
+        std::vector<double> packed_scores((size_t)live * W);
+        if (total > 0) CUDA_OK(cudaMemcpy(packed_ids.data(), d_nbest_ids, sizeof(int) * packed_ids.size(), cudaMemcpyDeviceToHost));
+        if (live > 0)
+            CUDA_OK(cudaMemcpy(packed_scores.data(), d_nbest_scores, sizeof(double) * packed_scores.size(), cudaMemcpyDeviceToHost));
+        nbest_host_ids.resize(total * W);
+        nbest_host_scores.assign((size_t)b * W, 0.0);
+        for (int i = 0, off = 0; i < live; off += W * g[order[i]].n_out, ++i) {
+            const int s = order[i];
+            std::copy(packed_ids.begin() + off, packed_ids.begin() + off + (size_t)W * g[s].n_out,
+                      nbest_host_ids.begin() + out_off[s] * W);
+            for (int w = 0; w < W; ++w) nbest_host_scores[(size_t)s * W + w] = packed_scores[(size_t)i * W + w];
+        }
+    }
+    // the cache holds streams of different lengths (and perhaps beams): the incremental API starts over
+    reset();
+    CUDA_OK(cudaStreamSynchronize(st));
+    nbest_b = b;
+    nbest_w = W > 1 ? W : 0;
+    nbest_n = (int)total;
+    scores_k = top_k;
+    scores_b = b;
+    scores_n = (int)total;
+    scores_pos.clear();
+    packed_results = true;
+    if (tm) {
+        int S4_long = 0;
+        for (const StreamGeom &x : g) S4_long = std::max(S4_long, x.S4);
+        tm->seq_len = S4_long;
+        tm->decode_tokens = n_max;
+    }
+}
+
+void Session::pack_uniform_results(int b, int n) {
+    const int K = scores_k, W = nbest_w;
+    scores_host_ids.assign((size_t)b * n * K, 0);
+    scores_host_lp.assign((size_t)b * n * K, 0.0f);
+    CUDA_OK(cudaStreamSynchronize(st));
+    for (int r = 0; r < b && n > 0 && K > 0; ++r) {   // row r's positions [0, n)
+        const size_t at = (size_t)r * out_ld * TOPK_MAX, dst = (size_t)r * n * K;
+        CUDA_OK(cudaMemcpy2D(scores_host_ids.data() + dst, sizeof(int) * K, d_top_ids + at, sizeof(int) * TOPK_MAX, sizeof(int) * K,
+                             n, cudaMemcpyDeviceToHost));
+        CUDA_OK(cudaMemcpy2D(scores_host_lp.data() + dst, sizeof(float) * K, d_top_lp + at, sizeof(float) * TOPK_MAX,
+                             sizeof(float) * K, n, cudaMemcpyDeviceToHost));
+    }
+    nbest_host_ids.assign((size_t)b * W * n, 0);
+    nbest_host_scores.assign((size_t)b * W, 0.0);
+    if (W > 0) {   // [b][W][n]: already stream after stream
+        if (n > 0) CUDA_OK(cudaMemcpy(nbest_host_ids.data(), d_nbest_ids, sizeof(int) * nbest_host_ids.size(), cudaMemcpyDeviceToHost));
+        CUDA_OK(cudaMemcpy(nbest_host_scores.data(), d_nbest_scores, sizeof(double) * nbest_host_scores.size(), cudaMemcpyDeviceToHost));
+    }
+    scores_n = nbest_n = b * n;
+    packed_results = true;
 }
 
 }  // namespace vox

@@ -93,6 +93,14 @@ void rope_rows(int hd, float theta, int64_t p0, int n, float *cos_out, float *si
 Q4Weight upload_q4(DeviceArena &arena, const std::vector<const uint8_t *> &raw, const std::vector<int> &n_rows,
                    int K, bool interleave, bool tc_layout = false);
 
+// What a transcribe call makes of one stream of n samples: the padded length (pad_audio), mel frames, audio positions
+// after the two stride-2 convolutions and the reshape, and decoder outputs (positions after the prefix; 0 when shorter).
+struct StreamGeom {
+    size_t padded = 0;
+    int frames = 0, S = 0, S4 = 0, n_out = 0;
+};
+StreamGeom stream_geometry(const vox_model_info &c, size_t n);
+
 // transcription delay of a new session or stream session, in tokens of 80 ms: the CLI default --delay 6
 // (transcribe.rs:49-51)
 constexpr float kDefaultDelay = 6.0f;
@@ -128,6 +136,9 @@ struct Session {
     float *h1 = nullptr, *x_enc = nullptr, *h_enc = nullptr, *qkv_enc = nullptr, *attn_enc = nullptr, *act_enc = nullptr;
     float *packed = nullptr, *adapter_h = nullptr, *audio = nullptr;
     int cur_B = 0, cur_S = 0, cur_S4 = 0;
+    int enc_rows = 0;           // encoder rows of the last encode: B * S, or the sum of the streams' S of a ragged one
+    int *d_seg = nullptr;       // [max_batch + 1] encoder row of each stream's first frame (ragged encode)
+    std::vector<int> seg_host;
     // decoder
     // decoder KV cache: page pools [L][n_pages][Hkv][KV_PAGE][hd] + per-row page tables (kernels.h KvView).  Whole-
     // utterance batches use the identity mapping (row b owns pages b*max_pages..); streaming sessions allocate pages
@@ -176,6 +187,7 @@ struct Session {
     // with the n-best results by the first set_beam(W > 1).
     int beam_w = 1;
     int beam_streams = 0;           // > 0 while a beam call runs: row r belongs to stream r % beam_streams
+    std::vector<int> row_streams;   // non-empty while a ragged call runs: row r belongs to stream row_streams[r]
     BeamWork beam;
     int *d_nbest_ids = nullptr;     // [b][W][n] of the last transcribe
     double *d_nbest_scores = nullptr;
@@ -188,6 +200,14 @@ struct Session {
     // position `step_pos` of each row), scored with k = scores_k (0: that call ran with scores off)
     int scores_k = 0, scores_b = 0, scores_n = 0;
     std::vector<int> scores_pos;    // per row, empty after a transcribe
+    // packed_results: the last transcribe was vox_transcribe_pcm_ragged, whose scores and n-best lists are kept here
+    // packed in the caller's stream order (stream s's entries after stream s-1's; scores_n / nbest_n their total count)
+    bool packed_results = false;
+    std::vector<int> scores_host_ids, nbest_host_ids;
+    std::vector<float> scores_host_lp;
+    std::vector<double> nbest_host_scores;
+    // packs the results of transcribe_from_mel over b streams of n outputs each like a ragged call's
+    void pack_uniform_results(int b, int n);
     // host mirror of d_outpos[] outside stream mode: outputs per row since reset (incremental calls / transcribe)
     std::vector<int> out_rows;
     StepGraph step_graph;   // the offline transcription's decode step, captured once per key and replayed
@@ -282,6 +302,13 @@ struct Session {
     void check_ids(const int32_t *ids, size_t n) const;
     // runs prefill + loop; returns tokens per stream
     int transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids, vox_timings *tm);
+    // encode() of b streams of T[s] mel frames packed one after the other in mel_tm: frames, conv rows and encoder rows
+    // packed by stream (d_seg); stream s's audio embeddings into the audio rows of rows[s] (S4_max apart)
+    void encode_ragged(int b, const int *T, const std::vector<std::vector<int>> &rows);
+    // vox_transcribe_pcm_ragged after its argument checks: b streams of lens[s] host samples, one after the other;
+    // n_out[s] ids of stream s after those of stream s - 1 in out_ids.  Records ev[0..4] like the other transcribe calls.
+    void transcribe_ragged(const float *samples, const size_t *lens, int b, int normalize, int32_t *out_ids,
+                           int32_t *n_out, vox_timings *tm);
     void reset();
     // re-bases the persistent kernel's step epoch once it has advanced far (see reset)
     void rebase_epoch();
