@@ -46,9 +46,9 @@ def _mel(i, seconds=SECONDS):
 class Geometry:
     """One window: the GPU model, the streams' mels, teacher ids and the f64 reference logits of positions 37..S4-1."""
 
-    def __init__(self, vx, window):
+    def __init__(self, vx, window, data=None):
         self.window = window
-        self.data = geometry_model_bytes(window)
+        self.data = geometry_model_bytes(window) if data is None else data
         self.model = vx.Q4ModelLoader.from_bytes(self.data).load(0, max_batch=N_STREAMS, max_mel_frames=MEL_FRAMES)
         self.vocab = self.model.info["vocab"]
         self.mels = np.concatenate([_mel(i) for i in range(N_STREAMS)])

@@ -56,9 +56,9 @@ def _report(what, err, bound):
 
 
 class Geometry:
-    def __init__(self, vx, window):
+    def __init__(self, vx, window, data=None):
         self.window = window
-        self.data = encoder_geometry_bytes(window)
+        self.data = encoder_geometry_bytes(window) if data is None else data
         self.model = vx.Q4ModelLoader.from_bytes(self.data).load(0, max_batch=MAX_BATCH, max_mel_frames=MEL_FRAMES)
         self.o64 = OracleModel(self.data, dtype=torch.float64)
         assert self.model.info["enc_window"] == window and self.model.info["enc_head_dim"] == 64

@@ -42,6 +42,47 @@ def tc_matvec_model(x: np.ndarray, raw: np.ndarray, n: int, k: int) -> np.ndarra
     return per_block.sum(axis=1, dtype=F32)
 
 
+def pack_q4(d: np.ndarray, q: np.ndarray) -> np.ndarray:
+    """Q4_0 bytes of f16 scales d [N, K/32] and nibbles q [N, K] (element i low, i + 16 high nibble of byte i)."""
+    n, kb = d.shape
+    qb = q.reshape(n, kb, 32).astype(np.uint8)
+    raw = np.empty((n, kb, 18), np.uint8)
+    raw[:, :, :2] = d.astype(np.float16).reshape(n, kb, 1).view(np.uint8)
+    raw[:, :, 2:] = qb[:, :, :16] | (qb[:, :, 16:] << 4)
+    return raw.reshape(-1)
+
+
+def gemm_split_weights(raw: np.ndarray, n: int, k: int):
+    """The wgmma GEMM's weight pieces: (q-8)*d' as f16 hi + the f16 residual lo, d' = f16(d * 2^8).  Exact inside the
+    kernel's |d| < 32 domain."""
+    blocks = raw.reshape(n, k // 32, 18)
+    d = blocks[:, :, :2].copy().view(np.float16)[:, :, 0]
+    qs = blocks[:, :, 2:]
+    n8 = np.concatenate([(qs & 0x0F), (qs >> 4)], axis=2).reshape(n, k).astype(np.float64) - 8.0
+    d2 = np.repeat((d.astype(np.float32) * 256).astype(np.float16), 32, 1).astype(np.float64)
+    hi = (n8 * d2).astype(np.float16)                                  # HMUL2: RN_f16(n8 * d')
+    lo = (n8 * d2 - hi.astype(np.float64)).astype(np.float16)          # HFMA2: the residual
+    return n8 * d2, hi, lo
+
+
+def gemm_split_model(x: np.ndarray, raw: np.ndarray, n: int, k: int) -> np.ndarray:
+    """numpy model of the wgmma GEMM (csrc/gemm_tc5.cu): x [M, K] times the per-token power of two that puts the row
+    maximum (x 1.0001) in [2^7, 2^8) (exponent clamped to +-100, all-zero rows scale 1) as f16 hi + mid; products
+    w_hi x_h + w_hi x_m + w_lo x_h in f64 (the MMA accumulates in f32).  Returns [M, N] in f64."""
+    _, hi, lo = gemm_split_weights(raw, n, k)
+    x64 = np.asarray(x, np.float32).astype(np.float64)
+    mx = np.abs(x64).max(1) * 1.0001
+    e0 = np.where(mx > 0, np.frexp(mx)[1] - 1, 7)                      # floor(log2(mx))
+    e = np.clip(e0, -100, 100)
+    sc = np.ldexp(1.0, 7 - e)[:, None]
+    xs = x64 * sc
+    xh = xs.astype(np.float16)
+    xm = (xs - xh.astype(np.float64)).astype(np.float16)
+    assert np.all(np.isfinite(xh.astype(np.float64))) and np.all((np.abs(xs).max(1) < 256.0) | (e != e0))
+    h, l = hi.astype(np.float64), lo.astype(np.float64)
+    return (xh.astype(np.float64) @ h.T + xm.astype(np.float64) @ h.T + xh.astype(np.float64) @ l.T) / sc / 256.0
+
+
 def _case(x, n=64, seed=0):
     k = x.size
     rng = np.random.default_rng(seed)
@@ -101,24 +142,17 @@ def test_gemm_f16_two_by_two_split_three_products():
     K, N, M = 5120, 48, 12
     for dscale in (1e-4, 1e-2, 3.0):
         d = (rng.uniform(0.5, 1.5, (N, K // 32)) * dscale).astype(np.float16)
-        n8 = (rng.integers(0, 16, (N, K)) - 8).astype(np.float64)
+        q = rng.integers(0, 16, (N, K))
+        n8 = (q - 8).astype(np.float64)
         w = n8 * np.repeat(d.astype(np.float64), 32, 1)
         x = (rng.standard_normal((M, K)) * rng.uniform(0.01, 30, (M, 1))).astype(np.float32)
         x[:, ::97] *= 50.0
-        d2 = np.repeat((d.astype(np.float32) * 256).astype(np.float16), 32, 1).astype(np.float64)
-        hi = (n8 * d2).astype(np.float16)                                  # HMUL2: RN_f16(n8 * d')
-        lo = (n8 * d2 - hi.astype(np.float64)).astype(np.float16)          # HFMA2: the residual
+        raw = pack_q4(d, q)
+        wd, hi, lo = gemm_split_weights(raw, N, K)
         assert np.all(np.isfinite(hi.astype(np.float64)))
         if dscale >= 1e-2:                                                 # normal range: the split is exact
-            assert np.array_equal(hi.astype(np.float64) + lo.astype(np.float64), n8 * d2)
-        mx = np.abs(x).max(1) * 1.0001
-        sc = 2.0 ** (7 - np.floor(np.log2(mx)))[:, None]
-        xs = x.astype(np.float64) * sc
-        xh = xs.astype(np.float16)
-        xm = (xs - xh.astype(np.float64)).astype(np.float16)
-        assert np.all(np.isfinite(xh.astype(np.float64))) and np.abs(xs).max() < 256.0
-        got = (xh.astype(np.float64) @ hi.astype(np.float64).T + xm.astype(np.float64) @ hi.astype(np.float64).T
-               + xh.astype(np.float64) @ lo.astype(np.float64).T) / sc / 256.0
+            assert np.array_equal(hi.astype(np.float64) + lo.astype(np.float64), wd)
+        got = gemm_split_model(x, raw, N, K)
         exact = x.astype(np.float64) @ w.T
         den = np.abs(x.astype(np.float64)) @ np.abs(w).T
         err = float((np.abs(got - exact) / den).max())

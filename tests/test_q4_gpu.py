@@ -98,11 +98,13 @@ def test_q4_vs_unquantised_f32(vx):
 
 @pytest.mark.parametrize("m", list(range(1, 10)) + [17, 64, 65])
 def test_q4_matmul_all_m_random_blocks(vx, m):
-    """Random nibbles (all 16 values incl. 0) and random scales; matvec (M<=8) and GEMM (M>8)."""
+    """Random nibbles (all 16 values incl. 0) and random scales of either sign (real files carry negative ones);
+    matvec (M<=8) and GEMM (M>8)."""
     n, k = 208, 2304  # N not a multiple of 16/64, K = 72 blocks (lanes unevenly loaded)
     rng = np.random.default_rng(m)
     raw = np.empty((n * k // 32, 18), np.uint8)
-    raw[:, :2] = (rng.uniform(0.001, 0.02, n * k // 32)).astype(np.float16).view(np.uint8).reshape(-1, 2)
+    d = rng.uniform(0.001, 0.02, n * k // 32) * rng.choice([-1.0, 1.0], n * k // 32)
+    raw[:, :2] = d.astype(np.float16).view(np.uint8).reshape(-1, 2)
     raw[:, 2:] = rng.integers(0, 256, (n * k // 32, 16), dtype=np.uint8)
     raw[::7, 2:] = 0  # whole blocks of nibble 0 => -8*d
     raw = raw.reshape(-1)
@@ -120,7 +122,8 @@ def test_q4_gemm_large_m_accuracy(vx, m, n, k):
     2x2 f16 split keeps f32-grade accuracy (error ~ f32 summation-order noise, far below 1e-3)."""
     rng = np.random.default_rng(m + n)
     raw = np.empty((n * k // 32, 18), np.uint8)
-    raw[:, :2] = rng.uniform(0.002, 0.02, n * k // 32).astype(np.float16).view(np.uint8).reshape(-1, 2)
+    d = rng.uniform(0.002, 0.02, n * k // 32) * rng.choice([-1.0, 1.0], n * k // 32)
+    raw[:, :2] = d.astype(np.float16).view(np.uint8).reshape(-1, 2)
     raw[:, 2:] = rng.integers(0, 256, (n * k // 32, 16), dtype=np.uint8)
     raw = raw.reshape(-1)
     x = (rng.standard_normal((1, m, k)) * rng.uniform(0.1, 3.0, (1, m, 1))).astype(np.float32)

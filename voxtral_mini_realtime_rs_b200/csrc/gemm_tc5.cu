@@ -7,6 +7,11 @@
 //                              product, lo = the exact tail; their f16 bit patterns are assembled with shifts and masks
 //                              (g5_pack_f16x2) -- no half2 arithmetic and no conversion instructions (d' = d * 2^8 keeps lo
 //                              out of the subnormal range)
+//                              Domain: every block scale finite with |d| < 32.  The packing keeps only the low five bits
+//                              of the re-biased exponent, so (q-8)*d*2^8 must stay below 2^16: from |d| = 32 on, nibble 0
+//                              gives inf, NaN or a wrong finite weight without any error.  upload_q4 records the domain
+//                              (Q4Weight::d_below_32) and gemm_tc5_supported refuses weights outside it, which then take
+//                              the SIMT GEMM (f32 scale, any finite d).
 //   x * 2^s_t = x_h + x_m      f16 pieces, 22 bits; s_t = per-token power of two that puts the row maximum in [2^7, 2^8)
 // and the product is accumulated in f32 registers from the three largest terms
 //   w_hi x_h + w_hi x_m + w_lo x_h            (dropped: w_lo x_m ~ 2^-22 |w||x|, the f32 rounding level)
@@ -521,7 +526,10 @@ __global__ void __launch_bounds__(256) split_tiles_kernel(const float *__restric
 
 }  // namespace
 
-bool gemm_tc5_supported(const Q4Weight &w, int M) { return w.N % G5_BM == 0 && w.K % G5_BK == 0 && M >= 1; }
+// shape, and the scales' domain (header): a weight with a block scale |d| >= 32 would be silently wrong here
+bool gemm_tc5_supported(const Q4Weight &w, int M) {
+    return w.N % G5_BM == 0 && w.K % G5_BK == 0 && M >= 1 && w.d_below_32;
+}
 
 // f16 elements of the split buffer: two pieces of tiles + the per-token output scales (floats) behind them.  Rows are
 // padded to TT * g5_bn(M), which grows with M, so a buffer sized for M rows serves every smaller launch.
@@ -578,7 +586,8 @@ static void g5_launch(const G5Args &a, int epi, int grid, cudaStream_t st) {
 
 void launch_q4_gemm_tc5(const Q4Weight &w, const void *xt, int M, float *y, int ldy, const float *bias, const float *res,
                         int epi, const GemmWork *gw, cudaStream_t st) {
-    VOX_CHECK(gemm_tc5_supported(w, M), VOX_EINVAL, "gemm_tc5: unsupported shape N=%d K=%d", w.N, w.K);
+    VOX_CHECK(gemm_tc5_supported(w, M), VOX_EINVAL, "gemm_tc5: unsupported weight N=%d K=%d (or a block scale |d| >= 32)",
+              w.N, w.K);
     const GemmWork need = gemm_tc5_work_size();
     VOX_CHECK(gw && gw->partial && gw->counters && gw->partial_floats >= need.partial_floats && gw->n_counters >= need.n_counters,
               VOX_EINVAL, "gemm_tc5: split scratch missing or smaller than gemm_tc5_work_size()");

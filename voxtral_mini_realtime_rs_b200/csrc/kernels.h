@@ -46,6 +46,9 @@ struct Q4Weight {
     const uint4 *qs_tc = nullptr;  // [N/16][K/64][32]
     const uint2 *d_tc = nullptr;   // [N/16][K/64][8]
     int N = 0, K = 0;
+    // every block scale is finite with |d| < 32: the domain in which the wgmma GEMM's f16 split of (q-8)*d*2^8 is exact
+    // (gemm_tc5.cu); set by upload_q4, which sees the scales on the host
+    bool d_below_32 = false;
     size_t bytes() const { return (size_t)N * (K / 32) * 18; }
 };
 

@@ -88,6 +88,8 @@ Q4Weight upload_q4(DeviceArena &arena, const std::vector<const uint8_t *> &raw, 
     Q4Weight w;
     w.N = N;
     w.K = K;
+    // f16 bits: |d| < 32 <=> exponent field < 16 (0x5000 = 32.0); inf and NaN fail too
+    w.d_below_32 = std::all_of(ds.begin(), ds.end(), [](uint16_t h) { return (h & 0x7FFFu) < 0x5000u; });
     w.qs = (const uint4 *)arena.upload(qs.data(), qs.size());
     w.d = (const __half *)arena.upload(ds.data(), ds.size());
     if (tc_layout) build_tc_layout(arena, w, qs, ds);
