@@ -588,17 +588,10 @@ static int32_t transcribe_pcm_impl(Session *s, const float *host, const float *d
     VOX_CHECK(frames >= 1, VOX_EINVAL, "Audio too short to produce mel frames");
     VOX_CHECK(frames <= (size_t)s->max_mel_frames, VOX_EINVAL,
               "audio needs %zu mel frames > session max_mel_frames %d (chunk it: vox_chunk_plan)", frames, s->max_mel_frames);
-    if ((size_t)b * padded > s->pcm_pad_cap) {
-        s->pcm_pad = s->arena.alloc_n<float>((size_t)b * padded);
-        s->pcm_pad_cap = (size_t)b * padded;
-    }
+    s->reserve_pcm(host ? (size_t)b * n : 0, (size_t)b * padded);
     CUDA_OK(cudaEventRecord(s->ev[0], s->st));
     const float *src = dev;
     if (host) {
-        if ((size_t)b * n > s->pcm_cap) {
-            s->pcm = s->arena.alloc_n<float>((size_t)b * n);
-            s->pcm_cap = (size_t)b * n;
-        }
         CUDA_OK(cudaMemcpyAsync(s->pcm, host, sizeof(float) * (size_t)b * n, cudaMemcpyHostToDevice, s->st));
         src = s->pcm;
     }
@@ -645,7 +638,7 @@ int32_t vox_transcribe_pcm_ragged(vox_session *sh, const float *samples, const s
         int32_t n = 0;
         const int32_t rc = transcribe_pcm_impl(s, samples, nullptr, b, lens[0], normalize, out_ids, cap, &n, tm);
         for (int i = 0; i < b; ++i) n_out[i] = n;
-        s->pack_uniform_results(b, n);
+        s->scores_n = s->nbest_n = b * n;   // a ragged call reports the total over its streams
         if (s->beam_w == 1) {   // like a ragged call, leave the decoder cache empty
             s->reset();
             CUDA_OK(cudaStreamSynchronize(s->st));
@@ -769,31 +762,30 @@ int32_t vox_session_token_scores(vox_session *sh, int32_t *top_ids, float *top_l
     VOX_API_BEGIN
     REQUIRE(sh);
     Session *s = sh->s;
-    const int B = s->scores_b, N = s->scores_n, K = s->scores_k;
+    const int K = s->scores_k;
     VOX_CHECK(K > 0, VOX_EINVAL, "no token scores: the last transcribe, prefill or decode step ran with top_k 0 (vox_session_set_top_k)");
-    if (b) *b = B;
-    if (n) *n = N;
+    if (b) *b = (int32_t)s->score_spans.size();
+    if (n) *n = s->scores_n;
     if (k) *k = K;
     if (!top_ids && !top_logprobs) return VOX_OK;
     REQUIRE(top_ids); REQUIRE(top_logprobs);
-    const size_t need = (size_t)(s->packed_results ? 1 : B) * N * K;
+    size_t need = 0;
+    for (const Session::ScoreSpan &r : s->score_spans) need += (size_t)r.n * K;
     VOX_CHECK(cap >= need, VOX_ECAPACITY, "token scores capacity %zu < %zu", cap, need);
     CUDA_OK(cudaSetDevice(s->m->device));
     CUDA_OK(cudaStreamSynchronize(s->st));
-    if (s->packed_results) {   // vox_transcribe_pcm_ragged: N entries of K over all streams, already on the host
-        memcpy(top_ids, s->scores_host_ids.data(), sizeof(int32_t) * N * K);
-        memcpy(top_logprobs, s->scores_host_lp.data(), sizeof(float) * N * K);
-        return VOX_OK;
-    }
-    // row r's entries [p0, p0 + N) of the device's [row][out_ld][VOX_MAX_TOP_K] buffers, the first K of each
+    // one stream after the other: entries [pos0, pos0 + n) of its row of the device's [row][out_ld][VOX_MAX_TOP_K]
+    // buffers, the first K of each
     const size_t pitch = sizeof(int32_t) * VOX_MAX_TOP_K;
-    for (int r = 0; r < B && N > 0; ++r) {
-        const size_t at = ((size_t)r * s->out_ld + (s->scores_pos.empty() ? 0 : s->scores_pos[r])) * VOX_MAX_TOP_K;
-        const size_t dst = (size_t)r * N * K;
-        CUDA_OK(cudaMemcpy2D(top_ids + dst, sizeof(int32_t) * K, s->d_top_ids + at, pitch, sizeof(int32_t) * K, N,
+    size_t dst = 0;
+    for (const Session::ScoreSpan &r : s->score_spans) {
+        if (r.n == 0) continue;
+        const size_t at = ((size_t)r.row * s->out_ld + r.pos0) * VOX_MAX_TOP_K;
+        CUDA_OK(cudaMemcpy2D(top_ids + dst, sizeof(int32_t) * K, s->d_top_ids + at, pitch, sizeof(int32_t) * K, r.n,
                              cudaMemcpyDeviceToHost));
-        CUDA_OK(cudaMemcpy2D(top_logprobs + dst, sizeof(float) * K, s->d_top_lp + at, pitch, sizeof(float) * K, N,
+        CUDA_OK(cudaMemcpy2D(top_logprobs + dst, sizeof(float) * K, s->d_top_lp + at, pitch, sizeof(float) * K, r.n,
                              cudaMemcpyDeviceToHost));
+        dst += (size_t)r.n * K;
     }
     VOX_API_END
 }
@@ -808,24 +800,25 @@ int32_t vox_session_nbest(vox_session *sh, int32_t *ids, double *scores, size_t 
     VOX_API_BEGIN
     REQUIRE(sh);
     Session *s = sh->s;
-    const int B = s->nbest_b, W = s->nbest_w, N = s->nbest_n;
+    const int W = s->nbest_w;
     VOX_CHECK(W > 0, VOX_EINVAL, "no n-best list: the last transcribe ran at beam width 1 (vox_session_set_beam)");
-    if (b) *b = B;
+    if (b) *b = (int32_t)s->nbest_spans.size();
     if (w) *w = W;
-    if (n) *n = N;
+    if (n) *n = s->nbest_n;
     if (!ids && !scores) return VOX_OK;
     REQUIRE(ids); REQUIRE(scores);
-    const size_t need = (size_t)(s->packed_results ? 1 : B) * W * N;
+    size_t need = 0;
+    for (const Session::NbestSpan &r : s->nbest_spans) need += (size_t)W * r.n;
     VOX_CHECK(cap >= need, VOX_ECAPACITY, "n-best capacity %zu < %zu", cap, need);
     CUDA_OK(cudaSetDevice(s->m->device));
     CUDA_OK(cudaStreamSynchronize(s->st));
-    if (s->packed_results) {   // vox_transcribe_pcm_ragged: stream s's W x n_out[s] ids after stream s-1's
-        memcpy(ids, s->nbest_host_ids.data(), sizeof(int32_t) * W * N);
-        memcpy(scores, s->nbest_host_scores.data(), sizeof(double) * B * W);
-        return VOX_OK;
+    // one stream after the other: its W hypotheses of n ids each, and its W scores
+    for (const Session::NbestSpan &r : s->nbest_spans) {
+        if (r.n > 0) CUDA_OK(cudaMemcpy(ids, s->d_nbest_ids + r.ids, sizeof(int32_t) * W * r.n, cudaMemcpyDeviceToHost));
+        CUDA_OK(cudaMemcpy(scores, s->d_nbest_scores + r.scores, sizeof(double) * W, cudaMemcpyDeviceToHost));
+        ids += (size_t)W * r.n;
+        scores += W;
     }
-    if (N > 0) CUDA_OK(cudaMemcpy(ids, s->d_nbest_ids, sizeof(int32_t) * B * W * N, cudaMemcpyDeviceToHost));
-    CUDA_OK(cudaMemcpy(scores, s->d_nbest_scores, sizeof(double) * B * W, cudaMemcpyDeviceToHost));
     VOX_API_END
 }
 int32_t vox_session_cache_len(const vox_session *s, int32_t *len) {

@@ -647,8 +647,19 @@ void Session::bind_delays(const int *streams, int n) {
 
 void Session::bind_row_delays(int B) {
     std::vector<int> id(B);
-    for (int b = 0; b < B; ++b) id[b] = !row_streams.empty() ? row_streams[b] : beam_streams > 0 ? b % beam_streams : b;
+    for (int b = 0; b < B; ++b) id[b] = row_streams.empty() ? b : row_streams[b];
     bind_delays(id.data(), B);
+}
+
+void Session::reserve_pcm(size_t in_floats, size_t padded_floats) {
+    if (in_floats > pcm_cap) {
+        pcm = arena.alloc_n<float>(in_floats);
+        pcm_cap = in_floats;
+    }
+    if (padded_floats > pcm_pad_cap) {
+        pcm_pad = arena.alloc_n<float>(padded_floats);
+        pcm_pad_cap = padded_floats;
+    }
 }
 
 void Session::check_batch(int b) const { VOX_CHECK(b >= 1 && b <= max_batch, VOX_EINVAL, "batch %d exceeds session max_batch %d", b, max_batch); }
@@ -656,30 +667,13 @@ void Session::check_ids(const int32_t *ids, size_t n) const {
     for (size_t i = 0; i < n; ++i) VOX_CHECK(ids[i] >= 0 && ids[i] < m->info.vocab, VOX_EINVAL, "token id %d out of range", ids[i]);
 }
 
-// Q4VoxtralModel::encode_audio (model.rs:783-788): conv -> 32 layers -> norm -> reshape x4 -> adapter
-void Session::encode(int B, int T) {
+void Session::encoder_layers(int rows, const std::function<void(int)> &attn) {
     const vox_model_info &c = m->info;
-    check_batch(B);
-    VOX_CHECK(T >= 1 && T <= max_mel_frames, VOX_EINVAL, "mel frames %d exceed session max_mel_frames %d", T, max_mel_frames);
-    const int T1 = conv_out(T), S = conv_out(T1), S4 = S / c.reshape_factor;
-    const int d = c.enc_dim, hdq = c.enc_heads * c.enc_head_dim;
-    const int rows = B * S;
-    // conv1 + GELU as implicit GEMM over the time-major mel [B][T][128] (K = 3*128)
-    launch_conv2_gemm(mel_tm, m->conv1_w, m->conv1_b, h1, B, T, T1, c.n_mels, d, st);
-    launch_conv2_gemm(h1, m->conv2_w, m->conv2_b, x_enc, B, T1, S, d, d, st);
-    if (debug_capture && dbg_conv) CUDA_OK(cudaMemcpyAsync(dbg_conv, x_enc, sizeof(float) * rows * d, cudaMemcpyDeviceToDevice, st));
-    const float scale = powf((float)c.enc_head_dim, -0.5f);
+    const int d = c.enc_dim;
     for (int i = 0; i < c.enc_layers; ++i) {
         const EncLayerW &l = m->enc[i];
-        linear(l.wqkv, x_enc, rows, qkv_enc, 3 * hdq, l.bqkv, nullptr, EPI_NONE, l.attn_norm, h_enc);
-        launch_rope_inplace(qkv_enc, rows, 3 * hdq, 0, c.enc_heads, hdq, c.enc_heads, c.enc_head_dim, S, 0,
-                            m->enc_cos, m->enc_sin, st);
-        if (use_enc_attn_tc && enc_attention_tc_supported(c.enc_head_dim, 3 * hdq, 0, hdq, 2 * hdq))
-            launch_enc_attention_tc(qkv_enc, attn_enc, B, S, c.enc_heads, c.enc_head_dim, 3 * hdq, 0, hdq, 2 * hdq,
-                                    c.enc_window, scale, st);
-        else
-            launch_enc_attention(qkv_enc, attn_enc, B, S, c.enc_heads, c.enc_head_dim, 3 * hdq, 0, hdq, 2 * hdq,
-                                 c.enc_window, scale, st);
+        linear(l.wqkv, x_enc, rows, qkv_enc, 3 * c.enc_heads * c.enc_head_dim, l.bqkv, nullptr, EPI_NONE, l.attn_norm, h_enc);
+        attn(i);
         linear(l.wo, attn_enc, rows, x_enc, d, l.bo, x_enc, EPI_RESIDUAL);
         linear(l.w13, x_enc, rows, act_enc, c.enc_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, h_enc);
         linear(l.w2, act_enc, rows, x_enc, d, l.b2, x_enc, EPI_RESIDUAL);
@@ -688,6 +682,30 @@ void Session::encode(int B, int T) {
                                     cudaMemcpyDeviceToDevice, st));
     }
     launch_rmsnorm(x_enc, m->enc_norm, h_enc, rows, d, m->norm_eps, st);
+}
+
+void Session::enc_rope_attention(int rows, int B, int S, const int *seg) {
+    const vox_model_info &c = m->info;
+    const int H = c.enc_heads, hd = c.enc_head_dim, hdq = H * hd;
+    const float scale = powf((float)hd, -0.5f);
+    launch_rope_inplace(qkv_enc, rows, 3 * hdq, 0, H, hdq, H, hd, S, 0, m->enc_cos, m->enc_sin, st, seg, seg ? B : 0);
+    const bool tc = use_enc_attn_tc && enc_attention_tc_supported(hd, 3 * hdq, 0, hdq, 2 * hdq);
+    (tc ? launch_enc_attention_tc : launch_enc_attention)(qkv_enc, attn_enc, B, S, H, hd, 3 * hdq, 0, hdq, 2 * hdq, c.enc_window,
+                                                          scale, st, seg);
+}
+
+// Q4VoxtralModel::encode_audio (model.rs:783-788): conv -> 32 layers -> norm -> reshape x4 -> adapter
+void Session::encode(int B, int T) {
+    const vox_model_info &c = m->info;
+    check_batch(B);
+    VOX_CHECK(T >= 1 && T <= max_mel_frames, VOX_EINVAL, "mel frames %d exceed session max_mel_frames %d", T, max_mel_frames);
+    const int T1 = conv_out(T), S = conv_out(T1), S4 = S / c.reshape_factor;
+    const int d = c.enc_dim, rows = B * S;
+    // conv1 + GELU as implicit GEMM over the time-major mel [B][T][128] (K = 3*128)
+    launch_conv2_gemm(mel_tm, m->conv1_w, m->conv1_b, h1, B, T, T1, c.n_mels, d, st);
+    launch_conv2_gemm(h1, m->conv2_w, m->conv2_b, x_enc, B, T1, S, d, d, st);
+    if (debug_capture && dbg_conv) CUDA_OK(cudaMemcpyAsync(dbg_conv, x_enc, sizeof(float) * rows * d, cudaMemcpyDeviceToDevice, st));
+    encoder_layers(rows, [&](int) { enc_rope_attention(rows, B, S, nullptr); });
     cur_B = B;
     cur_S = S;
     cur_S4 = S4;
@@ -937,7 +955,8 @@ void Session::alloc_scores() {
 
 // after the step's argmax and counter advance: row b's scores land at its output position d_outpos[b] - 1
 void Session::token_scores(int B) {
-    const int k = std::max(top_k, beam_streams > 0 ? beam_w : 0);
+    // at W > 1 every step belongs to a beam call (the incremental calls refuse to run), whose selection reads W candidates
+    const int k = std::max(top_k, beam_w > 1 ? beam_w : 0);
     if (k > 0) launch_token_scores(logits, B, m->info.vocab, k, d_outpos, out_ld, d_top_ids, d_top_lp, score_work, st);
 }
 
@@ -1075,11 +1094,9 @@ void Session::step_incremental(int b, int M, const int *ids_host, bool add_audio
     else mega_steps_host += decode_step(b, add_audio);
     cache_len += M;
     scores_k = top_k;
-    scores_b = b;
     scores_n = 1;
-    scores_pos.resize(b);
-    for (int r = 0; r < b; ++r) scores_pos[r] = out_rows[r]++;   // each row's output just emitted
-    packed_results = false;
+    score_spans.resize(b);
+    for (int r = 0; r < b; ++r) score_spans[r] = {r, out_rows[r]++, 1};   // each row's output just emitted
 }
 
 void Session::reset() {
@@ -1150,17 +1167,23 @@ void Session::run_steps(int R, int n, Step step) {
     }
 }
 
+namespace {
+// the rows of a transcribe call map to their streams for that call only, also when it throws
+struct RowStreams {
+    Session *s;
+    ~RowStreams() { s->row_streams.clear(); }
+};
+}  // namespace
+
 // Q4VoxtralModel::transcribe_streaming (model.rs:873-963).  Expects the mel in s->mel; records
 // ev[1] (after encode) and ev[2] (after decode) on the stream.  Returns tokens per stream.
 int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids, vox_timings *tm) {
     const vox_model_info &c = m->info;
     const int W = beam_w, R = B * W;   // decode rows: beam w of stream s in row w * B + s
     VOX_CHECK(W == 1 || R <= max_batch, VOX_EINVAL, "beam width %d x %d streams exceeds session max_batch %d", W, B, max_batch);
-    struct BeamRows {   // the rows map to their streams for this call only, also when it throws
-        Session *s;
-        ~BeamRows() { s->beam_streams = 0; }
-    } beam_rows{this};
-    beam_streams = W > 1 ? B : 0;
+    RowStreams row_guard{this};
+    if (W > 1)
+        for (int r = 0; r < R; ++r) row_streams.push_back(r % B);
     encode(B, T);
     CUDA_OK(cudaEventRecord(ev[2], st));
     const int S4 = cur_S4, P = c.prefix_len;
@@ -1193,10 +1216,6 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
     CUDA_OK(cudaStreamSynchronize(st));
     for (int b = 0; b < B; ++b)
         for (int i = 0; i < n_out; ++i) out_ids[(size_t)b * n_out + i] = host[(size_t)b * out_ld + i];
-    nbest_b = B;
-    nbest_w = W > 1 ? W : 0;
-    nbest_n = n_out;
-    packed_results = false;
     if (W > 1) {
         // the cache holds W hypotheses per stream, not one: the incremental API starts over, on the identity page table
         reset();
@@ -1207,9 +1226,14 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
             for (int b = 0; b < B; ++b) out_rows[b] = std::max(n_out, 1);
     }
     scores_k = top_k;
-    scores_b = B;
-    scores_n = n_out;
-    scores_pos.clear();
+    nbest_w = W > 1 ? W : 0;
+    scores_n = nbest_n = n_out;
+    score_spans.resize(B);
+    nbest_spans.resize(B);
+    for (int b = 0; b < B; ++b) {   // stream b's rank 0 beam is row b, the traceback's ids are [B][W][n_out]
+        score_spans[b] = {b, 0, n_out};
+        nbest_spans[b] = {(size_t)b * W * n_out, b * W, n_out};
+    }
     if (tm) {
         tm->seq_len = S4;
         tm->decode_tokens = n_out;
@@ -1227,7 +1251,7 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
 void Session::encode_ragged(int b, const int *T, const std::vector<std::vector<int>> &audio_rows) {
     const vox_model_info &c = m->info;
     check_batch(b);
-    const int d = c.enc_dim, hdq = c.enc_heads * c.enc_head_dim, f = c.reshape_factor, D = c.dec_dim;
+    const int d = c.enc_dim, f = c.reshape_factor, D = c.dec_dim;
     std::vector<int> T1(b), S(b), S4(b);
     seg_host.assign(b + 1, 0);
     int S_long = 0, sum_T = 0, sum_S4 = 0, n_rows = 0;
@@ -1256,26 +1280,7 @@ void Session::encode_ragged(int b, const int *T, const std::vector<std::vector<i
         launch_conv2_gemm(h1 + (size_t)t1 * d, m->conv2_w, m->conv2_b, x_enc + (size_t)seg_host[i] * d, 1, T1[i], S[i], d, d, st);
     }
     if (debug_capture && dbg_conv) CUDA_OK(cudaMemcpyAsync(dbg_conv, x_enc, sizeof(float) * rows * d, cudaMemcpyDeviceToDevice, st));
-    const float scale = powf((float)c.enc_head_dim, -0.5f);
-    for (int i = 0; i < c.enc_layers; ++i) {
-        const EncLayerW &l = m->enc[i];
-        linear(l.wqkv, x_enc, rows, qkv_enc, 3 * hdq, l.bqkv, nullptr, EPI_NONE, l.attn_norm, h_enc);
-        launch_rope_inplace(qkv_enc, rows, 3 * hdq, 0, c.enc_heads, hdq, c.enc_heads, c.enc_head_dim, S_long, 0,
-                            m->enc_cos, m->enc_sin, st, d_seg, b);
-        if (use_enc_attn_tc && enc_attention_tc_supported(c.enc_head_dim, 3 * hdq, 0, hdq, 2 * hdq))
-            launch_enc_attention_tc(qkv_enc, attn_enc, b, S_long, c.enc_heads, c.enc_head_dim, 3 * hdq, 0, hdq, 2 * hdq,
-                                    c.enc_window, scale, st, d_seg);
-        else
-            launch_enc_attention(qkv_enc, attn_enc, b, S_long, c.enc_heads, c.enc_head_dim, 3 * hdq, 0, hdq, 2 * hdq,
-                                 c.enc_window, scale, st, d_seg);
-        linear(l.wo, attn_enc, rows, x_enc, d, l.bo, x_enc, EPI_RESIDUAL);
-        linear(l.w13, x_enc, rows, act_enc, c.enc_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, h_enc);
-        linear(l.w2, act_enc, rows, x_enc, d, l.b2, x_enc, EPI_RESIDUAL);
-        if (debug_capture && dbg_layers)
-            CUDA_OK(cudaMemcpyAsync(dbg_layers + (size_t)i * rows * d, x_enc, sizeof(float) * rows * d,
-                                    cudaMemcpyDeviceToDevice, st));
-    }
-    launch_rmsnorm(x_enc, m->enc_norm, h_enc, rows, d, m->norm_eps, st);
+    encoder_layers(rows, [&](int) { enc_rope_attention(rows, b, S_long, d_seg); });
     enc_rows = rows;
     cur_B = n_rows;
     cur_S = S_max;
@@ -1295,6 +1300,14 @@ void Session::encode_ragged(int b, const int *T, const std::vector<std::vector<i
 // Streams sorted (stably) by decreasing output count own the rows: beams w of sorted stream i run in row i * W + w, so
 // the streams that still need tokens are always the rows [0, R).  Every stream with output takes the prefill; then the
 // steps run in segments, one per distinct output count, each over the rows still live.
+//
+// transcribe_from_mel is not this function at equal lengths, and moving it here would change what it costs and computes:
+//   - it prefills b rows and replicates them to the beam rows (beam_start).  Here the rows are stream-major, so that the
+//     live streams stay a prefix of the rows; a prefill row is then both a fork source and another stream's fork
+//     destination, and all b * W rows take the prefill: the prefill GEMMs' M grows W-fold (38 -> 304 at 1 stream x 8
+//     beams; not measured for that case).
+//   - another beam row layout moves a beam into another group of 8 rows when b * W > 8.  The persistent kernel's
+//     attn_chunks follows the group's row count, so the softmax merge order, and with it the low bits, would change.
 void Session::transcribe_ragged(const float *samples, const size_t *lens, int b, int normalize, int32_t *out_ids,
                                 int32_t *n_out, vox_timings *tm) {
     const vox_model_info &c = m->info;
@@ -1315,24 +1328,14 @@ void Session::transcribe_ragged(const float *samples, const size_t *lens, int b,
         pad_off[s + 1] = pad_off[s] + (g[s].padded + 3) / 4 * 4;   // each stream's padded signal 16-byte aligned
     }
     CUDA_OK(cudaSetDevice(m->device));
-    if (pad_off[b] > pcm_pad_cap) {
-        pcm_pad = arena.alloc_n<float>(pad_off[b]);
-        pcm_pad_cap = pad_off[b];
-    }
-    if (in_off[b] > pcm_cap) {
-        pcm = arena.alloc_n<float>(in_off[b]);
-        pcm_cap = in_off[b];
-    }
+    reserve_pcm(in_off[b], pad_off[b]);
     std::vector<int> order(b);
     for (int s = 0; s < b; ++s) order[s] = s;
     std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return g[x].n_out > g[y].n_out; });
     int live = 0;
     while (live < b && g[order[live]].n_out > 0) ++live;
     std::vector<std::vector<int>> rows(b);
-    struct RaggedRows {   // the rows map to their streams for this call only, also when it throws
-        Session *s;
-        ~RaggedRows() { s->row_streams.clear(); s->beam_streams = 0; }
-    } ragged_rows{this};
+    RowStreams row_guard{this};
     row_streams.assign((size_t)b * W, 0);
     for (int i = 0; i < b; ++i)
         for (int w = 0; w < W; ++w) {
@@ -1355,7 +1358,6 @@ void Session::transcribe_ragged(const float *samples, const size_t *lens, int b,
     const int n_max = live > 0 ? g[order[0]].n_out : 0;
     reset();
     if (live > 0) {
-        beam_streams = W > 1 ? live : 0;
         const int R0 = live * W;
         // prefix = [BOS] + [STREAMING_PAD]*37 (model.rs:883-892) in every row, each beam row of a stream included: the
         // first selection then reads one parent row per stream (its rank 0) and forks it into the others
@@ -1398,88 +1400,37 @@ void Session::transcribe_ragged(const float *samples, const size_t *lens, int b,
     }
     CUDA_OK(cudaEventRecord(ev[3], st));
 
-    // results back in the caller's stream order: stream s's outputs are in the row of its rank 0 beam, rows[s][0]
-    std::vector<size_t> out_off(b + 1, 0);
-    for (int s = 0; s < b; ++s) out_off[s + 1] = out_off[s] + g[s].n_out;
-    const size_t total = out_off[b];
+    if (W > 1 && live < b)   // a stream without output has no hypotheses: scores 0
+        CUDA_OK(cudaMemsetAsync(d_nbest_scores + live * W, 0, sizeof(double) * (b - live) * W, st));
+
+    // ids back in the caller's stream order: stream s's outputs are in the row of its rank 0 beam, rows[s][0]
     std::vector<int> host((size_t)live * W * out_ld);
     if (live > 0) CUDA_OK(cudaMemcpyAsync(host.data(), d_out, sizeof(int) * host.size(), cudaMemcpyDeviceToHost, st));
     CUDA_OK(cudaStreamSynchronize(st));
-    for (int s = 0; s < b; ++s)
-        for (int i = 0; i < g[s].n_out; ++i) out_ids[out_off[s] + i] = host[(size_t)rows[s][0] * out_ld + i];
-    scores_host_ids.clear();
-    scores_host_lp.clear();
-    if (top_k > 0) {
-        const int K = top_k;
-        scores_host_ids.resize(total * K);
-        scores_host_lp.resize(total * K);
-        const size_t pitch = sizeof(int) * TOPK_MAX;
-        for (int s = 0; s < b; ++s) {
-            if (g[s].n_out == 0) continue;
-            const size_t at = (size_t)rows[s][0] * out_ld * TOPK_MAX, dst = out_off[s] * K;
-            CUDA_OK(cudaMemcpy2D(scores_host_ids.data() + dst, sizeof(int) * K, d_top_ids + at, pitch, sizeof(int) * K, g[s].n_out,
-                                 cudaMemcpyDeviceToHost));
-            CUDA_OK(cudaMemcpy2D(scores_host_lp.data() + dst, sizeof(float) * K, d_top_lp + at, pitch, sizeof(float) * K, g[s].n_out,
-                                 cudaMemcpyDeviceToHost));
-        }
-    }
-    nbest_host_ids.clear();
-    nbest_host_scores.clear();
-    if (W > 1) {
-        // the tracebacks packed sorted stream i's W hypotheses after those of sorted stream i - 1
-        std::vector<int> packed_ids(total * W);
-        std::vector<double> packed_scores((size_t)live * W);
-        if (total > 0) CUDA_OK(cudaMemcpy(packed_ids.data(), d_nbest_ids, sizeof(int) * packed_ids.size(), cudaMemcpyDeviceToHost));
-        if (live > 0)
-            CUDA_OK(cudaMemcpy(packed_scores.data(), d_nbest_scores, sizeof(double) * packed_scores.size(), cudaMemcpyDeviceToHost));
-        nbest_host_ids.resize(total * W);
-        nbest_host_scores.assign((size_t)b * W, 0.0);
-        for (int i = 0, off = 0; i < live; off += W * g[order[i]].n_out, ++i) {
-            const int s = order[i];
-            std::copy(packed_ids.begin() + off, packed_ids.begin() + off + (size_t)W * g[s].n_out,
-                      nbest_host_ids.begin() + out_off[s] * W);
-            for (int w = 0; w < W; ++w) nbest_host_scores[(size_t)s * W + w] = packed_scores[(size_t)i * W + w];
-        }
+    size_t total = 0;
+    for (int s = 0; s < b; total += g[s].n_out, ++s)
+        for (int i = 0; i < g[s].n_out; ++i) out_ids[total + i] = host[(size_t)rows[s][0] * out_ld + i];
+    // scores and n-best stay on the device: the tracebacks packed sorted stream i's W hypotheses after those of sorted
+    // stream i - 1, and its W scores at i * W
+    scores_k = top_k;
+    nbest_w = W > 1 ? W : 0;
+    scores_n = nbest_n = (int)total;
+    score_spans.resize(b);
+    nbest_spans.resize(b);
+    for (size_t i = 0, off = 0; i < (size_t)b; off += (size_t)W * g[order[i]].n_out, ++i) {
+        const int s = order[i];
+        score_spans[s] = {rows[s][0], 0, g[s].n_out};
+        nbest_spans[s] = {off, (int)i * W, g[s].n_out};
     }
     // the cache holds streams of different lengths (and perhaps beams): the incremental API starts over
     reset();
     CUDA_OK(cudaStreamSynchronize(st));
-    nbest_b = b;
-    nbest_w = W > 1 ? W : 0;
-    nbest_n = (int)total;
-    scores_k = top_k;
-    scores_b = b;
-    scores_n = (int)total;
-    scores_pos.clear();
-    packed_results = true;
     if (tm) {
         int S4_long = 0;
         for (const StreamGeom &x : g) S4_long = std::max(S4_long, x.S4);
         tm->seq_len = S4_long;
         tm->decode_tokens = n_max;
     }
-}
-
-void Session::pack_uniform_results(int b, int n) {
-    const int K = scores_k, W = nbest_w;
-    scores_host_ids.assign((size_t)b * n * K, 0);
-    scores_host_lp.assign((size_t)b * n * K, 0.0f);
-    CUDA_OK(cudaStreamSynchronize(st));
-    for (int r = 0; r < b && n > 0 && K > 0; ++r) {   // row r's positions [0, n)
-        const size_t at = (size_t)r * out_ld * TOPK_MAX, dst = (size_t)r * n * K;
-        CUDA_OK(cudaMemcpy2D(scores_host_ids.data() + dst, sizeof(int) * K, d_top_ids + at, sizeof(int) * TOPK_MAX, sizeof(int) * K,
-                             n, cudaMemcpyDeviceToHost));
-        CUDA_OK(cudaMemcpy2D(scores_host_lp.data() + dst, sizeof(float) * K, d_top_lp + at, sizeof(float) * TOPK_MAX,
-                             sizeof(float) * K, n, cudaMemcpyDeviceToHost));
-    }
-    nbest_host_ids.assign((size_t)b * W * n, 0);
-    nbest_host_scores.assign((size_t)b * W, 0.0);
-    if (W > 0) {   // [b][W][n]: already stream after stream
-        if (n > 0) CUDA_OK(cudaMemcpy(nbest_host_ids.data(), d_nbest_ids, sizeof(int) * nbest_host_ids.size(), cudaMemcpyDeviceToHost));
-        CUDA_OK(cudaMemcpy(nbest_host_scores.data(), d_nbest_scores, sizeof(double) * nbest_host_scores.size(), cudaMemcpyDeviceToHost));
-    }
-    scores_n = nbest_n = b * n;
-    packed_results = true;
 }
 
 }  // namespace vox

@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 
 #include <cstdint>
+#include <functional>
 #include <string>
 #include <tuple>
 #include <vector>
@@ -130,6 +131,7 @@ struct Session {
     // audio
     float *pcm = nullptr, *pcm_pad = nullptr, *peak_scale = nullptr;
     size_t pcm_cap = 0, pcm_pad_cap = 0;
+    void reserve_pcm(size_t in_floats, size_t padded_floats);   // grows pcm / pcm_pad to hold that much
     float *mel = nullptr;     // [B][128][T] as handed in by callers (reference layout)
     float *mel_tm = nullptr;  // [B][T][128] time-major copy consumed by the conv1 implicit GEMM
     // encoder workspace
@@ -180,34 +182,33 @@ struct Session {
     ScoreWork score_work;
     void set_top_k(int k);
     void alloc_scores();        // the score buffers above (first use)
-    // launch over rows [0, B) of the step that just ran at k = max(top_k, beam width of a running beam call); no-op at 0
+    // launch over rows [0, B) of the step that just ran at k = max(top_k, beam width when it is > 1); no-op at 0
     void token_scores(int B);
     // beam search (vox_session_set_beam): beam_w beams per stream for the transcribe calls; 1 = greedy (no launch, no
     // memory).  A call over b streams at W > 1 runs rows w * b + s (beam w of stream s; kernels.h BeamWork), allocated
     // with the n-best results by the first set_beam(W > 1).
     int beam_w = 1;
-    int beam_streams = 0;           // > 0 while a beam call runs: row r belongs to stream r % beam_streams
-    std::vector<int> row_streams;   // non-empty while a ragged call runs: row r belongs to stream row_streams[r]
+    // the stream of each decoder row while a transcribe call runs whose rows are not its streams in order (beams, a
+    // ragged call's sorted streams); empty: row r belongs to stream r
+    std::vector<int> row_streams;
     BeamWork beam;
-    int *d_nbest_ids = nullptr;     // [b][W][n] of the last transcribe
+    int *d_nbest_ids = nullptr;     // every stream's [W][n] ids of the last transcribe, at NbestSpan::ids
     double *d_nbest_scores = nullptr;
-    int nbest_b = 0, nbest_w = 0, nbest_n = 0;   // nbest_w == 0: the last transcribe ran greedy
     bool page_table_forked = false; // a beam call has rewritten page-table rows: reset() re-uploads the identity table
     void set_beam(int w);
     void beam_start(int b);         // after the prefill of rows [0, b): replicate them to every beam row, select position 0
     void beam_step(int b, int n_live);   // selection + KV fork after a step over the b * beam_w rows
-    // what vox_session_token_scores returns: the last transcribe (positions [0, n) of `b` rows) or incremental call (the
-    // position `step_pos` of each row), scored with k = scores_k (0: that call ran with scores off)
-    int scores_k = 0, scores_b = 0, scores_n = 0;
-    std::vector<int> scores_pos;    // per row, empty after a transcribe
-    // packed_results: the last transcribe was vox_transcribe_pcm_ragged, whose scores and n-best lists are kept here
-    // packed in the caller's stream order (stream s's entries after stream s-1's; scores_n / nbest_n their total count)
-    bool packed_results = false;
-    std::vector<int> scores_host_ids, nbest_host_ids;
-    std::vector<float> scores_host_lp;
-    std::vector<double> nbest_host_scores;
-    // packs the results of transcribe_from_mel over b streams of n outputs each like a ragged call's
-    void pack_uniform_results(int b, int n);
+    // Where the results of the last call are, per stream in the caller's order; the getters copy them from the device
+    // when asked (the buffers outlive reset()).  Token scores, of the last transcribe or incremental call: entries
+    // [pos0, pos0 + n) of row `row` of d_top_ids / d_top_lp, scored with k = scores_k (0: that call ran with scores
+    // off).  N-best lists, of the last transcribe: W x n ids at d_nbest_ids + ids, W scores at d_nbest_scores + scores
+    // (nbest_w == 0: that transcribe ran greedy).  scores_n / nbest_n are the counts the getters report: per stream, or
+    // the total over the streams after vox_transcribe_pcm_ragged.
+    struct ScoreSpan { int row, pos0, n; };
+    struct NbestSpan { size_t ids; int scores, n; };
+    std::vector<ScoreSpan> score_spans;
+    std::vector<NbestSpan> nbest_spans;
+    int scores_k = 0, scores_n = 0, nbest_w = 0, nbest_n = 0;
     // host mirror of d_outpos[] outside stream mode: outputs per row since reset (incremental calls / transcribe)
     std::vector<int> out_rows;
     StepGraph step_graph;   // the offline transcription's decode step, captured once per key and replayed
@@ -270,10 +271,16 @@ struct Session {
     // streams' sets.  Launch-free, and copy-free when the row-to-stream mapping has not changed (so it may run inside a
     // stream capture); a delay change rewrites the sets in place and needs no new binding.
     void bind_delays(const int *streams, int n);
-    // row b = stream b, or stream b % beam_streams during a beam call (every call but the stream pool's)
+    // rows [0, B) as row_streams maps them (every call but the stream pool's)
     void bind_row_delays(int B);
     // mel already on device, time-major, in s->mel_tm
     void encode(int B, int T);
+    // The encoder layers over `rows` rows of x_enc, then the final norm into h_enc.  attn(layer) is the step between the
+    // layer's wqkv and wo: RoPE and attention from qkv_enc into attn_enc.
+    void encoder_layers(int rows, const std::function<void(int)> &attn);
+    // that step for B streams of up to S rows each: one after the other S rows apart, or, with a segment table `seg`
+    // (device, [B + 1]), packed at seg[b]
+    void enc_rope_attention(int rows, int B, int S, const int *seg);
     // launch_q4_linear with the session's GEMM scratch and path choice; `gamma`, `tmp`, `tc` and `ada_rows` as there
     void linear(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias, const float *res,
                 int epi, const float *gamma = nullptr, float *tmp = nullptr, const TcWork *tc = nullptr,

@@ -312,12 +312,10 @@ size_t StreamPool::poll(int id, int32_t *ids, int32_t *top_ids, float *top_lp, s
 // Encoder layers over `R` gathered rows in s->x_enc (Q4EncoderLayer::forward_with_cache, model.rs:300-315).
 void StreamPool::encoder_rows(int R) {
     const vox_model_info &c = m->info;
-    const int d = c.enc_dim, HQ = c.enc_heads * c.enc_head_dim;
+    const int HQ = c.enc_heads * c.enc_head_dim;
     const float scale = powf((float)c.enc_head_dim, -0.5f);
     const size_t ring_stride = (size_t)max_sessions * ring * HQ;
-    for (int i = 0; i < c.enc_layers; ++i) {
-        const EncLayerW &l = m->enc[i];
-        s->linear(l.wqkv, s->x_enc, R, s->qkv_enc, 3 * HQ, l.bqkv, nullptr, EPI_NONE, l.attn_norm, s->h_enc);
+    s->encoder_layers(R, [&](int i) {
         stream_rope_append_kernel<<<R, 256, 0, s->st>>>(s->qkv_enc, 3 * HQ, c.enc_heads, c.enc_head_dim, d_row_slot, d_row_pos,
                                                         ek + i * ring_stride, ev + i * ring_stride, ring,
                                                         unbounded ? enc_rope_cos : m->enc_cos, unbounded ? enc_rope_sin : m->enc_sin,
@@ -325,11 +323,7 @@ void StreamPool::encoder_rows(int R) {
         cuda_check(cudaGetLastError(), "stream_rope_append launch");
         launch_stream_attn(s->qkv_enc, R, 3 * HQ, c.enc_heads, c.enc_head_dim, d_row_slot, d_row_pos, ek + i * ring_stride,
                            ev + i * ring_stride, ring, c.enc_window, scale, s->attn_enc, s->st);
-        s->linear(l.wo, s->attn_enc, R, s->x_enc, d, l.bo, s->x_enc, EPI_RESIDUAL);
-        s->linear(l.w13, s->x_enc, R, s->act_enc, c.enc_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, s->h_enc);
-        s->linear(l.w2, s->act_enc, R, s->x_enc, d, l.b2, s->x_enc, EPI_RESIDUAL);
-    }
-    launch_rmsnorm(s->x_enc, m->enc_norm, s->h_enc, R, d, m->norm_eps, s->st);
+    });
 }
 
 void StreamPool::ensure_pages(Slot &sl, int positions) {
