@@ -233,6 +233,9 @@ int32_t vox_forward_streaming(vox_session *s, const float *mel, int32_t b, int32
  * [B][M][vocab] logits to the host).
  * vox_prefill: ids [B][M] at cache positions len..len+M-1; add_audio != 0 adds the session's audio embeddings of
  * those positions (after vox_encode_audio; model.rs:894-903); next_tok [B] (nullable) = argmax of the last row.
+ * After vox_transcribe_pcm_ragged, row i reads the call's stream i (caller order), B must be its stream count and
+ * only positions every stream has are allowed (those of the shortest stream), else VOX_EINVAL; the same for
+ * vox_decode_step.
  * vox_decode_step: one position; tok [B] NULL = use the device-side token left by the previous call;
  * next_tok NULL with tok NULL = fully asynchronous (no host sync). */
 int32_t vox_prefill(vox_session *s, const int32_t *ids, int32_t b, int32_t m, int32_t add_audio, int32_t *next_tok);

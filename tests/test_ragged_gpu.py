@@ -12,6 +12,8 @@ ragged calls).
     reference run on each stream alone: packed encoder output and audio embeddings, tensor-core and SIMT attention.
   * Rows retire: persistent-kernel launches per step = ceil(live rows / 8), and max n_out - 1 steps.
   * Per-stream delays, token scores and beams (W = 2, 4) compose.
+  * After a ragged call, vox_prefill / vox_decode_step with add_audio read the streams in the caller's order, up to the
+    shortest stream's positions.
   * transcribe_long equals per-chunk vox_transcribe_pcm of the host-normalised chunks (overlap 0 and > 0).
   * Bad arguments are refused before device work and leave the session usable; a ragged call leaves the cache empty.
 """
@@ -22,7 +24,7 @@ import pytest
 import torch
 
 from oracle import mel as omel
-from oracle.model import OracleModel
+from oracle.model import PREFIX_LEN, OracleModel
 from test_encoder_geometry_ref import EMBED_REL_BOUND, encoder_geometry_bytes, rel_err
 from test_golden_gpu import NEAR_TIE, assert_ids_match
 from voxtral_mini_realtime_rs_b200 import synth
@@ -220,13 +222,46 @@ def test_beams_compose(vx, tiny, W):
     print(f"\n[ragged] W={W}: every stream's n-best equals its single-stream beam call")
 
 
+def test_add_audio_after_ragged_call_reads_caller_order(vx, tiny):
+    """Streams given shortest first, so the caller's order is the reverse of the sorted decoder rows.  A prefill and
+    decode steps teacher-forced along the ragged ids, with add_audio, read stream i's embeddings in row i: they give
+    stream i's ragged ids (near-tie runner-ups allowed), up to the shortest stream's positions, and refuse the next."""
+    lens = [9000, 21000 + 160 * 7, 44000]
+    audios = [_stream(n, 1000 + i) for i, n in enumerate(lens)]
+    b = len(audios)
+    tiny.set_top_k(2)
+    try:
+        ids = tiny.transcribe_pcm_ragged(audios)
+        sc = tiny.token_scores_ragged()
+    finally:
+        tiny.set_top_k(0)
+    assert ids[0].size < ids[1].size < ids[2].size
+    n = ids[0].size   # the shortest stream's S4 is PREFIX_LEN + n
+    try:
+        got = [tiny.prefill(np.tile([1] + [32] * (PREFIX_LEN - 1), (b, 1)), add_audio=True)]
+        for t in range(1, n + 1):   # position PREFIX_LEN + n - 1 has audio too; its id is the one no call emits
+            got.append(tiny.decode_step(tok=[x[t - 1] for x in ids], add_audio=True))
+        assert tiny.cache_len() == PREFIX_LEN + n
+        with pytest.raises(vx.VoxtralError) as e:
+            tiny.decode_step(tok=[x[n - 1] for x in ids], add_audio=True)
+        assert e.value.code == 1
+    finally:
+        tiny.reset_cache()
+    got = np.stack(got[:n], 1)
+    for i in range(b):
+        top, lp = sc[i]
+        for j in np.nonzero(got[i] != ids[i][:n])[0]:
+            assert lp[j, 0] - lp[j, 1] < NEAR_TIE and got[i][j] == top[j, 1], (i, j)
+        print(f"\n[ragged] add_audio after a ragged call: stream {i} {int((got[i] == ids[i][:n]).sum())}/{n} ids equal")
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 def _gpu_mel(vx, audio):
     return vx.MelSpectrogram.voxtral(0).compute_log(vx.pad_audio(audio)).T[None]
 
 
 @pytest.mark.parametrize("attn", ["enc_attn_tc", "enc_attn_simt"])
-def test_ragged_encoder_vs_f64(vx, attn):
+def test_ragged_encoder_packed_embeds_vs_f64(vx, attn):
     """Window 750: streams of 30, 16 and 7 s (S = 938, 588, 363 encoder frames): the window bites inside the first."""
     data = encoder_geometry_bytes(750)
     m = vx.Q4ModelLoader.from_bytes(data).load(0, max_batch=3, max_mel_frames=4000)
@@ -240,10 +275,8 @@ def test_ragged_encoder_vs_f64(vx, attn):
             m.debug("enc_attn_tc")
         d, D = o64.cfg.enc_dim, o64.cfg.dec_dim
         enc = m.debug("enc_out").reshape(-1, d)
-        emb = m.debug("audio_embeds").reshape(3, -1, D)   # rows in decreasing-length order, S4_max apart
-        n_out = [vx.stream_n_out(a.size) for a in audios]
-        order = sorted(range(3), key=lambda i: -n_out[i])
-        r0 = 0
+        emb = m.debug("audio_embeds").reshape(-1, D)   # stream after stream, in the caller's order
+        r0 = e0 = 0
         for i, a in enumerate(audios):
             mel = _gpu_mel(vx, a)
             cap = {}
@@ -252,12 +285,13 @@ def test_ragged_encoder_vs_f64(vx, attn):
             S = ref_enc.shape[0]
             got_enc = enc[r0:r0 + S]
             r0 += S
-            got_emb = emb[order.index(i), :ref_emb.shape[0]]
+            got_emb = emb[e0:e0 + ref_emb.shape[0]]
+            e0 += ref_emb.shape[0]
             e1, e2 = rel_err(got_enc, ref_enc), rel_err(got_emb, ref_emb)
             print(f"\n[ragged encoder] {attn} stream {i} S={S}: enc_out {e1:.2e}, embeds {e2:.2e} (bound {EMBED_REL_BOUND:.0e})")
             assert S > 750 or i > 0
             assert e1 <= EMBED_REL_BOUND and e2 <= EMBED_REL_BOUND
-        assert r0 == enc.shape[0]
+        assert r0 == enc.shape[0] and e0 == emb.shape[0]
     finally:
         m.close()
 

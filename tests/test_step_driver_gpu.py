@@ -5,7 +5,8 @@ Model: the production decoder geometry (test_decode_geometry_ref.geometry_model_
 - The captured step reads the op table the host built for its token capacity; an incremental call at another row count
   rebuilds that table in between, so a later replay must find the table of its own capacity again.
 - Every host-side choice the captured kernels depend on is in the graph's key: the per-op path at 11 rows (the wgmma
-  GEMM) is captured again after gemm_simt.
+  GEMM) is captured again after gemm_simt.  The streams' length is not: the rows' audio offsets are bound per call, so
+  a step captured for one length replays for another.
 - The host counts the persistent kernel's launches exactly as the device epoch advances (one per launch, ceil(R / 8)
   per step over R rows), through graph replays, incremental steps, beam calls and reset.
 """
@@ -81,6 +82,18 @@ def test_q4_path_is_in_the_graph_key(drv):
         m.debug("mega_auto")
     _assert_same(graph, eager, "gemm_simt")
     assert graph[2] == eager[2]
+
+
+def test_replay_across_stream_lengths(drv):
+    """Two transcriptions at 4 rows whose streams differ in length: the second replays the step graph the first captured,
+    and gives the ids and last-step logits of an eager run."""
+    m, mels = drv
+    m.debug("mega_auto")
+    full = _transcribe(m, mels[:4])
+    short = np.ascontiguousarray(mels[:4, :, :MEL_FRAMES // 2])
+    again = _transcribe(m, short)
+    assert again[0].shape[1] < full[0].shape[1]
+    _assert_same(again, _eager(m, short), "shorter streams")
 
 
 def _assert_epoch(m, what):

@@ -720,9 +720,9 @@ int32_t vox_prefill(vox_session *sh, const int32_t *ids, int32_t b, int32_t m, i
     VOX_CHECK(s->beam_w == 1, VOX_EINVAL, "vox_prefill runs greedy only: the session's beam width is %d", s->beam_w);
     VOX_CHECK(s->cache_len + m <= s->out_ld, VOX_EINVAL, "KV cache full (%d + %d > %d)", s->cache_len, m, s->out_ld);
     if (add_audio)
-        VOX_CHECK(b == s->cur_B && s->cache_len + m <= s->cur_S4, VOX_EINVAL,
+        VOX_CHECK(b == (int)s->audio_offs.size() && s->cache_len + m <= s->cur_S4, VOX_EINVAL,
                   "add_audio: positions %d..%d need audio embeddings of %d streams (have %d positions for %d streams; call vox_encode_audio first)",
-                  s->cache_len, s->cache_len + m, b, s->cur_S4, s->cur_B);
+                  s->cache_len, s->cache_len + m, b, s->cur_S4, (int)s->audio_offs.size());
     s->check_ids(ids, (size_t)b * m);
     CUDA_OK(cudaSetDevice(s->m->device));
     s->step_incremental(b, m, ids, add_audio != 0);
@@ -738,8 +738,9 @@ int32_t vox_decode_step(vox_session *sh, const int32_t *tok, int32_t b, int32_t 
     VOX_CHECK(s->beam_w == 1, VOX_EINVAL, "vox_decode_step runs greedy only: the session's beam width is %d", s->beam_w);
     VOX_CHECK(s->cache_len + 1 <= s->out_ld, VOX_EINVAL, "KV cache full (%d + 1 > %d)", s->cache_len, s->out_ld);
     if (add_audio)
-        VOX_CHECK(b == s->cur_B && s->cache_len < s->cur_S4, VOX_EINVAL,
-                  "add_audio: position %d has no audio embedding (%d positions, %d streams encoded)", s->cache_len, s->cur_S4, s->cur_B);
+        VOX_CHECK(b == (int)s->audio_offs.size() && s->cache_len < s->cur_S4, VOX_EINVAL,
+                  "add_audio: position %d has no audio embedding (%d positions, %d streams encoded)", s->cache_len, s->cur_S4,
+                  (int)s->audio_offs.size());
     CUDA_OK(cudaSetDevice(s->m->device));
     if (tok) {
         s->check_ids(tok, b);
@@ -926,7 +927,7 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
         }
         return VOX_OK;
     } else if (w == "enc_out") { src = s->h_enc; n = rows * c.enc_dim; }
-    else if (w == "audio_embeds") { src = s->audio; n = (size_t)s->cur_B * s->cur_S4 * c.dec_dim; }
+    else if (w == "audio_embeds") { src = s->audio; n = (size_t)s->audio_n * c.dec_dim; }   // stream after stream
     else if (w == "mel") { src = s->mel; n = 0; /* size unknown here */ }
     else if (w == "conv") { src = s->dbg_conv; n = rows * c.enc_dim; }
     else if (w == "logits") { src = s->logits; n = (size_t)s->cur_B * c.vocab; }

@@ -1132,8 +1132,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
             for (int b = cta; b < B; b += nctas) {
                 cbar();
                 const int id = p.d_tok[b];
-                const float *arow = p.audio_rows ? p.audio_rows[b]
-                                                 : (p.audio ? p.audio + ((size_t)b * p.audio_seq + p.d_pos[b]) * D : nullptr);
+                const float *arow = p.audio ? p.audio + p.audio_off[b] + (int64_t)p.d_pos[b] * D : nullptr;
                 for (int base = 0; base < n; base += MG_CTHREADS) {
                     const int i = base + tid;
                     const bool act = i < n;

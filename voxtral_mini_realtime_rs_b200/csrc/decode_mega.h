@@ -9,7 +9,7 @@
 namespace vox {
 
 enum MegaKind : int {
-    MG_EMBED = 0,   // x_dec[b] = audio[b][pos-?] + dequant(E[tok[b]])  (+ sums of squares for the first norm)
+    MG_EMBED = 0,   // x_dec[b] = audio of row b at pos[b] + dequant(E[tok[b]])  (+ sums of squares for the first norm)
     MG_MATVEC = 1,  // y = epi(norm?(x) . W^T), weights streamed through the CTA's TMA ring
     MG_ATTN = 2,    // RoPE + KV append + GQA attention of one layer (key chunks combined by the last chunk's CTA)
     MG_ARGMAX = 3,  // combine the per-CTA lm_head candidates, write the token, advance the counters
@@ -72,9 +72,9 @@ struct MegaParams {
     const uint4 *emb_qs = nullptr;
     const __half *emb_d = nullptr;
     int D = 0;
+    // audio embeddings (nullptr: none); row b's position p at audio + audio_off[b] + p * D (kernels.h launch_embed)
     const float *audio = nullptr;
-    int audio_seq = 0;
-    const float *const *audio_rows = nullptr;  // optional [B]: the audio embedding of each row's current position (streaming)
+    const int64_t *audio_off = nullptr;
     float *x_dec = nullptr, *ssq_x = nullptr;
     uint2 *emb_fbf = nullptr;         // fragments of the embedded row (x first layer's attn_norm) for layer 0
     float2 *emb_foff = nullptr;

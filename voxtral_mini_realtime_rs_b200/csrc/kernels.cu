@@ -786,21 +786,15 @@ void launch_dec_attention(const float *qkv, int B, int M, int ld, int H, int Hkv
 // Embedding gather from the Q4 table + audio add (model.rs:584-618, 942-948), device-side ids.
 // =====================================================================================
 __global__ void embed_kernel(const uint4 *__restrict__ qs, const __half *__restrict__ ds, int K,
-                             const int *__restrict__ ids, const float *__restrict__ audio, int audio_seq, int M,
-                             const int *__restrict__ pos_ptr, float *__restrict__ x, float *__restrict__ ssq_out,
-                             const int rows_total, const float *const *__restrict__ audio_rows) {
+                             const int *__restrict__ ids, const float *__restrict__ audio,
+                             const int64_t *__restrict__ audio_off, int M, const int *__restrict__ pos_ptr,
+                             float *__restrict__ x, float *__restrict__ ssq_out, const int rows_total) {
     asm volatile("griddepcontrol.launch_dependents;\n" ::: "memory");  // PDL: next kernel may prefetch weights
     const int i = blockIdx.x, b = blockIdx.y;
     const int r = b * M + i;
     const int id = ids[r];
     const int bpr = K >> 5;
-    const float *arow = nullptr;
-    if (audio_rows) {
-        arow = audio_rows[b] ? audio_rows[b] + (size_t)i * K : nullptr;
-    } else if (audio) {
-        const int pos = (pos_ptr ? pos_ptr[b] : 0) + i;
-        arow = audio + ((size_t)b * audio_seq + pos) * K;
-    }
+    const float *arow = audio ? audio + audio_off[b] + (int64_t)(pos_ptr[b] + i) * K : nullptr;
     for (int t = threadIdx.x; t < bpr * 16; t += blockDim.x) {
         const int blk = t >> 4, j = t & 15;
         const uint8_t byte = reinterpret_cast<const uint8_t *>(qs + (size_t)id * bpr + blk)[j];
@@ -827,10 +821,10 @@ __global__ void embed_kernel(const uint4 *__restrict__ qs, const __half *__restr
     }
 }
 
-void launch_embed(const Q4Weight &emb, const int *ids, const float *audio, int audio_seq, int B, int M,
-                  const int *pos_ptr, float *x, float *ssq_out, cudaStream_t st, const float *const *audio_rows) {
+void launch_embed(const Q4Weight &emb, const int *ids, const float *audio, const int64_t *audio_off, int B, int M,
+                  const int *pos_ptr, float *x, float *ssq_out, cudaStream_t st) {
     dim3 grid(M, B);
-    embed_kernel<<<grid, 256, 0, st>>>(emb.qs, emb.d, emb.K, ids, audio, audio_seq, M, pos_ptr, x, ssq_out, B * M, audio_rows);
+    embed_kernel<<<grid, 256, 0, st>>>(emb.qs, emb.d, emb.K, ids, audio, audio_off, M, pos_ptr, x, ssq_out, B * M);
     post_launch("embed");
 }
 

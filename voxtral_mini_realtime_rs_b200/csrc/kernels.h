@@ -206,12 +206,12 @@ void launch_dec_rope_append(float *qkv, int B, int M, int ld, int H, int Hkv, in
 // decoder GQA attention over the cache (keys 0..kv.pos[b]+i, window), out [B*M][H*hd].
 void launch_dec_attention(const float *qkv, int B, int M, int ld, int H, int Hkv, int hd, const KvView &kv, int window,
                           float scale, float *out, cudaStream_t st);
-// x[r][:] = audio_row(b, pos[b] + i) + dequant(E[ids[r]]),  r = b*M + i; the audio row is audio_rows[b] + i*K when the
-// pointer table is given (streaming sessions: one pointer per row), else audio + (b*audio_seq + pos[b] + i)*K, else 0
-// (pos == nullptr: position 0).
+// x[r][:] = audio[audio_off[b] + (pos[b] + i)*K ..] + dequant(E[ids[r]]),  r = b*M + i; without audio (nullptr) the
+// embedding alone.  audio_off [B]: element offset of row b's stream's position 0, signed (an unbounded stream pool's
+// buffer slides past it).
 // ssq_out (optional): [K/16][B*M] per-16-element sums of squares of the written rows (TcWork::ssq_in)
-void launch_embed(const Q4Weight &emb, const int *ids, const float *audio, int audio_seq, int B, int M,
-                  const int *pos, float *x, float *ssq_out, cudaStream_t st, const float *const *audio_rows = nullptr);
+void launch_embed(const Q4Weight &emb, const int *ids, const float *audio, const int64_t *audio_off, int B, int M,
+                  const int *pos, float *x, float *ssq_out, cudaStream_t st);
 // greedy argmax (lowest index wins ties) over logits [B][V]; writes tok[b] and, if out_ids,
 // out_ids[b*out_ld + out_pos[b]]
 void launch_argmax(const float *logits, int B, int V, int *tok, int *out_ids, int out_ld,

@@ -466,6 +466,7 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ri
         s->delays.assign(B, 0.0f);
         s->d_ada_rows = (const float **)s->arena.alloc(sizeof(float *) * B);
         s->d_fga_rows = (const float **)s->arena.alloc(sizeof(float *) * B);
+        s->d_audio_off = s->arena.alloc_n<int64_t>(B);
         s->t_embed = s->arena.alloc_n<float>(c.dec_dim);
         s->ada_tmp = s->arena.alloc_n<float>(c.t_cond_dim);
         s->d_pos = s->arena.alloc_n<int>(B);      // per row (kernels.h KvView::pos)
@@ -632,23 +633,28 @@ void Session::set_stream_delay(int i, float d) {
     delays[i] = d;
 }
 
-void Session::bind_delays(const int *streams, int n) {
-    if (ada_row_streams.size() >= (size_t)n && std::equal(streams, streams + n, ada_row_streams.begin())) return;
-    std::vector<const float *> a(n), f(n);
-    for (int i = 0; i < n; ++i) {
-        a[i] = ada_sets + (size_t)streams[i] * ada_set_floats();
-        f[i] = a[i] + ada_set_floats() / 2;
+void Session::bind_rows(int B) {
+    std::vector<int> streams(B);
+    std::vector<int64_t> offs(B);
+    for (int r = 0; r < B; ++r) {
+        const int s = row_streams.empty() ? r : row_streams[r];
+        streams[r] = s;
+        offs[r] = s < (int)audio_offs.size() ? audio_offs[s] : 0;   // (a stream without embeddings reads none)
     }
-    CUDA_OK(cudaMemcpyAsync(d_ada_rows, a.data(), sizeof(float *) * n, cudaMemcpyHostToDevice, st));
-    CUDA_OK(cudaMemcpyAsync(d_fga_rows, f.data(), sizeof(float *) * n, cudaMemcpyHostToDevice, st));
+    if (bound_streams.size() >= (size_t)B && std::equal(streams.begin(), streams.end(), bound_streams.begin()) &&
+        std::equal(offs.begin(), offs.end(), bound_offs.begin()))
+        return;
+    std::vector<const float *> a(B), f(B);
+    for (int r = 0; r < B; ++r) {
+        a[r] = ada_sets + (size_t)streams[r] * ada_set_floats();
+        f[r] = a[r] + ada_set_floats() / 2;
+    }
+    CUDA_OK(cudaMemcpyAsync(d_ada_rows, a.data(), sizeof(float *) * B, cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(d_fga_rows, f.data(), sizeof(float *) * B, cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(d_audio_off, offs.data(), sizeof(int64_t) * B, cudaMemcpyHostToDevice, st));
     CUDA_OK(cudaStreamSynchronize(st));   // the staging vectors die with this frame
-    ada_row_streams.assign(streams, streams + n);
-}
-
-void Session::bind_row_delays(int B) {
-    std::vector<int> id(B);
-    for (int b = 0; b < B; ++b) id[b] = row_streams.empty() ? b : row_streams[b];
-    bind_delays(id.data(), B);
+    bound_streams = std::move(streams);
+    bound_offs = std::move(offs);
 }
 
 void Session::reserve_pcm(size_t in_floats, size_t padded_floats) {
@@ -707,9 +713,11 @@ void Session::encode(int B, int T) {
     if (debug_capture && dbg_conv) CUDA_OK(cudaMemcpyAsync(dbg_conv, x_enc, sizeof(float) * rows * d, cudaMemcpyDeviceToDevice, st));
     encoder_layers(rows, [&](int) { enc_rope_attention(rows, B, S, nullptr); });
     cur_B = B;
-    cur_S = S;
     cur_S4 = S4;
     enc_rows = rows;
+    audio_n = B * S4;
+    audio_offs.resize(B);
+    for (int s = 0; s < B; ++s) audio_offs[s] = (int64_t)s * S4 * c.dec_dim;
     if (S4 > 0) {
         launch_reshape_rows(h_enc, packed, B, S, S4, d, c.reshape_factor, st);
         linear(m->adapter0, packed, B * S4, adapter_h, c.dec_dim, nullptr, nullptr, EPI_GELU);
@@ -748,7 +756,6 @@ bool Session::decoder_forward(int B, int M) {
     const int D = c.dec_dim, H = c.dec_heads, Hkv = c.dec_kv_heads, hd = c.dec_head_dim;
     const int qkvd = (H + 2 * Hkv) * hd, rows = B * M;
     const float scale = powf((float)hd, -0.5f);
-    if (!stream_mode) bind_row_delays(B);   // (a stream pool binds its rows' sessions itself)
     // decode-sized problems: RMSNorm fused into the consuming matvec, RoPE + KV append fused into the
     // attention kernel => 5 launches per layer instead of 8
     const bool fused = fused_decode(rows);
@@ -783,9 +790,10 @@ void Session::lm_head_rows(int rows, bool norm_pending, float *dst) {
 }
 
 void Session::forward_logits(int b, int M, const int *ids_host, bool with_audio, float *dst) {
+    bind_rows(b);
     CUDA_OK(cudaMemcpyAsync(d_ids, ids_host, sizeof(int) * (size_t)b * M, cudaMemcpyHostToDevice, st));
-    launch_embed(m->tok_emb, d_ids, with_audio ? audio : nullptr, with_audio ? cur_S4 : 0, b, M, with_audio ? d_pos : nullptr,
-                 x_dec, fused_decode(b * M) ? ssq_x : nullptr, st);
+    launch_embed(m->tok_emb, d_ids, with_audio ? audio : nullptr, d_audio_off, b, M, d_pos, x_dec,
+                 fused_decode(b * M) ? ssq_x : nullptr, st);
     const bool pending = decoder_forward(b, M);
     lm_head_rows(b * M, pending, dst);
     launch_advance(d_pos, M, nullptr, 0, b, st);
@@ -908,9 +916,9 @@ void Session::mega_clear_fragments() {
 // More than 8 rows: the rows are independent streams, so the step runs as consecutive launches of the persistent
 // kernel over groups of 8 rows (each group streams the weights once; the per-op GEMMs would pad 16-32 rows to a
 // 128-token tile).  The scratch activations are reused by the groups; the per-row state (token, positions, page table,
-// audio row, output row, logits) is addressed from the group's first row.
+// audio offset, output row, logits) is addressed from the group's first row.
 unsigned Session::prepare_step(int R) {
-    if (!stream_mode) bind_row_delays(R);   // (a stream pool binds its rows' sessions itself)
+    bind_rows(R);
     return mega_prepare(std::min(R, 8)) ? (unsigned)(R + 7) / 8 : 0u;
 }
 
@@ -921,12 +929,11 @@ unsigned Session::decode_step(int B, bool add_audio) {
     if (mega_launches > 0) {
         for (int b0 = 0; b0 < B; b0 += 8) decode_step_mega(b0, std::min(8, B - b0), add_audio);
     } else {
-        launch_embed(m->tok_emb, d_tok, add_audio ? audio : nullptr, cur_S4, B, 1, d_pos, x_dec, fused_decode(B) ? ssq_x : nullptr,
-                     st, add_audio ? audio_rows_dev : nullptr);
+        launch_embed(m->tok_emb, d_tok, add_audio ? audio : nullptr, d_audio_off, B, 1, d_pos, x_dec,
+                     fused_decode(B) ? ssq_x : nullptr, st);
         const bool pending = decoder_forward(B, 1);
         lm_head_rows(B, pending, logits);
-        launch_argmax_multi(logits, B, m->info.vocab, d_tok, stream_mode ? nullptr : d_out, out_ld, d_outpos, am_vals, am_idx,
-                            am_cnt, st);
+        launch_argmax_multi(logits, B, m->info.vocab, d_tok, d_out, out_ld, d_outpos, am_vals, am_idx, am_cnt, st);
         launch_advance(d_pos, 1, d_outpos, 1, B, st);
     }
     token_scores(B);   // one launch over every row (every group of the persistent kernel's)
@@ -978,14 +985,12 @@ void Session::set_beam(int w) {
     beam_w = w;
 }
 
-// The prefill left stream s's prefix in row s.  Beam rows w * b + s take stream s's audio embeddings and step counters;
-// the selection at position 0 has one live rank per stream (the prefix, score 0), whose top-W ids become the W beams,
-// and the fork hands the prefix's KV to the other rows.
+// The prefill left stream s's prefix in row s.  Beam rows w * b + s take stream s's step counters (and read its audio
+// embeddings through row_streams); the selection at position 0 has one live rank per stream (the prefix, score 0), whose
+// top-W ids become the W beams, and the fork hands the prefix's KV to the other rows.
 void Session::beam_start(int b) {
     const int W = beam_w;
-    const size_t per = (size_t)cur_S4 * m->info.dec_dim;
     for (int w = 1; w < W; ++w) {
-        CUDA_OK(cudaMemcpyAsync(audio + (size_t)w * b * per, audio, sizeof(float) * b * per, cudaMemcpyDeviceToDevice, st));
         CUDA_OK(cudaMemcpyAsync(d_pos + w * b, d_pos, sizeof(int) * b, cudaMemcpyDeviceToDevice, st));
         CUDA_OK(cudaMemcpyAsync(d_outpos + w * b, d_outpos, sizeof(int) * b, cudaMemcpyDeviceToDevice, st));
     }
@@ -1044,9 +1049,8 @@ void Session::decode_step_mega(int b0, int B, bool add_audio) {
     p.emb_qs = m->tok_emb.qs;
     p.emb_d = m->tok_emb.d;
     p.D = c.dec_dim;
-    p.audio = add_audio && audio ? audio + (size_t)b0 * cur_S4 * c.dec_dim : nullptr;
-    p.audio_rows = add_audio && audio_rows_dev ? audio_rows_dev + b0 : nullptr;
-    p.audio_seq = cur_S4;
+    p.audio = add_audio ? audio : nullptr;
+    p.audio_off = d_audio_off + b0;
     p.ffn_ada_rows = d_fga_rows + b0;
     p.x_dec = x_dec;
     p.ssq_x = ssq_x;
@@ -1058,7 +1062,7 @@ void Session::decode_step_mega(int b0, int B, bool add_audio) {
     p.d_pos = d_pos + b0;
     p.d_outpos = d_outpos + b0;
     p.d_tok = d_tok + b0;
-    p.d_out = stream_mode ? nullptr : d_out + (size_t)b0 * out_ld;
+    p.d_out = d_out + (size_t)b0 * out_ld;
     p.out_ld = out_ld;
     p.logits_out = logits + (size_t)b0 * c.vocab;
     p.am_vals = mega_am_vals;
@@ -1074,8 +1078,9 @@ void Session::decode_step_mega(int b0, int B, bool add_audio) {
 // Prefill of M positions for B streams (model.rs:894-923 with M = 38; also the incremental vox_prefill).
 void Session::prefill(int B, int M, const int *ids_host, bool add_audio) {
     const vox_model_info &c = m->info;
+    bind_rows(B);
     CUDA_OK(cudaMemcpyAsync(d_ids, ids_host, sizeof(int) * (size_t)B * M, cudaMemcpyHostToDevice, st));
-    launch_embed(m->tok_emb, d_ids, add_audio ? (audio_base ? audio_base : audio) : nullptr, audio_base ? S4_max : cur_S4, B, M, d_pos, x_dec,
+    launch_embed(m->tok_emb, d_ids, add_audio ? audio : nullptr, d_audio_off, B, M, d_pos, x_dec,
                  fused_decode(B * M) ? ssq_x : nullptr, st);
     const bool pending = decoder_forward(B, M);
     if (pending) {   // decode-sized prefill (B*M <= 8): final norm still pending in x_dec
@@ -1084,7 +1089,7 @@ void Session::prefill(int B, int M, const int *ids_host, bool add_audio) {
     // lm_head on the last row only (the reference computes all M rows and keeps one)
     launch_gather_last(h_dec, last_h, B, M, c.dec_dim, st);
     linear(m->tok_emb, last_h, B, logits, c.vocab, nullptr, nullptr, EPI_NONE);
-    launch_argmax(logits, B, c.vocab, d_tok, stream_mode ? nullptr : d_out, out_ld, d_outpos, st);
+    launch_argmax(logits, B, c.vocab, d_tok, d_out, out_ld, d_outpos, st);
     launch_advance(d_pos, M, d_outpos, 1, B, st);
     token_scores(B);
 }
@@ -1126,14 +1131,14 @@ void Session::rebase_epoch() {
     }
 }
 
-// A replay reads the op table and the ADA bindings the host built for the captured step's shape: prepare_step re-builds
-// them before the first replay (an incremental call in between may have built them for another row count), and every
-// other host-side choice the captured kernels depend on is in the key.  `step()` returns its persistent-kernel launches.
+// A replay reads the op table and the row tables (ADA sets, audio offsets) the host built: prepare_step re-builds them
+// before the first replay (an incremental call or another encode in between may have changed them), and every other
+// host-side choice the captured kernels depend on is in the key.  `step()` returns its persistent-kernel launches.
 template <class Step>
 void Session::run_steps(int R, int n, Step step) {
     if (n <= 0) return;
     prepare_step(R);
-    const StepKey key{R, cur_S4, top_k, beam_w, path.matvec_tc, path.gemm_tc, use_mega};
+    const StepKey key{R, top_k, beam_w, path.matvec_tc, path.gemm_tc, use_mega};
     if (use_graph && !(step_graph.exec && step_graph.key == key)) {
         // first step eagerly (also performs any one-time kernel attribute setup), then capture one step and replay it
         mega_steps_host += step();
@@ -1248,13 +1253,14 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
 // encode() on streams packed one after the other: the convolutions run per stream (their zero padding is at each
 // stream's own ends), the layers' linears run over all rows at once, RoPE and attention read the segment table, and
 // each stream keeps its own S / 4 embeddings.  Work follows the sum of the lengths, not b x the longest.
-void Session::encode_ragged(int b, const int *T, const std::vector<std::vector<int>> &audio_rows) {
+void Session::encode_ragged(int b, const int *T) {
     const vox_model_info &c = m->info;
     check_batch(b);
     const int d = c.enc_dim, f = c.reshape_factor, D = c.dec_dim;
     std::vector<int> T1(b), S(b), S4(b);
     seg_host.assign(b + 1, 0);
-    int S_long = 0, sum_T = 0, sum_S4 = 0, n_rows = 0;
+    audio_offs.resize(b);
+    int S_long = 0, sum_T = 0, sum_S4 = 0, S4_short = S4_max;
     for (int i = 0; i < b; ++i) {
         VOX_CHECK(T[i] >= 1 && T[i] <= max_mel_frames, VOX_EINVAL, "mel frames %d exceed session max_mel_frames %d", T[i],
                   max_mel_frames);
@@ -1263,15 +1269,15 @@ void Session::encode_ragged(int b, const int *T, const std::vector<std::vector<i
         S4[i] = S[i] / f;
         seg_host[i + 1] = seg_host[i] + S[i];
         S_long = std::max(S_long, S[i]);
+        S4_short = std::min(S4_short, S4[i]);
         sum_T += T[i];
+        audio_offs[i] = (int64_t)sum_S4 * D;
         sum_S4 += S4[i];
-        for (int r : audio_rows[i]) n_rows = std::max(n_rows, r + 1);
     }
     const int rows = seg_host[b];
     // b <= max_batch streams of <= max_mel_frames frames: the scratch Session::create sized for max_batch uniform streams
-    // holds them packed; the adapter's output passes through x_enc on its way to the audio rows
-    if (!(sum_T <= max_batch * max_mel_frames && rows <= max_batch * S_max && n_rows <= max_batch &&
-          (size_t)sum_S4 * D <= (size_t)max_batch * S_max * d))
+    // holds them packed
+    if (!(sum_T <= max_batch * max_mel_frames && rows <= max_batch * S_max))
         fail(VOX_EINVAL, "encode_ragged: packed streams exceed the session scratch");
     CUDA_OK(cudaMemcpyAsync(d_seg, seg_host.data(), sizeof(int) * (b + 1), cudaMemcpyHostToDevice, st));
     for (int i = 0, t0 = 0, t1 = 0; i < b; t0 += T[i], t1 += T1[i], ++i) {
@@ -1282,19 +1288,14 @@ void Session::encode_ragged(int b, const int *T, const std::vector<std::vector<i
     if (debug_capture && dbg_conv) CUDA_OK(cudaMemcpyAsync(dbg_conv, x_enc, sizeof(float) * rows * d, cudaMemcpyDeviceToDevice, st));
     encoder_layers(rows, [&](int) { enc_rope_attention(rows, b, S_long, d_seg); });
     enc_rows = rows;
-    cur_B = n_rows;
-    cur_S = S_max;
-    cur_S4 = S4_max;   // the decoder reads row r's embeddings at audio + r * S4_max
+    cur_B = b * beam_w;   // the call's decoder rows, whose logits debug "logits" reads
+    cur_S4 = S4_short;    // positions every stream has
+    audio_n = sum_S4;
     if (sum_S4 == 0) return;
     for (int i = 0, o = 0; i < b; o += S4[i], ++i)
         launch_reshape_rows(h_enc + (size_t)seg_host[i] * d, packed + (size_t)o * d * f, 1, S[i], S4[i], d, f, st);
     linear(m->adapter0, packed, sum_S4, adapter_h, D, nullptr, nullptr, EPI_GELU);
-    linear(m->adapter2, adapter_h, sum_S4, x_enc, D, nullptr, nullptr, EPI_NONE);
-    for (int i = 0, o = 0; i < b; o += S4[i], ++i)
-        for (int r : audio_rows[i])
-            if (S4[i] > 0)
-                CUDA_OK(cudaMemcpyAsync(audio + (size_t)r * S4_max * D, x_enc + (size_t)o * D, sizeof(float) * S4[i] * D,
-                                        cudaMemcpyDeviceToDevice, st));
+    linear(m->adapter2, adapter_h, sum_S4, audio, D, nullptr, nullptr, EPI_NONE);
 }
 
 // Streams sorted (stably) by decreasing output count own the rows: beams w of sorted stream i run in row i * W + w, so
@@ -1334,14 +1335,13 @@ void Session::transcribe_ragged(const float *samples, const size_t *lens, int b,
     std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return g[x].n_out > g[y].n_out; });
     int live = 0;
     while (live < b && g[order[live]].n_out > 0) ++live;
-    std::vector<std::vector<int>> rows(b);
+    std::vector<int> row0(b);   // stream s's rank 0 beam
     RowStreams row_guard{this};
     row_streams.assign((size_t)b * W, 0);
-    for (int i = 0; i < b; ++i)
-        for (int w = 0; w < W; ++w) {
-            rows[order[i]].push_back(i * W + w);
-            row_streams[(size_t)i * W + w] = order[i];
-        }
+    for (int i = 0; i < b; ++i) {
+        row0[order[i]] = i * W;
+        for (int w = 0; w < W; ++w) row_streams[(size_t)i * W + w] = order[i];
+    }
 
     CUDA_OK(cudaEventRecord(ev[0], st));
     CUDA_OK(cudaMemcpyAsync(pcm, samples, sizeof(float) * in_off[b], cudaMemcpyHostToDevice, st));
@@ -1352,7 +1352,7 @@ void Session::transcribe_ragged(const float *samples, const size_t *lens, int b,
                    m->mel.fb_len, m->mel.fb_stride, mel_tm + (size_t)t0 * c.n_mels, T[s], 0, st);
     }
     CUDA_OK(cudaEventRecord(ev[1], st));
-    encode_ragged(b, T.data(), rows);
+    encode_ragged(b, T.data());
     CUDA_OK(cudaEventRecord(ev[2], st));
 
     const int n_max = live > 0 ? g[order[0]].n_out : 0;
@@ -1403,13 +1403,13 @@ void Session::transcribe_ragged(const float *samples, const size_t *lens, int b,
     if (W > 1 && live < b)   // a stream without output has no hypotheses: scores 0
         CUDA_OK(cudaMemsetAsync(d_nbest_scores + live * W, 0, sizeof(double) * (b - live) * W, st));
 
-    // ids back in the caller's stream order: stream s's outputs are in the row of its rank 0 beam, rows[s][0]
+    // ids back in the caller's stream order: stream s's outputs are in the row of its rank 0 beam, row0[s]
     std::vector<int> host((size_t)live * W * out_ld);
     if (live > 0) CUDA_OK(cudaMemcpyAsync(host.data(), d_out, sizeof(int) * host.size(), cudaMemcpyDeviceToHost, st));
     CUDA_OK(cudaStreamSynchronize(st));
     size_t total = 0;
     for (int s = 0; s < b; total += g[s].n_out, ++s)
-        for (int i = 0; i < g[s].n_out; ++i) out_ids[total + i] = host[(size_t)rows[s][0] * out_ld + i];
+        for (int i = 0; i < g[s].n_out; ++i) out_ids[total + i] = host[(size_t)row0[s] * out_ld + i];
     // scores and n-best stay on the device: the tracebacks packed sorted stream i's W hypotheses after those of sorted
     // stream i - 1, and its W scores at i * W
     scores_k = top_k;
@@ -1419,7 +1419,7 @@ void Session::transcribe_ragged(const float *samples, const size_t *lens, int b,
     nbest_spans.resize(b);
     for (size_t i = 0, off = 0; i < (size_t)b; off += (size_t)W * g[order[i]].n_out, ++i) {
         const int s = order[i];
-        score_spans[s] = {rows[s][0], 0, g[s].n_out};
+        score_spans[s] = {row0[s], 0, g[s].n_out};
         nbest_spans[s] = {off, (int)i * W, g[s].n_out};
     }
     // the cache holds streams of different lengths (and perhaps beams): the incremental API starts over

@@ -109,9 +109,9 @@ constexpr float kDefaultDelay = 6.0f;
 // Everything a captured decode step depends on that is chosen on the host: a step captured under another key launches
 // other kernels or reads another op table.
 struct StepKey {
-    int rows = 0, S4 = 0, top_k = 0, beam_w = 1;
+    int rows = 0, top_k = 0, beam_w = 1;
     bool matvec_tc = true, gemm_tc = true, use_mega = true;
-    auto tie() const { return std::tie(rows, S4, top_k, beam_w, matvec_tc, gemm_tc, use_mega); }
+    auto tie() const { return std::tie(rows, top_k, beam_w, matvec_tc, gemm_tc, use_mega); }
     bool operator==(const StepKey &o) const { return tie() == o.tie(); }
 };
 struct StepGraph {
@@ -137,7 +137,14 @@ struct Session {
     // encoder workspace
     float *h1 = nullptr, *x_enc = nullptr, *h_enc = nullptr, *qkv_enc = nullptr, *attn_enc = nullptr, *act_enc = nullptr;
     float *packed = nullptr, *adapter_h = nullptr, *audio = nullptr;
-    int cur_B = 0, cur_S = 0, cur_S4 = 0;
+    // read on the host only (argument checks, step counts, debug reads), never by a launch: rows of the last call's
+    // logits, and positions every stream of the last encode has audio embeddings for
+    int cur_B = 0, cur_S4 = 0;
+    // stream s's audio embedding of position p is at audio + audio_offs[s] + p * dec_dim, for the streams of the last
+    // encode (s * S4 * dec_dim; a ragged encode packs them one after the other) or the slots of a stream pool;
+    // audio_n: the embeddings of the last encode, all its streams together
+    std::vector<int64_t> audio_offs;
+    int audio_n = 0;
     int enc_rows = 0;           // encoder rows of the last encode: B * S, or the sum of the streams' S of a ragged one
     int *d_seg = nullptr;       // [max_batch + 1] encoder row of each stream's first frame (ragged encode)
     std::vector<int> seg_host;
@@ -161,18 +168,15 @@ struct Session {
     std::vector<float> delays;
     float *ada_sets = nullptr, *t_embed = nullptr, *ada_tmp = nullptr;
     size_t ada_set_floats() const { return (size_t)2 * m->info.dec_layers * m->info.dec_dim; }
-    // row i of a launch uses stream ada_row_streams[i]'s set through the pointer tables [max_batch] (kernels.h AdaRows,
-    // MegaParams::ffn_ada_rows)
+    // row i of a launch reads its stream's ADA set and audio embeddings through the tables [max_batch] bind_rows
+    // fills: the ADA set pointers (kernels.h AdaRows, MegaParams::ffn_ada_rows) and the audio offsets (launch_embed)
     const float **d_ada_rows = nullptr, **d_fga_rows = nullptr;
-    std::vector<int> ada_row_streams;
+    int64_t *d_audio_off = nullptr;
+    std::vector<int> bound_streams;     // what the tables hold, per row
+    std::vector<int64_t> bound_offs;
     int *d_pos = nullptr, *d_outpos = nullptr, *d_tok = nullptr, *d_ids = nullptr, *d_out = nullptr;
     int out_ld = 0;
     int cache_len = 0;  // host mirror of d_pos[] (all rows equal) for the incremental API
-    // streaming pool (stream.cu): rows of a step belong to sessions of different ages -- no d_out history, audio
-    // embeddings through a per-row pointer table (decode) or a per-launch base pointer (single-session prefill)
-    bool stream_mode = false;
-    const float *const *audio_rows_dev = nullptr;
-    const float *audio_base = nullptr;
     // token confidences (vox_session_set_top_k): 0 = off (no launch, no memory).  k > 0: every prefill and decode step
     // ends with launch_token_scores over its rows into [max_batch][out_ld][TOPK_MAX] ids / log-probabilities, allocated
     // by the first set_top_k(k > 0)
@@ -189,14 +193,14 @@ struct Session {
     // with the n-best results by the first set_beam(W > 1).
     int beam_w = 1;
     // the stream of each decoder row while a transcribe call runs whose rows are not its streams in order (beams, a
-    // ragged call's sorted streams); empty: row r belongs to stream r
+    // ragged call's sorted streams), or the slot of each row of a stream pool's launch; empty: row r belongs to stream r
     std::vector<int> row_streams;
     BeamWork beam;
     int *d_nbest_ids = nullptr;     // every stream's [W][n] ids of the last transcribe, at NbestSpan::ids
     double *d_nbest_scores = nullptr;
     bool page_table_forked = false; // a beam call has rewritten page-table rows: reset() re-uploads the identity table
     void set_beam(int w);
-    void beam_start(int b);         // after the prefill of rows [0, b): replicate them to every beam row, select position 0
+    void beam_start(int b);         // after the prefill of rows [0, b): start every beam row there, select position 0
     void beam_step(int b, int n_live);   // selection + KV fork after a step over the b * beam_w rows
     // Where the results of the last call are, per stream in the caller's order; the getters copy them from the device
     // when asked (the buffers outlive reset()).  Token scores, of the last transcribe or incremental call: entries
@@ -209,7 +213,8 @@ struct Session {
     std::vector<ScoreSpan> score_spans;
     std::vector<NbestSpan> nbest_spans;
     int scores_k = 0, scores_n = 0, nbest_w = 0, nbest_n = 0;
-    // host mirror of d_outpos[] outside stream mode: outputs per row since reset (incremental calls / transcribe)
+    // host mirror of d_outpos[] (the stream pool's session aside): outputs per row since reset (incremental calls /
+    // transcribe)
     std::vector<int> out_rows;
     StepGraph step_graph;   // the offline transcription's decode step, captured once per key and replayed
     bool use_graph = true;
@@ -267,12 +272,11 @@ struct Session {
     // stream i at delays[i] for i < b; streams >= b keep theirs
     void set_delays(const float *delays, int b);
     void set_stream_delay(int stream, float delay);
-    // the ADA sets of the next launches, whose row i belongs to stream streams[i]: points the per-row tables at the
-    // streams' sets.  Launch-free, and copy-free when the row-to-stream mapping has not changed (so it may run inside a
-    // stream capture); a delay change rewrites the sets in place and needs no new binding.
-    void bind_delays(const int *streams, int n);
-    // rows [0, B) as row_streams maps them (every call but the stream pool's)
-    void bind_row_delays(int B);
+    // the per-row tables of launches over rows [0, B), as row_streams maps them to streams: each row's stream's ADA set
+    // and audio offset.  Runs at the start of every prefill, decode step and teacher-forced pass.  Launch-free, and
+    // copy-free when no row's stream or offset has changed (so it may run inside a stream capture); a delay change
+    // rewrites the sets in place and needs no new binding.
+    void bind_rows(int B);
     // mel already on device, time-major, in s->mel_tm
     void encode(int B, int T);
     // The encoder layers over `rows` rows of x_enc, then the final norm into h_enc.  attn(layer) is the step between the
@@ -290,8 +294,7 @@ struct Session {
     // teacher-forced pass over ids [b][M] (+ the audio embeddings at positions *d_pos.. when with_audio): logits of every
     // row into dst [b * M][vocab], positions advanced by M
     void forward_logits(int b, int M, const int *ids_host, bool with_audio, float *dst);
-    // host-side preparation a decode step over R rows depends on (row delays outside stream mode, the persistent
-    // kernel's op table); returns the step's persistent-kernel launches, 0 on the per-op path.  Copy- and sync-free when
+    // host-side preparation a decode step over R rows depends on (bind_rows, the persistent kernel's op table); returns the step's persistent-kernel launches, 0 on the per-op path.  Copy- and sync-free when
     // the last step had the same shape, so that it may run under stream capture.
     unsigned prepare_step(int R);
     // returns prepare_step(B); advances no host counter (it also runs under stream capture)
@@ -309,9 +312,9 @@ struct Session {
     void check_ids(const int32_t *ids, size_t n) const;
     // runs prefill + loop; returns tokens per stream
     int transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids, vox_timings *tm);
-    // encode() of b streams of T[s] mel frames packed one after the other in mel_tm: frames, conv rows and encoder rows
-    // packed by stream (d_seg); stream s's audio embeddings into the audio rows of rows[s] (S4_max apart)
-    void encode_ragged(int b, const int *T, const std::vector<std::vector<int>> &rows);
+    // encode() of b streams of T[s] mel frames packed one after the other in mel_tm: frames, conv rows, encoder rows
+    // (d_seg) and audio embeddings (audio_offs) packed by stream
+    void encode_ragged(int b, const int *T);
     // vox_transcribe_pcm_ragged after its argument checks: b streams of lens[s] host samples, one after the other;
     // n_out[s] ids of stream s after those of stream s - 1 in out_ids.  Records ev[0..4] like the other transcribe calls.
     void transcribe_ragged(const float *samples, const size_t *lens, int b, int normalize, int32_t *out_ids,

@@ -204,7 +204,7 @@ StreamPool *StreamPool::create(Model *m, int max_sessions, float max_seconds) {
         const size_t max_rows = (size_t)B * p->max_new;
         p->d_row_slot = s->arena.alloc_n<int>(max_rows);
         p->d_row_pos = s->arena.alloc_n<int>(max_rows);
-        p->d_audio_rows = (const float **)s->arena.alloc(sizeof(float *) * B);
+        s->audio_offs.assign(B, 0);   // slot id's embeddings: audio + (id * S4_max - emb0) * dec_dim, set per launch
         if (unbounded) {
             const size_t enc_rows = B * p->ring * (c.enc_head_dim / 2), dec_rows = (size_t)kDecRopeRing * (c.dec_head_dim / 2);
             p->enc_rope_cos = s->arena.alloc_n<float>(enc_rows);
@@ -219,7 +219,6 @@ StreamPool *StreamPool::create(Model *m, int max_sessions, float max_seconds) {
         p->slots.resize(max_sessions);
         // decoder KV pages: the session's identity tables are replaced by a free list
         for (int i = s->kv_n_pages - 1; i >= 0; --i) p->free_pages.push_back(i);
-        s->stream_mode = true;
     } catch (...) {
         delete p;
         throw;
@@ -337,26 +336,25 @@ void StreamPool::ensure_pages(Slot &sl, int positions) {
     }
 }
 
-// rows[i] = slot id of batch row i: page tables, positions, fed-back tokens, audio pointers of this step, and the rows'
-// ADA sets (the sessions' delays)
+// rows[i] = slot id of batch row i: page tables, positions and fed-back tokens of this launch; the rows' slots and
+// their audio offsets for the session to bind (Session::bind_rows: ADA sets and audio embeddings)
 void StreamPool::upload_rows(const std::vector<int> &rows, bool with_tokens) {
-    s->bind_delays(rows.data(), (int)rows.size());
     const vox_model_info &c = m->info;
     const int nb = (int)rows.size(), mp = s->kv_max_pages;
     std::vector<int> pt((size_t)nb * mp, 0), pos(nb), tok(nb), zero(nb, 0);
-    std::vector<const float *> ar(nb);
     for (int i = 0; i < nb; ++i) {
         const Slot &sl = slots[rows[i]];
         for (size_t k = 0; k < sl.pages.size(); ++k) pt[(size_t)i * mp + k] = sl.pages[k];
         pos[i] = sl.pos;
         tok[i] = sl.last_tok;
-        ar[i] = s->audio + ((size_t)rows[i] * s->S4_max + (sl.pos - sl.emb0)) * c.dec_dim;
+        // negative once the buffer has slid: position p's embedding sits at buffer row p - emb0
+        s->audio_offs[rows[i]] = ((int64_t)rows[i] * s->S4_max - sl.emb0) * c.dec_dim;
     }
+    s->row_streams = rows;
     CUDA_OK(cudaMemcpyAsync(s->d_page_table, pt.data(), sizeof(int) * pt.size(), cudaMemcpyHostToDevice, s->st));
     CUDA_OK(cudaMemcpyAsync(s->d_pos, pos.data(), sizeof(int) * nb, cudaMemcpyHostToDevice, s->st));
     CUDA_OK(cudaMemcpyAsync(s->d_outpos, zero.data(), sizeof(int) * nb, cudaMemcpyHostToDevice, s->st));
     if (with_tokens) CUDA_OK(cudaMemcpyAsync(s->d_tok, tok.data(), sizeof(int) * nb, cudaMemcpyHostToDevice, s->st));
-    CUDA_OK(cudaMemcpyAsync(d_audio_rows, ar.data(), sizeof(float *) * nb, cudaMemcpyHostToDevice, s->st));
     CUDA_OK(cudaStreamSynchronize(s->st));  // the staging vectors die with this frame
 }
 
@@ -460,10 +458,7 @@ void StreamPool::tick(vox_stream_stats *st_out) {
             upload_rows({id}, false);
             std::vector<int> prefix((size_t)P, 32);
             prefix[0] = 1;
-            s->audio_rows_dev = nullptr;
-            s->audio_base = s->audio + (size_t)id * s->S4_max * D;  // row 0 of the launch = this session
             s->prefill(1, P, prefix.data(), true);
-            s->audio_base = nullptr;
             int tok = 0;
             std::vector<int32_t> top((size_t)s->top_k);
             std::vector<float> lp((size_t)s->top_k);
@@ -499,9 +494,7 @@ void StreamPool::tick(vox_stream_stats *st_out) {
                 if (unbounded) fill_rope(dec_rope_cos, dec_rope_sin, c.dec_head_dim, kDecRopeRing, 0, slots[id].pos, 1);
             }
             upload_rows(rows, true);
-            s->audio_rows_dev = d_audio_rows;
             s->mega_steps_host += s->decode_step((int)rows.size(), true);
-            s->audio_rows_dev = nullptr;
             std::vector<int> toks(rows.size());
             std::vector<int32_t> top(rows.size() * s->top_k);
             std::vector<float> lp(rows.size() * s->top_k);
@@ -614,7 +607,7 @@ void StreamPool::session_info(int id, struct vox_stream_session_info *out) {
     out->kv_pages = (int32_t)sl.pages.size();
 }
 
-// stream mode resets every row's output position before a step, so its scores sit at position 0 of the row
+// upload_rows resets every row's output position before a step, so its token and scores sit at position 0 of the row
 void StreamPool::fetch_scores(int n, int32_t *top_ids, float *top_lp) {
     const int k = s->top_k;
     if (k == 0) return;

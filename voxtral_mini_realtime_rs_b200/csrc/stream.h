@@ -43,7 +43,6 @@ struct StreamPool {
     float *dec_rope_cos = nullptr, *dec_rope_sin = nullptr;
     float *slide_tmp = nullptr;  // unbounded pools: bounce buffer of slide() (stream.cu), the size of the largest session buffer
     int *d_row_slot = nullptr, *d_row_pos = nullptr;
-    const float **d_audio_rows = nullptr;
     std::vector<Slot> slots;
     std::vector<int> free_pages;
 
