@@ -46,7 +46,7 @@ def main():
             t3 = t2
         a = agg.setdefault(nm, [0] + [0.0] * 6)
         a[0] += 1
-        a[1] += t1 - t0            # staging (matvec) / q,k,v load + RoPE (attention)
+        a[1] += t1 - t0            # staging (matvec) / q and the first K tile landed (attention)
         a[2] += t4 - t1            # wait for the first weight stage / KV walk
         a[3] += t5 - t4            # weight loop (matvec)
         a[4] += t2 - max(t5, t4)   # last reduce + epilogue / softmax merge

@@ -24,8 +24,12 @@
 //     next fused RMSNorm / SiLU*up / running argmax / activation fragments of the next matvec) => no atomics, no split-K
 //     scratch, bitwise deterministic.  When the activation fragments of all of K do not fit shared memory (M > 2 and
 //     K > 3072) the CTA walks K in private slices and keeps tile sums in shared memory.
-//   * attention: RoPE + KV append + GQA as in decode_attn.cu, one CTA per (stream, kv head, key chunk); the chunks' softmax
-//     states travel as 8-byte {value, (step, layer) tag} words that the merging CTA polls directly.
+//   * RoPE and the KV append run in the qkv phase's epilogue (an epilogue thread's quad of rows is two whole RoPE pairs):
+//     once that phase's grid barrier has passed, the step's key is in the cache like every other.
+//   * attention: GQA, one CTA per (stream, kv head, key chunk).  The chunk's K and V pass through the scratch region in
+//     tiles; a consumer thread scores one key against the G heads, one CTA-wide max per head, then P.V with one thread per
+//     (head, dim), online softmax across tiles.  The chunks' softmax states travel as 8-byte {value, (step, layer) tag}
+//     words that the merging CTA polls directly.
 //
 // All activations written by other CTAs are read with ld.global.cg (L1 is not coherent).
 // Every spin loop has a watchdog that traps instead of hanging the GPU.
@@ -83,6 +87,16 @@ __host__ __device__ constexpr int mg_misc_bytes(int MT) {
     return ((592 + 2048 * mg_nt(MT) * MT + 64 * MG_ACC_TILES * MT + 4 * mg_vals(MT) + 256) + 127) & ~127;  // + s_op
 }
 __host__ __device__ constexpr int mg_pair_bytes(int MT) { return 272 * MT; }  // fragments + offsets of one block pair
+// Attention phase in the scratch region: q [G][HD] + per-warp maxima [MG_CWARPS][G], then per key of a tile its G scores,
+// its K row padded by one float4 (HD + 4) and its V row.  Keys per tile: what the scratch holds, in whole warps (one key
+// per consumer thread, at most MG_CTHREADS).
+__host__ __device__ constexpr int mg_attn_fixed_bytes(int G, int HD) { return (G * HD + MG_CWARPS * G) * 4; }
+__host__ __device__ constexpr int mg_attn_key_bytes(int G, int HD) { return (G + 2 * HD + 4) * 4; }
+__host__ __device__ constexpr int mg_attn_tile(int scratch_bytes, int G, int HD) {
+    return (scratch_bytes - mg_attn_fixed_bytes(G, HD)) / mg_attn_key_bytes(G, HD) / 32 * 32 > MG_CTHREADS
+               ? MG_CTHREADS
+               : (scratch_bytes - mg_attn_fixed_bytes(G, HD)) / mg_attn_key_bytes(G, HD) / 32 * 32;
+}
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
@@ -144,6 +158,13 @@ __device__ __forceinline__ float2 ld_tagged(const float2 *p) {
 __device__ __forceinline__ void red_release_add(unsigned *p, unsigned v) {
     asm volatile("red.release.gpu.global.add.u32 [%0], %1;\n" ::"l"(p), "r"(v) : "memory");
 }
+// 16-byte copy global -> shared through L2 (cp.async.cg: rows written by other CTAs in the previous phase)
+__device__ __forceinline__ void cp_async16(void *dst_smem, const void *src_gmem) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(smem_u32(dst_smem)), "l"(src_gmem) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void prefetch_l1(const void *p) { asm volatile("prefetch.global.L1 [%0];\n" ::"l"(p)); }
 // L2 prefetch of a byte range (16-byte multiple)
 __device__ __forceinline__ void bulk_prefetch_l2(const void *p, uint32_t bytes) {
@@ -639,6 +660,31 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                                             out.z = 0.5f * out.z * (1.0f + erff(out.z * 0.70710678118654752440f));
                                             out.w = 0.5f * out.w * (1.0f + erff(out.w * 0.70710678118654752440f));
                                         }
+                                        // the qkv phase (kc set): q and k rows go through RoPE (rope.rs:103-141; interleaved pairs
+                                        // (2i, 2i+1): the quad is two whole pairs), k and v rows are appended to the layer's KV cache
+                                        // at the token's position.  (Loaded here, not ahead of the hand-off barrier: live across the
+                                        // partial-sum tree these operands made this 64-register role spill.)
+                                        if (vop->kc != nullptr) {
+                                            const int pos = p.d_pos[q_tok];
+                                            if (RING || pos < p.max_seq) {
+                                                const int hrow = r_row % HD, qk_rows = (p.H + p.Hkv) * HD;
+                                                if (r_row < qk_rows) {
+                                                    const size_t rr = (size_t)(RING ? pos % p.rope_rows : pos) * (HD / 2) + (hrow >> 1);
+                                                    const float2 c = *reinterpret_cast<const float2 *>(p.cos_t + rr);
+                                                    const float2 sn = *reinterpret_cast<const float2 *>(p.sin_t + rr);
+                                                    out = make_float4(out.x * c.x - out.y * sn.x, out.x * sn.x + out.y * c.x,
+                                                                      out.z * c.y - out.w * sn.y, out.z * sn.y + out.w * c.y);
+                                                }
+                                                if (r_row >= p.H * HD) {
+                                                    KvView kvw;
+                                                    kvw.page_table = p.page_table;
+                                                    kvw.max_pages = p.max_pages;
+                                                    const int kvh = ((r_row - p.H * HD) / HD) % p.Hkv;
+                                                    float *dst = (r_row < qk_rows ? vop->kc : vop->vc) + kv_index<RING>(kvw, q_tok, p.Hkv, kvh, pos, HD) + hrow;
+                                                    *reinterpret_cast<float4 *>(dst) = out;
+                                                }
+                                            }
+                                        }
                                         if (yout) {
                                             float *yd = yout + (size_t)q_tok * ldy + r_row;
                                             if (vec_ok && quad_in) {
@@ -904,170 +950,155 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                 }
             }
         } else if (kind == MG_ATTN) {
-            // unit = (stream, kv head, key chunk): the 4 query heads of a GQA group share one pass over their
-            // chunk of K and V; the chunks' softmax states are combined by the last chunk's CTA (tagged words, below).  (With
-            // one CTA per (stream, kv head), a few CTAs walk all keys -- issue-bound -- while the other SMs wait.)
-            float *qs = reinterpret_cast<float *>(scratch);       // [G][HD]
-            float *kvs = qs + G * HD;                              // [2][HD]
-            float *red_m = kvs + 2 * HD;                           // [MG_CWARPS][G]
-            float *red_l = red_m + MG_CWARPS * G;                  // [MG_CWARPS][G]
-            float *red_acc = red_l + MG_CWARPS * G;                // [MG_CWARPS][G][HD]
-            const int H = p.H, Hkv = p.Hkv, max_seq = p.max_seq, NC = p.attn_chunks;
+            // unit = (stream, kv head, key chunk): the G query heads of a GQA group share one pass over their chunk of the
+            // keys; the chunks' softmax states are combined by the last chunk's CTA (tagged words, below).  The qkv phase left
+            // q rotated in p.qkv and the step's k, v in the cache, so every key of the chunk comes from the cache.
+            // The chunk goes through shared memory KT keys at a time (online softmax across tiles): consumer thread j scores
+            // key j against the G heads (q read as a broadcast; K rows padded to HD + 4 floats, an odd number of float4, so
+            // the 8 threads of a quarter-warp read 8 distinct bank groups), one CTA-wide max per head, then P.V with
+            // thread = (head, dim).
+            const int KT = mg_attn_tile(p.scratch_bytes, G, HD);
+            constexpr int KLD = HD + 4;
+            float *qs = reinterpret_cast<float *>(scratch);  // [G][HD]
+            float *red_m = qs + G * HD;                       // [MG_CWARPS][G] tile max per warp
+            float *ps = red_m + MG_CWARPS * G;                // [G][KT] scores, then probabilities
+            float *ks = ps + G * KT;                          // [KT][KLD]
+            float *vs = ks + KT * KLD;                        // [KT][HD]
+            const int H = p.H, Hkv = p.Hkv, NC = p.attn_chunks;
             KvView kvw;
             kvw.k = op.kc;
             kvw.v = op.vc;
             kvw.page_table = p.page_table;
             kvw.max_pages = p.max_pages;
+            const int oh = tid / HD, od = tid - oh * HD;      // output (head, dim) of thread tid < G * HD
             for (int unit = cta; unit < B * Hkv * NC; unit += nctas) {
                 const int ch = unit % NC, bk = unit / NC;
                 const int b = bk / Hkv, kvh = bk - b * Hkv;
                 const int pos = p.d_pos[b];              // per row: sessions of different ages share the step
-                if (!RING && pos >= max_seq) continue;
+                if (!RING && pos >= p.max_seq) continue;
                 const int j_lo = pos - p.window > 0 ? pos - p.window : 0;
                 const int per = (pos - j_lo + NC) / NC;  // ceil((pos - j_lo + 1) / NC) keys per chunk
                 const int j0 = j_lo + ch * per, j1 = min(pos + 1, j0 + per);  // keys [j0, j1)
-                const bool has_new = j0 <= pos && pos < j1;                    // this chunk holds the new row
-                const float *row = p.qkv + (size_t)b * p.ld_qkv;
-                cbar();  // scratch free (previous unit / previous op)
-                // q (G heads) and k through RoPE on the way in (rope.rs:103-141: interleaved pairs), v as is
-                constexpr int half = HD / 2;
-                for (int i = tid; i < (G + 1) * half; i += MG_CTHREADS) {
-                    const int h = i / half, pi = i - h * half;
-                    const float *src = (h < G) ? row + (size_t)(kvh * G + h) * HD + 2 * pi : row + (size_t)H * HD + kvh * HD + 2 * pi;
-                    const float2 xv = __ldcg(reinterpret_cast<const float2 *>(src));
-                    const size_t rr = (size_t)(RING ? pos % p.rope_rows : pos) * half + pi;
-                    const float c = p.cos_t[rr], sn = p.sin_t[rr];
-                    float *dst = (h < G) ? &qs[h * HD + 2 * pi] : &kvs[2 * pi];
-                    dst[0] = xv.x * c - xv.y * sn;
-                    dst[1] = xv.x * sn + xv.y * c;
-                }
-                for (int i = tid; i < HD; i += MG_CTHREADS) kvs[HD + i] = __ldcg(row + (size_t)(H + Hkv) * HD + kvh * HD + i);
-                cbar();
-                if (tracing) p.trace[oi * 6 + 1] = (unsigned long long)clock64();
-                if (tr_all) ta[3] = (unsigned long long)clock64();
-                if (has_new) {
-                    const size_t at = kv_index<RING>(kvw, b, Hkv, kvh, pos, HD);
-                    for (int i = tid; i < HD; i += MG_CTHREADS) {
-                        kvw.k[at + i] = kvs[i];
-                        kvw.v[at + i] = kvs[HD + i];
+                float m_run[G];
+#pragma unroll
+                for (int h = 0; h < G; ++h) m_run[h] = -INFINITY;
+                float o_acc = 0.0f, o_sum = 0.0f;        // thread (oh, od): unnormalised P.V and sum of P
+                for (int jt = j0; jt < j1; jt += KT) {
+                    const int n = min(KT, j1 - jt);
+                    cbar();  // scratch free (previous tile / unit / op)
+                    // K (with q on the first tile), then V: two copy groups, the scores start once K has landed
+                    if (jt == j0)
+                        for (int i = tid; i < G * HD / 4; i += MG_CTHREADS)
+                            cp_async16(qs + 4 * i, p.qkv + (size_t)b * p.ld_qkv + (size_t)kvh * G * HD + 4 * i);
+                    for (int f = tid; f < n * (HD / 4); f += MG_CTHREADS) {
+                        const int jj = f / (HD / 4), c4 = f - jj * (HD / 4);
+                        cp_async16(ks + jj * KLD + 4 * c4, kvw.k + kv_index<RING>(kvw, b, Hkv, kvh, jt + jj, HD) + 4 * c4);
                     }
-                }
-                float q[G][DPL];
+                    cp_async_commit();
+                    for (int f = tid; f < n * (HD / 4); f += MG_CTHREADS) {
+                        const int jj = f / (HD / 4), c4 = f - jj * (HD / 4);
+                        cp_async16(vs + jj * HD + 4 * c4, kvw.v + kv_index<RING>(kvw, b, Hkv, kvh, jt + jj, HD) + 4 * c4);
+                    }
+                    cp_async_commit();
+                    cp_async_wait<1>();
+                    cbar();  // q and the K tile have landed
+                    if (jt == j0) {
+                        if (tracing) p.trace[oi * 6 + 1] = (unsigned long long)clock64();
+                        if (tr_all) ta[3] = (unsigned long long)clock64();
+                    }
+                    // ---- scores: thread j = key jt + j
+                    float sj[G];
 #pragma unroll
-                for (int h = 0; h < G; ++h)
+                    for (int h = 0; h < G; ++h) sj[h] = -INFINITY;
+                    if (tid < n) {
+                        const float4 *kr = reinterpret_cast<const float4 *>(ks + tid * KLD);
+                        float d0[G], d1[G];   // two chains per head
 #pragma unroll
-                    for (int i = 0; i < DPL; ++i) q[h][i] = qs[h * HD + lane * DPL + i];
-                float m_run[G], l_run[G], acc[G][DPL];
+                        for (int h = 0; h < G; ++h) d0[h] = d1[h] = 0.0f;
+#pragma unroll 4
+                        for (int c = 0; c < HD / 4; c += 2) {
+                            const float4 ka = kr[c], kb = kr[c + 1];
 #pragma unroll
-                for (int h = 0; h < G; ++h) {
-                    m_run[h] = -INFINITY;
-                    l_run[h] = 0.0f;
-#pragma unroll
-                    for (int i = 0; i < DPL; ++i) acc[h][i] = 0.0f;
-                }
-                constexpr int KU = 4;  // keys in flight per warp; one softmax rescale per KU keys
-                for (int jb = j0 + warp; jb < j1; jb += KU * MG_CWARPS) {
-                    float kk[KU][DPL], vv[KU][DPL];
-#pragma unroll
-                    for (int u = 0; u < KU; ++u) {
-                        const int j = jb + u * MG_CWARPS;
-                        if (j < j1 && j != pos) {
-                            const size_t at = kv_index<RING>(kvw, b, Hkv, kvh, j, HD) + lane * DPL;
-                            const float *kr = kvw.k + at;
-                            const float *vr = kvw.v + at;
-                            if constexpr (DPL == 4) {
-                                const float4 k4 = *reinterpret_cast<const float4 *>(kr);
-                                const float4 v4 = *reinterpret_cast<const float4 *>(vr);
-                                kk[u][0] = k4.x; kk[u][1] = k4.y; kk[u][2] = k4.z; kk[u][3] = k4.w;
-                                vv[u][0] = v4.x; vv[u][1] = v4.y; vv[u][2] = v4.z; vv[u][3] = v4.w;
-                            } else {
-#pragma unroll
-                                for (int i = 0; i < DPL; ++i) {
-                                    kk[u][i] = kr[i];
-                                    vv[u][i] = vr[i];
-                                }
-                            }
-                        } else {  // j == pos: the row appended above, still in shared memory (j >= j1: unused)
-#pragma unroll
-                            for (int i = 0; i < DPL; ++i) {
-                                kk[u][i] = kvs[lane * DPL + i];
-                                vv[u][i] = kvs[HD + lane * DPL + i];
+                            for (int h = 0; h < G; ++h) {
+                                const float4 qa = reinterpret_cast<const float4 *>(qs + h * HD)[c];
+                                const float4 qb = reinterpret_cast<const float4 *>(qs + h * HD)[c + 1];
+                                d0[h] = fmaf(qa.x, ka.x, fmaf(qa.y, ka.y, fmaf(qa.z, ka.z, fmaf(qa.w, ka.w, d0[h]))));
+                                d1[h] = fmaf(qb.x, kb.x, fmaf(qb.y, kb.y, fmaf(qb.z, kb.z, fmaf(qb.w, kb.w, d1[h]))));
                             }
                         }
-                    }
-                    float sc[KU][G];
-#pragma unroll
-                    for (int u = 0; u < KU; ++u)
 #pragma unroll
                         for (int h = 0; h < G; ++h) {
-                            float d = 0.0f;
-#pragma unroll
-                            for (int i = 0; i < DPL; ++i) d = fmaf(q[h][i], kk[u][i], d);
-                            sc[u][h] = d;
+                            sj[h] = (d0[h] + d1[h]) * p.scale;
+                            ps[h * KT + tid] = sj[h];
                         }
-#pragma unroll
-                    for (int o = 16; o > 0; o >>= 1)
-#pragma unroll
-                        for (int u = 0; u < KU; ++u)
-#pragma unroll
-                            for (int h = 0; h < G; ++h) sc[u][h] += __shfl_xor_sync(0xffffffffu, sc[u][h], o);
+                    }
 #pragma unroll
                     for (int h = 0; h < G; ++h) {
-                        float m_new = m_run[h];
+                        float mw = sj[h];
 #pragma unroll
-                        for (int u = 0; u < KU; ++u) {
-                            sc[u][h] = (jb + u * MG_CWARPS < j1) ? sc[u][h] * p.scale : -INFINITY;
-                            m_new = fmaxf(m_new, sc[u][h]);
-                        }
-                        const float alpha = fast_exp(m_run[h] - m_new);  // exp(-inf) = 0 on the first batch
-                        float pe[KU], ps = 0.0f;
-#pragma unroll
-                        for (int u = 0; u < KU; ++u) {
-                            pe[u] = fast_exp(sc[u][h] - m_new);  // masked keys: exp(-inf) = 0
-                            ps += pe[u];
-                        }
-                        l_run[h] = l_run[h] * alpha + ps;
-                        m_run[h] = m_new;
-#pragma unroll
-                        for (int i = 0; i < DPL; ++i) {
-                            float a = acc[h][i] * alpha;
-#pragma unroll
-                            for (int u = 0; u < KU; ++u) a = fmaf(pe[u], vv[u][i], a);
-                            acc[h][i] = a;
-                        }
+                        for (int o = 16; o > 0; o >>= 1) mw = fmaxf(mw, __shfl_xor_sync(0xffffffffu, mw, o));
+                        if (lane == 0) red_m[warp * G + h] = mw;
                     }
+                    cbar();
+                    // ---- running max over the tile; probabilities of key tid
+                    float m_new[G];
+#pragma unroll
+                    for (int h = 0; h < G; ++h) {
+                        float mt = m_run[h];
+#pragma unroll
+                        for (int w = 0; w < MG_CWARPS; ++w) mt = fmaxf(mt, red_m[w * G + h]);
+                        m_new[h] = mt;
+                        if (tid < n) ps[h * KT + tid] = fast_exp(sj[h] - mt);
+                    }
+                    cp_async_wait<0>();
+                    cbar();  // V tile landed, probabilities visible
+                    // ---- P.V: thread (head, dim)
+                    if (tid < G * HD) {
+                        float mo = m_run[0], mn = m_new[0];
+#pragma unroll
+                        for (int h = 1; h < G; ++h)
+                            if (oh == h) {
+                                mo = m_run[h];
+                                mn = m_new[h];
+                            }
+                        const float alpha = fast_exp(mo - mn);  // exp(-inf) = 0 on the first tile
+                        const float *pr = ps + oh * KT;
+                        const float *vc = vs + od;
+                        float a0 = 0.0f, a1 = 0.0f, s0 = 0.0f, s1 = 0.0f;
+                        int j = 0;
+#pragma unroll 4
+                        for (; j + 1 < n; j += 2) {
+                            const float2 pj = *reinterpret_cast<const float2 *>(pr + j);
+                            a0 = fmaf(pj.x, vc[j * HD], a0);
+                            a1 = fmaf(pj.y, vc[(j + 1) * HD], a1);
+                            s0 += pj.x;
+                            s1 += pj.y;
+                        }
+                        if (j < n) {
+                            a0 = fmaf(pr[j], vc[j * HD], a0);
+                            s0 += pr[j];
+                        }
+                        o_acc = fmaf(o_acc, alpha, a0 + a1);
+                        o_sum = fmaf(o_sum, alpha, s0 + s1);
+                    }
+#pragma unroll
+                    for (int h = 0; h < G; ++h) m_run[h] = m_new[h];
                 }
                 if (tracing) p.trace[oi * 6 + 4] = (unsigned long long)clock64();
-#pragma unroll
-                for (int h = 0; h < G; ++h) {
-                    if (lane == 0) {
-                        red_m[warp * G + h] = m_run[h];
-                        red_l[warp * G + h] = l_run[h];
-                    }
-#pragma unroll
-                    for (int i = 0; i < DPL; ++i) red_acc[((size_t)warp * G + h) * HD + lane * DPL + i] = acc[h][i];
-                }
-                cbar();
-                // ---- combine the warps; with several key chunks per (stream, kv head) the last chunk's CTA also
-                // combines the chunks (pairwise release/acquire flags: no grid-wide phase for the merge)
+                // ---- with several key chunks per (stream, kv head) the last chunk's CTA combines the chunks (pairwise
+                // tagged words: no grid-wide phase for the merge)
                 const int u0 = bk * NC;
                 const int target = epoch * 64 + op.layer + 1;  // unique per (decode step, layer), never 0
                 float2 *const acc2 = reinterpret_cast<float2 *>(p.att_acc);   // [unit][G][hd] {value, tag}
                 float2 *const ml2 = reinterpret_cast<float2 *>(p.att_ml);     // [unit][G][2]  {value, tag}
                 float o_final = 0.0f;                           // thread i < G*HD: output (head i / HD, dim i % HD)
-                for (int i = tid; i < G * HD; i += MG_CTHREADS) {
-                    const int h = i / HD, d = i - h * HD;
-                    float mx = -INFINITY;
+                if (tid < G * HD) {
+                    const int h = oh, d = od;
+                    float mx = m_run[0];
 #pragma unroll
-                    for (int w = 0; w < MG_CWARPS; ++w) mx = fmaxf(mx, red_m[w * G + h]);
-                    float num = 0.0f, den = 0.0f;
-#pragma unroll
-                    for (int w = 0; w < MG_CWARPS; ++w) {
-                        const float mw = red_m[w * G + h];
-                        const float f = (mw == -INFINITY) ? 0.0f : fast_exp(mw - mx);
-                        num = fmaf(red_acc[((size_t)w * G + h) * HD + d], f, num);
-                        den = fmaf(red_l[w * G + h], f, den);
-                    }
+                    for (int hh = 1; hh < G; ++hh)
+                        if (oh == hh) mx = m_run[hh];
+                    const float num = o_acc, den = o_sum;
                     if (NC == 1) {
                         o_final = num / den;
                     } else if (ch != NC - 1) {
@@ -1288,7 +1319,7 @@ MegaPlan decode_mega_plan(int B, int max_pairs, int H, int Hkv, int hd) {
     MegaPlan pl;
     pl.MT = B <= 1 ? 1 : (B <= 2 ? 2 : (B <= 4 ? 4 : 8));
     const int G = H / Hkv;
-    const int attn_bytes = ((G + 2) * hd + 2 * MG_CWARPS * G + MG_CWARPS * G * hd) * (int)sizeof(float);
+    const int attn_bytes = mg_attn_fixed_bytes(G, hd) + 32 * mg_attn_key_bytes(G, hd);   // a tile of at least 32 keys
     const int per_pair = mg_pair_bytes(pl.MT);
     int cap_pairs = MG_SCRATCH_CAP / per_pair;
     if (cap_pairs >= MG_CHUNK) cap_pairs = cap_pairs / MG_CHUNK * MG_CHUNK;

@@ -11,7 +11,7 @@ namespace vox {
 enum MegaKind : int {
     MG_EMBED = 0,   // x_dec[b] = audio of row b at pos[b] + dequant(E[tok[b]])  (+ sums of squares for the first norm)
     MG_MATVEC = 1,  // y = epi(norm?(x) . W^T), weights streamed through the CTA's TMA ring
-    MG_ATTN = 2,    // RoPE + KV append + GQA attention of one layer (key chunks combined by the last chunk's CTA)
+    MG_ATTN = 2,    // GQA attention of one layer over its KV cache (key chunks combined by the last chunk's CTA)
     MG_ARGMAX = 3,  // combine the per-CTA lm_head candidates, write the token, advance the counters
 };
 
@@ -42,7 +42,7 @@ struct MegaOp {
     int ssq_in_parts = 0;
     float *ssq_out = nullptr;       // [n_tiles][B]
     int track_argmax = 0;
-    // MG_ATTN
+    // MG_ATTN, and the layer's qkv MG_MATVEC, whose epilogue applies RoPE to the q and k rows and appends k and v
     float *kc = nullptr, *vc = nullptr;  // this layer's KV page pools [n_pages][Hkv][KV_PAGE][hd] (kernels.h KvView)
     int layer = 0;
     // MG_MATVEC whose output fragments take layer j's ffn_norm x ADA scale (wo): j, else -1.  Token b's fragments are

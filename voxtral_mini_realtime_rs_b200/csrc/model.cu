@@ -869,7 +869,10 @@ bool Session::mega_prepare(int B) {
     }
     for (int j = 0; j < c.dec_layers; ++j) {
         const DecLayerW &l = m->dec[j];
+        // wqkv: its epilogue applies RoPE to q and k and appends k, v to layer j's cache
         matvec(l.wqkv, XF, qkv_dec, qkvd, nullptr, EPI_NONE, l.attn_norm, false, false, 1, none, nullptr);
+        ops.back().kc = kc + (size_t)j * layer_stride;
+        ops.back().vc = vc + (size_t)j * layer_stride;
         MegaOp a;
         a.kind = MG_ATTN;
         a.kc = kc + (size_t)j * layer_stride;
@@ -1039,9 +1042,13 @@ void Session::decode_step_mega(int b0, int B, bool add_audio) {
     p.rope_rows = dec_rope.rows;
     p.ring = kv_ring ? 1 : 0;
     p.attn_out = attn_dec;
-    // key chunks per (stream, kv head): spread the KV walk over idle SMs, but no more than 4 -- the merging CTA waits
-    // for the other chunks' states one after the other (an L2 round trip each), and a CTA walks 64 keys per round
-    // trip anyway, so more chunks add merge latency without shortening the walk
+    // key chunks per (stream, kv head): spread the keys over idle SMs in one wave, but no more than 4.  A CTA stages a
+    // chunk's keys in tiles (32 keys at B = 1, 64 at B = 2, 96 at B = 3..8 in this decoder's
+    // scratch region, decode_mega_plan) with one L2 round trip and four CTA
+    // barriers per tile, while the merging CTA polls the other chunks' states one after the other, so chunks beyond
+    // what keeps a unit to a tile or two add merge latency without shortening the walk.  B = 8: 64 (stream, kv head)
+    // pairs, 2 chunks = 128 units on 132 SMs (3 would take a second wave).  B = 1: 8 pairs, 4 chunks = 32 units, at
+    // most 2 tiles each for the first ~250 positions.
     p.attn_chunks = std::max(1, std::min(4, std::min(mega_grid, mega_att_units - 8 * c.dec_kv_heads) / (B * c.dec_kv_heads)));
     p.att_acc = mega_att_acc;
     p.att_ml = mega_att_ml;
