@@ -281,7 +281,9 @@ int32_t vox_session_reset(vox_session *s);                                      
 /* debugging / parity: copy an internal activation by name ("enc_out","audio_embeds","conv","enc<i>",
  * "logits","ada") to host; "mega_trace" = SM-clock phase stamps of the last persistent decode step
  * (6 floats per phase, microseconds); "mega_epoch" = {persistent-kernel launches the host has counted
- * since the last epoch re-base, the device epoch} (equal between calls); names of the form "<switch>_on|_off|_auto" (graph, tc, gemm_tc |
+ * since the last epoch re-base, the device epoch} (equal between calls); "mega_attn" = the attention
+ * tiling of each persistent launch of the last decode step, 4 floats per launch {rows, token capacity,
+ * keys per K/V tile, key chunks per (stream, kv head)} (none after a per-op step); names of the form "<switch>_on|_off|_auto" (graph, tc, gemm_tc |
  * gemm_simt, enc_attn_tc | enc_attn_simt, mega, capture) flip a kernel-selection switch and return no
  * data (INTEGRATION.md section 5) */
 int32_t vox_session_debug_read(vox_session *s, const char *what, float *out, size_t cap_floats,

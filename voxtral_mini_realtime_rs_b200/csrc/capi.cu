@@ -892,6 +892,16 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
             memcpy(out, v, sizeof(v));
         }
         return VOX_OK;
+    } else if (w == "mega_attn") {
+        // attention tiling of the last decode step: per persistent launch {rows, token capacity, keys per K/V tile, key
+        // chunks per (stream, kv head)}; nothing after a step on the per-op path
+        const size_t cnt = s->mega_attn_log.size() * 4;
+        if (n_floats) *n_floats = cnt;
+        if (out) {
+            VOX_CHECK(cap >= cnt, VOX_ECAPACITY, "debug_read capacity %zu < %zu", cap, cnt);
+            for (size_t i = 0; i < cnt; ++i) out[i] = (float)s->mega_attn_log[i / 4][i % 4];
+        }
+        return VOX_OK;
     } else if (w == "mega_trace") {
         // phase trace of the last persistent decode step (CTA 0): per op {start, staged, body done,
         // barrier passed, first weights ready | KV walked, last stage consumed} in microseconds since the first stamp; ops 0..mega_n_ops-1

@@ -1328,6 +1328,7 @@ MegaPlan decode_mega_plan(int B, int max_pairs, int H, int Hkv, int hd) {
     int scratch = pl.Ps_cap * per_pair;
     if (scratch < attn_bytes) scratch = attn_bytes;
     pl.scratch_bytes = (scratch + 127) & ~127;
+    pl.attn_tile = mg_attn_tile(pl.scratch_bytes, G, hd);
     const int left = MG_SMEM_MAX - mg_misc_bytes(pl.MT) - pl.scratch_bytes;
     const int stage_bytes = mg_nt(pl.MT) * MG_SLOT_BYTES;
     int ns = left / stage_bytes;

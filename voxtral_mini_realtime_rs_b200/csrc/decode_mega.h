@@ -111,6 +111,7 @@ struct MegaPlan {
     int Ps_cap = 0;         // pairs per K slice that fit the scratch region
     int scratch_bytes = 0;
     int nstage = 0;
+    int attn_tile = 0;      // keys per K/V tile of the attention phase (what the scratch region holds)
     size_t smem_bytes = 0;
 };
 

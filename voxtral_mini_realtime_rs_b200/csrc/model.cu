@@ -929,6 +929,7 @@ unsigned Session::prepare_step(int R) {
 // 26 layers, lm_head, argmax, device-side feedback; all positions read from device counters.
 unsigned Session::decode_step(int B, bool add_audio) {
     const unsigned mega_launches = prepare_step(B);
+    mega_attn_log.clear();
     if (mega_launches > 0) {
         for (int b0 = 0; b0 < B; b0 += 8) decode_step_mega(b0, std::min(8, B - b0), add_audio);
     } else {
@@ -1079,6 +1080,7 @@ void Session::decode_step_mega(int b0, int B, bool add_audio) {
     p.scratch_bytes = mega_plan.scratch_bytes;
     p.trace = mega_trace;
     p.trace_all = mega_trace_all;
+    mega_attn_log.push_back({B, mega_plan.MT, mega_plan.attn_tile, p.attn_chunks});
     launch_decode_mega(p, mega_plan, mega_grid, st);
 }
 

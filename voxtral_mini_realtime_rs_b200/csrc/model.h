@@ -3,6 +3,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <array>
 #include <cstdint>
 #include <functional>
 #include <string>
@@ -241,6 +242,9 @@ struct Session {
     // persistent-kernel launches executed since the device epoch was last re-based (Session::reset): advanced by the
     // code that issues or replays steps, never under stream capture
     unsigned mega_steps_host = 0;
+    // attention tiling of each persistent launch of the last decode step issued or captured (debug "mega_attn"): {rows,
+    // token capacity MT, keys per K/V tile, key chunks per (stream, kv head)}; empty after a per-op step
+    std::vector<std::array<int, 4>> mega_attn_log;
     // activation fragments (decode_mega.cu frag_build): residual stream x norm weight, attention output, SwiGLU output
     uint2 *mega_xf_bf = nullptr, *mega_af_bf = nullptr, *mega_cf_bf = nullptr;
     float2 *mega_xf_off = nullptr, *mega_af_off = nullptr, *mega_cf_off = nullptr;
