@@ -276,6 +276,36 @@ int32_t vox_session_set_beam(vox_session *s, int32_t width);
  * (descending per stream); ids needs cap >= b * w * n elements and scores b * w.  Synchronises the session's stream.  Both
  * buffers NULL: only *b, *w, *n are set.  VOX_EINVAL if that call ran at width 1, VOX_ECAPACITY if cap is short. */
 int32_t vox_session_nbest(vox_session *s, int32_t *ids, double *scores, size_t cap, int32_t *b, int32_t *w, int32_t *n);
+/* Phrase boosting (custom vocabulary) for greedy decoding: vox_transcribe_streaming, vox_transcribe_pcm,
+ * vox_transcribe_pcm_ragged, vox_transcribe_pcm_dev, vox_prefill, vox_decode_step and streaming pools.
+ *   - A stream's bias list holds up to VOX_MAX_BIAS_PHRASES phrases.  A phrase is 1 to VOX_MAX_BIAS_LEN token ids, each
+ *     in [VOX_FIRST_TEXT_ID, vocab), with a boost b > 0 (finite, in logit units).  Callers tokenize their phrases
+ *     themselves; a word's ids depend on its leading space, so a list may hold both forms.
+ *   - The stream's history h is the sequence of text ids (>= VOX_FIRST_TEXT_ID) it has emitted since the history was
+ *     last cleared; lower (special) ids, [STREAMING_PAD] among them, never enter it.  The history is cleared whenever the
+ *     decoder cache is emptied (every transcribe call, vox_session_reset, a pool session's prefill) and when the stream's
+ *     list is set.
+ *   - At every position the stream emits (the prefill's output included), candidate id t gets
+ *         boost(t) = max { b_i : phrase i, 0 <= j < len_i, the last j ids of h equal phrase_i[0..j), phrase_i[j] = t }
+ *     or 0 when no phrase offers t: the first id of every phrase is always offered, a continuation only while the
+ *     history ends in the phrase's prefix.  The emitted id is the argmax of (float)(logit(t) + boost(t)) over the whole
+ *     vocabulary, the lowest id winning a tie: the greedy rule applied to boosted logits.  The logits themselves are
+ *     unchanged (vox_session_debug_read "logits", token scores: top_ids[0] is the unboosted argmax and need not be the
+ *     emitted id).
+ *   - With no list (the default) a stream decodes exactly as before.  While some stream of a session has a list, every
+ *     prefill and decode step costs one extra kernel launch; device memory (about 18 KB per stream) is allocated by the
+ *     first non-empty list.
+ *   - A transcribe call at beam width > 1 while any stream has a list returns VOX_EINVAL before any device work.
+ *     vox_generate_step_with_cache and vox_forward_streaming emit nothing and are unaffected.
+ * Phrase p is ids[off_p .. off_p + lens[p]) with off_p = lens[0] + ... + lens[p-1]; n_phrases = 0 clears the list.
+ * stream in [0, max_batch), or -1 for every stream.  VOX_EINVAL for an unknown stream, n_phrases outside
+ * [0, VOX_MAX_BIAS_PHRASES], a length outside [1, VOX_MAX_BIAS_LEN], an id outside [VOX_FIRST_TEXT_ID, vocab), a boost
+ * that is not finite and > 0, or NULL buffers with n_phrases > 0; a refused call changes nothing. */
+#define VOX_FIRST_TEXT_ID 1000
+#define VOX_MAX_BIAS_PHRASES 256
+#define VOX_MAX_BIAS_LEN 16
+int32_t vox_session_set_bias(vox_session *s, int32_t stream, const int32_t *ids, const int32_t *lens, const float *boosts,
+                             int32_t n_phrases);
 int32_t vox_session_cache_len(const vox_session *s, int32_t *len);             /* LayerCaches::seq_len */
 int32_t vox_session_reset(vox_session *s);                                       /* LayerCaches::reset  */
 /* debugging / parity: copy an internal activation by name ("enc_out","audio_embeds","conv","enc<i>",
@@ -320,6 +350,10 @@ int32_t vox_stream_open(vox_stream_pool *p, int32_t *session);
  * unknown session or a delay that is not finite and >= 0.  VOX_ECUDA without a device, before the arguments are checked.
  * Sessions at different delays share one decode step. */
 int32_t vox_stream_set_delay(vox_stream_pool *p, int32_t session, float delay_tokens);
+/* the session's bias list (see vox_session_set_bias), same arguments and errors; VOX_EINVAL for a session that is not
+ * open.  It takes effect at the session's next decoder position and clears its history; vox_stream_open empties it. */
+int32_t vox_stream_set_bias(vox_stream_pool *p, int32_t session, const int32_t *ids, const int32_t *lens, const float *boosts,
+                            int32_t n_phrases);
 int32_t vox_stream_push_pcm(vox_stream_pool *p, int32_t session, const float *samples, size_t n);
 int32_t vox_stream_finish(vox_stream_pool *p, int32_t session);        /* end of utterance: right padding, pad.rs:89-103 */
 int32_t vox_stream_tick(vox_stream_pool *p, vox_stream_stats *stats /* nullable */);

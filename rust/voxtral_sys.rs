@@ -78,6 +78,10 @@ extern "C" {
     pub fn vox_session_set_beam(s: *mut vox_session, width: i32) -> i32;
     pub fn vox_session_nbest(s: *mut vox_session, ids: *mut i32, scores: *mut f64, cap: usize, b: *mut i32, w: *mut i32,
                              n: *mut i32) -> i32;
+    // phrase boosting (custom vocabulary): phrase p is ids[off_p .. off_p + lens[p]); stream -1 = every stream;
+    // n_phrases = 0 clears
+    pub fn vox_session_set_bias(s: *mut vox_session, stream: i32, ids: *const i32, lens: *const i32, boosts: *const f32,
+                                n_phrases: i32) -> i32;
     pub fn vox_session_free(s: *mut vox_session);
     // src/gguf/{tensor,linear,op}.rs
     pub fn vox_q4_tensor_create(bytes: *const u8, nbytes: usize, n: i64, k: i64, device: i32,
@@ -102,6 +106,8 @@ extern "C" {
     pub fn vox_stream_pool_create(m: *mut vox_model, max_sessions: i32, max_seconds: f32, out: *mut *mut vox_stream_pool) -> i32;
     pub fn vox_stream_open(p: *mut vox_stream_pool, session: *mut i32) -> i32;
     pub fn vox_stream_set_delay(p: *mut vox_stream_pool, session: i32, delay_tokens: f32) -> i32;
+    pub fn vox_stream_set_bias(p: *mut vox_stream_pool, session: i32, ids: *const i32, lens: *const i32, boosts: *const f32,
+                               n_phrases: i32) -> i32;
     pub fn vox_stream_push_pcm(p: *mut vox_stream_pool, session: i32, samples: *const f32, n: usize) -> i32;
     pub fn vox_stream_finish(p: *mut vox_stream_pool, session: i32) -> i32;
     pub fn vox_stream_tick(p: *mut vox_stream_pool, stats: *mut vox_stream_stats) -> i32;

@@ -139,6 +139,7 @@ _SIGS = {
     "vox_session_set_beam": (C.c_int32, [_P, C.c_int32]),
     "vox_session_nbest": (C.c_int32, [_P, _P, _P, C.c_size_t, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
                                       C.POINTER(C.c_int32)]),
+    "vox_session_set_bias": (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32]),
     "vox_session_cache_len": (C.c_int32, [_P, C.POINTER(C.c_int32)]),
     "vox_session_reset": (C.c_int32, [_P]),
     "vox_session_debug_read": (C.c_int32, [_P, C.c_char_p, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
@@ -147,6 +148,7 @@ _SIGS = {
     "vox_stream_pool_create": (C.c_int32, [_P, C.c_int32, C.c_float, C.POINTER(_P)]),
     "vox_stream_open": (C.c_int32, [_P, C.POINTER(C.c_int32)]),
     "vox_stream_set_delay": (C.c_int32, [_P, C.c_int32, C.c_float]),
+    "vox_stream_set_bias": (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32]),
     "vox_stream_push_pcm": (C.c_int32, [_P, C.c_int32, _P, C.c_size_t]),
     "vox_stream_finish": (C.c_int32, [_P, C.c_int32]),
     "vox_stream_tick": (C.c_int32, [_P, _P]),
@@ -194,6 +196,18 @@ def _check(code: int):
 
 def device_count() -> int:
     return int(lib().vox_device_count())
+
+
+def _bias_args(phrases, boost):
+    """(ids, lens, boosts, n) of vox_session_set_bias for a list of id phrases and one boost or one per phrase."""
+    phrases = [[int(t) for t in p] for p in phrases]
+    n = len(phrases)
+    boosts = np.broadcast_to(np.asarray(boost, np.float32), (n,)).copy()
+    lens = np.array([len(p) for p in phrases], np.int32)
+    ids = np.array([t for p in phrases for t in p], np.int32)
+    keep = [ids, lens, boosts]
+    ptr = (lambda a: _ptr(a) if a.size else None)
+    return keep, ptr(ids), ptr(lens), ptr(boosts), n
 
 
 def _f32(a) -> np.ndarray:
@@ -775,6 +789,15 @@ class Q4VoxtralModel:
         _check(lib().vox_session_nbest(self._s, _ptr(ids), _ptr(scores), ids.size, C.byref(b), C.byref(w), C.byref(n)))
         return ids, scores
 
+    def set_bias(self, phrases, boost, stream: int | None = None):
+        """Phrase boosting for greedy decoding: `phrases` is a list of token-id lists (ids >= 1000, up to 16 each, up to
+        256 phrases), `boost` one float > 0 (logit units) or one per phrase.  At every emitted position the first id of
+        every phrase, and the next id of every phrase whose prefix the stream's recent text ids end in, are boosted; the
+        emitted id is the argmax of the boosted logits.  stream None: every stream; an empty list clears.  See
+        vox_session_set_bias in include/voxtral.h."""
+        _keep, ids, lens, boosts, n = _bias_args(phrases, boost)
+        _check(lib().vox_session_set_bias(self._s, -1 if stream is None else stream, ids, lens, boosts, n))
+
     def cache_len(self) -> int:
         v = C.c_int32()
         _check(lib().vox_session_cache_len(self._s, C.byref(v)))
@@ -856,6 +879,12 @@ class StreamingPool:
     def set_delay(self, session: int, delay: float):
         """The session's transcription delay; only before its prefill (session_info()["decoder_positions"] == 0)."""
         _check(lib().vox_stream_set_delay(self._p, session, delay))
+
+    def set_bias(self, session: int, phrases, boost):
+        """The session's phrase list (Q4VoxtralModel.set_bias); from its next decoder position.  open() starts a session
+        with none."""
+        _keep, ids, lens, boosts, n = _bias_args(phrases, boost)
+        _check(lib().vox_stream_set_bias(self._p, session, ids, lens, boosts, n))
 
     def push(self, session: int, samples):
         s = _f32(samples).reshape(-1)

@@ -567,6 +567,7 @@ int32_t vox_transcribe_streaming(vox_session *sh, const float *mel, int32_t b, i
     VOX_API_BEGIN
     REQUIRE(sh); REQUIRE(mel); REQUIRE(out_ids); REQUIRE(n_out);
     Session *s = sh->s;
+    s->check_beam_bias();
     CUDA_OK(cudaSetDevice(s->m->device));
     CUDA_OK(cudaEventRecord(s->ev[0], s->st));
     upload_mel(s, mel, b, t);
@@ -579,6 +580,7 @@ int32_t vox_transcribe_streaming(vox_session *sh, const float *mel, int32_t b, i
 static int32_t transcribe_pcm_impl(Session *s, const float *host, const float *dev, int b, size_t n, int normalize,
                                    int32_t *out_ids, size_t cap, int32_t *n_out, vox_timings *tm) {
     s->check_batch(b);
+    s->check_beam_bias();
     VOX_CHECK(n >= 1, VOX_EINVAL, "empty audio");
     CUDA_OK(cudaSetDevice(s->m->device));
     vox_pad_config pc;
@@ -621,6 +623,7 @@ int32_t vox_transcribe_pcm_ragged(vox_session *sh, const float *samples, const s
     s->check_batch(b);
     VOX_CHECK(s->beam_w == 1 || b * s->beam_w <= s->max_batch, VOX_EINVAL, "beam width %d x %d streams exceeds session max_batch %d",
               s->beam_w, b, s->max_batch);
+    s->check_beam_bias();
     size_t total = 0;
     bool equal = true;
     for (int i = 0; i < b; ++i) {
@@ -795,6 +798,17 @@ int32_t vox_session_set_beam(vox_session *s, int32_t width) {
     VOX_API_BEGIN
     REQUIRE(s);
     s->s->set_beam(width);
+    VOX_API_END
+}
+static_assert(VOX_MAX_BIAS_PHRASES == BIAS_MAX_PHRASES && VOX_MAX_BIAS_LEN == BIAS_MAX_LEN &&
+                  VOX_FIRST_TEXT_ID == BIAS_FIRST_TEXT_ID,
+              "the bias kernel's limits are the header's");
+int32_t vox_session_set_bias(vox_session *sh, int32_t stream, const int32_t *ids, const int32_t *lens, const float *boosts,
+                             int32_t n_phrases) {
+    VOX_API_BEGIN
+    require_any_device();
+    REQUIRE(sh);
+    sh->s->set_bias(stream, ids, lens, boosts, n_phrases);
     VOX_API_END
 }
 int32_t vox_session_nbest(vox_session *sh, int32_t *ids, double *scores, size_t cap, int32_t *b, int32_t *w, int32_t *n) {
@@ -1070,6 +1084,14 @@ int32_t vox_stream_set_delay(vox_stream_pool *p, int32_t session, float delay_to
     require_any_device();
     REQUIRE(p);
     p->p->set_delay(session, delay_tokens);
+    VOX_API_END
+}
+int32_t vox_stream_set_bias(vox_stream_pool *p, int32_t session, const int32_t *ids, const int32_t *lens, const float *boosts,
+                            int32_t n_phrases) {
+    VOX_API_BEGIN
+    require_any_device();
+    REQUIRE(p);
+    p->p->set_bias(session, ids, lens, boosts, n_phrases);
     VOX_API_END
 }
 int32_t vox_stream_session_info(vox_stream_pool *p, int32_t session, struct vox_stream_session_info *out) {

@@ -260,6 +260,27 @@ void launch_beam_fork(float *kc, float *vc, size_t layer_stride, int layers, int
                       const int *src, int rows, int Hkv, int hd, cudaStream_t st);
 void launch_beam_traceback(const BeamWork &w, int b, int W, int n, int out_ld, int *ids, double *scores, int *out,
                            int *top_ids, float *top_lp, cudaStream_t st, int s0 = 0, int out_stride = 1);
+// Phrase boosting (vox_session_set_bias, bias.cu).  Stream s's list: n_phrases[s] phrases, phrase i of lens[...] ids at
+// ids + (s * BIAS_MAX_PHRASES + i) * BIAS_MAX_LEN with boost boosts[s * BIAS_MAX_PHRASES + i]; its history: the last
+// hist[s][BIAS_HIST] (<= BIAS_HIST) text ids it emitted, oldest first, in hist[s][0..).  Every stream's list sits at a
+// fixed offset, so a captured step reads whatever list is set when it replays.
+constexpr int BIAS_MAX_PHRASES = 256;   // VOX_MAX_BIAS_PHRASES
+constexpr int BIAS_MAX_LEN = 16;        // VOX_MAX_BIAS_LEN
+constexpr int BIAS_FIRST_TEXT_ID = 1000;   // VOX_FIRST_TEXT_ID: lower ids never enter a history
+constexpr int BIAS_HIST = BIAS_MAX_LEN - 1;   // a phrase's longest matched prefix
+struct BiasLists {
+    int *ids = nullptr;        // [streams][BIAS_MAX_PHRASES][BIAS_MAX_LEN]
+    int *lens = nullptr;       // [streams][BIAS_MAX_PHRASES]
+    float *boosts = nullptr;   // [streams][BIAS_MAX_PHRASES]
+    int *n_phrases = nullptr;  // [streams]
+    int *hist = nullptr;       // [streams][BIAS_HIST + 1]: ids, then their count
+};
+// After the step's argmax and counter advance, per row r of stream row_stream[r] with a non-empty list: the argmax of
+// fl32(logit(t) + boost(t)) (lowest id on ties) over the greedy id tok[r] and the ids the list offers after the stream's
+// history, into tok[r] and out_ids[r * out_ld + out_pos[r] - 1]; a winner >= BIAS_FIRST_TEXT_ID joins the history.
+// One CTA per row; a row whose stream has no list leaves at once.
+void launch_bias_select(const float *logits, int B, int V, const int *row_stream, const BiasLists &lists, int *tok, int *out_ids,
+                        int out_ld, const int *out_pos, cudaStream_t st);
 // a[i] += da; b[i] += db for i < n  (device-side per-row step counters for graph replay)
 void launch_advance(int *a, int da, int *b, int db, int n, cudaStream_t st);
 // gather rows: dst[b][:] = src[b*M + (M-1)][:]

@@ -464,6 +464,7 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ri
         s->logits = s->arena.alloc_n<float>(B * c.vocab);
         s->ada_sets = s->arena.alloc_n<float>(B * s->ada_set_floats());
         s->delays.assign(B, 0.0f);
+        s->bias_n.assign(B, 0);
         s->d_ada_rows = (const float **)s->arena.alloc(sizeof(float *) * B);
         s->d_fga_rows = (const float **)s->arena.alloc(sizeof(float *) * B);
         s->d_audio_off = s->arena.alloc_n<int64_t>(B);
@@ -652,6 +653,7 @@ void Session::bind_rows(int B) {
     CUDA_OK(cudaMemcpyAsync(d_ada_rows, a.data(), sizeof(float *) * B, cudaMemcpyHostToDevice, st));
     CUDA_OK(cudaMemcpyAsync(d_fga_rows, f.data(), sizeof(float *) * B, cudaMemcpyHostToDevice, st));
     CUDA_OK(cudaMemcpyAsync(d_audio_off, offs.data(), sizeof(int64_t) * B, cudaMemcpyHostToDevice, st));
+    if (d_row_stream) CUDA_OK(cudaMemcpyAsync(d_row_stream, streams.data(), sizeof(int) * B, cudaMemcpyHostToDevice, st));
     CUDA_OK(cudaStreamSynchronize(st));   // the staging vectors die with this frame
     bound_streams = std::move(streams);
     bound_offs = std::move(offs);
@@ -940,7 +942,8 @@ unsigned Session::decode_step(int B, bool add_audio) {
         launch_argmax_multi(logits, B, m->info.vocab, d_tok, d_out, out_ld, d_outpos, am_vals, am_idx, am_cnt, st);
         launch_advance(d_pos, 1, d_outpos, 1, B, st);
     }
-    token_scores(B);   // one launch over every row (every group of the persistent kernel's)
+    bias_select(B);    // one launch over every row (every group of the persistent kernel's) ...
+    token_scores(B);   // ... and so is this one
     return mega_launches;
 }
 
@@ -969,6 +972,70 @@ void Session::token_scores(int B) {
     // at W > 1 every step belongs to a beam call (the incremental calls refuse to run), whose selection reads W candidates
     const int k = std::max(top_k, beam_w > 1 ? beam_w : 0);
     if (k > 0) launch_token_scores(logits, B, m->info.vocab, k, d_outpos, out_ld, d_top_ids, d_top_lp, score_work, st);
+}
+
+void Session::set_bias(int stream, const int32_t *ids, const int32_t *lens, const float *boosts, int n) {
+    VOX_CHECK(stream >= -1 && stream < max_batch, VOX_EINVAL, "set_bias: stream %d out of range [0,%d) (or -1 for every stream)",
+              stream, max_batch);
+    VOX_CHECK(n >= 0 && n <= BIAS_MAX_PHRASES, VOX_EINVAL, "set_bias: %d phrases out of range [0,%d]", n, BIAS_MAX_PHRASES);
+    VOX_CHECK(n == 0 || (ids && lens && boosts), VOX_EINVAL, "set_bias: NULL ids, lens or boosts with %d phrases", n);
+    // phrase p is ids[off_p .. off_p + lens[p]), padded to BIAS_MAX_LEN ids in the device layout
+    std::vector<int> packed((size_t)n * BIAS_MAX_LEN, 0), hist(BIAS_HIST + 1, 0);
+    for (int p = 0, off = 0; p < n; off += lens[p], ++p) {
+        VOX_CHECK(lens[p] >= 1 && lens[p] <= BIAS_MAX_LEN, VOX_EINVAL, "set_bias: phrase %d has %d ids (1..%d)", p, lens[p],
+                  BIAS_MAX_LEN);
+        VOX_CHECK(std::isfinite(boosts[p]) && boosts[p] > 0.0f, VOX_EINVAL, "set_bias: boost %g of phrase %d must be finite and > 0",
+                  boosts[p], p);
+        for (int j = 0; j < lens[p]; ++j) {
+            const int t = ids[off + j];
+            VOX_CHECK(t >= BIAS_FIRST_TEXT_ID && t < m->info.vocab, VOX_EINVAL, "set_bias: id %d of phrase %d outside [%d,%d)", t, p,
+                      BIAS_FIRST_TEXT_ID, m->info.vocab);
+            packed[(size_t)p * BIAS_MAX_LEN + j] = t;
+        }
+    }
+    if (n == 0 && !bias.ids) return;   // nothing was ever set: nothing to clear
+    CUDA_OK(cudaSetDevice(m->device));
+    if (!bias.ids) {
+        const size_t S = max_batch;
+        bias.ids = arena.alloc_n<int>(S * BIAS_MAX_PHRASES * BIAS_MAX_LEN);
+        bias.lens = arena.alloc_n<int>(S * BIAS_MAX_PHRASES);
+        bias.boosts = arena.alloc_n<float>(S * BIAS_MAX_PHRASES);
+        bias.n_phrases = arena.alloc_n<int>(S);
+        bias.hist = arena.alloc_n<int>(S * (BIAS_HIST + 1));
+        d_row_stream = arena.alloc_n<int>(S);
+        CUDA_OK(cudaMemsetAsync(bias.n_phrases, 0, sizeof(int) * S, st));
+        CUDA_OK(cudaMemsetAsync(bias.hist, 0, sizeof(int) * S * (BIAS_HIST + 1), st));
+        bound_streams.clear();   // the next bind_rows fills the row table
+    }
+    for (int s = stream < 0 ? 0 : stream; s < (stream < 0 ? max_batch : stream + 1); ++s) {
+        const size_t p0 = (size_t)s * BIAS_MAX_PHRASES;
+        if (n > 0) {
+            CUDA_OK(cudaMemcpyAsync(bias.ids + p0 * BIAS_MAX_LEN, packed.data(), sizeof(int) * packed.size(), cudaMemcpyHostToDevice, st));
+            CUDA_OK(cudaMemcpyAsync(bias.lens + p0, lens, sizeof(int) * n, cudaMemcpyHostToDevice, st));
+            CUDA_OK(cudaMemcpyAsync(bias.boosts + p0, boosts, sizeof(float) * n, cudaMemcpyHostToDevice, st));
+        }
+        CUDA_OK(cudaMemcpyAsync(bias.n_phrases + s, &n, sizeof(int), cudaMemcpyHostToDevice, st));
+        CUDA_OK(cudaMemcpyAsync(bias.hist + (size_t)s * (BIAS_HIST + 1), hist.data(), sizeof(int) * hist.size(),
+                                cudaMemcpyHostToDevice, st));
+        bias_n[s] = n;
+    }
+    CUDA_OK(cudaStreamSynchronize(st));   // the staging vectors and the caller's buffers
+}
+
+void Session::clear_bias_history(int stream) {
+    if (!bias.hist) return;
+    const size_t per = BIAS_HIST + 1;
+    if (stream < 0) CUDA_OK(cudaMemsetAsync(bias.hist, 0, sizeof(int) * max_batch * per, st));
+    else CUDA_OK(cudaMemsetAsync(bias.hist + (size_t)stream * per, 0, sizeof(int) * per, st));
+}
+
+void Session::bias_select(int B) {
+    if (bias_on()) launch_bias_select(logits, B, m->info.vocab, d_row_stream, bias, d_tok, d_out, out_ld, d_outpos, st);
+}
+
+void Session::check_beam_bias() const {
+    VOX_CHECK(beam_w == 1 || !bias_on(), VOX_EINVAL, "beam search (width %d) does not take phrase boosting: clear the bias lists",
+              beam_w);
 }
 
 static_assert(BEAM_MAX <= TOPK_MAX, "a beam's candidates are the first W entries of its row's top-k list");
@@ -1100,6 +1167,7 @@ void Session::prefill(int B, int M, const int *ids_host, bool add_audio) {
     linear(m->tok_emb, last_h, B, logits, c.vocab, nullptr, nullptr, EPI_NONE);
     launch_argmax(logits, B, c.vocab, d_tok, d_out, out_ld, d_outpos, st);
     launch_advance(d_pos, M, d_outpos, 1, B, st);
+    bias_select(B);
     token_scores(B);
 }
 
@@ -1123,6 +1191,7 @@ void Session::reset() {
                                 cudaMemcpyHostToDevice, st));
         page_table_forked = false;
     }
+    clear_bias_history(-1);
     rebase_epoch();
 }
 
@@ -1147,7 +1216,7 @@ template <class Step>
 void Session::run_steps(int R, int n, Step step) {
     if (n <= 0) return;
     prepare_step(R);
-    const StepKey key{R, top_k, beam_w, path.matvec_tc, path.gemm_tc, use_mega};
+    const StepKey key{R, top_k, beam_w, path.matvec_tc, path.gemm_tc, use_mega, bias_on()};
     if (use_graph && !(step_graph.exec && step_graph.key == key)) {
         // first step eagerly (also performs any one-time kernel attribute setup), then capture one step and replay it
         mega_steps_host += step();

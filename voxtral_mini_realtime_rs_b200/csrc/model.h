@@ -3,6 +3,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <array>
 #include <cstdint>
 #include <functional>
@@ -111,8 +112,8 @@ constexpr float kDefaultDelay = 6.0f;
 // other kernels or reads another op table.
 struct StepKey {
     int rows = 0, top_k = 0, beam_w = 1;
-    bool matvec_tc = true, gemm_tc = true, use_mega = true;
-    auto tie() const { return std::tie(rows, top_k, beam_w, matvec_tc, gemm_tc, use_mega); }
+    bool matvec_tc = true, gemm_tc = true, use_mega = true, bias = false;
+    auto tie() const { return std::tie(rows, top_k, beam_w, matvec_tc, gemm_tc, use_mega, bias); }
     bool operator==(const StepKey &o) const { return tie() == o.tie(); }
 };
 struct StepGraph {
@@ -203,6 +204,19 @@ struct Session {
     void set_beam(int w);
     void beam_start(int b);         // after the prefill of rows [0, b): start every beam row there, select position 0
     void beam_step(int b, int n_live);   // selection + KV fork after a step over the b * beam_w rows
+    // phrase boosting (vox_session_set_bias): per-stream lists and histories at fixed offsets (kernels.h BiasLists),
+    // allocated by the first non-empty list, with the stream of each row (bind_rows fills it once they exist).  While
+    // some stream has a list, every prefill and decode step ends with one launch_bias_select over its rows.
+    BiasLists bias;
+    std::vector<int> bias_n;        // phrases per stream
+    int *d_row_stream = nullptr;    // [max_batch]
+    bool bias_on() const { return std::any_of(bias_n.begin(), bias_n.end(), [](int n) { return n > 0; }); }
+    // stream's list (-1: every stream's) := the n phrases of ids / lens / boosts (vox_session_set_bias), its history
+    // cleared; every argument is checked before anything changes
+    void set_bias(int stream, const int32_t *ids, const int32_t *lens, const float *boosts, int n);
+    void clear_bias_history(int stream);   // -1: every stream's; on st
+    void bias_select(int B);               // rows [0, B) of the step that just ran; no-op while no stream has a list
+    void check_beam_bias() const;          // a beam transcribe call with a list set is refused
     // Where the results of the last call are, per stream in the caller's order; the getters copy them from the device
     // when asked (the buffers outlive reset()).  Token scores, of the last transcribe or incremental call: entries
     // [pos0, pos0 + n) of row `row` of d_top_ids / d_top_lp, scored with k = scores_k (0: that call ran with scores

@@ -238,7 +238,8 @@ int StreamPool::open() {
             sl.n_samples = pad_left(pad);
             CUDA_OK(cudaSetDevice(m->device));
             CUDA_OK(cudaMemsetAsync(pcm + (size_t)i * cap_samples, 0, sizeof(float) * cap_samples, s->st));
-            s->set_stream_delay(i, kDefaultDelay);   // a reused slot does not inherit the previous session's delay
+            s->set_stream_delay(i, kDefaultDelay);   // a reused slot does not inherit the previous session's delay ...
+            if (s->bias_n[i] > 0) s->set_bias(i, nullptr, nullptr, nullptr, 0);   // ... or its phrase list
             return i;
         }
     fail(VOX_ECAPACITY, fmt("all %d stream sessions are in use", max_sessions));
@@ -250,6 +251,11 @@ void StreamPool::set_delay(int id, float delay) {
     VOX_CHECK(std::isfinite(delay) && delay >= 0.0f, VOX_EINVAL, "delay %g must be finite and >= 0", delay);
     CUDA_OK(cudaSetDevice(m->device));
     s->set_stream_delay(id, delay);
+}
+
+void StreamPool::set_bias(int id, const int32_t *ids, const int32_t *lens, const float *boosts, int n) {
+    slot(id);
+    s->set_bias(id, ids, lens, boosts, n);
 }
 
 StreamPool::Slot &StreamPool::slot(int id) {
@@ -456,6 +462,7 @@ void StreamPool::tick(vox_stream_stats *st_out) {
             ensure_pages(sl, P + 1);
             if (unbounded) fill_rope(dec_rope_cos, dec_rope_sin, c.dec_head_dim, kDecRopeRing, 0, 0, P);
             upload_rows({id}, false);
+            s->clear_bias_history(id);   // the slot's decoder cache starts empty
             std::vector<int> prefix((size_t)P, 32);
             prefix[0] = 1;
             s->prefill(1, P, prefix.data(), true);

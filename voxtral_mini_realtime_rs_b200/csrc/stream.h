@@ -52,6 +52,8 @@ struct StreamPool {
     int open();   // the new session runs at kDefaultDelay
     // the session's transcription delay (its own ADA set); only before its prefill has run
     void set_delay(int id, float delay);
+    // session id's phrase list (Session::set_bias on its slot); open() empties it, and its prefill clears its history
+    void set_bias(int id, const int32_t *ids, const int32_t *lens, const float *boosts, int n);
     void push(int id, const float *samples, size_t n);
     void finish(int id);
     void close(int id);
