@@ -169,6 +169,19 @@ typedef struct {
 } vox_timings;
 /* max_batch concurrent streams, up to max_mel_frames mel frames per stream */
 int32_t vox_session_create(vox_model *m, int32_t max_batch, int32_t max_mel_frames, vox_session **out);
+/* Decoder KV cache element type, chosen at creation and fixed for the session's (or pool's) lifetime.
+ *   VOX_DTYPE_F32 (what vox_session_create / vox_stream_pool_create use): K after RoPE and V are cached as computed.
+ *   VOX_DTYPE_F16: half the KV memory and half the attention's K/V traffic.  K after RoPE and V are stored as IEEE
+ *     binary16: each value is clamped to [-65504, 65504], then rounded to nearest even, so a value outside the f16 range
+ *     stores +-65504, never +-inf; NaN stays NaN.  Every attention path (prefill, decode step, persistent kernel,
+ *     per-op paths) reads the stored values, including the current position's own key and value, widens them exactly to
+ *     f32 and computes as with an f32 cache, so all paths compute the same function.  Nothing else changes:
+ *     activations, logits, weights, the encoder and its K/V rings, token scores, beams and bias work as before.
+ *   Any other kv_dtype: VOX_EINVAL, and *out is left untouched. */
+int32_t vox_session_create_ex(vox_model *m, int32_t max_batch, int32_t max_mel_frames, int32_t kv_dtype, vox_session **out);
+/* bytes of device memory the session allocated (all of it at creation; the first set_top_k / set_beam / set_bias and
+ * the debug captures add their buffers) -- for sizing servers without querying the shared device */
+int32_t vox_session_device_bytes(const vox_session *s, uint64_t *bytes);
 /* TimeEmbedding::embed(delay) + the 26 ADA scale vectors (model.rs:250-255), once per session: every stream at
  * delay_tokens (80 ms each; 6.0 when the session is created) */
 int32_t vox_session_set_delay(vox_session *s, float delay_tokens);
@@ -313,7 +326,9 @@ int32_t vox_session_reset(vox_session *s);                                      
  * (6 floats per phase, microseconds); "mega_epoch" = {persistent-kernel launches the host has counted
  * since the last epoch re-base, the device epoch} (equal between calls); "mega_attn" = the attention
  * tiling of each persistent launch of the last decode step, 4 floats per launch {rows, token capacity,
- * keys per K/V tile, key chunks per (stream, kv head)} (none after a per-op step); names of the form "<switch>_on|_off|_auto" (graph, tc, gemm_tc |
+ * keys per K/V tile, key chunks per (stream, kv head)} (none after a per-op step); "kv_k<l>" / "kv_v<l>" = decoder layer l's
+ * cached K (after RoPE) or V for the rows of the last call, positions [0, cache length), as f32 [row][pos][kv_head][hd]
+ * (an f16 cache widened exactly; not on the ring-indexed sessions of an unbounded stream pool); names of the form "<switch>_on|_off|_auto" (graph, tc, gemm_tc |
  * gemm_simt, enc_attn_tc | enc_attn_simt, mega, capture) flip a kernel-selection switch and return no
  * data (INTEGRATION.md section 5) */
 int32_t vox_session_debug_read(vox_session *s, const char *what, float *out, size_t cap_floats,
@@ -344,6 +359,12 @@ typedef struct {
  * fixed when the pool is created.  push_pcm then fails with VOX_ECAPACITY while the audio not yet consumed by a tick
  * would exceed those 30 s; encode_chunk is not available.  Absolute positions stay int32: ~248 days of audio. */
 int32_t vox_stream_pool_create(vox_model *m, int32_t max_sessions, float max_seconds, vox_stream_pool **out);
+/* kv_dtype as vox_session_create_ex: every session of the pool shares its page pool, so they share the element type.
+ * An unbounded pool's state is dominated by the decoder KV ring; VOX_DTYPE_F16 halves it (INTEGRATION.md section 3b). */
+int32_t vox_stream_pool_create_ex(vox_model *m, int32_t max_sessions, float max_seconds, int32_t kv_dtype,
+                                  vox_stream_pool **out);
+/* bytes of device memory the pool allocated (its session's arena, which holds every per-session buffer) */
+int32_t vox_stream_pool_device_bytes(const vox_stream_pool *p, uint64_t *bytes);
 int32_t vox_stream_open(vox_stream_pool *p, int32_t *session);
 /* the session's transcription delay in tokens (80 ms each); default 6.0 on vox_stream_open.  Only before the session's
  * 38-position prefill has run (vox_stream_session_info.decoder_positions == 0), else VOX_EINVAL; also VOX_EINVAL for an

@@ -48,6 +48,10 @@ extern "C" {
     // src/gguf/model.rs
     pub fn vox_session_create(m: *mut vox_model, max_batch: i32, max_mel_frames: i32,
                               out: *mut *mut vox_session) -> i32;
+    // kv_dtype: VOX_DTYPE_F32 (0) or VOX_DTYPE_F16 (1), the decoder KV cache's element type
+    pub fn vox_session_create_ex(m: *mut vox_model, max_batch: i32, max_mel_frames: i32, kv_dtype: i32,
+                                 out: *mut *mut vox_session) -> i32;
+    pub fn vox_session_device_bytes(s: *const vox_session, bytes: *mut u64) -> i32;
     pub fn vox_session_set_delay(s: *mut vox_session, delay_tokens: f32) -> i32;
     pub fn vox_session_set_delays(s: *mut vox_session, delays: *const f32, b: i32) -> i32;
     pub fn vox_encode_audio(s: *mut vox_session, mel: *const f32, b: i32, t: i32,
@@ -104,6 +108,9 @@ extern "C" {
     pub fn vox_stream_progress(n_samples: usize, ended: i32, reshape_factor: i32, prefix_len: i32, out: *mut i64) -> i32;
     // streaming sessions: Q4AudioEncoder::forward_with_cache (model.rs:437-452), encode_audio_with_cache (790-799)
     pub fn vox_stream_pool_create(m: *mut vox_model, max_sessions: i32, max_seconds: f32, out: *mut *mut vox_stream_pool) -> i32;
+    pub fn vox_stream_pool_create_ex(m: *mut vox_model, max_sessions: i32, max_seconds: f32, kv_dtype: i32,
+                                     out: *mut *mut vox_stream_pool) -> i32;
+    pub fn vox_stream_pool_device_bytes(p: *const vox_stream_pool, bytes: *mut u64) -> i32;
     pub fn vox_stream_open(p: *mut vox_stream_pool, session: *mut i32) -> i32;
     pub fn vox_stream_set_delay(p: *mut vox_stream_pool, session: i32, delay_tokens: f32) -> i32;
     pub fn vox_stream_set_bias(p: *mut vox_stream_pool, session: i32, ids: *const i32, lens: *const i32, boosts: *const f32,

@@ -118,6 +118,8 @@ _SIGS = {
     "vox_model_get_info": (C.c_int32, [_P, C.POINTER(_ModelInfo)]),
     "vox_model_free": (None, [_P]),
     "vox_session_create": (C.c_int32, [_P, C.c_int32, C.c_int32, C.POINTER(_P)]),
+    "vox_session_create_ex": (C.c_int32, [_P, C.c_int32, C.c_int32, C.c_int32, C.POINTER(_P)]),
+    "vox_session_device_bytes": (C.c_int32, [_P, C.POINTER(C.c_uint64)]),
     "vox_session_set_delay": (C.c_int32, [_P, C.c_float]),
     "vox_session_set_delays": (C.c_int32, [_P, _P, C.c_int32]),
     "vox_encode_audio": (C.c_int32, [_P, _P, C.c_int32, C.c_int32, _P, C.c_size_t, C.POINTER(C.c_int32)]),
@@ -146,6 +148,8 @@ _SIGS = {
     "vox_session_launch_count": (C.c_int32, [_P, C.POINTER(C.c_uint64)]),
     "vox_session_free": (None, [_P]),
     "vox_stream_pool_create": (C.c_int32, [_P, C.c_int32, C.c_float, C.POINTER(_P)]),
+    "vox_stream_pool_create_ex": (C.c_int32, [_P, C.c_int32, C.c_float, C.c_int32, C.POINTER(_P)]),
+    "vox_stream_pool_device_bytes": (C.c_int32, [_P, C.POINTER(C.c_uint64)]),
     "vox_stream_open": (C.c_int32, [_P, C.POINTER(C.c_int32)]),
     "vox_stream_set_delay": (C.c_int32, [_P, C.c_int32, C.c_float]),
     "vox_stream_set_bias": (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32]),
@@ -559,11 +563,22 @@ def q4_matmul_bench(weights, m: int, iters: int = 200, warmup: int = 20) -> floa
     return ms.value
 
 
+# decoder KV cache element types (include/voxtral.h vox_session_create_ex): VOX_DTYPE_F32, VOX_DTYPE_F16
+KV_DTYPES = {"f32": 0, "f16": 1}
+
+
+def _kv_dtype(kv_dtype: str) -> int:
+    if kv_dtype not in KV_DTYPES:
+        raise ValueError(f"kv_dtype {kv_dtype!r}: one of {sorted(KV_DTYPES)}")
+    return KV_DTYPES[kv_dtype]
+
+
 # ------------------------------------------------------------------------------ model
 class Q4VoxtralModel:
     """Q4VoxtralModel (model.rs:759-989) + its session state (LayerCaches, workspace, stream)."""
 
-    def __init__(self, model_handle, device: int, max_batch: int = 1, max_mel_frames: int = 3000):
+    def __init__(self, model_handle, device: int, max_batch: int = 1, max_mel_frames: int = 3000,
+                 kv_dtype: str = "f32"):
         self._m = model_handle
         self.device = device
         info = _ModelInfo()
@@ -571,7 +586,14 @@ class Q4VoxtralModel:
         self.info = {f[0]: getattr(info, f[0]) for f in _ModelInfo._fields_}
         self._s = _P()
         self.max_batch, self.max_mel_frames = max_batch, max_mel_frames
-        _check(lib().vox_session_create(self._m, max_batch, max_mel_frames, C.byref(self._s)))
+        self.kv_dtype = kv_dtype
+        _check(lib().vox_session_create_ex(self._m, max_batch, max_mel_frames, _kv_dtype(kv_dtype), C.byref(self._s)))
+
+    def device_bytes(self) -> int:
+        """Device memory the session holds, in bytes (vox_session_device_bytes)."""
+        n = C.c_uint64()
+        _check(lib().vox_session_device_bytes(self._s, C.byref(n)))
+        return n.value
 
     def set_delay(self, delay_tokens: float):
         _check(lib().vox_session_set_delay(self._s, delay_tokens))
@@ -851,13 +873,21 @@ class StreamingPool:
     and must outlive the pool.  max_seconds=None: sessions of any length, with fixed device state (30 s of padded audio
     resident per session; see include/voxtral.h)."""
 
-    def __init__(self, model: "Q4VoxtralModel", max_sessions: int = 8, max_seconds: float | None = 30.0):
+    def __init__(self, model: "Q4VoxtralModel", max_sessions: int = 8, max_seconds: float | None = 30.0,
+                 kv_dtype: str = "f32"):
+        """kv_dtype: element type of the decoder KV cache the sessions share, "f32" or "f16" (include/voxtral.h)."""
         self._model = model
         self._p = _P()
-        _check(lib().vox_stream_pool_create(model._m, max_sessions, 0.0 if max_seconds is None else max_seconds,
-                                            C.byref(self._p)))
+        _check(lib().vox_stream_pool_create_ex(model._m, max_sessions, 0.0 if max_seconds is None else max_seconds,
+                                               _kv_dtype(kv_dtype), C.byref(self._p)))
         self.dec_dim = model.info["dec_dim"]
         self.top_k = 0
+
+    def device_bytes(self) -> int:
+        """Device memory the pool holds, in bytes (vox_stream_pool_device_bytes)."""
+        n = C.c_uint64()
+        _check(lib().vox_stream_pool_device_bytes(self._p, C.byref(n)))
+        return n.value
 
     def set_top_k(self, k: int):
         """Token confidences (Q4VoxtralModel.set_top_k) for every session of the pool; only while no session is open."""
@@ -983,10 +1013,13 @@ class Q4ModelLoader:
     def from_shards(shards) -> "Q4ModelLoader":
         return Q4ModelLoader(GgufReader.from_shards(shards))
 
-    def load(self, device: int = 0, max_batch: int = 1, max_mel_frames: int = 3000) -> Q4VoxtralModel:
+    def load(self, device: int = 0, max_batch: int = 1, max_mel_frames: int = 3000,
+             kv_dtype: str = "f32") -> Q4VoxtralModel:
+        """kv_dtype: element type of the session's decoder KV cache, "f32" or "f16" (include/voxtral.h)."""
+        _kv_dtype(kv_dtype)
         h = _P()
         _check(lib().vox_model_load_gguf_handle(self._reader._h, device, C.byref(h)))
-        return Q4VoxtralModel(h, device, max_batch, max_mel_frames)
+        return Q4VoxtralModel(h, device, max_batch, max_mel_frames, kv_dtype)
 
 
 # ------------------------------------------------------------------------------ tokenizer

@@ -89,8 +89,9 @@ void launch_beam_select(const int *top_ids, const float *top_lp, const int *out_
 // grid (rows, layers): a row whose beam came from another row q takes q's page-table entries of the full pages and a
 // copy of the filled part of q's current page into its own current page.  Full pages are never written again (a row
 // writes only its own page at the current logical index, which only grows), so sharing them is safe.
+template <typename KV>
 __global__ void __launch_bounds__(256)
-beam_fork_kernel(float *kc, float *vc, size_t layer_stride, int *page_table, int max_pages, const int *__restrict__ pos,
+beam_fork_kernel(KV *kc, KV *vc, size_t layer_stride, int *page_table, int max_pages, const int *__restrict__ pos,
                  const int *__restrict__ src, int Hkv, int hd) {
     const int row = blockIdx.x, layer = blockIdx.y, q = src[row];
     if (q == row) return;
@@ -101,9 +102,9 @@ beam_fork_kernel(float *kc, float *vc, size_t layer_stride, int *page_table, int
     if (layer == 0)
         for (int lp = threadIdx.x; lp < c; lp += blockDim.x) dst_pt[lp] = src_pt[lp];
     if (rem == 0) return;
-    const int n4 = rem * hd / 4;   // positions [0, rem) of one kv head are contiguous in a page
+    const int n4 = rem * hd / (16 / (int)sizeof(KV));   // 16-byte chunks: positions [0, rem) of one kv head are contiguous in a page
     for (int kv = 0; kv < 2; ++kv) {
-        float *base = (kv ? vc : kc) + (size_t)layer * layer_stride;
+        KV *base = (kv ? vc : kc) + (size_t)layer * layer_stride;
         for (int h = 0; h < Hkv; ++h) {
             const float4 *s4 = reinterpret_cast<const float4 *>(base + ((size_t)from * Hkv + h) * KV_PAGE * hd);
             float4 *d4 = reinterpret_cast<float4 *>(base + ((size_t)own * Hkv + h) * KV_PAGE * hd);
@@ -112,9 +113,14 @@ beam_fork_kernel(float *kc, float *vc, size_t layer_stride, int *page_table, int
     }
 }
 
-void launch_beam_fork(float *kc, float *vc, size_t layer_stride, int layers, int *page_table, int max_pages, const int *pos,
-                      const int *src, int rows, int Hkv, int hd, cudaStream_t st) {
-    beam_fork_kernel<<<dim3(rows, layers), 256, 0, st>>>(kc, vc, layer_stride, page_table, max_pages, pos, src, Hkv, hd);
+void launch_beam_fork(void *kc, void *vc, KvType type, size_t layer_stride, int layers, int *page_table, int max_pages,
+                      const int *pos, const int *src, int rows, int Hkv, int hd, cudaStream_t st) {
+    if (type == KvType::F16)
+        beam_fork_kernel<__half><<<dim3(rows, layers), 256, 0, st>>>((__half *)kc, (__half *)vc, layer_stride, page_table,
+                                                                     max_pages, pos, src, Hkv, hd);
+    else
+        beam_fork_kernel<float><<<dim3(rows, layers), 256, 0, st>>>((float *)kc, (float *)vc, layer_stride, page_table,
+                                                                    max_pages, pos, src, Hkv, hd);
     tc_count_launch("beam_fork");
 }
 

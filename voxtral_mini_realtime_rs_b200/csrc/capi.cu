@@ -499,11 +499,26 @@ void vox_model_free(vox_model *m) {
 }
 
 // ---------------------------------------------------------------- session
+// the element type vox_session_create_ex / vox_stream_pool_create_ex accept
+static KvType kv_type_of(int32_t kv_dtype) {
+    VOX_CHECK(kv_dtype == VOX_DTYPE_F32 || kv_dtype == VOX_DTYPE_F16, VOX_EINVAL,
+              "kv_dtype %d: VOX_DTYPE_F32 or VOX_DTYPE_F16", (int)kv_dtype);
+    return kv_dtype == VOX_DTYPE_F16 ? KvType::F16 : KvType::F32;
+}
 int32_t vox_session_create(vox_model *m, int32_t max_batch, int32_t max_mel_frames, vox_session **out) {
+    return vox_session_create_ex(m, max_batch, max_mel_frames, VOX_DTYPE_F32, out);
+}
+int32_t vox_session_create_ex(vox_model *m, int32_t max_batch, int32_t max_mel_frames, int32_t kv_dtype, vox_session **out) {
     VOX_API_BEGIN
     REQUIRE(m); REQUIRE(out);
-    Session *s = Session::create(m->m, max_batch, max_mel_frames);
+    Session *s = Session::create(m->m, max_batch, max_mel_frames, false, kv_type_of(kv_dtype));
     *out = new vox_session{s};
+    VOX_API_END
+}
+int32_t vox_session_device_bytes(const vox_session *s, uint64_t *bytes) {
+    VOX_API_BEGIN
+    REQUIRE(s); REQUIRE(bytes);
+    *bytes = s->s->arena.total;
     VOX_API_END
 }
 int32_t vox_session_set_delay(vox_session *s, float delay) {
@@ -916,6 +931,37 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
             for (size_t i = 0; i < cnt; ++i) out[i] = (float)s->mega_attn_log[i / 4][i % 4];
         }
         return VOX_OK;
+    } else if ((w.rfind("kv_k", 0) == 0 || w.rfind("kv_v", 0) == 0) && w.size() > 4) {
+        // layer l's cached K or V of rows [0, cur_B) at positions [0, cache length), f32 [row][pos][kv_head][hd]
+        const int l = atoi(w.c_str() + 4);
+        VOX_CHECK(l >= 0 && l < c.dec_layers && std::to_string(l) == w.substr(4), VOX_EINVAL, "no decoder layer in '%s'", what);
+        VOX_CHECK(!s->kv_ring, VOX_EINVAL, "'%s': not on ring-indexed sessions", what);
+        const int B = s->cur_B, Hkv = c.dec_kv_heads, hd = c.dec_head_dim;
+        std::vector<int> pos(B);
+        CUDA_OK(cudaStreamSynchronize(s->st));
+        if (B) CUDA_OK(cudaMemcpy(pos.data(), s->d_pos, sizeof(int) * B, cudaMemcpyDeviceToHost));
+        const int L = B ? std::min(pos[0], s->kv_max_pages * KV_PAGE) : 0;
+        for (int b = 0; b < B; ++b) VOX_CHECK(pos[b] == pos[0], VOX_EINVAL, "'%s': rows at different positions", what);
+        const size_t cnt = (size_t)B * L * Hkv * hd;
+        if (n_floats) *n_floats = cnt;
+        if (out && cnt) {
+            VOX_CHECK(cap >= cnt, VOX_ECAPACITY, "debug_read capacity %zu < %zu", cap, cnt);
+            std::vector<int> pt((size_t)B * s->kv_max_pages);
+            CUDA_OK(cudaMemcpy(pt.data(), s->d_page_table, sizeof(int) * pt.size(), cudaMemcpyDeviceToHost));
+            const size_t eb = kv_elem_bytes(s->kv_type), stride = s->kv_layer_stride();
+            std::vector<unsigned char> layer(stride * eb);
+            CUDA_OK(cudaMemcpy(layer.data(), s->kv_layer(w[3] == 'k' ? s->kc : s->vc, l), layer.size(), cudaMemcpyDeviceToHost));
+            size_t o = 0;
+            for (int b = 0; b < B; ++b)
+                for (int j = 0; j < L; ++j)
+                    for (int h = 0; h < Hkv; ++h) {
+                        const size_t at = (((size_t)pt[(size_t)b * s->kv_max_pages + j / KV_PAGE] * Hkv + h) * KV_PAGE + j % KV_PAGE) * hd;
+                        for (int d = 0; d < hd; ++d, ++o)
+                            out[o] = s->kv_type == KvType::F16 ? __half2float(reinterpret_cast<const __half *>(layer.data())[at + d])
+                                                                : reinterpret_cast<const float *>(layer.data())[at + d];
+                    }
+        }
+        return VOX_OK;
     } else if (w == "mega_trace") {
         // phase trace of the last persistent decode step (CTA 0): per op {start, staged, body done,
         // barrier passed, first weights ready | KV walked, last stage consumed} in microseconds since the first stamp; ops 0..mega_n_ops-1
@@ -986,10 +1032,21 @@ void vox_session_free(vox_session *s) {
 
 // ---------------------------------------------------------------- streaming sessions
 int32_t vox_stream_pool_create(vox_model *m, int32_t max_sessions, float max_seconds, vox_stream_pool **out) {
+    return vox_stream_pool_create_ex(m, max_sessions, max_seconds, VOX_DTYPE_F32, out);
+}
+int32_t vox_stream_pool_create_ex(vox_model *m, int32_t max_sessions, float max_seconds, int32_t kv_dtype,
+                                  vox_stream_pool **out) {
     VOX_API_BEGIN
     REQUIRE(m); REQUIRE(out);
+    const KvType t = kv_type_of(kv_dtype);
     CUDA_OK(cudaSetDevice(m->m->device));
-    *out = new vox_stream_pool{StreamPool::create(m->m, max_sessions, max_seconds)};
+    *out = new vox_stream_pool{StreamPool::create(m->m, max_sessions, max_seconds, t)};
+    VOX_API_END
+}
+int32_t vox_stream_pool_device_bytes(const vox_stream_pool *p, uint64_t *bytes) {
+    VOX_API_BEGIN
+    REQUIRE(p); REQUIRE(bytes);
+    *bytes = p->p->s->arena.total;
     VOX_API_END
 }
 int32_t vox_stream_open(vox_stream_pool *p, int32_t *session) {

@@ -18,7 +18,7 @@ namespace {
 constexpr int DA_WARPS = 8;
 constexpr int DA_THREADS = DA_WARPS * 32;
 
-template <int G, int DPL, bool RING>
+template <int G, int DPL, bool RING, typename KV>
 __global__ void __launch_bounds__(DA_THREADS)
 dec_attn_fused_kernel(const float *__restrict__ qkv, const int ld, const int H, const int Hkv, const KvView kv, const int window,
                       const float scale, const RopeView rope, float *__restrict__ out) {
@@ -57,8 +57,8 @@ dec_attn_fused_kernel(const float *__restrict__ qkv, const int ld, const int H, 
     {
         const size_t at = kv_index<RING>(kv, b, Hkv, kvh, pos, HD);
         for (int i = threadIdx.x; i < HD; i += DA_THREADS) {
-            kv.k[at + i] = kvs[0][i];
-            kv.v[at + i] = kvs[1][i];
+            kv_store(kv_ptr<KV>(kv.k) + at + i, kvs[0][i]);
+            kv_store(kv_ptr<KV>(kv.v) + at + i, kvs[1][i]);
         }
     }
     __syncthreads();  // the CTA's own global writes are visible to all its threads after the barrier
@@ -82,12 +82,12 @@ dec_attn_fused_kernel(const float *__restrict__ qkv, const int ld, const int H, 
         const int pg = RING ? (j / KV_PAGE) % kv.max_pages : j / KV_PAGE;
         const int phys = pg < 64 ? pts[pg] : kv.page_table[(size_t)b * kv.max_pages + pg];
         const size_t at = (((size_t)phys * Hkv + kvh) * KV_PAGE + (j % KV_PAGE)) * HD + lane * DPL;
-        const float *kr = kv.k + at;
-        const float *vr = kv.v + at;
+        const KV *kr = kv_ptr<KV>(kv.k) + at;
+        const KV *vr = kv_ptr<KV>(kv.v) + at;
 #pragma unroll
         for (int i = 0; i < DPL; ++i) {
-            kk[i] = kr[i];
-            vv[i] = vr[i];
+            kk[i] = kv_load(kr[i]);
+            vv[i] = kv_load(vr[i]);
         }
         float s[G];
 #pragma unroll
@@ -140,13 +140,13 @@ dec_attn_fused_kernel(const float *__restrict__ qkv, const int ld, const int H, 
     }
 }
 
-template <int G, bool RING>
+template <int G, bool RING, typename KV>
 void launch_g(int dpl, dim3 grid, cudaStream_t st, const float *qkv, int ld, int H, int Hkv, const KvView &kv, int window,
               float scale, const RopeView &rope, float *out) {
     switch (dpl) {
-        case 1: dec_attn_fused_kernel<G, 1, RING><<<grid, DA_THREADS, 0, st>>>(qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
-        case 2: dec_attn_fused_kernel<G, 2, RING><<<grid, DA_THREADS, 0, st>>>(qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
-        case 4: dec_attn_fused_kernel<G, 4, RING><<<grid, DA_THREADS, 0, st>>>(qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        case 1: dec_attn_fused_kernel<G, 1, RING, KV><<<grid, DA_THREADS, 0, st>>>(qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        case 2: dec_attn_fused_kernel<G, 2, RING, KV><<<grid, DA_THREADS, 0, st>>>(qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        case 4: dec_attn_fused_kernel<G, 4, RING, KV><<<grid, DA_THREADS, 0, st>>>(qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
         default: fail(VOX_EINVAL, "dec_attn_fused: unsupported head_dim");
     }
 }
@@ -163,13 +163,20 @@ void launch_dec_attn_fused(float *qkv, int B, int ld, int H, int Hkv, int hd, co
     VOX_CHECK(dec_attn_fused_supported(H, Hkv, hd), VOX_EINVAL, "dec_attn_fused: unsupported shape");
     const int G = H / Hkv, dpl = hd / 32;
     dim3 grid(Hkv, B);
-    switch (G * 2 + (kv.ring ? 1 : 0)) {
-        case 2: launch_g<1, false>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
-        case 3: launch_g<1, true>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
-        case 4: launch_g<2, false>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
-        case 5: launch_g<2, true>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
-        case 8: launch_g<4, false>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
-        default: launch_g<4, true>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+    const bool f16 = kv.type == KvType::F16;
+    switch (G * 4 + (kv.ring ? 2 : 0) + (f16 ? 1 : 0)) {
+        case 4: launch_g<1, false, float>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        case 5: launch_g<1, false, __half>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        case 6: launch_g<1, true, float>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        case 7: launch_g<1, true, __half>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        case 8: launch_g<2, false, float>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        case 9: launch_g<2, false, __half>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        case 10: launch_g<2, true, float>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        case 11: launch_g<2, true, __half>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        case 16: launch_g<4, false, float>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        case 17: launch_g<4, false, __half>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        case 18: launch_g<4, true, float>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        default: launch_g<4, true, __half>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
     }
     tc_count_launch("dec_attn_fused");
 }

@@ -88,14 +88,14 @@ __host__ __device__ constexpr int mg_misc_bytes(int MT) {
 }
 __host__ __device__ constexpr int mg_pair_bytes(int MT) { return 272 * MT; }  // fragments + offsets of one block pair
 // Attention phase in the scratch region: q [G][HD] + per-warp maxima [MG_CWARPS][G], then per key of a tile its G scores,
-// its K row padded by one float4 (HD + 4) and its V row.  Keys per tile: what the scratch holds, in whole warps (one key
-// per consumer thread, at most MG_CTHREADS).
+// its K row padded by one 16-byte chunk (HD + 16 / KB elements of KB bytes: 4 f32 or 8 f16) and its V row.  Keys per
+// tile: what the scratch holds, in whole warps (one key per consumer thread, at most MG_CTHREADS).
 __host__ __device__ constexpr int mg_attn_fixed_bytes(int G, int HD) { return (G * HD + MG_CWARPS * G) * 4; }
-__host__ __device__ constexpr int mg_attn_key_bytes(int G, int HD) { return (G + 2 * HD + 4) * 4; }
-__host__ __device__ constexpr int mg_attn_tile(int scratch_bytes, int G, int HD) {
-    return (scratch_bytes - mg_attn_fixed_bytes(G, HD)) / mg_attn_key_bytes(G, HD) / 32 * 32 > MG_CTHREADS
+__host__ __device__ constexpr int mg_attn_key_bytes(int G, int HD, int KB) { return G * 4 + (2 * HD + 16 / KB) * KB; }
+__host__ __device__ constexpr int mg_attn_tile(int scratch_bytes, int G, int HD, int KB) {
+    return (scratch_bytes - mg_attn_fixed_bytes(G, HD)) / mg_attn_key_bytes(G, HD, KB) / 32 * 32 > MG_CTHREADS
                ? MG_CTHREADS
-               : (scratch_bytes - mg_attn_fixed_bytes(G, HD)) / mg_attn_key_bytes(G, HD) / 32 * 32;
+               : (scratch_bytes - mg_attn_fixed_bytes(G, HD)) / mg_attn_key_bytes(G, HD, KB) / 32 * 32;
 }
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -387,7 +387,7 @@ __device__ __forceinline__ void mg_pair(const unsigned char *__restrict__ sb, co
 // rows come from p.cos_t / p.sin_t at pos % p.rope_rows; positions have no cap.  RING = false is the plain walk.
 // Each row is a stream at its own transcription delay: the wo phases scale token b's w13 input fragments by its own
 // ffn_norm x ADA vector (p.ffn_ada_rows[b]).
-template <int MT, int G, int DPL, bool RING>
+template <int MT, int G, int DPL, bool RING, typename KV>
 __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaParams p) {
     constexpr int CG = (MT + 3) / 4;
     constexpr int HD = DPL * 32;
@@ -538,8 +538,8 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                                 for (int pg = j0 / KV_PAGE; pg * KV_PAGE < j1; ++pg) {     // pages are the contiguous unit
                                     const int ka = max(j0, pg * KV_PAGE), ke = min(j1, (pg + 1) * KV_PAGE);
                                     const size_t off = (((size_t)p.page_table[(size_t)b * p.max_pages + (RING ? pg % p.max_pages : pg)] * p.Hkv + kvh) * KV_PAGE + (ka - pg * KV_PAGE)) * HD;
-                                    bulk_prefetch_l2(nx.kc + off, (uint32_t)(ke - ka) * HD * 4u);
-                                    bulk_prefetch_l2(nx.vc + off, (uint32_t)(ke - ka) * HD * 4u);
+                                    bulk_prefetch_l2(kv_ptr<KV>(nx.kc) + off, (uint32_t)(ke - ka) * HD * (uint32_t)sizeof(KV));
+                                    bulk_prefetch_l2(kv_ptr<KV>(nx.vc) + off, (uint32_t)(ke - ka) * HD * (uint32_t)sizeof(KV));
                                 }
                             }
                         }
@@ -664,7 +664,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                                         // (2i, 2i+1): the quad is two whole pairs), k and v rows are appended to the layer's KV cache
                                         // at the token's position.  (Loaded here, not ahead of the hand-off barrier: live across the
                                         // partial-sum tree these operands made this 64-register role spill.)
-                                        if (vop->kc != nullptr) {
+                                        if (kv_ptr<KV>(vop->kc) != nullptr) {
                                             const int pos = p.d_pos[q_tok];
                                             if (RING || pos < p.max_seq) {
                                                 const int hrow = r_row % HD, qk_rows = (p.H + p.Hkv) * HD;
@@ -680,8 +680,8 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                                                     kvw.page_table = p.page_table;
                                                     kvw.max_pages = p.max_pages;
                                                     const int kvh = ((r_row - p.H * HD) / HD) % p.Hkv;
-                                                    float *dst = (r_row < qk_rows ? vop->kc : vop->vc) + kv_index<RING>(kvw, q_tok, p.Hkv, kvh, pos, HD) + hrow;
-                                                    *reinterpret_cast<float4 *>(dst) = out;
+                                                    KV *dst = (r_row < qk_rows ? kv_ptr<KV>(vop->kc) : kv_ptr<KV>(vop->vc)) + kv_index<RING>(kvw, q_tok, p.Hkv, kvh, pos, HD) + hrow;
+                                                    kv_store4(dst, out);
                                                 }
                                             }
                                         }
@@ -956,14 +956,16 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
             // The chunk goes through shared memory KT keys at a time (online softmax across tiles): consumer thread j scores
             // key j against the G heads (q read as a broadcast; K rows padded to HD + 4 floats, an odd number of float4, so
             // the 8 threads of a quarter-warp read 8 distinct bank groups), one CTA-wide max per head, then P.V with
-            // thread = (head, dim).
-            const int KT = mg_attn_tile(p.scratch_bytes, G, HD);
-            constexpr int KLD = HD + 4;
+            // thread = (head, dim).  An f16 cache is staged as stored (EPC = 8 elements per 16-byte copy, K rows padded
+            // by 8 halves: again an odd number of chunks at HD 128 and 32) and widened exactly where it is read.
+            constexpr int EPC = 16 / (int)sizeof(KV);
+            const int KT = mg_attn_tile(p.scratch_bytes, G, HD, (int)sizeof(KV));
+            constexpr int KLD = HD + EPC;
             float *qs = reinterpret_cast<float *>(scratch);  // [G][HD]
             float *red_m = qs + G * HD;                       // [MG_CWARPS][G] tile max per warp
             float *ps = red_m + MG_CWARPS * G;                // [G][KT] scores, then probabilities
-            float *ks = ps + G * KT;                          // [KT][KLD]
-            float *vs = ks + KT * KLD;                        // [KT][HD]
+            KV *ks = reinterpret_cast<KV *>(ps + G * KT);     // [KT][KLD]
+            KV *vs = ks + KT * KLD;                           // [KT][HD]
             const int H = p.H, Hkv = p.Hkv, NC = p.attn_chunks;
             KvView kvw;
             kvw.k = op.kc;
@@ -990,14 +992,14 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                     if (jt == j0)
                         for (int i = tid; i < G * HD / 4; i += MG_CTHREADS)
                             cp_async16(qs + 4 * i, p.qkv + (size_t)b * p.ld_qkv + (size_t)kvh * G * HD + 4 * i);
-                    for (int f = tid; f < n * (HD / 4); f += MG_CTHREADS) {
-                        const int jj = f / (HD / 4), c4 = f - jj * (HD / 4);
-                        cp_async16(ks + jj * KLD + 4 * c4, kvw.k + kv_index<RING>(kvw, b, Hkv, kvh, jt + jj, HD) + 4 * c4);
+                    for (int f = tid; f < n * (HD / EPC); f += MG_CTHREADS) {
+                        const int jj = f / (HD / EPC), c4 = f - jj * (HD / EPC);
+                        cp_async16(ks + jj * KLD + EPC * c4, kv_ptr<KV>(kvw.k) + kv_index<RING>(kvw, b, Hkv, kvh, jt + jj, HD) + EPC * c4);
                     }
                     cp_async_commit();
-                    for (int f = tid; f < n * (HD / 4); f += MG_CTHREADS) {
-                        const int jj = f / (HD / 4), c4 = f - jj * (HD / 4);
-                        cp_async16(vs + jj * HD + 4 * c4, kvw.v + kv_index<RING>(kvw, b, Hkv, kvh, jt + jj, HD) + 4 * c4);
+                    for (int f = tid; f < n * (HD / EPC); f += MG_CTHREADS) {
+                        const int jj = f / (HD / EPC), c4 = f - jj * (HD / EPC);
+                        cp_async16(vs + jj * HD + EPC * c4, kv_ptr<KV>(kvw.v) + kv_index<RING>(kvw, b, Hkv, kvh, jt + jj, HD) + EPC * c4);
                     }
                     cp_async_commit();
                     cp_async_wait<1>();
@@ -1011,13 +1013,14 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
 #pragma unroll
                     for (int h = 0; h < G; ++h) sj[h] = -INFINITY;
                     if (tid < n) {
-                        const float4 *kr = reinterpret_cast<const float4 *>(ks + tid * KLD);
+                        const KV *kr = ks + tid * KLD;
                         float d0[G], d1[G];   // two chains per head
 #pragma unroll
                         for (int h = 0; h < G; ++h) d0[h] = d1[h] = 0.0f;
 #pragma unroll 4
                         for (int c = 0; c < HD / 4; c += 2) {
-                            const float4 ka = kr[c], kb = kr[c + 1];
+                            float4 ka, kb;
+                            kv_load8(kr, c, ka, kb);
 #pragma unroll
                             for (int h = 0; h < G; ++h) {
                                 const float4 qa = reinterpret_cast<const float4 *>(qs + h * HD)[c];
@@ -1063,19 +1066,19 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                             }
                         const float alpha = fast_exp(mo - mn);  // exp(-inf) = 0 on the first tile
                         const float *pr = ps + oh * KT;
-                        const float *vc = vs + od;
+                        const KV *vc = vs + od;
                         float a0 = 0.0f, a1 = 0.0f, s0 = 0.0f, s1 = 0.0f;
                         int j = 0;
 #pragma unroll 4
                         for (; j + 1 < n; j += 2) {
                             const float2 pj = *reinterpret_cast<const float2 *>(pr + j);
-                            a0 = fmaf(pj.x, vc[j * HD], a0);
-                            a1 = fmaf(pj.y, vc[(j + 1) * HD], a1);
+                            a0 = fmaf(pj.x, kv_load(vc[j * HD]), a0);
+                            a1 = fmaf(pj.y, kv_load(vc[(j + 1) * HD]), a1);
                             s0 += pj.x;
                             s1 += pj.y;
                         }
                         if (j < n) {
-                            a0 = fmaf(pr[j], vc[j * HD], a0);
+                            a0 = fmaf(pr[j], kv_load(vc[j * HD]), a0);
                             s0 += pr[j];
                         }
                         o_acc = fmaf(o_acc, alpha, a0 + a1);
@@ -1274,10 +1277,10 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
     }
 }
 
-template <int MT, int G, int DPL, bool RING>
+template <int MT, int G, int DPL, bool RING, typename KV>
 void launch_t(const MegaParams &p, const MegaPlan &plan, int grid, cudaStream_t st) {
     static SmemAttr smem_attr;
-    cuda_check_mg(ensure_dyn_smem(decode_mega_kernel<MT, G, DPL, RING>, MG_SMEM_MAX, smem_attr), "cudaFuncSetAttribute(decode_mega)");
+    cuda_check_mg(ensure_dyn_smem(decode_mega_kernel<MT, G, DPL, RING, KV>, MG_SMEM_MAX, smem_attr), "cudaFuncSetAttribute(decode_mega)");
     // cooperative launch: the runtime refuses the launch (instead of the grid barrier hanging) if the
     // `grid` CTAs cannot all be resident at once
     cudaLaunchConfig_t cfg{};
@@ -1290,13 +1293,14 @@ void launch_t(const MegaParams &p, const MegaPlan &plan, int grid, cudaStream_t 
     attr[0].val.cooperative = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    cuda_check_mg(cudaLaunchKernelEx(&cfg, decode_mega_kernel<MT, G, DPL, RING>, p), "decode_mega launch");
+    cuda_check_mg(cudaLaunchKernelEx(&cfg, decode_mega_kernel<MT, G, DPL, RING, KV>, p), "decode_mega launch");
     tc_count_launch("decode_mega");
 }
 
 template <int MT, int G, int DPL>
 void launch_g(const MegaParams &p, const MegaPlan &plan, int grid, cudaStream_t st) {
-    (p.ring ? launch_t<MT, G, DPL, true> : launch_t<MT, G, DPL, false>)(p, plan, grid, st);
+    if (plan.kv_bytes == 2) (p.ring ? launch_t<MT, G, DPL, true, __half> : launch_t<MT, G, DPL, false, __half>)(p, plan, grid, st);
+    else (p.ring ? launch_t<MT, G, DPL, true, float> : launch_t<MT, G, DPL, false, float>)(p, plan, grid, st);
 }
 
 template <int MT>
@@ -1315,11 +1319,13 @@ bool decode_mega_supported(int B, int H, int Hkv, int hd) {
     return (G == 4 && hd == 128) || (G == 2 && hd == 32);
 }
 
-MegaPlan decode_mega_plan(int B, int max_pairs, int H, int Hkv, int hd) {
+MegaPlan decode_mega_plan(int B, int max_pairs, int H, int Hkv, int hd, int kv_bytes) {
+    VOX_CHECK(kv_bytes == 4 || kv_bytes == 2, VOX_EINVAL, "decode_mega: KV element of %d bytes", kv_bytes);
     MegaPlan pl;
+    pl.kv_bytes = kv_bytes;
     pl.MT = B <= 1 ? 1 : (B <= 2 ? 2 : (B <= 4 ? 4 : 8));
     const int G = H / Hkv;
-    const int attn_bytes = mg_attn_fixed_bytes(G, hd) + 32 * mg_attn_key_bytes(G, hd);   // a tile of at least 32 keys
+    const int attn_bytes = mg_attn_fixed_bytes(G, hd) + 32 * mg_attn_key_bytes(G, hd, kv_bytes);   // a tile of at least 32 keys
     const int per_pair = mg_pair_bytes(pl.MT);
     int cap_pairs = MG_SCRATCH_CAP / per_pair;
     if (cap_pairs >= MG_CHUNK) cap_pairs = cap_pairs / MG_CHUNK * MG_CHUNK;
@@ -1328,7 +1334,7 @@ MegaPlan decode_mega_plan(int B, int max_pairs, int H, int Hkv, int hd) {
     int scratch = pl.Ps_cap * per_pair;
     if (scratch < attn_bytes) scratch = attn_bytes;
     pl.scratch_bytes = (scratch + 127) & ~127;
-    pl.attn_tile = mg_attn_tile(pl.scratch_bytes, G, hd);
+    pl.attn_tile = mg_attn_tile(pl.scratch_bytes, G, hd, kv_bytes);
     const int left = MG_SMEM_MAX - mg_misc_bytes(pl.MT) - pl.scratch_bytes;
     const int stage_bytes = mg_nt(pl.MT) * MG_SLOT_BYTES;
     int ns = left / stage_bytes;

@@ -6,6 +6,8 @@
 #include <cstddef>
 #include <cstdint>
 
+#include "kernels.h"
+
 namespace vox {
 
 enum MegaKind : int {
@@ -43,7 +45,7 @@ struct MegaOp {
     float *ssq_out = nullptr;       // [n_tiles][B]
     int track_argmax = 0;
     // MG_ATTN, and the layer's qkv MG_MATVEC, whose epilogue applies RoPE to the q and k rows and appends k and v
-    float *kc = nullptr, *vc = nullptr;  // this layer's KV page pools [n_pages][Hkv][KV_PAGE][hd] (kernels.h KvView)
+    KvPool kc, vc;   // this layer's KV page pools [n_pages][Hkv][KV_PAGE][hd] of MegaPlan::kv_bytes elements (kernels.h)
     int layer = 0;
     // MG_MATVEC whose output fragments take layer j's ffn_norm x ADA scale (wo): j, else -1.  Token b's fragments are
     // scaled by MegaParams::ffn_ada_rows[b] + j * D (fout_gamma is unset).
@@ -112,13 +114,15 @@ struct MegaPlan {
     int scratch_bytes = 0;
     int nstage = 0;
     int attn_tile = 0;      // keys per K/V tile of the attention phase (what the scratch region holds)
+    int kv_bytes = 4;       // KV cache element: 4 (f32) or 2 (f16); selects the kernel instantiation
     size_t smem_bytes = 0;
 };
 
 // Shapes the persistent kernel is instantiated for.
 bool decode_mega_supported(int B, int H, int Hkv, int hd);
-// Shared-memory plan for B streams given the largest K (in block pairs) of any matvec of the step.
-MegaPlan decode_mega_plan(int B, int max_pairs, int H, int Hkv, int hd);
+// Shared-memory plan for B streams given the largest K (in block pairs) of any matvec of the step and the KV cache's
+// element size in bytes (4: f32, 2: f16).
+MegaPlan decode_mega_plan(int B, int max_pairs, int H, int Hkv, int hd, int kv_bytes);
 int decode_mega_grid(int device);
 void launch_decode_mega(const MegaParams &p, const MegaPlan &plan, int grid, cudaStream_t st);
 

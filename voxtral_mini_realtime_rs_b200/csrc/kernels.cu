@@ -671,7 +671,7 @@ void launch_enc_attention(const float *qkv, float *out, int B, int S, int H, int
 // cache without materialising the repeated K/V (model.rs:125-197).  Positions come from a device
 // counter so the same CUDA graph can be replayed for every step.
 // =====================================================================================
-template <bool RING>
+template <bool RING, typename KV>
 __global__ void dec_rope_append_kernel(float *qkv, int M, int ld, int H, int Hkv, int hd, const KvView kv, const RopeView rope) {
     const int i = blockIdx.x, b = blockIdx.y;
     const int pos = kv.pos[b] + i;
@@ -692,26 +692,30 @@ __global__ void dec_rope_append_kernel(float *qkv, int M, int ld, int H, int Hkv
     for (int t = threadIdx.x; t < Hkv * half; t += blockDim.x) {
         const int h = t / half, p = t - h * half;
         const float xr = krow[h * hd + 2 * p], xi = krow[h * hd + 2 * p + 1];
-        float *dst = kv.k + kv_index<RING>(kv, b, Hkv, h, pos, hd) + 2 * p;
-        dst[0] = xr * cr[p] - xi * sr[p];
-        dst[1] = xr * sr[p] + xi * cr[p];
+        KV *dst = kv_ptr<KV>(kv.k) + kv_index<RING>(kv, b, Hkv, h, pos, hd) + 2 * p;
+        kv_store(dst, xr * cr[p] - xi * sr[p]);
+        kv_store(dst + 1, xr * sr[p] + xi * cr[p]);
     }
     for (int t = threadIdx.x; t < Hkv * hd; t += blockDim.x) {
         const int h = t / hd, d = t - h * hd;
-        kv.v[kv_index<RING>(kv, b, Hkv, h, pos, hd) + d] = vrow[t];
+        const float x = vrow[t];
+        kv_store(kv_ptr<KV>(kv.v) + kv_index<RING>(kv, b, Hkv, h, pos, hd) + d, x);
     }
 }
 
 void launch_dec_rope_append(float *qkv, int B, int M, int ld, int H, int Hkv, int hd, const KvView &kv,
                             const RopeView &rope, cudaStream_t st) {
     dim3 grid(M, B);
-    if (kv.ring) dec_rope_append_kernel<true><<<grid, 256, 0, st>>>(qkv, M, ld, H, Hkv, hd, kv, rope);
-    else dec_rope_append_kernel<false><<<grid, 256, 0, st>>>(qkv, M, ld, H, Hkv, hd, kv, rope);
+    const bool f16 = kv.type == KvType::F16;
+    if (kv.ring && f16) dec_rope_append_kernel<true, __half><<<grid, 256, 0, st>>>(qkv, M, ld, H, Hkv, hd, kv, rope);
+    else if (kv.ring) dec_rope_append_kernel<true, float><<<grid, 256, 0, st>>>(qkv, M, ld, H, Hkv, hd, kv, rope);
+    else if (f16) dec_rope_append_kernel<false, __half><<<grid, 256, 0, st>>>(qkv, M, ld, H, Hkv, hd, kv, rope);
+    else dec_rope_append_kernel<false, float><<<grid, 256, 0, st>>>(qkv, M, ld, H, Hkv, hd, kv, rope);
     post_launch("dec_rope_append");
 }
 
 // grid (Hkv, M, B); block = 32 * (H/Hkv): one warp per query head of the group.
-template <bool RING>
+template <bool RING, typename KV>
 __global__ void dec_attention_kernel(const float *__restrict__ qkv, int M, int ld, int H, int Hkv, int hd, const KvView kv,
                                      int window, float scale, float *__restrict__ out) {
     extern __shared__ float sm[];
@@ -731,11 +735,11 @@ __global__ void dec_attention_kernel(const float *__restrict__ qkv, int M, int l
     const int base = RING ? j_lo : 0;
     float mx = -INFINITY;
     for (int j = j_lo + lane; j <= pos; j += 32) {
-        const float4 *kr = reinterpret_cast<const float4 *>(kv.k + kv_index<RING>(kv, b, Hkv, kvh, j, hd));
+        const KV *kr = kv_ptr<KV>(kv.k) + kv_index<RING>(kv, b, Hkv, kvh, j, hd);
         const float4 *q4 = reinterpret_cast<const float4 *>(qsm);
         float acc = 0.0f;
         for (int d = 0; d < (hd >> 2); ++d) {
-            const float4 kk = kr[d];
+            const float4 kk = kv_load4(kr, d);
             const float4 qv = q4[d];
             acc = fmaf(qv.x, kk.x, acc);
             acc = fmaf(qv.y, kk.y, acc);
@@ -759,7 +763,8 @@ __global__ void dec_attention_kernel(const float *__restrict__ qkv, int M, int l
     float *orow = out + ((size_t)b * M + i) * (H * hd) + h * hd;
     for (int d = lane; d < hd; d += 32) {
         float acc = 0.0f;
-        for (int j = j_lo; j <= pos; ++j) acc = fmaf(sc[j - base], kv.v[kv_index<RING>(kv, b, Hkv, kvh, j, hd) + d], acc);
+        for (int j = j_lo; j <= pos; ++j)
+            acc = fmaf(sc[j - base], kv_load(kv_ptr<KV>(kv.v)[kv_index<RING>(kv, b, Hkv, kvh, j, hd) + d]), acc);
         orow[d] = acc * inv;
     }
 }
@@ -770,15 +775,17 @@ void launch_dec_attention(const float *qkv, int B, int M, int ld, int H, int Hkv
     dim3 grid(Hkv, M, B);
     const size_t smem = (size_t)G * (hd + kv.max_seq()) * sizeof(float);
     VOX_CHECK(smem <= 200 * 1024, VOX_EINVAL, "dec_attention: max_seq %d too large for the v1 kernel", kv.max_seq());
-    static SmemAttr attr, attr_ring;
-    if (kv.ring) {
-        VOX_CHECK(window < kv.max_seq(), VOX_EINVAL, "dec_attention: window %d does not fit the KV ring", window);
-        if (smem > 48 * 1024) smem_attr_check(ensure_dyn_smem(dec_attention_kernel<true>, smem, attr_ring), "dec_attention");
-        dec_attention_kernel<true><<<grid, 32 * G, smem, st>>>(qkv, M, ld, H, Hkv, hd, kv, window, scale, out);
-    } else {
-        if (smem > 48 * 1024) smem_attr_check(ensure_dyn_smem(dec_attention_kernel<false>, smem, attr), "dec_attention");
-        dec_attention_kernel<false><<<grid, 32 * G, smem, st>>>(qkv, M, ld, H, Hkv, hd, kv, window, scale, out);
-    }
+    static SmemAttr attr, attr_ring, attr16, attr_ring16;
+    if (kv.ring) VOX_CHECK(window < kv.max_seq(), VOX_EINVAL, "dec_attention: window %d does not fit the KV ring", window);
+    auto go = [&](auto kernel, SmemAttr &a) {
+        if (smem > 48 * 1024) smem_attr_check(ensure_dyn_smem(kernel, smem, a), "dec_attention");
+        kernel<<<grid, 32 * G, smem, st>>>(qkv, M, ld, H, Hkv, hd, kv, window, scale, out);
+    };
+    const bool f16 = kv.type == KvType::F16;
+    if (kv.ring && f16) go(dec_attention_kernel<true, __half>, attr_ring16);
+    else if (kv.ring) go(dec_attention_kernel<true, float>, attr_ring);
+    else if (f16) go(dec_attention_kernel<false, __half>, attr16);
+    else go(dec_attention_kernel<false, float>, attr);
     post_launch("dec_attention");
 }
 

@@ -103,11 +103,35 @@ TcWork q4_matvec_tc_work_size(int N, int K);
 // sessions of an unbounded stream pool, stream.cu; safe while max_pages * KV_PAGE > window + the rows a prefill writes
 // before reading).  The kernels take it as a template flag, so the non-ring code is the plain table walk.
 constexpr int KV_PAGE = 16;
+// Element type of the decoder KV cache, fixed for a session's lifetime (vox_session_create_ex kv_dtype): f32, or IEEE
+// binary16 (__half).  Kernels take the C++ type as a template parameter KV next to RING; every load and store of a
+// cached K or V element goes through kv_load / kv_store below, the one place the f16 format is decided.
+enum class KvType : uint8_t { F32 = 0, F16 = 1 };
+inline size_t kv_elem_bytes(KvType t) { return t == KvType::F16 ? 2 : 4; }
+// Base address of a KV page pool, typed by its element: kv_pool sets the member of the pool's KvType, kv_ptr<KV> reads
+// the member of the kernel's KV (the same type: a kernel instantiation is chosen by the view's KvType).
+union KvPool {
+    float *f32 = nullptr;
+    __half *f16;
+};
+inline KvPool kv_pool(void *p, KvType t) {
+    KvPool r;
+    if (t == KvType::F16) r.f16 = static_cast<__half *>(p);
+    else r.f32 = static_cast<float *>(p);
+    return r;
+}
+template <typename KV> __host__ __device__ __forceinline__ KV *kv_ptr(const KvPool &p);
+template <> __host__ __device__ __forceinline__ float *kv_ptr<float>(const KvPool &p) { return p.f32; }
+template <> __host__ __device__ __forceinline__ __half *kv_ptr<__half>(const KvPool &p) { return p.f16; }
+template <typename KV> __host__ __device__ __forceinline__ KV *kv_ptr(const volatile KvPool &p);
+template <> __host__ __device__ __forceinline__ float *kv_ptr<float>(const volatile KvPool &p) { return p.f32; }
+template <> __host__ __device__ __forceinline__ __half *kv_ptr<__half>(const volatile KvPool &p) { return p.f16; }
 struct KvView {
-    float *k = nullptr, *v = nullptr;  // [n_pages][Hkv][KV_PAGE][hd]
+    KvPool k, v;                       // [n_pages][Hkv][KV_PAGE][hd] of `type`
     const int *page_table = nullptr;   // [B][max_pages] physical page ids
     int max_pages = 0;                 // logical pages per row; capacity = max_pages * KV_PAGE positions (ring: slots)
     bool ring = false;
+    KvType type = KvType::F32;
     const int *pos = nullptr;          // [B]
     __host__ __device__ int max_seq() const { return max_pages * KV_PAGE; }
 };
@@ -117,6 +141,46 @@ __device__ __forceinline__ size_t kv_index(const KvView &kv, const int b, const 
     const int lp = j / KV_PAGE;
     const int phys = kv.page_table[(size_t)b * kv.max_pages + (RING ? lp % kv.max_pages : lp)];
     return (((size_t)phys * Hkv + kvh) * KV_PAGE + (j % KV_PAGE)) * hd;
+}
+// Stored value of x: f32 as is; f16 clamped to [-65504, 65504] (a value past the f16 range stores +-65504, never
+// +-inf), then rounded to nearest even.  NaN fails both comparisons and stays NaN.
+__device__ __forceinline__ float kv_clamp16(const float x) { return x > 65504.0f ? 65504.0f : (x < -65504.0f ? -65504.0f : x); }
+__device__ __forceinline__ void kv_store(float *p, const float x) { *p = x; }
+__device__ __forceinline__ void kv_store(__half *p, const float x) { *p = __float2half_rn(kv_clamp16(x)); }
+// four consecutive elements (16-byte aligned for f32, 8-byte for f16)
+__device__ __forceinline__ void kv_store4(float *p, const float4 x) { *reinterpret_cast<float4 *>(p) = x; }
+__device__ __forceinline__ void kv_store4(__half *p, const float4 x) {
+    const __half2 lo = __halves2half2(__float2half_rn(kv_clamp16(x.x)), __float2half_rn(kv_clamp16(x.y)));
+    const __half2 hi = __halves2half2(__float2half_rn(kv_clamp16(x.z)), __float2half_rn(kv_clamp16(x.w)));
+    uint2 u;
+    u.x = *reinterpret_cast<const uint32_t *>(&lo);
+    u.y = *reinterpret_cast<const uint32_t *>(&hi);
+    *reinterpret_cast<uint2 *>(p) = u;
+}
+// exact widening to f32
+__device__ __forceinline__ float kv_load(const float x) { return x; }
+__device__ __forceinline__ float kv_load(const __half x) { return __half2float(x); }
+// elements [4d, 4d + 4) of a row (16-byte aligned f32, 8-byte aligned f16)
+__device__ __forceinline__ float4 kv_load4(const float *row, const int d) { return reinterpret_cast<const float4 *>(row)[d]; }
+__device__ __forceinline__ float4 kv_load4(const __half *row, const int d) {
+    const uint2 u = reinterpret_cast<const uint2 *>(row)[d];
+    const float2 lo = __half22float2(*reinterpret_cast<const __half2 *>(&u.x));
+    const float2 hi = __half22float2(*reinterpret_cast<const __half2 *>(&u.y));
+    return make_float4(lo.x, lo.y, hi.x, hi.y);
+}
+// elements [4c, 4c + 8) of a row, c even (the shared-memory K tiles of decode_mega.cu: the row is 16-byte aligned)
+__device__ __forceinline__ void kv_load8(const float *row, const int c, float4 &a, float4 &b) {
+    a = reinterpret_cast<const float4 *>(row)[c];
+    b = reinterpret_cast<const float4 *>(row)[c + 1];
+}
+__device__ __forceinline__ void kv_load8(const __half *row, const int c, float4 &a, float4 &b) {
+    const uint4 u = reinterpret_cast<const uint4 *>(row)[c >> 1];
+    const float2 f0 = __half22float2(*reinterpret_cast<const __half2 *>(&u.x));
+    const float2 f1 = __half22float2(*reinterpret_cast<const __half2 *>(&u.y));
+    const float2 f2 = __half22float2(*reinterpret_cast<const __half2 *>(&u.z));
+    const float2 f3 = __half22float2(*reinterpret_cast<const __half2 *>(&u.w));
+    a = make_float4(f0.x, f0.y, f1.x, f1.y);
+    b = make_float4(f2.x, f2.y, f3.x, f3.y);
 }
 #endif
 // Decoder RoPE tables as the kernels read them: cos / sin [rows][hd/2], position p at row p -- or, for a ring KvView, at
@@ -256,8 +320,9 @@ struct BeamWork {
 };
 void launch_beam_select(const int *top_ids, const float *top_lp, const int *out_pos, int out_ld, int b, int W, int n_live,
                         const BeamWork &w, int *tok, cudaStream_t st);
-void launch_beam_fork(float *kc, float *vc, size_t layer_stride, int layers, int *page_table, int max_pages, const int *pos,
-                      const int *src, int rows, int Hkv, int hd, cudaStream_t st);
+// kc / vc: KV page pools of element type `type`, layer_stride elements per layer
+void launch_beam_fork(void *kc, void *vc, KvType type, size_t layer_stride, int layers, int *page_table, int max_pages,
+                      const int *pos, const int *src, int rows, int Hkv, int hd, cudaStream_t st);
 void launch_beam_traceback(const BeamWork &w, int b, int W, int n, int out_ld, int *ids, double *scores, int *out,
                            int *top_ids, float *top_lp, cudaStream_t st, int s0 = 0, int out_stride = 1);
 // Phrase boosting (vox_session_set_bias, bias.cu).  Stream s's list: n_phrases[s] phrases, phrase i of lens[...] ids at

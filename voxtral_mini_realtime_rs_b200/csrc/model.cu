@@ -405,7 +405,7 @@ StreamGeom stream_geometry(const vox_model_info &c, size_t n) {
     return g;
 }
 
-Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ring) {
+Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ring, KvType kv_type) {
     VOX_CHECK(max_batch >= 1 && max_batch <= 64, VOX_EINVAL, "max_batch %d out of range [1,64]", max_batch);
     VOX_CHECK(max_mel_frames >= 16, VOX_EINVAL, "max_mel_frames %d too small", max_mel_frames);
     CUDA_OK(cudaSetDevice(m->device));
@@ -447,8 +447,9 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ri
         s->kv_ring = kv_ring;
         s->dec_rope = m->dec_rope();
         const size_t kv_elems = (size_t)c.dec_layers * s->kv_n_pages * c.dec_kv_heads * KV_PAGE * c.dec_head_dim;
-        s->kc = s->arena.alloc_n<float>(kv_elems);
-        s->vc = s->arena.alloc_n<float>(kv_elems);
+        s->kv_type = kv_type;
+        s->kc = s->arena.alloc(kv_elems * kv_elem_bytes(kv_type));
+        s->vc = s->arena.alloc(kv_elems * kv_elem_bytes(kv_type));
         s->page_table_host.resize((size_t)max_batch * s->kv_max_pages);
         for (int b = 0; b < max_batch; ++b)
             for (int pg = 0; pg < s->kv_max_pages; ++pg) s->page_table_host[(size_t)b * s->kv_max_pages + pg] = b * s->kv_max_pages + pg;
@@ -744,8 +745,9 @@ TcWork Session::tc_work(bool norm_in, bool ssq_out_) const {
 
 KvView Session::kv_view(int layer) const {
     KvView v;
-    v.k = kc + (size_t)layer * kv_layer_stride();
-    v.v = vc + (size_t)layer * kv_layer_stride();
+    v.k = kv_pool(kv_layer(kc, layer), kv_type);
+    v.v = kv_pool(kv_layer(vc, layer), kv_type);
+    v.type = kv_type;
     v.page_table = d_page_table;
     v.max_pages = kv_max_pages;
     v.ring = kv_ring;
@@ -817,8 +819,7 @@ bool Session::mega_prepare(int B) {
         if (!m->dec[j].wqkv.qs_tc || !m->dec[j].wo.qs_tc || !m->dec[j].w13.qs_tc || !m->dec[j].w2.qs_tc) return false;
     auto pairs = [](int K) { return (K / 32 + 1) / 2; };
     const int max_pairs = std::max(std::max(pairs(D), pairs(H * hd)), pairs(c.dec_ffn));
-    mega_plan = decode_mega_plan(B, max_pairs, H, Hkv, hd);
-    const size_t layer_stride = kv_layer_stride();
+    mega_plan = decode_mega_plan(B, max_pairs, H, Hkv, hd, (int)kv_elem_bytes(kv_type));
     const int parts = (D + 15) / 16;
     std::vector<MegaOp> ops;
     bool ok = true;
@@ -873,12 +874,12 @@ bool Session::mega_prepare(int B) {
         const DecLayerW &l = m->dec[j];
         // wqkv: its epilogue applies RoPE to q and k and appends k, v to layer j's cache
         matvec(l.wqkv, XF, qkv_dec, qkvd, nullptr, EPI_NONE, l.attn_norm, false, false, 1, none, nullptr);
-        ops.back().kc = kc + (size_t)j * layer_stride;
-        ops.back().vc = vc + (size_t)j * layer_stride;
+        ops.back().kc = kv_pool(kv_layer(kc, j), kv_type);
+        ops.back().vc = kv_pool(kv_layer(vc, j), kv_type);
         MegaOp a;
         a.kind = MG_ATTN;
-        a.kc = kc + (size_t)j * layer_stride;
-        a.vc = vc + (size_t)j * layer_stride;
+        a.kc = kv_pool(kv_layer(kc, j), kv_type);
+        a.vc = kv_pool(kv_layer(vc, j), kv_type);
         a.layer = j;
         ops.push_back(a);
         // wo: h += attn . Wo^T; leaves fragments of h x (ffn_norm x ADA) for w13
@@ -1078,7 +1079,7 @@ void Session::beam_start(int b) {
 void Session::beam_step(int b, int n_live) {
     const vox_model_info &c = m->info;
     launch_beam_select(d_top_ids, d_top_lp, d_outpos, out_ld, b, beam_w, n_live, beam, d_tok, st);
-    launch_beam_fork(kc, vc, kv_layer_stride(), c.dec_layers, d_page_table, kv_max_pages, d_pos, beam.src, b * beam_w,
+    launch_beam_fork(kc, vc, kv_type, kv_layer_stride(), c.dec_layers, d_page_table, kv_max_pages, d_pos, beam.src, b * beam_w,
                      c.dec_kv_heads, c.dec_head_dim, st);
 }
 

@@ -153,11 +153,14 @@ struct Session {
     // decoder
     // decoder KV cache: page pools [L][n_pages][Hkv][KV_PAGE][hd] + per-row page tables (kernels.h KvView).  Whole-
     // utterance batches use the identity mapping (row b owns pages b*max_pages..); streaming sessions allocate pages
-    float *kc = nullptr, *vc = nullptr;
+    // of kv_type elements (vox_session_create_ex kv_dtype; fixed for the session's lifetime)
+    void *kc = nullptr, *vc = nullptr;
+    KvType kv_type = KvType::F32;
     int kv_max_pages = 0, kv_n_pages = 0;
     int *d_page_table = nullptr;          // [max_batch][kv_max_pages]
     std::vector<int> page_table_host;
-    size_t kv_layer_stride() const { return (size_t)kv_n_pages * m->info.dec_kv_heads * KV_PAGE * m->info.dec_head_dim; }
+    size_t kv_layer_stride() const { return (size_t)kv_n_pages * m->info.dec_kv_heads * KV_PAGE * m->info.dec_head_dim; }  // elements
+    void *kv_layer(void *pool, int layer) const { return (char *)pool + (size_t)layer * kv_layer_stride() * kv_elem_bytes(kv_type); }
     bool kv_ring = false;                 // KvView::ring (Session::create)
     KvView kv_view(int layer) const;
     RopeView dec_rope;                    // the model's tables, or an unbounded stream pool's ring
@@ -283,7 +286,8 @@ struct Session {
     // kv_ring: each row's decoder KV is a ring of pages just long enough for the decoder window plus the rows one launch
     // appends before reading (16 L > dec_window + M_max), and positions are unbounded (stream pools with no length
     // limit; the pool owner points dec_rope at its RoPE ring)
-    static Session *create(Model *m, int max_batch, int max_mel_frames, bool kv_ring = false);
+    // kv_type: element type of the decoder KV cache
+    static Session *create(Model *m, int max_batch, int max_mel_frames, bool kv_ring = false, KvType kv_type = KvType::F32);
     ~Session();
     // every stream at `delay` (tokens of 80 ms)
     void set_delay(float delay);

@@ -171,7 +171,7 @@ size_t pcm_keep(int n_mel) { return (size_t)std::max<int64_t>(0, (int64_t)n_mel 
 }  // namespace
 
 // ======================================================================================================
-StreamPool *StreamPool::create(Model *m, int max_sessions, float max_seconds) {
+StreamPool *StreamPool::create(Model *m, int max_sessions, float max_seconds, KvType kv_type) {
     VOX_CHECK(max_sessions >= 1 && max_sessions <= 64, VOX_EINVAL, "max_sessions %d out of range [1,64]", max_sessions);
     const bool unbounded = max_seconds == 0.0f;
     VOX_CHECK(unbounded || (max_seconds >= 1.0f && max_seconds <= 60.0f), VOX_EINVAL,
@@ -189,7 +189,7 @@ StreamPool *StreamPool::create(Model *m, int max_sessions, float max_seconds) {
         p->cap_samples = pad_audio_len((size_t)std::ceil((unbounded ? kResidentSeconds : max_seconds) * 16000.0f), pc);
         const int cap_mel = (int)mel_num_frames(p->cap_samples);
         // unbounded: the frame buffers get a few frames beyond the resident audio for the rows their consumers still read
-        p->s = Session::create(m, max_sessions, unbounded ? cap_mel + 16 : cap_mel, unbounded);
+        p->s = Session::create(m, max_sessions, unbounded ? cap_mel + 16 : cap_mel, unbounded, kv_type);
         Session *s = p->s;
         VOX_CHECK(s->S_max <= m->enc_rope_len, VOX_EINVAL, "max_seconds exceeds the encoder RoPE table");
         p->max_new = 256;

@@ -47,7 +47,8 @@ struct StreamPool {
     std::vector<int> free_pages;
 
     // max_seconds in [1, 60]: sessions up to that long, all their state resident.  0: sessions of any length.
-    static StreamPool *create(Model *m, int max_sessions, float max_seconds);
+    // kv_type: element type of the decoder KV pages every session of the pool shares (Session::create)
+    static StreamPool *create(Model *m, int max_sessions, float max_seconds, KvType kv_type = KvType::F32);
     ~StreamPool();
     int open();   // the new session runs at kDefaultDelay
     // the session's transcription delay (its own ADA set); only before its prefill has run
