@@ -913,8 +913,8 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
         // {persistent-kernel launches counted on the host since the last re-base, the device epoch}: equal between calls
         int epoch = 0;
         CUDA_OK(cudaStreamSynchronize(s->st));
-        CUDA_OK(cudaMemcpy(&epoch, s->mega_epoch, sizeof(int), cudaMemcpyDeviceToHost));
-        const float v[2] = {(float)s->mega_steps_host, (float)epoch};
+        CUDA_OK(cudaMemcpy(&epoch, s->mega.epoch, sizeof(int), cudaMemcpyDeviceToHost));
+        const float v[2] = {(float)s->mega.launches, (float)epoch};
         if (n_floats) *n_floats = 2;
         if (out) {
             VOX_CHECK(cap >= 2, VOX_ECAPACITY, "debug_read capacity %zu < 2", cap);
@@ -924,11 +924,11 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
     } else if (w == "mega_attn") {
         // attention tiling of the last decode step: per persistent launch {rows, token capacity, keys per K/V tile, key
         // chunks per (stream, kv head)}; nothing after a step on the per-op path
-        const size_t cnt = s->mega_attn_log.size() * 4;
+        const size_t cnt = s->mega.attn_log.size() * 4;
         if (n_floats) *n_floats = cnt;
         if (out) {
             VOX_CHECK(cap >= cnt, VOX_ECAPACITY, "debug_read capacity %zu < %zu", cap, cnt);
-            for (size_t i = 0; i < cnt; ++i) out[i] = (float)s->mega_attn_log[i / 4][i % 4];
+            for (size_t i = 0; i < cnt; ++i) out[i] = (float)s->mega.attn_log[i / 4][i % 4];
         }
         return VOX_OK;
     } else if ((w.rfind("kv_k", 0) == 0 || w.rfind("kv_v", 0) == 0) && w.size() > 4) {
@@ -964,14 +964,14 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
         return VOX_OK;
     } else if (w == "mega_trace") {
         // phase trace of the last persistent decode step (CTA 0): per op {start, staged, body done,
-        // barrier passed, first weights ready | KV walked, last stage consumed} in microseconds since the first stamp; ops 0..mega_n_ops-1
-        const size_t cnt = (size_t)s->mega_n_ops * 6;
+        // barrier passed, first weights ready | KV walked, last stage consumed} in microseconds since the first stamp; ops 0..mega.n_ops-1
+        const size_t cnt = (size_t)s->mega.n_ops * 6;
         if (n_floats) *n_floats = cnt;
         if (out) {
             VOX_CHECK(cap >= cnt, VOX_ECAPACITY, "debug_read capacity %zu < %zu", cap, cnt);
             CUDA_OK(cudaStreamSynchronize(s->st));
             std::vector<unsigned long long> t(cnt);
-            if (cnt) CUDA_OK(cudaMemcpy(t.data(), s->mega_trace, sizeof(unsigned long long) * cnt, cudaMemcpyDeviceToHost));
+            if (cnt) CUDA_OK(cudaMemcpy(t.data(), s->mega.trace, sizeof(unsigned long long) * cnt, cudaMemcpyDeviceToHost));
             int khz = 0;
             CUDA_OK(cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, s->m->device));
             for (size_t i = 0; i < cnt; ++i) out[i] = (float)((double)(t[i] - t[0]) / ((double)khz * 1e-3));
@@ -979,17 +979,17 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
         return VOX_OK;
     } else if (w == "mega_trace_all") {
         // [grid][n_ops][4] microseconds relative to each CTA's exit from the first grid barrier (VOX_MEGA_TRACE_ALL=1)
-        VOX_CHECK(s->mega_trace_all != nullptr, VOX_ENOTFOUND, "all-CTA trace not enabled (VOX_MEGA_TRACE_ALL=1 at session creation)");
-        const size_t per = (size_t)s->mega_n_ops * 4, cnt = per * s->mega_grid;
+        VOX_CHECK(s->mega.trace_all != nullptr, VOX_ENOTFOUND, "all-CTA trace not enabled (VOX_MEGA_TRACE_ALL=1 at session creation)");
+        const size_t per = (size_t)s->mega.n_ops * 4, cnt = per * s->mega.grid;
         if (n_floats) *n_floats = cnt;
         if (out) {
             VOX_CHECK(cap >= cnt, VOX_ECAPACITY, "debug_read capacity %zu < %zu", cap, cnt);
             CUDA_OK(cudaStreamSynchronize(s->st));
             std::vector<unsigned long long> t(cnt);
-            if (cnt) CUDA_OK(cudaMemcpy(t.data(), s->mega_trace_all, sizeof(unsigned long long) * cnt, cudaMemcpyDeviceToHost));
+            if (cnt) CUDA_OK(cudaMemcpy(t.data(), s->mega.trace_all, sizeof(unsigned long long) * cnt, cudaMemcpyDeviceToHost));
             int khz = 0;
             CUDA_OK(cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, s->m->device));
-            for (int ctai = 0; ctai < s->mega_grid; ++ctai) {
+            for (int ctai = 0; ctai < s->mega.grid; ++ctai) {
                 const unsigned long long t0 = t[(size_t)ctai * per + 2];
                 for (size_t i = 0; i < per; ++i)
                     out[(size_t)ctai * per + i] = (float)((double)((long long)(t[(size_t)ctai * per + i] - t0)) / ((double)khz * 1e-3));

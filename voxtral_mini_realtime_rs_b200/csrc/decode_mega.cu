@@ -36,21 +36,125 @@
 #include <cuda_fp16.h>
 
 #include <cfloat>
+#include <cmath>
 #include <cstdlib>
 
 #include "common.h"
-#include "decode_mega.h"
-#include "kernels.h"
+#include "model.h"
 
 namespace vox {
+
+enum MegaKind : int {
+    MG_EMBED = 0,   // x_dec[b] = audio of row b at pos[b] + dequant(E[tok[b]])  (+ sums of squares for the first norm)
+    MG_MATVEC = 1,  // y = epi(norm?(x) . W^T), weights streamed through the CTA's TMA ring
+    MG_ATTN = 2,    // GQA attention of one layer over its KV cache (key chunks combined by the last chunk's CTA)
+    MG_ARGMAX = 3,  // combine the per-CTA lm_head candidates, write the token, advance the counters
+};
+
+// One grid-wide phase.  A grid barrier separates consecutive phases.
+struct MegaOp {
+    int kind = 0, epi = 0;
+    // MG_MATVEC
+    const uint4 *qs_tc = nullptr;
+    const uint2 *d_tc = nullptr;
+    int N = 0, K = 0, n_tiles = 0, n_pairs = 0;
+    int S = 1, Ps = 0;  // CTA-private K slices: the activation fragments of one slice fit the scratch region
+    // activation fragments (tensor-core B operands + per-block offsets, see decode_mega.cu) of the input,
+    // written by the phase that produced the activations; bulk-copied into shared memory, never re-derived
+    const uint2 *fin_bf = nullptr;    // [K/32 (+pad)][2][2*MT][4]
+    const float2 *fin_off = nullptr;  // [K/32 (+pad)][MT]
+    // fragments of this op's OUTPUT for the next matvec (nullptr: plain output only): one 32-value block per
+    // unit of `unit_tiles` consecutive tiles (2: plain rows, 4: SiLU pairs), scaled by fout_gamma if set (or per row:
+    // fout_ada_layer)
+    uint2 *fout_bf = nullptr;
+    float2 *fout_off = nullptr;
+    const float *fout_gamma = nullptr;
+    int unit_tiles = 1;
+    float *y = nullptr;               // plain output (nullptr: fragments only)
+    int ldy = 0;
+    const float *bias = nullptr, *res = nullptr;
+    const float *gamma = nullptr;   // fused RMSNorm weight (x ADA scale where the layer has one)
+    const float *ssq_in = nullptr;  // [ssq_in_parts][B]
+    int ssq_in_parts = 0;
+    float *ssq_out = nullptr;       // [n_tiles][B]
+    int track_argmax = 0;
+    // MG_ATTN, and the layer's qkv MG_MATVEC, whose epilogue applies RoPE to the q and k rows and appends k and v
+    KvPool kc, vc;   // this layer's KV page pools [n_pages][Hkv][KV_PAGE][hd] of MegaPlan::kv_bytes elements (kernels.h)
+    int layer = 0;
+    // MG_MATVEC whose output fragments take layer j's ffn_norm x ADA scale (wo): j, else -1.  Token b's fragments are
+    // scaled by MegaParams::ffn_ada_rows[b] + j * D (fout_gamma is unset).
+    int fout_ada_layer = -1;
+};
+
+struct MegaParams {
+    const MegaOp *ops = nullptr;
+    int n_ops = 0;
+    int B = 0;  // streams (= token rows of every matvec)
+    float eps = 0.f;
+    // attention
+    float *qkv = nullptr;
+    int ld_qkv = 0, H = 0, Hkv = 0, hd = 0, max_seq = 0, window = 0;  // max_seq = max_pages * KV_PAGE
+    const int *page_table = nullptr;  // [B][max_pages] physical KV pages of each batch row
+    int max_pages = 0;
+    float scale = 0.f;
+    const float *cos_t = nullptr, *sin_t = nullptr;
+    float *attn_out = nullptr;
+    int attn_chunks = 1;          // key chunks per (stream, kv head): spreads the KV walk over the grid
+    // chunk states as 8-byte words {value, tag}, tag = epoch * 64 + layer + 1 (unique per decode step and layer, never 0):
+    float *att_acc = nullptr;     // [B*Hkv*chunks][G][hd][2] unnormalised weighted V per chunk
+    float *att_ml = nullptr;      // [B*Hkv*chunks][G][2][2]  running max, sum of exp
+    int *d_epoch = nullptr;       // decode steps executed by this session (never reset)
+    // embedding (row-major planes of the tied table)
+    const uint4 *emb_qs = nullptr;
+    const __half *emb_d = nullptr;
+    int D = 0;
+    // audio embeddings (nullptr: none); row b's position p at audio + audio_off[b] + p * D (kernels.h launch_embed)
+    const float *audio = nullptr;
+    const int64_t *audio_off = nullptr;
+    float *x_dec = nullptr, *ssq_x = nullptr;
+    uint2 *emb_fbf = nullptr;         // fragments of the embedded row (x first layer's attn_norm) for layer 0
+    float2 *emb_foff = nullptr;
+    const float *emb_gamma = nullptr;
+    uint2 *att_fbf = nullptr;         // fragments of the attention output (input of wo)
+    float2 *att_foff = nullptr;
+    // device-side step state; d_pos / d_outpos are PER ROW ([B]): sessions of different ages share a step
+    int *d_pos = nullptr, *d_outpos = nullptr, *d_tok = nullptr, *d_out = nullptr;
+    int out_ld = 0;
+    // per-CTA argmax candidates [grid][8]
+    float *am_vals = nullptr;
+    int *am_idx = nullptr;
+    // grid barrier: [0] arrivals, [1] finished CTAs, [2] watchdog code
+    unsigned *bar = nullptr;
+    // shared-memory plan
+    int nstage = 0, scratch_bytes = 0;
+    // optional phase trace of CTA 0: 6 SM-clock stamps per op (start, staged, body done, barrier passed,
+    // first weights ready | KV walked, last weight stage consumed)
+    unsigned long long *trace = nullptr;
+    // optional all-CTA trace [grid][n_ops][4]: op start, body done, barrier passed, first weights ready / KV walk
+    // start (SM clocks; the host aligns the CTAs on their exit from the first grid barrier)
+    unsigned long long *trace_all = nullptr;
+    float *logits_out = nullptr;  // != nullptr: where the lm_head op writes its rows (row groups of a larger batch)
+    // sessions of an unbounded stream pool: page_table rows are rings of max_pages slots, positions are uncapped and
+    // RoPE row of position pos is pos % rope_rows of cos_t / sin_t (kernels.h KvView, RopeView)
+    int ring = 0;
+    int rope_rows = 0;
+    // [B]: each row's [L][D] ffn_norm x ADA set (the rows' streams may be at different transcription delays)
+    const float *const *ffn_ada_rows = nullptr;
+};
+
+struct MegaPlan {
+    int MT = 0;             // token capacity of the instantiation (1, 2, 4, 8)
+    int Ps_cap = 0;         // pairs per K slice that fit the scratch region
+    int scratch_bytes = 0;
+    int nstage = 0;
+    int attn_tile = 0;      // keys per K/V tile of the attention phase (what the scratch region holds)
+    int kv_bytes = 4;       // KV cache element: 4 (f32) or 2 (f16); selects the kernel instantiation
+    size_t smem_bytes = 0;
+};
 
 void tc_count_launch(const char *name);
 
 namespace {
-
-inline void cuda_check_mg(cudaError_t e, const char *what) {
-    if (e != cudaSuccess) fail(VOX_ECUDA, fmt("CUDA error: %s: %s", what, cudaGetErrorString(e)));
-}
 
 constexpr int MG_CWARPS = 16;                    // consumer warps
 constexpr int MG_CTHREADS = MG_CWARPS * 32;
@@ -74,6 +178,9 @@ constexpr int MG_ACC_TILES = 2;                  // tiles per CTA whose sums may
 constexpr int MG_SMEM_MAX = 227 * 1024;
 constexpr int MG_SCRATCH_CAP = 104448;           // 48 pairs at 8 tokens
 constexpr long long MG_SPIN_CYCLES = 4000000000ll;  // ~2 s: watchdog
+constexpr int MG_ROWS = 8;                       // rows of one launch: the largest token capacity MT
+// block pairs of a matvec's K: its activation fragments take 2 x as many 32-value blocks (the last one padding when odd)
+constexpr int mg_pairs(int K) { return (K / 32 + 1) / 2; }
 
 // tiles a CTA advances together (independent accumulation chains per warp, shared activation fragments)
 __host__ __device__ constexpr int mg_nt(int MT) { return MT <= 2 ? 4 : 2; }
@@ -1280,7 +1387,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
 template <int MT, int G, int DPL, bool RING, typename KV>
 void launch_t(const MegaParams &p, const MegaPlan &plan, int grid, cudaStream_t st) {
     static SmemAttr smem_attr;
-    cuda_check_mg(ensure_dyn_smem(decode_mega_kernel<MT, G, DPL, RING, KV>, MG_SMEM_MAX, smem_attr), "cudaFuncSetAttribute(decode_mega)");
+    CUDA_OK(ensure_dyn_smem(decode_mega_kernel<MT, G, DPL, RING, KV>, MG_SMEM_MAX, smem_attr));
     // cooperative launch: the runtime refuses the launch (instead of the grid barrier hanging) if the
     // `grid` CTAs cannot all be resident at once
     cudaLaunchConfig_t cfg{};
@@ -1293,7 +1400,7 @@ void launch_t(const MegaParams &p, const MegaPlan &plan, int grid, cudaStream_t 
     attr[0].val.cooperative = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    cuda_check_mg(cudaLaunchKernelEx(&cfg, decode_mega_kernel<MT, G, DPL, RING, KV>, p), "decode_mega launch");
+    CUDA_OK(cudaLaunchKernelEx(&cfg, decode_mega_kernel<MT, G, DPL, RING, KV>, p));
     tc_count_launch("decode_mega");
 }
 
@@ -1303,22 +1410,24 @@ void launch_g(const MegaParams &p, const MegaPlan &plan, int grid, cudaStream_t 
     else (p.ring ? launch_t<MT, G, DPL, true, float> : launch_t<MT, G, DPL, false, float>)(p, plan, grid, st);
 }
 
-template <int MT>
-void launch_m(const MegaParams &p, const MegaPlan &plan, int grid, cudaStream_t st) {
-    const int G = p.H / p.Hkv;
-    if (G == 4 && p.hd == 128) launch_g<MT, 4, 4>(p, plan, grid, st);
-    else if (G == 2 && p.hd == 32) launch_g<MT, 2, 1>(p, plan, grid, st);
-    else fail(VOX_EINVAL, "decode_mega: unsupported attention shape");
+
+using MegaLaunch = void (*)(const MegaParams &, const MegaPlan &, int, cudaStream_t);
+template <int G, int DPL>
+MegaLaunch mt_launch(int MT) {
+    return MT == 1 ? launch_g<1, G, DPL> : MT == 2 ? launch_g<2, G, DPL> : MT == 4 ? launch_g<4, G, DPL>
+                                                                             : launch_g<8, G, DPL>;
+}
+// The launch of token capacity MT for the attention shape, nullptr where the kernel is not instantiated for it.  The
+// shapes: G = H / Hkv query heads per kv head at head dim hd, with hd / 32 head dims per lane.
+MegaLaunch find_launch(int MT, int H, int Hkv, int hd) {
+    const int G = Hkv > 0 && H % Hkv == 0 ? H / Hkv : 0;
+    if (G == 4 && hd == 128) return mt_launch<4, 4>(MT);
+    if (G == 2 && hd == 32) return mt_launch<2, 1>(MT);
+    return nullptr;
 }
 
-}  // namespace
-
-bool decode_mega_supported(int B, int H, int Hkv, int hd) {
-    if (B < 1 || B > 8 || Hkv <= 0 || H % Hkv != 0) return false;
-    const int G = H / Hkv;
-    return (G == 4 && hd == 128) || (G == 2 && hd == 32);
-}
-
+// Shared-memory plan for B streams given the largest K (in block pairs) of any matvec of the step and the KV cache's
+// element size in bytes (4: f32, 2: f16).
 MegaPlan decode_mega_plan(int B, int max_pairs, int H, int Hkv, int hd, int kv_bytes) {
     VOX_CHECK(kv_bytes == 4 || kv_bytes == 2, VOX_EINVAL, "decode_mega: KV element of %d bytes", kv_bytes);
     MegaPlan pl;
@@ -1344,21 +1453,256 @@ MegaPlan decode_mega_plan(int B, int max_pairs, int H, int Hkv, int hd, int kv_b
     return pl;
 }
 
-int decode_mega_grid(int device) {
-    int sms = 0;
-    cuda_check_mg(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device), "cudaDeviceGetAttribute(SM count)");
-    return sms;
+}  // namespace
+
+// activation fragments of one matvec input (frag_build): [blocks][16 * MG_ROWS] B operands, [blocks][MG_ROWS] offsets
+struct MegaFrag {
+    uint2 *bf = nullptr;
+    float2 *off = nullptr;
+    size_t blocks = 0;
+};
+
+struct DecodeMega::State {
+    MegaParams p;            // the launch parameters fixed for the session's lifetime, and n_ops of the current table
+    MegaPlan plan;           // of the current table
+    MegaOp *ops = nullptr;   // [ops_cap] on the device
+    int ops_cap = 0;
+    int rows = 0;            // rows per group the current table was built for (0: none yet)
+    // (stream, kv head, key chunk) units a launch spreads its attention over, at most; the chunk states hold 8 Hkv more
+    int att_units = 0;
+    size_t acc_floats = 0, ml_floats = 0;   // of the chunk states att_acc / att_ml
+    MegaFrag xf, af, cf;     // inputs of wqkv and w13 (residual stream x norm weight), of wo, of w2 (SwiGLU output)
+    // padding tokens (capacity MT > B) and padding blocks must read as zero fragments
+    void clear_fragments(cudaStream_t st) const {
+        for (const MegaFrag *f : {&xf, &af, &cf}) CUDA_OK(cudaMemsetAsync(f->bf, 0, sizeof(uint2) * f->blocks * 16 * MG_ROWS, st));
+        for (const MegaFrag *f : {&xf, &af, &cf}) CUDA_OK(cudaMemsetAsync(f->off, 0, sizeof(float2) * f->blocks * MG_ROWS, st));
+    }
+};
+
+DecodeMega::DecodeMega() : state(new State) {}
+DecodeMega::~DecodeMega() = default;
+
+void DecodeMega::create(Session &s) {
+    const Model &m = *s.m;
+    const vox_model_info &c = m.info;
+    State &g = *state;
+    MegaParams &p = g.p;
+    CUDA_OK(cudaDeviceGetAttribute(&grid, cudaDevAttrMultiProcessorCount, m.device));
+    g.ops_cap = 6 * c.dec_layers + 4;
+    p.ops = g.ops = s.arena.alloc_n<MegaOp>(g.ops_cap);
+    p.bar = s.arena.alloc_n<unsigned>(4);
+    CUDA_OK(cudaMemset(p.bar, 0, sizeof(unsigned) * 4));
+    p.am_vals = s.arena.alloc_n<float>((size_t)grid * MG_ROWS);
+    p.am_idx = s.arena.alloc_n<int>((size_t)grid * MG_ROWS);
+    g.att_units = std::max(grid, MG_ROWS * c.dec_kv_heads);
+    const size_t units = g.att_units + MG_ROWS * c.dec_kv_heads, G = c.dec_heads / c.dec_kv_heads;
+    g.acc_floats = 2 * units * G * c.dec_head_dim;   // {value, tag}
+    g.ml_floats = 2 * units * G * 2;                 // {value, tag}
+    p.att_acc = s.arena.alloc_n<float>(g.acc_floats);
+    p.att_ml = s.arena.alloc_n<float>(g.ml_floats);
+    p.d_epoch = epoch = s.arena.alloc_n<int>(1);
+    // chunk states carry their own validity tag (decode step, layer): never 0
+    CUDA_OK(cudaMemset(p.att_acc, 0, sizeof(float) * g.acc_floats));
+    CUDA_OK(cudaMemset(p.att_ml, 0, sizeof(float) * g.ml_floats));
+    CUDA_OK(cudaMemset(epoch, 0, sizeof(int)));
+    g.xf.blocks = 2 * mg_pairs(c.dec_dim);
+    g.af.blocks = 2 * mg_pairs(c.dec_heads * c.dec_head_dim);
+    g.cf.blocks = 2 * mg_pairs(c.dec_ffn);
+    for (MegaFrag *f : {&g.xf, &g.af, &g.cf}) f->bf = s.arena.alloc_n<uint2>(f->blocks * 16 * MG_ROWS);
+    for (MegaFrag *f : {&g.xf, &g.af, &g.cf}) f->off = s.arena.alloc_n<float2>(f->blocks * MG_ROWS);
+    p.trace = trace = s.arena.alloc_n<unsigned long long>((size_t)g.ops_cap * 6);
+    CUDA_OK(cudaMemset(trace, 0, sizeof(unsigned long long) * g.ops_cap * 6));
+    if (const char *ta = getenv("VOX_MEGA_TRACE_ALL"); ta && ta[0] == '1') {
+        const size_t n = (size_t)grid * g.ops_cap * 4;
+        p.trace_all = trace_all = s.arena.alloc_n<unsigned long long>(n);
+        CUDA_OK(cudaMemset(trace_all, 0, sizeof(unsigned long long) * n));
+    }
+    p.eps = m.norm_eps;
+    p.qkv = s.qkv_dec;
+    p.ld_qkv = (c.dec_heads + 2 * c.dec_kv_heads) * c.dec_head_dim;
+    p.H = c.dec_heads;
+    p.Hkv = c.dec_kv_heads;
+    p.hd = c.dec_head_dim;
+    p.max_seq = s.out_ld;
+    p.page_table = s.d_page_table;
+    p.max_pages = s.kv_max_pages;
+    p.window = c.dec_window;
+    p.scale = powf((float)c.dec_head_dim, -0.5f);
+    p.ring = s.kv_ring ? 1 : 0;
+    p.attn_out = s.attn_dec;
+    p.emb_qs = m.tok_emb.qs;
+    p.emb_d = m.tok_emb.d;
+    p.D = c.dec_dim;
+    p.audio_off = s.d_audio_off;
+    p.ffn_ada_rows = s.d_fga_rows;
+    p.x_dec = s.x_dec;
+    p.ssq_x = s.ssq_x;
+    p.emb_fbf = g.xf.bf;
+    p.emb_foff = g.xf.off;
+    p.emb_gamma = m.dec[0].attn_norm;
+    p.att_fbf = g.af.bf;
+    p.att_foff = g.af.off;
+    p.d_pos = s.d_pos;
+    p.d_outpos = s.d_outpos;
+    p.d_tok = s.d_tok;
+    p.d_out = s.d_out;
+    p.out_ld = s.out_ld;
 }
 
-void launch_decode_mega(const MegaParams &p, const MegaPlan &plan, int grid, cudaStream_t st) {
-    VOX_CHECK(p.nstage == plan.nstage && p.scratch_bytes == plan.scratch_bytes, VOX_EINVAL, "decode_mega: plan mismatch");
-    VOX_CHECK(p.ffn_ada_rows != nullptr, VOX_EINVAL, "decode_mega: no per-row ADA table");
-    switch (plan.MT) {
-        case 1: launch_m<1>(p, plan, grid, st); break;
-        case 2: launch_m<2>(p, plan, grid, st); break;
-        case 4: launch_m<4>(p, plan, grid, st); break;
-        case 8: launch_m<8>(p, plan, grid, st); break;
-        default: fail(VOX_EINVAL, "decode_mega: bad token capacity");
+unsigned DecodeMega::prepare(const Session &s, int R) {
+    const Model &m = *s.m;
+    const vox_model_info &c = m.info;
+    State &g = *state;
+    const int B = std::min(R, MG_ROWS);
+    const unsigned groups = (unsigned)(R + MG_ROWS - 1) / MG_ROWS;
+    const int D = c.dec_dim, H = c.dec_heads, Hkv = c.dec_kv_heads, hd = c.dec_head_dim;
+    if (B < 1 || !find_launch(1, H, Hkv, hd)) return 0;
+    if (g.rows == B) return n_ops > 0 ? groups : 0;
+    g.rows = B;
+    n_ops = 0;
+    for (int j = 0; j < c.dec_layers; ++j)
+        if (!m.dec[j].wqkv.qs_tc || !m.dec[j].wo.qs_tc || !m.dec[j].w13.qs_tc || !m.dec[j].w2.qs_tc) return 0;
+    const int max_pairs = std::max(std::max(mg_pairs(D), mg_pairs(H * hd)), mg_pairs(c.dec_ffn));
+    g.plan = decode_mega_plan(B, max_pairs, H, Hkv, hd, (int)kv_elem_bytes(s.kv_type));
+    const int parts = (D + 15) / 16;
+    std::vector<MegaOp> ops;
+    bool ok = true;
+    auto matvec = [&](const Q4Weight &w, const MegaFrag &fin, float *y, int ldy, const float *res, int epi, const float *norm_w,
+                      bool ssq_out_, bool track, int unit_tiles, const MegaFrag &fout, const float *fout_gamma) {
+        MegaOp o;
+        o.kind = MG_MATVEC;
+        o.epi = epi;
+        o.qs_tc = w.qs_tc;
+        o.d_tc = w.d_tc;
+        o.N = w.N;
+        o.K = w.K;
+        o.n_tiles = (w.N + 15) / 16;
+        o.n_pairs = mg_pairs(w.K);
+        int S = (o.n_pairs + g.plan.Ps_cap - 1) / g.plan.Ps_cap;
+        int Ps = (o.n_pairs + S - 1) / S;
+        if (S > 1) Ps = std::min(g.plan.Ps_cap, (Ps + 15) / 16 * 16);
+        S = (o.n_pairs + Ps - 1) / Ps;
+        o.S = S;
+        o.Ps = Ps;
+        o.unit_tiles = unit_tiles;
+        if (o.n_tiles % unit_tiles != 0) ok = false;
+        const int n_units = o.n_tiles / unit_tiles;
+        // tile sums kept in shared memory across K slices: MG_ACC_TILES tiles per CTA
+        if (S > 1 && ((n_units + grid - 1) / grid) * unit_tiles > MG_ACC_TILES) ok = false;
+        o.fin_bf = fin.bf;
+        o.fin_off = fin.off;
+        o.fout_bf = fout.bf;
+        o.fout_off = fout.off;
+        o.fout_gamma = fout_gamma;
+        o.y = y;
+        o.ldy = ldy;
+        o.res = res;
+        o.gamma = norm_w;  // != nullptr: the input is RMS-normalised (1/rms applied in the epilogue)
+        if (norm_w) {
+            o.ssq_in = s.ssq_x;
+            o.ssq_in_parts = parts;
+        }
+        if (ssq_out_) o.ssq_out = s.ssq_x;
+        o.track_argmax = track ? 1 : 0;
+        ops.push_back(o);
+    };
+    const MegaFrag none;
+    {
+        MegaOp e;
+        e.kind = MG_EMBED;
+        ops.push_back(e);
+    }
+    for (int j = 0; j < c.dec_layers; ++j) {
+        const DecLayerW &l = m.dec[j];
+        // wqkv: its epilogue applies RoPE to q and k and appends k, v to layer j's cache
+        matvec(l.wqkv, g.xf, s.qkv_dec, g.p.ld_qkv, nullptr, EPI_NONE, l.attn_norm, false, false, 1, none, nullptr);
+        ops.back().kc = kv_pool(s.kv_layer(s.kc, j), s.kv_type);
+        ops.back().vc = kv_pool(s.kv_layer(s.vc, j), s.kv_type);
+        MegaOp a;
+        a.kind = MG_ATTN;
+        a.kc = kv_pool(s.kv_layer(s.kc, j), s.kv_type);
+        a.vc = kv_pool(s.kv_layer(s.vc, j), s.kv_type);
+        a.layer = j;
+        ops.push_back(a);
+        // wo: h += attn . Wo^T; leaves fragments of h x (ffn_norm x ADA) for w13
+        matvec(l.wo, g.af, s.x_dec, D, s.x_dec, EPI_RESIDUAL, nullptr, true, false, 2, g.xf, nullptr);
+        ops.back().fout_ada_layer = j;   // each row's own ffn_norm x ADA vector of layer j
+        // w13: SwiGLU of the normed stream; leaves fragments of the activation for w2 (no plain copy)
+        matvec(l.w13, g.xf, nullptr, c.dec_ffn, nullptr, EPI_SILU_MUL, l.ffn_norm, false, false, 4, g.cf, nullptr);
+        // w2: h += act . W2^T; leaves fragments of h x (next attention norm | final norm)
+        const float *next_norm = j + 1 < c.dec_layers ? m.dec[j + 1].attn_norm : m.dec_norm;
+        matvec(l.w2, g.cf, s.x_dec, D, s.x_dec, EPI_RESIDUAL, nullptr, true, false, 2, g.xf, next_norm);
+    }
+    matvec(m.tok_emb, g.xf, s.logits, c.vocab, nullptr, EPI_NONE, m.dec_norm, false, true, 1, none, nullptr);
+    {
+        MegaOp f;
+        f.kind = MG_ARGMAX;
+        ops.push_back(f);
+    }
+    if (c.dec_ffn % 32 != 0 || (H * hd) % 32 != 0 || c.dec_layers > 63) ok = false;
+    // the residual epilogues and the embedding must leave exactly `parts` partial sums of squares
+    if ((D + 15) / 16 != parts || D % 32 != 0) ok = false;
+    if (!ok || (int)ops.size() > g.ops_cap) return 0;
+    g.clear_fragments(s.st);
+    CUDA_OK(cudaMemcpyAsync(g.ops, ops.data(), sizeof(MegaOp) * ops.size(), cudaMemcpyHostToDevice, s.st));
+    CUDA_OK(cudaStreamSynchronize(s.st));
+    n_ops = g.p.n_ops = (int)ops.size();
+    return groups;
+}
+
+// More than 8 rows: the rows are independent streams, so the step runs as consecutive launches over groups of 8 rows
+// (each group streams the weights once; the per-op GEMMs would pad 16-32 rows to a 128-token tile).  The scratch
+// activations are reused by the groups; the per-row state (token, positions, page table, audio offset, output row,
+// logits) is addressed from the group's first row.
+void DecodeMega::step(const Session &s, int R, bool add_audio) {
+    const State &g = *state;
+    for (int b0 = 0; b0 < R; b0 += MG_ROWS) {
+        const int B = std::min(MG_ROWS, R - b0);
+        if (B < g.rows) {
+            // a ragged last group on the 8-token instantiation: its padding tokens must read as zero fragments, not as
+            // the previous group's rows
+            g.clear_fragments(s.st);
+        }
+        MegaParams p = g.p;
+        p.B = B;
+        p.page_table += (size_t)b0 * p.max_pages;
+        p.audio_off += b0;
+        p.ffn_ada_rows += b0;
+        p.d_pos += b0;
+        p.d_outpos += b0;
+        p.d_tok += b0;
+        p.d_out += (size_t)b0 * p.out_ld;
+        p.audio = add_audio ? s.audio : nullptr;
+        p.logits_out = s.logits + (size_t)b0 * s.m->info.vocab;
+        // read per launch: an unbounded stream pool points the session's RoPE tables at its ring after creating it
+        p.cos_t = s.dec_rope.cos_t;
+        p.sin_t = s.dec_rope.sin_t;
+        p.rope_rows = s.dec_rope.rows;
+        // key chunks per (stream, kv head): spread the keys over idle SMs in one wave, but no more than 4.  A CTA stages a
+        // chunk's keys in tiles (32 keys at B = 1, 64 at B = 2, 96 at B = 3..8 in this decoder's
+        // scratch region, decode_mega_plan) with one L2 round trip and four CTA
+        // barriers per tile, while the merging CTA polls the other chunks' states one after the other, so chunks beyond
+        // what keeps a unit to a tile or two add merge latency without shortening the walk.  B = 8: 64 (stream, kv head)
+        // pairs, 2 chunks = 128 units on 132 SMs (3 would take a second wave).  B = 1: 8 pairs, 4 chunks = 32 units, at
+        // most 2 tiles each for the first ~250 positions.
+        p.attn_chunks = std::max(1, std::min(4, std::min(grid, g.att_units) / (B * p.Hkv)));
+        p.nstage = g.plan.nstage;
+        p.scratch_bytes = g.plan.scratch_bytes;
+        attn_log.push_back({B, g.plan.MT, g.plan.attn_tile, p.attn_chunks});
+        find_launch(g.plan.MT, p.H, p.Hkv, p.hd)(p, g.plan, grid, s.st);
+        if (!capturing) ++launches;
+    }
+}
+
+void DecodeMega::rebase_epoch(cudaStream_t st) {
+    // the persistent kernel's attention-chunk states carry the tag epoch * 64 + layer + 1 (int): re-base the device
+    // epoch long before that can overflow (2^24 launches ~ 10 hours of continuous decoding) -- and wipe the tagged words, so
+    // that no stale state can match a tag of the new numbering
+    if (launches > (1u << 24)) {
+        CUDA_OK(cudaMemsetAsync(state->p.att_acc, 0, sizeof(float) * state->acc_floats, st));
+        CUDA_OK(cudaMemsetAsync(state->p.att_ml, 0, sizeof(float) * state->ml_floats, st));
+        CUDA_OK(cudaMemsetAsync(epoch, 0, sizeof(int), st));
+        launches = 0;
     }
 }
 

@@ -509,46 +509,9 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ri
             s->am_cnt = s->arena.alloc_n<int>(max_batch);
             CUDA_OK(cudaMemset(s->am_cnt, 0, sizeof(int) * max_batch));
         }
-        {   // persistent decode-step kernel
-            const char *mv = getenv("VOX_MEGA");
-            s->use_mega = !(mv && mv[0] == '0');
-            s->mega_grid = decode_mega_grid(m->device);
-            s->mega_ops_cap = 6 * c.dec_layers + 4;
-            s->mega_ops = s->arena.alloc_n<MegaOp>(s->mega_ops_cap);
-            s->mega_bar = s->arena.alloc_n<unsigned>(4);
-            CUDA_OK(cudaMemset(s->mega_bar, 0, sizeof(unsigned) * 4));
-            s->mega_am_vals = s->arena.alloc_n<float>((size_t)s->mega_grid * 8);
-            s->mega_am_idx = s->arena.alloc_n<int>((size_t)s->mega_grid * 8);
-            s->mega_att_units = std::max(s->mega_grid, 8 * c.dec_kv_heads) + 8 * c.dec_kv_heads;
-            s->mega_att_acc = s->arena.alloc_n<float>((size_t)2 * s->mega_att_units * (c.dec_heads / c.dec_kv_heads) * c.dec_head_dim);  // {value, tag}
-            s->mega_att_ml = s->arena.alloc_n<float>((size_t)2 * s->mega_att_units * (c.dec_heads / c.dec_kv_heads) * 2);  // {value, tag}
-            s->mega_epoch = s->arena.alloc_n<int>(1);
-            // chunk states carry their own validity tag (decode step, layer): never 0
-            CUDA_OK(cudaMemset(s->mega_att_acc, 0, sizeof(float) * 2 * s->mega_att_units * (c.dec_heads / c.dec_kv_heads) * c.dec_head_dim));
-            CUDA_OK(cudaMemset(s->mega_att_ml, 0, sizeof(float) * 2 * s->mega_att_units * (c.dec_heads / c.dec_kv_heads) * 2));
-            CUDA_OK(cudaMemset(s->mega_epoch, 0, sizeof(int)));
-            {
-                auto blocks = [](int K) { return (size_t)((K / 32 + 1) / 2) * 2; };
-                s->mega_xf_blocks = blocks(c.dec_dim);
-                s->mega_af_blocks = blocks(c.dec_heads * c.dec_head_dim);
-                s->mega_cf_blocks = blocks(c.dec_ffn);
-                s->mega_xf_bf = s->arena.alloc_n<uint2>(s->mega_xf_blocks * 16 * 8);
-                s->mega_af_bf = s->arena.alloc_n<uint2>(s->mega_af_blocks * 16 * 8);
-                s->mega_cf_bf = s->arena.alloc_n<uint2>(s->mega_cf_blocks * 16 * 8);
-                s->mega_xf_off = s->arena.alloc_n<float2>(s->mega_xf_blocks * 8);
-                s->mega_af_off = s->arena.alloc_n<float2>(s->mega_af_blocks * 8);
-                s->mega_cf_off = s->arena.alloc_n<float2>(s->mega_cf_blocks * 8);
-            }
-            s->mega_trace = s->arena.alloc_n<unsigned long long>((size_t)s->mega_ops_cap * 6);
-            CUDA_OK(cudaMemset(s->mega_trace, 0, sizeof(unsigned long long) * s->mega_ops_cap * 6));
-            if (const char *ta = getenv("VOX_MEGA_TRACE_ALL")) {
-                if (ta[0] == '1') {
-                    const size_t n = (size_t)s->mega_grid * s->mega_ops_cap * 4;
-                    s->mega_trace_all = s->arena.alloc_n<unsigned long long>(n);
-                    CUDA_OK(cudaMemset(s->mega_trace_all, 0, sizeof(unsigned long long) * n));
-                }
-            }
-        }
+        const char *mv = getenv("VOX_MEGA");
+        s->use_mega = !(mv && mv[0] == '0');
+        s->mega.create(*s);
         CUDA_OK(cudaMemset(s->d_pos, 0, sizeof(int) * B));
         CUDA_OK(cudaMemset(s->d_outpos, 0, sizeof(int) * B));
         s->out_rows.assign(B, 0);
@@ -804,138 +767,19 @@ void Session::forward_logits(int b, int M, const int *ids_host, bool with_audio,
     cache_len += M;
 }
 
-// Builds (once per batch size) the op table of the persistent decode-step kernel.  Returns false when
-// the shapes are outside what decode_mega.cu is instantiated for; the caller then uses per-op launches.
-bool Session::mega_prepare(int B) {
-    const vox_model_info &c = m->info;
-    if (!use_mega || !path.matvec_tc || !fused_decode(B)) return false;
-    if (!decode_mega_supported(B, c.dec_heads, c.dec_kv_heads, c.dec_head_dim)) return false;
-    if (mega_B == B) return mega_n_ops > 0;
-    mega_B = B;
-    mega_n_ops = 0;
-    const int D = c.dec_dim, H = c.dec_heads, Hkv = c.dec_kv_heads, hd = c.dec_head_dim;
-    const int qkvd = (H + 2 * Hkv) * hd;
-    for (int j = 0; j < c.dec_layers; ++j)
-        if (!m->dec[j].wqkv.qs_tc || !m->dec[j].wo.qs_tc || !m->dec[j].w13.qs_tc || !m->dec[j].w2.qs_tc) return false;
-    auto pairs = [](int K) { return (K / 32 + 1) / 2; };
-    const int max_pairs = std::max(std::max(pairs(D), pairs(H * hd)), pairs(c.dec_ffn));
-    mega_plan = decode_mega_plan(B, max_pairs, H, Hkv, hd, (int)kv_elem_bytes(kv_type));
-    const int parts = (D + 15) / 16;
-    std::vector<MegaOp> ops;
-    bool ok = true;
-    struct Frag { uint2 *bf; float2 *off; };
-    const Frag XF{mega_xf_bf, mega_xf_off}, AF{mega_af_bf, mega_af_off}, CF{mega_cf_bf, mega_cf_off};
-    auto matvec = [&](const Q4Weight &w, Frag fin, float *y, int ldy, const float *res, int epi, const float *norm_w,
-                      bool ssq_out_, bool track, int unit_tiles, Frag fout, const float *fout_gamma) {
-        MegaOp o;
-        o.kind = MG_MATVEC;
-        o.epi = epi;
-        o.qs_tc = w.qs_tc;
-        o.d_tc = w.d_tc;
-        o.N = w.N;
-        o.K = w.K;
-        o.n_tiles = (w.N + 15) / 16;
-        o.n_pairs = pairs(w.K);
-        int S = (o.n_pairs + mega_plan.Ps_cap - 1) / mega_plan.Ps_cap;
-        int Ps = (o.n_pairs + S - 1) / S;
-        if (S > 1) Ps = std::min(mega_plan.Ps_cap, (Ps + 15) / 16 * 16);
-        S = (o.n_pairs + Ps - 1) / Ps;
-        o.S = S;
-        o.Ps = Ps;
-        o.unit_tiles = unit_tiles;
-        if (o.n_tiles % unit_tiles != 0) ok = false;
-        const int n_units = o.n_tiles / unit_tiles;
-        // tile sums kept in shared memory across K slices: 2 tiles per CTA
-        if (S > 1 && ((n_units + mega_grid - 1) / mega_grid) * unit_tiles > 2) ok = false;
-        o.fin_bf = fin.bf;
-        o.fin_off = fin.off;
-        o.fout_bf = fout.bf;
-        o.fout_off = fout.off;
-        o.fout_gamma = fout_gamma;
-        o.y = y;
-        o.ldy = ldy;
-        o.res = res;
-        o.gamma = norm_w;  // != nullptr: the input is RMS-normalised (1/rms applied in the epilogue)
-        if (norm_w) {
-            o.ssq_in = ssq_x;
-            o.ssq_in_parts = parts;
-        }
-        if (ssq_out_) o.ssq_out = ssq_x;
-        o.track_argmax = track ? 1 : 0;
-        ops.push_back(o);
-    };
-    const Frag none{nullptr, nullptr};
-    {
-        MegaOp e;
-        e.kind = MG_EMBED;
-        ops.push_back(e);
-    }
-    for (int j = 0; j < c.dec_layers; ++j) {
-        const DecLayerW &l = m->dec[j];
-        // wqkv: its epilogue applies RoPE to q and k and appends k, v to layer j's cache
-        matvec(l.wqkv, XF, qkv_dec, qkvd, nullptr, EPI_NONE, l.attn_norm, false, false, 1, none, nullptr);
-        ops.back().kc = kv_pool(kv_layer(kc, j), kv_type);
-        ops.back().vc = kv_pool(kv_layer(vc, j), kv_type);
-        MegaOp a;
-        a.kind = MG_ATTN;
-        a.kc = kv_pool(kv_layer(kc, j), kv_type);
-        a.vc = kv_pool(kv_layer(vc, j), kv_type);
-        a.layer = j;
-        ops.push_back(a);
-        // wo: h += attn . Wo^T; leaves fragments of h x (ffn_norm x ADA) for w13
-        matvec(l.wo, AF, x_dec, D, x_dec, EPI_RESIDUAL, nullptr, true, false, 2, XF, nullptr);
-        ops.back().fout_ada_layer = j;   // each row's own ffn_norm x ADA vector of layer j
-        // w13: SwiGLU of the normed stream; leaves fragments of the activation for w2 (no plain copy)
-        matvec(l.w13, XF, nullptr, c.dec_ffn, nullptr, EPI_SILU_MUL, l.ffn_norm, false, false, 4, CF, nullptr);
-        // w2: h += act . W2^T; leaves fragments of h x (next attention norm | final norm)
-        const float *next_norm = j + 1 < c.dec_layers ? m->dec[j + 1].attn_norm : m->dec_norm;
-        matvec(l.w2, CF, x_dec, D, x_dec, EPI_RESIDUAL, nullptr, true, false, 2, XF, next_norm);
-    }
-    matvec(m->tok_emb, XF, logits, c.vocab, nullptr, EPI_NONE, m->dec_norm, false, true, 1, none, nullptr);
-    {
-        MegaOp f;
-        f.kind = MG_ARGMAX;
-        ops.push_back(f);
-    }
-    if (c.dec_ffn % 32 != 0 || (H * hd) % 32 != 0 || c.dec_layers > 63) ok = false;
-    // the residual epilogues and the embedding must leave exactly `parts` partial sums of squares
-    if ((D + 15) / 16 != parts || D % 32 != 0) ok = false;
-    if (!ok || (int)ops.size() > mega_ops_cap) return false;
-    // padding tokens (capacity MT > B) and padding blocks must read as zero fragments
-    mega_clear_fragments();
-    mega_ops_host = ops;
-    CUDA_OK(cudaMemcpyAsync(mega_ops, mega_ops_host.data(), sizeof(MegaOp) * ops.size(), cudaMemcpyHostToDevice, st));
-    CUDA_OK(cudaStreamSynchronize(st));
-    mega_n_ops = (int)ops.size();
-    return true;
-}
-
-void Session::mega_clear_fragments() {
-    CUDA_OK(cudaMemsetAsync(mega_xf_bf, 0, sizeof(uint2) * mega_xf_blocks * 16 * 8, st));
-    CUDA_OK(cudaMemsetAsync(mega_af_bf, 0, sizeof(uint2) * mega_af_blocks * 16 * 8, st));
-    CUDA_OK(cudaMemsetAsync(mega_cf_bf, 0, sizeof(uint2) * mega_cf_blocks * 16 * 8, st));
-    CUDA_OK(cudaMemsetAsync(mega_xf_off, 0, sizeof(float2) * mega_xf_blocks * 8, st));
-    CUDA_OK(cudaMemsetAsync(mega_af_off, 0, sizeof(float2) * mega_af_blocks * 8, st));
-    CUDA_OK(cudaMemsetAsync(mega_cf_off, 0, sizeof(float2) * mega_cf_blocks * 8, st));
-}
-
-// More than 8 rows: the rows are independent streams, so the step runs as consecutive launches of the persistent
-// kernel over groups of 8 rows (each group streams the weights once; the per-op GEMMs would pad 16-32 rows to a
-// 128-token tile).  The scratch activations are reused by the groups; the per-row state (token, positions, page table,
-// audio offset, output row, logits) is addressed from the group's first row.
 unsigned Session::prepare_step(int R) {
     bind_rows(R);
-    return mega_prepare(std::min(R, 8)) ? (unsigned)(R + 7) / 8 : 0u;
+    // the persistent kernel runs the step as row groups of a fused-decode size
+    return use_mega && fused_decode(1) ? mega.prepare(*this, R) : 0u;
 }
 
 // One autoregressive step for B streams (model.rs:938-960): embed(prev token) + audio[pos-1],
 // 26 layers, lm_head, argmax, device-side feedback; all positions read from device counters.
 unsigned Session::decode_step(int B, bool add_audio) {
     const unsigned mega_launches = prepare_step(B);
-    mega_attn_log.clear();
-    if (mega_launches > 0) {
-        for (int b0 = 0; b0 < B; b0 += 8) decode_step_mega(b0, std::min(8, B - b0), add_audio);
-    } else {
+    mega.attn_log.clear();
+    if (mega_launches > 0) mega.step(*this, B, add_audio);
+    else {
         launch_embed(m->tok_emb, d_tok, add_audio ? audio : nullptr, d_audio_off, B, 1, d_pos, x_dec,
                      fused_decode(B) ? ssq_x : nullptr, st);
         const bool pending = decoder_forward(B, 1);
@@ -1083,75 +927,6 @@ void Session::beam_step(int b, int n_live) {
                      c.dec_kv_heads, c.dec_head_dim, st);
 }
 
-// One launch of the persistent kernel for rows [b0, b0 + B) (B <= 8) of the session; mega_prepare() has built the op table.
-void Session::decode_step_mega(int b0, int B, bool add_audio) {
-    const vox_model_info &c = m->info;
-    if (B < mega_B) {
-        // a ragged last group on the 8-token instantiation: its padding tokens must read as zero fragments, not as
-        // the previous group's rows
-        mega_clear_fragments();
-    }
-    MegaParams p;
-    p.ops = mega_ops;
-    p.n_ops = mega_n_ops;
-    p.B = B;
-    p.eps = m->norm_eps;
-    p.qkv = qkv_dec;
-    p.ld_qkv = (c.dec_heads + 2 * c.dec_kv_heads) * c.dec_head_dim;
-    p.H = c.dec_heads;
-    p.Hkv = c.dec_kv_heads;
-    p.hd = c.dec_head_dim;
-    p.max_seq = out_ld;
-    p.page_table = d_page_table + (size_t)b0 * kv_max_pages;
-    p.max_pages = kv_max_pages;
-    p.window = c.dec_window;
-    p.scale = powf((float)c.dec_head_dim, -0.5f);
-    p.cos_t = dec_rope.cos_t;
-    p.sin_t = dec_rope.sin_t;
-    p.rope_rows = dec_rope.rows;
-    p.ring = kv_ring ? 1 : 0;
-    p.attn_out = attn_dec;
-    // key chunks per (stream, kv head): spread the keys over idle SMs in one wave, but no more than 4.  A CTA stages a
-    // chunk's keys in tiles (32 keys at B = 1, 64 at B = 2, 96 at B = 3..8 in this decoder's
-    // scratch region, decode_mega_plan) with one L2 round trip and four CTA
-    // barriers per tile, while the merging CTA polls the other chunks' states one after the other, so chunks beyond
-    // what keeps a unit to a tile or two add merge latency without shortening the walk.  B = 8: 64 (stream, kv head)
-    // pairs, 2 chunks = 128 units on 132 SMs (3 would take a second wave).  B = 1: 8 pairs, 4 chunks = 32 units, at
-    // most 2 tiles each for the first ~250 positions.
-    p.attn_chunks = std::max(1, std::min(4, std::min(mega_grid, mega_att_units - 8 * c.dec_kv_heads) / (B * c.dec_kv_heads)));
-    p.att_acc = mega_att_acc;
-    p.att_ml = mega_att_ml;
-    p.d_epoch = mega_epoch;
-    p.emb_qs = m->tok_emb.qs;
-    p.emb_d = m->tok_emb.d;
-    p.D = c.dec_dim;
-    p.audio = add_audio ? audio : nullptr;
-    p.audio_off = d_audio_off + b0;
-    p.ffn_ada_rows = d_fga_rows + b0;
-    p.x_dec = x_dec;
-    p.ssq_x = ssq_x;
-    p.emb_fbf = mega_xf_bf;
-    p.emb_foff = mega_xf_off;
-    p.emb_gamma = m->dec[0].attn_norm;
-    p.att_fbf = mega_af_bf;
-    p.att_foff = mega_af_off;
-    p.d_pos = d_pos + b0;
-    p.d_outpos = d_outpos + b0;
-    p.d_tok = d_tok + b0;
-    p.d_out = d_out + (size_t)b0 * out_ld;
-    p.out_ld = out_ld;
-    p.logits_out = logits + (size_t)b0 * c.vocab;
-    p.am_vals = mega_am_vals;
-    p.am_idx = mega_am_idx;
-    p.bar = mega_bar;
-    p.nstage = mega_plan.nstage;
-    p.scratch_bytes = mega_plan.scratch_bytes;
-    p.trace = mega_trace;
-    p.trace_all = mega_trace_all;
-    mega_attn_log.push_back({B, mega_plan.MT, mega_plan.attn_tile, p.attn_chunks});
-    launch_decode_mega(p, mega_plan, mega_grid, st);
-}
-
 // Prefill of M positions for B streams (model.rs:894-923 with M = 38; also the incremental vox_prefill).
 void Session::prefill(int B, int M, const int *ids_host, bool add_audio) {
     const vox_model_info &c = m->info;
@@ -1174,7 +949,7 @@ void Session::prefill(int B, int M, const int *ids_host, bool add_audio) {
 
 void Session::step_incremental(int b, int M, const int *ids_host, bool add_audio) {
     if (ids_host) prefill(b, M, ids_host, add_audio);
-    else mega_steps_host += decode_step(b, add_audio);
+    else decode_step(b, add_audio);
     cache_len += M;
     scores_k = top_k;
     scores_n = 1;
@@ -1196,20 +971,6 @@ void Session::reset() {
     rebase_epoch();
 }
 
-void Session::rebase_epoch() {
-    // the persistent kernel's attention-chunk states carry the tag epoch * 64 + layer + 1 (int): re-base the device
-    // epoch long before that can overflow (2^24 launches ~ 10 hours of continuous decoding) -- and wipe the tagged words, so
-    // that no stale state can match a tag of the new numbering
-    if (mega_steps_host > (1u << 24)) {
-        const vox_model_info &ci = m->info;
-        const size_t gq = (size_t)(ci.dec_heads / ci.dec_kv_heads);
-        CUDA_OK(cudaMemsetAsync(mega_att_acc, 0, sizeof(float) * 2 * mega_att_units * gq * ci.dec_head_dim, st));
-        CUDA_OK(cudaMemsetAsync(mega_att_ml, 0, sizeof(float) * 2 * mega_att_units * gq * 2, st));
-        CUDA_OK(cudaMemsetAsync(mega_epoch, 0, sizeof(int), st));
-        mega_steps_host = 0;
-    }
-}
-
 // A replay reads the op table and the row tables (ADA sets, audio offsets) the host built: prepare_step re-builds them
 // before the first replay (an incremental call or another encode in between may have changed them), and every other
 // host-side choice the captured kernels depend on is in the key.  `step()` returns its persistent-kernel launches.
@@ -1220,20 +981,23 @@ void Session::run_steps(int R, int n, Step step) {
     const StepKey key{R, top_k, beam_w, path.matvec_tc, path.gemm_tc, use_mega, bias_on()};
     if (use_graph && !(step_graph.exec && step_graph.key == key)) {
         // first step eagerly (also performs any one-time kernel attribute setup), then capture one step and replay it
-        mega_steps_host += step();
+        step();
         --n;
         if (step_graph.exec) { cudaGraphExecDestroy(step_graph.exec); step_graph.exec = nullptr; }
         if (n > 0) {
             cudaGraph_t graph = nullptr;
             const uint64_t before = kernel_launch_count();
             CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+            mega.capturing = true;   // captured, not executed: not counted
             try {
-                step_graph.mega_launches = step();   // captured, not executed: not counted
+                step_graph.mega_launches = step();
             } catch (...) {
+                mega.capturing = false;
                 cudaStreamEndCapture(st, &graph);
                 if (graph) cudaGraphDestroy(graph);
                 throw;
             }
+            mega.capturing = false;
             CUDA_OK(cudaStreamEndCapture(st, &graph));
             step_graph.nodes = kernel_launch_count() - before;
             add_graph_launches(-(int64_t)step_graph.nodes);  // captured, not executed
@@ -1244,10 +1008,10 @@ void Session::run_steps(int R, int n, Step step) {
         }
     }
     for (int i = 0; i < n; ++i) {
-        if (!use_graph) { mega_steps_host += step(); continue; }
+        if (!use_graph) { step(); continue; }
         CUDA_OK(cudaGraphLaunch(step_graph.exec, st));
         add_graph_launches((int64_t)step_graph.nodes);
-        mega_steps_host += step_graph.mega_launches;
+        mega.launches += step_graph.mega_launches;
     }
 }
 

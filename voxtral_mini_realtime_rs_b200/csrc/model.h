@@ -4,7 +4,6 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <array>
 #include <cstdint>
 #include <functional>
 #include <string>
@@ -174,7 +173,7 @@ struct Session {
     float *ada_sets = nullptr, *t_embed = nullptr, *ada_tmp = nullptr;
     size_t ada_set_floats() const { return (size_t)2 * m->info.dec_layers * m->info.dec_dim; }
     // row i of a launch reads its stream's ADA set and audio embeddings through the tables [max_batch] bind_rows
-    // fills: the ADA set pointers (kernels.h AdaRows, MegaParams::ffn_ada_rows) and the audio offsets (launch_embed)
+    // fills: the ADA set pointers (kernels.h AdaRows, the persistent kernel's ffn_ada_rows) and the audio offsets (launch_embed)
     const float **d_ada_rows = nullptr, **d_fga_rows = nullptr;
     int64_t *d_audio_off = nullptr;
     std::vector<int> bound_streams;     // what the tables hold, per row
@@ -243,35 +242,11 @@ struct Session {
     float *am_vals = nullptr;
     int *am_idx = nullptr, *am_cnt = nullptr;
     TcWork tc_work(bool norm_in, bool ssq_out) const;
-    // persistent decode-step kernel (decode_mega.cu): op table per batch size, grid barrier words,
-    // per-CTA argmax candidates.  VOX_MEGA=0 (or debug "mega_off") selects the per-op launches.
+    // persistent decode-step kernel (decode_mega.h): its op table, scratch, launches and step epoch.  VOX_MEGA=0 (or
+    // debug "mega_off") selects the per-op launches.
     bool use_mega = true;
-    int mega_B = 0, mega_grid = 0, mega_n_ops = 0, mega_ops_cap = 0;
-    MegaPlan mega_plan;
-    std::vector<MegaOp> mega_ops_host;
-    MegaOp *mega_ops = nullptr;
-    unsigned *mega_bar = nullptr;
-    float *mega_am_vals = nullptr;
-    int *mega_am_idx = nullptr;
-    float *mega_att_acc = nullptr, *mega_att_ml = nullptr;  // key-chunk softmax states (MG_ATTN -> MG_ATTN_MERGE)
-    int mega_att_units = 0;
-    int *mega_epoch = nullptr;
-    // persistent-kernel launches executed since the device epoch was last re-based (Session::reset): advanced by the
-    // code that issues or replays steps, never under stream capture
-    unsigned mega_steps_host = 0;
-    // attention tiling of each persistent launch of the last decode step issued or captured (debug "mega_attn"): {rows,
-    // token capacity MT, keys per K/V tile, key chunks per (stream, kv head)}; empty after a per-op step
-    std::vector<std::array<int, 4>> mega_attn_log;
-    // activation fragments (decode_mega.cu frag_build): residual stream x norm weight, attention output, SwiGLU output
-    uint2 *mega_xf_bf = nullptr, *mega_af_bf = nullptr, *mega_cf_bf = nullptr;
-    float2 *mega_xf_off = nullptr, *mega_af_off = nullptr, *mega_cf_off = nullptr;
-    size_t mega_xf_blocks = 0, mega_af_blocks = 0, mega_cf_blocks = 0;
-    void mega_clear_fragments();   // zero all three (padding tokens and blocks must read as zero), on st
-    unsigned long long *mega_trace_all = nullptr;  // [grid][mega_ops_cap][4] (debug "mega_trace_all", VOX_MEGA_TRACE_ALL=1)
-    unsigned long long *mega_trace = nullptr;  // [mega_ops_cap][6] SM-clock stamps of CTA 0 (debug "mega_trace")
-    bool mega_prepare(int B);
+    DecodeMega mega;
     bool fused_decode(int rows) const;
-    void decode_step_mega(int b0, int B, bool add_audio);
     void *xt_buf = nullptr;   // f16 split tiles feeding the wgmma GEMM
     size_t xt_elems = 0;
     GemmWork gemm_work;       // split-K scratch of the wgmma GEMM
@@ -319,7 +294,7 @@ struct Session {
     // host-side preparation a decode step over R rows depends on (bind_rows, the persistent kernel's op table); returns the step's persistent-kernel launches, 0 on the per-op path.  Copy- and sync-free when
     // the last step had the same shape, so that it may run under stream capture.
     unsigned prepare_step(int R);
-    // returns prepare_step(B); advances no host counter (it also runs under stream capture)
+    // returns prepare_step(B), the persistent-kernel launches it issues (mega counts them unless it is capturing)
     unsigned decode_step(int B, bool add_audio = true);
     // `n` decode steps over R rows, each one `step()`: CUDA-graph replay of one captured step when use_graph, else eager
     template <class Step> void run_steps(int R, int n, Step step);
@@ -327,8 +302,8 @@ struct Session {
     // last row, argmax -> d_tok (device feedback) and d_out; advances the device counters
     void prefill(int B, int M, const int *ids_host, bool add_audio);
     // the incremental API after argument validation: vox_prefill over ids_host [b][M], or vox_decode_step (ids_host
-    // nullptr, M = 1) over rows [0, b); then advances cache_len, out_rows, the epoch count and the positions
-    // vox_session_token_scores reads
+    // nullptr, M = 1) over rows [0, b); then advances cache_len, out_rows and the positions vox_session_token_scores
+    // reads
     void step_incremental(int b, int M, const int *ids_host, bool add_audio);
     void check_batch(int b) const;
     void check_ids(const int32_t *ids, size_t n) const;
@@ -343,7 +318,7 @@ struct Session {
                            int32_t *n_out, vox_timings *tm);
     void reset();
     // re-bases the persistent kernel's step epoch once it has advanced far (see reset)
-    void rebase_epoch();
+    void rebase_epoch() { mega.rebase_epoch(st); }
 };
 
 }  // namespace vox

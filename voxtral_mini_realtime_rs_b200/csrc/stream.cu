@@ -501,7 +501,7 @@ void StreamPool::tick(vox_stream_stats *st_out) {
                 if (unbounded) fill_rope(dec_rope_cos, dec_rope_sin, c.dec_head_dim, kDecRopeRing, 0, slots[id].pos, 1);
             }
             upload_rows(rows, true);
-            s->mega_steps_host += s->decode_step((int)rows.size(), true);
+            s->decode_step((int)rows.size(), true);
             std::vector<int> toks(rows.size());
             std::vector<int32_t> top(rows.size() * s->top_k);
             std::vector<float> lp(rows.size() * s->top_k);
