@@ -158,6 +158,7 @@ void vox_model_free(vox_model *m);
 /* ------------------------------------------------------------------ session
  * caller-owned mutable state (LayerCaches kv_cache.rs:208-259 + workspace + stream). */
 typedef struct vox_session vox_session;
+typedef struct vox_tokenizer vox_tokenizer;   /* the tokenizer section below */
 typedef struct {
     float preprocess_ms; /* pad + H2D + mel                       (e2e_bench.rs:147-149) */
     float encode_ms;     /* conv + encoder + adapter              (e2e_bench.rs:161-167) */
@@ -292,8 +293,8 @@ int32_t vox_session_nbest(vox_session *s, int32_t *ids, double *scores, size_t c
 /* Phrase boosting (custom vocabulary) for greedy decoding: vox_transcribe_streaming, vox_transcribe_pcm,
  * vox_transcribe_pcm_ragged, vox_transcribe_pcm_dev, vox_prefill, vox_decode_step and streaming pools.
  *   - A stream's bias list holds up to VOX_MAX_BIAS_PHRASES phrases.  A phrase is 1 to VOX_MAX_BIAS_LEN token ids, each
- *     in [VOX_FIRST_TEXT_ID, vocab), with a boost b > 0 (finite, in logit units).  Callers tokenize their phrases
- *     themselves; a word's ids depend on its leading space, so a list may hold both forms.
+ *     in [VOX_FIRST_TEXT_ID, vocab), with a boost b > 0 (finite, in logit units).  A word's ids depend on its leading
+ *     space, so a list may hold both forms; vox_session_set_bias_text builds them from words.
  *   - The stream's history h is the sequence of text ids (>= VOX_FIRST_TEXT_ID) it has emitted since the history was
  *     last cleared; lower (special) ids, [STREAMING_PAD] among them, never enter it.  The history is cleared whenever the
  *     decoder cache is emptied (every transcribe call, vox_session_reset, a pool session's prefill) and when the stream's
@@ -319,6 +320,20 @@ int32_t vox_session_nbest(vox_session *s, int32_t *ids, double *scores, size_t c
 #define VOX_MAX_BIAS_LEN 16
 int32_t vox_session_set_bias(vox_session *s, int32_t stream, const int32_t *ids, const int32_t *lens, const float *boosts,
                              int32_t n_phrases);
+/* vox_session_set_bias with the phrases given as words: phrases[p] is NUL-terminated UTF-8, boosts[p] its boost.
+ * Expansion rule (the whole contract): phrase p gives the id phrase vox_tokenizer_encode(p), then the id phrase
+ * vox_tokenizer_encode(" " + p) unless p starts with White_Space (a word in running text carries its leading space); the
+ * second form is dropped when it equals the first.  Both forms get boosts[p].  The forms go in phrase order, and the
+ * result goes to vox_session_set_bias unchanged: the same replacement of the stream's list, history clearing and device
+ * rule.  No other variant is added: case ("Zurich" / "zurich"), plural or other spellings are separate phrases the caller
+ * lists.  n_phrases = 0 clears the list (t, phrases and boosts may then be NULL).
+ * VOX_EINVAL, changing nothing, for an empty phrase, a NULL phrase or buffer, invalid UTF-8, a form longer than
+ * VOX_MAX_BIAS_LEN ids (the message names the phrase index), more than VOX_MAX_BIAS_PHRASES forms after expansion, and
+ * every case vox_session_set_bias refuses (a form id outside the model's vocabulary, a boost that is not finite and > 0,
+ * an unknown stream); VOX_EFORMAT for a tokenizer that cannot encode (vox_tokenizer_encode).  All of it is checked on the
+ * host before any device work. */
+int32_t vox_session_set_bias_text(vox_session *s, int32_t stream, const vox_tokenizer *t, const char *const *phrases,
+                                  const float *boosts, int32_t n_phrases);
 int32_t vox_session_cache_len(const vox_session *s, int32_t *len);             /* LayerCaches::seq_len */
 int32_t vox_session_reset(vox_session *s);                                       /* LayerCaches::reset  */
 /* debugging / parity: copy an internal activation by name ("enc_out","audio_embeds","conv","enc<i>",
@@ -375,6 +390,9 @@ int32_t vox_stream_set_delay(vox_stream_pool *p, int32_t session, float delay_to
  * open.  It takes effect at the session's next decoder position and clears its history; vox_stream_open empties it. */
 int32_t vox_stream_set_bias(vox_stream_pool *p, int32_t session, const int32_t *ids, const int32_t *lens, const float *boosts,
                             int32_t n_phrases);
+/* the session's bias list from words: vox_session_set_bias_text's expansion, then vox_stream_set_bias */
+int32_t vox_stream_set_bias_text(vox_stream_pool *p, int32_t session, const vox_tokenizer *t, const char *const *phrases,
+                                 const float *boosts, int32_t n_phrases);
 int32_t vox_stream_push_pcm(vox_stream_pool *p, int32_t session, const float *samples, size_t n);
 int32_t vox_stream_finish(vox_stream_pool *p, int32_t session);        /* end of utterance: right padding, pad.rs:89-103 */
 int32_t vox_stream_tick(vox_stream_pool *p, vox_stream_stats *stats /* nullable */);
@@ -413,8 +431,7 @@ int32_t vox_stream_close(vox_stream_pool *p, int32_t session);
 void vox_stream_pool_free(vox_stream_pool *p);
 
 /* ------------------------------------------------------------------ tokenizer (host)
- * VoxtralTokenizer, src/tokenizer/mod.rs:70-214 */
-typedef struct vox_tokenizer vox_tokenizer;
+ * VoxtralTokenizer, src/tokenizer/mod.rs:70-214 (vox_tokenizer is declared with the session) */
 int32_t vox_tokenizer_from_file(const char *path, vox_tokenizer **out);         /* mod.rs:70  */
 int32_t vox_tokenizer_from_json(const char *json, size_t len, vox_tokenizer **out); /* mod.rs:125 */
 int32_t vox_tokenizer_decode(const vox_tokenizer *t, const uint32_t *ids, size_t n, char *buf,
@@ -422,6 +439,16 @@ int32_t vox_tokenizer_decode(const vox_tokenizer *t, const uint32_t *ids, size_t
 int32_t vox_tokenizer_decode_token(const vox_tokenizer *t, uint32_t id, char *buf, size_t cap,
                                    size_t *written, int32_t *found);             /* mod.rs:194 */
 int32_t vox_tokenizer_vocab_size(const vox_tokenizer *t, size_t *n);            /* mod.rs:211 */
+/* Tekken encode (mistral_common's Tekkenizer.encode(text, bos=False, eos=False), tiktoken's encode with no special
+ * tokens): UTF-8 text[len] -> text ids (>= VOX_FIRST_TEXT_ID) in ids[cap]; *n = ids needed.  ids NULL: only *n.
+ * Special-token text such as "[INST]" is plain text; no Unicode normalisation (NFC and NFD text give different ids).
+ * The ids decode back to the text: vox_tokenizer_decode(encode(s)) == s.  The rank table (the text ranks below
+ * default_vocab_size - 1000, the lowest position winning for a repeated byte string) is built by the first call and kept;
+ * concurrent calls on one handle are safe.
+ * VOX_EINVAL invalid UTF-8 (overlong forms, surrogates, > U+10FFFF, truncated sequences); VOX_EFORMAT a pattern other
+ * than Tekken's or a vocabulary without the 256 byte tokens (decoding still works); VOX_ECAPACITY cap < *n (and *n is
+ * set). */
+int32_t vox_tokenizer_encode(const vox_tokenizer *t, const char *text, size_t len, int32_t *ids, size_t cap, size_t *n);
 void vox_tokenizer_free(vox_tokenizer *t);
 
 #ifdef __cplusplus

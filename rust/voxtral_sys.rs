@@ -86,6 +86,9 @@ extern "C" {
     // n_phrases = 0 clears
     pub fn vox_session_set_bias(s: *mut vox_session, stream: i32, ids: *const i32, lens: *const i32, boosts: *const f32,
                                 n_phrases: i32) -> i32;
+    // the same from words (NUL-terminated UTF-8): each word and its leading-space form (include/voxtral.h)
+    pub fn vox_session_set_bias_text(s: *mut vox_session, stream: i32, t: *const vox_tokenizer, phrases: *const *const c_char,
+                                     boosts: *const f32, n_phrases: i32) -> i32;
     pub fn vox_session_free(s: *mut vox_session);
     // src/gguf/{tensor,linear,op}.rs
     pub fn vox_q4_tensor_create(bytes: *const u8, nbytes: usize, n: i64, k: i64, device: i32,
@@ -115,6 +118,8 @@ extern "C" {
     pub fn vox_stream_set_delay(p: *mut vox_stream_pool, session: i32, delay_tokens: f32) -> i32;
     pub fn vox_stream_set_bias(p: *mut vox_stream_pool, session: i32, ids: *const i32, lens: *const i32, boosts: *const f32,
                                n_phrases: i32) -> i32;
+    pub fn vox_stream_set_bias_text(p: *mut vox_stream_pool, session: i32, t: *const vox_tokenizer,
+                                    phrases: *const *const c_char, boosts: *const f32, n_phrases: i32) -> i32;
     pub fn vox_stream_push_pcm(p: *mut vox_stream_pool, session: i32, samples: *const f32, n: usize) -> i32;
     pub fn vox_stream_finish(p: *mut vox_stream_pool, session: i32) -> i32;
     pub fn vox_stream_tick(p: *mut vox_stream_pool, stats: *mut vox_stream_stats) -> i32;
@@ -135,4 +140,7 @@ extern "C" {
     pub fn vox_tokenizer_decode(t: *const vox_tokenizer, ids: *const u32, n: usize, buf: *mut c_char,
                                 cap: usize, written: *mut usize) -> i32;
     pub fn vox_tokenizer_free(t: *mut vox_tokenizer);
+    // Tekken encode, which the crate's tokenizer lacks: UTF-8 text -> text ids; ids NULL: only *n
+    pub fn vox_tokenizer_encode(t: *const vox_tokenizer, text: *const c_char, len: usize, ids: *mut i32, cap: usize,
+                                n: *mut usize) -> i32;
 }

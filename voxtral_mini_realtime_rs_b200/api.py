@@ -142,6 +142,7 @@ _SIGS = {
     "vox_session_nbest": (C.c_int32, [_P, _P, _P, C.c_size_t, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
                                       C.POINTER(C.c_int32)]),
     "vox_session_set_bias": (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32]),
+    "vox_session_set_bias_text": (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32]),
     "vox_session_cache_len": (C.c_int32, [_P, C.POINTER(C.c_int32)]),
     "vox_session_reset": (C.c_int32, [_P]),
     "vox_session_debug_read": (C.c_int32, [_P, C.c_char_p, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
@@ -153,6 +154,7 @@ _SIGS = {
     "vox_stream_open": (C.c_int32, [_P, C.POINTER(C.c_int32)]),
     "vox_stream_set_delay": (C.c_int32, [_P, C.c_int32, C.c_float]),
     "vox_stream_set_bias": (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32]),
+    "vox_stream_set_bias_text": (C.c_int32, [_P, C.c_int32, _P, _P, _P, C.c_int32]),
     "vox_stream_push_pcm": (C.c_int32, [_P, C.c_int32, _P, C.c_size_t]),
     "vox_stream_finish": (C.c_int32, [_P, C.c_int32]),
     "vox_stream_tick": (C.c_int32, [_P, _P]),
@@ -172,6 +174,7 @@ _SIGS = {
     "vox_tokenizer_decode_token": (C.c_int32, [_P, C.c_uint32, _P, C.c_size_t, C.POINTER(C.c_size_t),
                                                C.POINTER(C.c_int32)]),
     "vox_tokenizer_vocab_size": (C.c_int32, [_P, C.POINTER(C.c_size_t)]),
+    "vox_tokenizer_encode": (C.c_int32, [_P, C.c_char_p, C.c_size_t, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
     "vox_tokenizer_free": (None, [_P]),
 }
 
@@ -212,6 +215,21 @@ def _bias_args(phrases, boost):
     keep = [ids, lens, boosts]
     ptr = (lambda a: _ptr(a) if a.size else None)
     return keep, ptr(ids), ptr(lens), ptr(boosts), n
+
+
+def _bias_text_args(phrases, boost):
+    """(keep, phrases, boosts, n) of vox_session_set_bias_text for a list of words and one boost or one per word."""
+    words = [p.encode("utf-8") if isinstance(p, str) else bytes(p) for p in phrases]
+    if any(b"\0" in w for w in words):
+        raise ValueError("a phrase contains a NUL character")
+    n = len(words)
+    arr = (C.c_char_p * max(n, 1))(*words)
+    boosts = np.broadcast_to(np.asarray(boost, np.float32), (n,)).copy()
+    return (arr, boosts), (C.cast(arr, _P) if n else None), (_ptr(boosts) if n else None), n
+
+
+def _tok_handle(tokenizer):
+    return None if tokenizer is None else tokenizer._h
 
 
 def _f32(a) -> np.ndarray:
@@ -820,6 +838,14 @@ class Q4VoxtralModel:
         _keep, ids, lens, boosts, n = _bias_args(phrases, boost)
         _check(lib().vox_session_set_bias(self._s, -1 if stream is None else stream, ids, lens, boosts, n))
 
+    def set_bias_text(self, phrases, boost, tokenizer: "VoxtralTokenizer", stream: int | None = None):
+        """set_bias with the phrases given as words (str, UTF-8): each word boosts its Tekken ids, and those of its
+        leading-space form unless it starts with whitespace (vox_session_set_bias_text in include/voxtral.h: the
+        expansion runs in the library).  `boost`: one float > 0 or one per word; an empty list clears."""
+        _keep, words, boosts, n = _bias_text_args(phrases, boost)
+        _check(lib().vox_session_set_bias_text(self._s, -1 if stream is None else stream, _tok_handle(tokenizer), words,
+                                               boosts, n))
+
     def cache_len(self) -> int:
         v = C.c_int32()
         _check(lib().vox_session_cache_len(self._s, C.byref(v)))
@@ -915,6 +941,11 @@ class StreamingPool:
         with none."""
         _keep, ids, lens, boosts, n = _bias_args(phrases, boost)
         _check(lib().vox_stream_set_bias(self._p, session, ids, lens, boosts, n))
+
+    def set_bias_text(self, session: int, phrases, boost, tokenizer: "VoxtralTokenizer"):
+        """The session's phrase list from words (Q4VoxtralModel.set_bias_text)."""
+        _keep, words, boosts, n = _bias_text_args(phrases, boost)
+        _check(lib().vox_stream_set_bias_text(self._p, session, _tok_handle(tokenizer), words, boosts, n))
 
     def push(self, session: int, samples):
         s = _f32(samples).reshape(-1)
@@ -1024,7 +1055,7 @@ class Q4ModelLoader:
 
 # ------------------------------------------------------------------------------ tokenizer
 class VoxtralTokenizer:
-    """VoxtralTokenizer (tokenizer/mod.rs:56-214), decode-only."""
+    """VoxtralTokenizer (tokenizer/mod.rs:56-214), plus the Tekken encoder the reference lacks."""
 
     def __init__(self, handle):
         self._h = handle
@@ -1058,6 +1089,16 @@ class VoxtralTokenizer:
         buf = C.create_string_buffer(n.value + 1)
         _check(lib().vox_tokenizer_decode_token(self._h, token_id, buf, n.value + 1, C.byref(n), C.byref(found)))
         return buf.raw[: n.value].decode("utf-8")
+
+    def encode(self, text) -> np.ndarray:
+        """Text ids (int32, >= 1000) of `text` (str, or bytes that must be UTF-8): mistral_common's
+        Tekkenizer.encode(text, bos=False, eos=False)."""
+        raw = text.encode("utf-8") if isinstance(text, str) else bytes(text)
+        n = C.c_size_t()
+        _check(lib().vox_tokenizer_encode(self._h, raw, len(raw), None, 0, C.byref(n)))
+        ids = np.empty(n.value, np.int32)
+        _check(lib().vox_tokenizer_encode(self._h, raw, len(raw), _ptr(ids), ids.size, C.byref(n)))
+        return ids
 
     def vocab_size(self) -> int:
         n = C.c_size_t()

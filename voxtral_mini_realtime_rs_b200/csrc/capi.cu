@@ -826,6 +826,54 @@ int32_t vox_session_set_bias(vox_session *sh, int32_t stream, const int32_t *ids
     sh->s->set_bias(stream, ids, lens, boosts, n_phrases);
     VOX_API_END
 }
+// vox_session_set_bias_text's expansion: phrase p -> encode(p), then encode(" " + p) unless p starts with White_Space
+// (and unless it equals the first form), both at boosts[p], in phrase order.  Checked here, on the host, in full.
+struct BiasText {
+    std::vector<int32_t> ids, lens;
+    std::vector<float> boosts;
+};
+static BiasText expand_bias_text(const vox_tokenizer *t, const char *const *phrases, const float *boosts, int32_t n) {
+    BiasText o;
+    VOX_CHECK(n >= 0, VOX_EINVAL, "set_bias_text: %d phrases", n);
+    if (n == 0) return o;
+    REQUIRE(t); REQUIRE(phrases); REQUIRE(boosts);
+    auto add = [&](const std::vector<int32_t> &form, int p) {
+        VOX_CHECK(form.size() <= VOX_MAX_BIAS_LEN, VOX_EINVAL, "set_bias_text: phrase %d encodes to %zu ids (at most %d)", p,
+                  form.size(), VOX_MAX_BIAS_LEN);
+        VOX_CHECK(o.lens.size() < VOX_MAX_BIAS_PHRASES, VOX_EINVAL,
+                  "set_bias_text: phrase %d: more than %d id phrases after adding the leading-space forms", p, VOX_MAX_BIAS_PHRASES);
+        o.ids.insert(o.ids.end(), form.begin(), form.end());
+        o.lens.push_back((int32_t)form.size());
+        o.boosts.push_back(boosts[p]);
+    };
+    for (int p = 0; p < n; ++p) {
+        VOX_CHECK(phrases[p] != nullptr, VOX_EINVAL, "set_bias_text: phrase %d is NULL", p);
+        const std::string word(phrases[p]);
+        VOX_CHECK(!word.empty(), VOX_EINVAL, "set_bias_text: phrase %d is empty", p);
+        std::vector<int32_t> bare;
+        try {
+            bare = t->t->encode(word.data(), word.size());
+        } catch (const Error &e) {
+            fail(e.code, fmt("set_bias_text: phrase %d: %s", p, e.what()));
+        }
+        add(bare, p);
+        // a phrase that starts with White_Space keeps its one form: " " + p would only lengthen its leading run
+        if (Tokenizer::starts_with_white_space(word.data(), word.size())) continue;
+        const std::string with_space = " " + word;
+        const std::vector<int32_t> spaced = t->t->encode(with_space.data(), with_space.size());
+        if (spaced != bare) add(spaced, p);
+    }
+    return o;
+}
+int32_t vox_session_set_bias_text(vox_session *sh, int32_t stream, const vox_tokenizer *t, const char *const *phrases,
+                                  const float *boosts, int32_t n_phrases) {
+    VOX_API_BEGIN
+    require_any_device();
+    REQUIRE(sh);
+    const BiasText b = expand_bias_text(t, phrases, boosts, n_phrases);
+    sh->s->set_bias(stream, b.ids.data(), b.lens.data(), b.boosts.data(), (int)b.lens.size());
+    VOX_API_END
+}
 int32_t vox_session_nbest(vox_session *sh, int32_t *ids, double *scores, size_t cap, int32_t *b, int32_t *w, int32_t *n) {
     VOX_API_BEGIN
     REQUIRE(sh);
@@ -1151,6 +1199,15 @@ int32_t vox_stream_set_bias(vox_stream_pool *p, int32_t session, const int32_t *
     p->p->set_bias(session, ids, lens, boosts, n_phrases);
     VOX_API_END
 }
+int32_t vox_stream_set_bias_text(vox_stream_pool *p, int32_t session, const vox_tokenizer *t, const char *const *phrases,
+                                 const float *boosts, int32_t n_phrases) {
+    VOX_API_BEGIN
+    require_any_device();
+    REQUIRE(p);
+    const BiasText b = expand_bias_text(t, phrases, boosts, n_phrases);
+    p->p->set_bias(session, b.ids.data(), b.lens.data(), b.boosts.data(), (int)b.lens.size());
+    VOX_API_END
+}
 int32_t vox_stream_session_info(vox_stream_pool *p, int32_t session, struct vox_stream_session_info *out) {
     VOX_API_BEGIN
     require_any_device();
@@ -1212,6 +1269,18 @@ int32_t vox_tokenizer_decode_token(const vox_tokenizer *t, uint32_t id, char *bu
     const bool ok = t->t->decode_token(id, &s);
     if (found) *found = ok ? 1 : 0;
     copy_out(ok ? s : std::string(), buf, cap, written);
+    VOX_API_END
+}
+int32_t vox_tokenizer_encode(const vox_tokenizer *t, const char *text, size_t len, int32_t *ids, size_t cap, size_t *n) {
+    VOX_API_BEGIN
+    REQUIRE(t); REQUIRE(n);
+    if (len) REQUIRE(text);
+    const std::vector<int32_t> out = t->t->encode(text, len);
+    *n = out.size();
+    if (ids) {
+        VOX_CHECK(cap >= out.size(), VOX_ECAPACITY, "id buffer too small (%zu < %zu)", cap, out.size());
+        std::copy(out.begin(), out.end(), ids);
+    }
     VOX_API_END
 }
 int32_t vox_tokenizer_vocab_size(const vox_tokenizer *t, size_t *n) {

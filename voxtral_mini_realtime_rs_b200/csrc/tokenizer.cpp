@@ -1,9 +1,11 @@
-// tokenizer.cpp -- Tekken decode-only tokenizer (reference src/tokenizer/mod.rs:70-214).
+// tokenizer.cpp -- Tekken tokenizer (reference src/tokenizer/mod.rs:70-214, decode only there).
 // tekken.json -> per-vocab-index byte strings (base64 `token_bytes`, else UTF-8 of `token_str`);
 // control entries (is_control) are kept in a rank->string map; decode() skips ids < 1000, maps
 // id-1000 to the vocab *position*, silently skips unknown ids and returns lossy UTF-8.
+// encode() is tiktoken's encode over the same positions (mistral_common's Tekkenizer.encode without BOS/EOS).
 #include "tokenizer.h"
 
+#include <algorithm>
 #include <cstdlib>
 #include <cctype>
 #include <cstring>
@@ -11,6 +13,7 @@
 #include <sstream>
 
 #include "common.h"
+#include "unicode_tables.h"
 
 namespace vox {
 namespace {
@@ -225,7 +228,202 @@ std::string utf8_lossy(const std::string &in) {
     return o;
 }
 
+// ---- Tekken encoder: pre-tokenizer over code points, then tiktoken's byte-pair merge inside each piece ----------
+// The one pattern the encoder knows (config.pattern of every Tekken vocabulary), matched by match_piece() below.
+const char kTekkenPattern[] =
+    R"([^\r\n\p{L}\p{N}]?[\p{Lu}\p{Lt}\p{Lm}\p{Lo}\p{M}]*[\p{Ll}\p{Lm}\p{Lo}\p{M}]+|)"
+    R"([^\r\n\p{L}\p{N}]?[\p{Lu}\p{Lt}\p{Lm}\p{Lo}\p{M}]+[\p{Ll}\p{Lm}\p{Lo}\p{M}]*|)"
+    R"(\p{N}| ?[^\s\p{L}\p{N}]+[\r\n/]*|\s*[\r\n]+|\s+(?!\S)|\s+)";
+
+// per-code-point flags: the pattern's classes
+enum : uint8_t {
+    fL = 1,      // \p{L}
+    fN = 2,      // \p{N}
+    fWS = 4,     // \s (White_Space)
+    fU = 8,      // [\p{Lu}\p{Lt}\p{Lm}\p{Lo}\p{M}]
+    fLw = 16,    // [\p{Ll}\p{Lm}\p{Lo}\p{M}]
+    fCRLF = 32,  // [\r\n]
+    fTail = 64,  // [\r\n/]
+};
+
+uint8_t char_flags(uint32_t c) {
+    int lo = 0, hi = uni::kNumRanges - 1, cls = 0;
+    while (lo <= hi) {
+        const int mid = (lo + hi) / 2;
+        if (c < uni::kUniRanges[mid].lo) hi = mid - 1;
+        else if (c > uni::kUniRanges[mid].hi) lo = mid + 1;
+        else { cls = uni::kUniRanges[mid].cls; break; }
+    }
+    uint8_t f = 0;
+    switch (cls) {
+        case uni::kLu: case uni::kLt: f = fL | fU; break;
+        case uni::kLl: f = fL | fLw; break;
+        case uni::kLm: case uni::kLo: f = fL | fU | fLw; break;
+        case uni::kM: f = fU | fLw; break;
+        case uni::kN: f = fN; break;
+        default: break;
+    }
+    for (uint32_t w : uni::kWhiteSpace)
+        if (c == w) f |= fWS;
+    if (c == '\r' || c == '\n') f |= fCRLF | fTail;
+    if (c == '/') f |= fTail;
+    return f;
+}
+
+// [^\r\n\p{L}\p{N}] and [^\s\p{L}\p{N}]
+bool is_lead(uint8_t f) { return !(f & (fL | fN | fCRLF)); }
+bool is_punct(uint8_t f) { return !(f & (fL | fN | fWS)); }
+
+// strict UTF-8 -> code points and their byte offsets (offs has one more entry: the end)
+void utf8_decode(const uint8_t *s, size_t n, std::vector<uint32_t> &cps, std::vector<size_t> &offs) {
+    size_t i = 0;
+    while (i < n) {
+        const uint8_t c = s[i];
+        offs.push_back(i);
+        if (c < 0x80) { cps.push_back(c); ++i; continue; }
+        int need;
+        uint8_t lo = 0x80, hi = 0xBF;
+        uint32_t cp;
+        if (c >= 0xC2 && c <= 0xDF) { need = 1; cp = c & 0x1F; }
+        else if (c >= 0xE0 && c <= 0xEF) { need = 2; cp = c & 0x0F; if (c == 0xE0) lo = 0xA0; if (c == 0xED) hi = 0x9F; }
+        else if (c >= 0xF0 && c <= 0xF4) { need = 3; cp = c & 0x07; if (c == 0xF0) lo = 0x90; if (c == 0xF4) hi = 0x8F; }
+        else fail(VOX_EINVAL, fmt("encode: invalid UTF-8 byte 0x%02X at offset %zu", c, i));
+        VOX_CHECK(n - i > (size_t)need, VOX_EINVAL, "encode: truncated UTF-8 sequence at offset %zu", i);
+        for (int k = 1; k <= need; ++k) {
+            const uint8_t d = s[i + k];
+            VOX_CHECK(d >= (k == 1 ? lo : 0x80) && d <= (k == 1 ? hi : 0xBF), VOX_EINVAL,
+                      "encode: invalid UTF-8 sequence at offset %zu", i);
+            cp = (cp << 6) | (d & 0x3F);
+        }
+        cps.push_back(cp);
+        i += need + 1;
+    }
+    offs.push_back(n);
+}
+
+// end of the maximal run of code points from k that have one of `mask`'s flags
+size_t run_end(const std::vector<uint8_t> &f, size_t k, uint8_t mask) {
+    while (k < f.size() && (f[k] & mask)) ++k;
+    return k;
+}
+
+// The pattern's match at code point i (regex semantics: the first alternative that matches, greedy quantifiers that
+// give back characters); returns its end.  Every code point starts a match, so pieces tile the text.
+size_t match_piece(const std::vector<uint32_t> &cp, const std::vector<uint8_t> &f, size_t i) {
+    const size_t n = f.size(), none = SIZE_MAX;
+    // U* Lw+ from j: the star gives back characters (U and Lw overlap on Lm, Lo, M) until the plus can match
+    auto upper_lower = [&](size_t j) -> size_t {
+        const size_t kmax = run_end(f, j, fU);
+        for (size_t k = kmax + 1; k-- > j;)
+            if (k < n && (f[k] & fLw)) return run_end(f, k, fLw);
+        return none;
+    };
+    // U+ Lw*
+    auto upper_then = [&](size_t j) -> size_t {
+        const size_t kmax = run_end(f, j, fU);
+        return kmax > j ? run_end(f, kmax, fLw) : none;
+    };
+    const bool lead = is_lead(f[i]);   // the optional leading character: tried with it first, then without
+    size_t e;
+    if (lead && (e = upper_lower(i + 1)) != none) return e;                  // 1
+    if ((e = upper_lower(i)) != none) return e;
+    if (lead && (e = upper_then(i + 1)) != none) return e;                   // 2
+    if ((e = upper_then(i)) != none) return e;
+    if (f[i] & fN) return i + 1;                                              // 3
+    const size_t p0 = (cp[i] == ' ' && i + 1 < n && is_punct(f[i + 1])) ? i + 1 : i;   // 4
+    if (is_punct(f[p0])) {
+        size_t k = p0;
+        while (k < n && is_punct(f[k])) ++k;
+        return run_end(f, k, fTail);
+    }
+    const size_t w = run_end(f, i, fWS);
+    for (size_t k = w; k-- > i;)                                              // 5: \s* gives back to [\r\n]+
+        if (f[k] & fCRLF) return run_end(f, k, fCRLF);
+    if (w > i && w == n) return w;                                            // 6: \s+(?!\S)
+    if (w > i + 1) return w - 1;                                              //    the last space goes to the next word
+    if (w > i) return w;                                                      // 7
+    return i + 1;   // unreachable: a code point is a letter, a number, White_Space or [^\s\p{L}\p{N}]
+}
+
 }  // namespace
+
+bool Tokenizer::starts_with_white_space(const char *text, size_t len) {
+    if (len == 0) return false;
+    const size_t first = (uint8_t)text[0] < 0x80 ? 1 : (uint8_t)text[0] < 0xE0 ? 2 : (uint8_t)text[0] < 0xF0 ? 3 : 4;
+    std::vector<uint32_t> cps;
+    std::vector<size_t> offs;
+    utf8_decode((const uint8_t *)text, std::min(first, len), cps, offs);
+    return (char_flags(cps[0]) & fWS) != 0;
+}
+
+void Tokenizer::build_ranks() const {
+    if (pattern_ != kTekkenPattern) {
+        ranks_err_ = VOX_EFORMAT;
+        ranks_msg_ = "encode: the tokenizer's pattern is not Tekken's; only decoding is available";
+        return;
+    }
+    // text ranks below default_vocab_size - 1000, as mistral_common cuts them; the lowest position of a byte string wins
+    const size_t cut = std::min(vocab_bytes_.size(), vocab_size_ > kTextTokenOffset ? vocab_size_ - kTextTokenOffset : 0);
+    ranks_.reserve(cut);
+    for (size_t p = 0; p < cut; ++p)
+        if (has_bytes_[p] && !vocab_bytes_[p].empty()) ranks_.emplace(std::string_view(vocab_bytes_[p]), (uint32_t)p);
+    for (int b = 0; b < 256; ++b) {
+        const char c = (char)b;
+        if (!ranks_.count(std::string_view(&c, 1))) {
+            ranks_err_ = VOX_EFORMAT;
+            ranks_msg_ = fmt("encode: the vocabulary (cut at %zu text ranks) has no token for byte 0x%02X", cut, b);
+            ranks_.clear();
+            return;
+        }
+    }
+}
+
+std::vector<int32_t> Tokenizer::encode(const char *text, size_t len) const {
+    std::call_once(ranks_once_, [this] { build_ranks(); });
+    if (ranks_err_) fail(ranks_err_, ranks_msg_);
+    std::vector<uint32_t> cps;
+    std::vector<size_t> offs;
+    utf8_decode((const uint8_t *)text, len, cps, offs);
+    std::vector<uint8_t> f(cps.size());
+    for (size_t k = 0; k < cps.size(); ++k) f[k] = char_flags(cps[k]);
+    std::vector<int32_t> out;
+    std::vector<std::pair<size_t, uint32_t>> parts;   // (byte start, rank of the pair starting here)
+    auto rank_of = [&](std::string_view v) -> uint32_t {
+        auto it = ranks_.find(v);
+        return it == ranks_.end() ? UINT32_MAX : it->second;
+    };
+    for (size_t i = 0; i < cps.size();) {
+        const size_t e = match_piece(cps, f, i);
+        const std::string_view piece(text + offs[i], offs[e] - offs[i]);
+        i = e;
+        const uint32_t whole = rank_of(piece);
+        if (whole != UINT32_MAX) { out.push_back((int32_t)(whole + kTextTokenOffset)); continue; }
+        // tiktoken's byte_pair_merge: merge the adjacent pair of lowest rank (the leftmost on a tie) until none is a token
+        const size_t m = piece.size();
+        parts.clear();
+        for (size_t k = 0; k + 1 < m; ++k) parts.emplace_back(k, rank_of(piece.substr(k, 2)));
+        parts.emplace_back(m - 1, UINT32_MAX);
+        parts.emplace_back(m, UINT32_MAX);
+        auto pair_rank = [&](size_t k) {
+            return k + 3 < parts.size() ? rank_of(piece.substr(parts[k].first, parts[k + 3].first - parts[k].first)) : UINT32_MAX;
+        };
+        for (;;) {
+            size_t best = SIZE_MAX;
+            uint32_t r = UINT32_MAX;
+            for (size_t k = 0; k + 1 < parts.size(); ++k)
+                if (parts[k].second < r) { r = parts[k].second; best = k; }
+            if (best == SIZE_MAX) break;
+            if (best > 0) parts[best - 1].second = pair_rank(best - 1);
+            parts[best].second = pair_rank(best);
+            parts.erase(parts.begin() + best + 1);
+        }
+        for (size_t k = 0; k + 1 < parts.size(); ++k) {
+            const uint32_t t = rank_of(piece.substr(parts[k].first, parts[k + 1].first - parts[k].first));
+            out.push_back((int32_t)(t + kTextTokenOffset));   // every part is a token: the 256 bytes are
+        }
+    }
+    return out;
+}
 
 Tokenizer *Tokenizer::from_json(const char *json, size_t len) {
     JParser jp{json, json + len};
@@ -239,6 +437,8 @@ Tokenizer *Tokenizer::from_json(const char *json, size_t len) {
     VOX_CHECK(dvs && dvs->t == JVal::Num, VOX_EIO, "Failed to parse tekken JSON: missing field `default_vocab_size`");
     Tokenizer *t = new Tokenizer();
     t->vocab_size_ = (size_t)dvs->num;
+    const JVal *pat = cfg->get("pattern");
+    if (pat && pat->t == JVal::Str) t->pattern_ = pat->s;
     t->vocab_bytes_.resize(vocab->arr.size());
     t->has_bytes_.assign(vocab->arr.size(), 0);
     for (size_t idx = 0; idx < vocab->arr.size(); ++idx) {
