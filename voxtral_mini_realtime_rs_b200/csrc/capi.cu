@@ -983,31 +983,17 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
         // layer l's cached K or V of rows [0, cur_B) at positions [0, cache length), f32 [row][pos][kv_head][hd]
         const int l = atoi(w.c_str() + 4);
         VOX_CHECK(l >= 0 && l < c.dec_layers && std::to_string(l) == w.substr(4), VOX_EINVAL, "no decoder layer in '%s'", what);
-        VOX_CHECK(!s->kv_ring, VOX_EINVAL, "'%s': not on ring-indexed sessions", what);
-        const int B = s->cur_B, Hkv = c.dec_kv_heads, hd = c.dec_head_dim;
+        const int B = s->cur_B;
         std::vector<int> pos(B);
         CUDA_OK(cudaStreamSynchronize(s->st));
         if (B) CUDA_OK(cudaMemcpy(pos.data(), s->d_pos, sizeof(int) * B, cudaMemcpyDeviceToHost));
-        const int L = B ? std::min(pos[0], s->kv_max_pages * KV_PAGE) : 0;
+        const int L = B ? std::min(pos[0], s->kv.capacity()) : 0;
         for (int b = 0; b < B; ++b) VOX_CHECK(pos[b] == pos[0], VOX_EINVAL, "'%s': rows at different positions", what);
-        const size_t cnt = (size_t)B * L * Hkv * hd;
+        const size_t cnt = (size_t)B * L * c.dec_kv_heads * c.dec_head_dim;
         if (n_floats) *n_floats = cnt;
         if (out && cnt) {
             VOX_CHECK(cap >= cnt, VOX_ECAPACITY, "debug_read capacity %zu < %zu", cap, cnt);
-            std::vector<int> pt((size_t)B * s->kv_max_pages);
-            CUDA_OK(cudaMemcpy(pt.data(), s->d_page_table, sizeof(int) * pt.size(), cudaMemcpyDeviceToHost));
-            const size_t eb = kv_elem_bytes(s->kv_type), stride = s->kv_layer_stride();
-            std::vector<unsigned char> layer(stride * eb);
-            CUDA_OK(cudaMemcpy(layer.data(), s->kv_layer(w[3] == 'k' ? s->kc : s->vc, l), layer.size(), cudaMemcpyDeviceToHost));
-            size_t o = 0;
-            for (int b = 0; b < B; ++b)
-                for (int j = 0; j < L; ++j)
-                    for (int h = 0; h < Hkv; ++h) {
-                        const size_t at = (((size_t)pt[(size_t)b * s->kv_max_pages + j / KV_PAGE] * Hkv + h) * KV_PAGE + j % KV_PAGE) * hd;
-                        for (int d = 0; d < hd; ++d, ++o)
-                            out[o] = s->kv_type == KvType::F16 ? __half2float(reinterpret_cast<const __half *>(layer.data())[at + d])
-                                                                : reinterpret_cast<const float *>(layer.data())[at + d];
-                    }
+            s->kv.read(l, w[3] == 'v', B, L, out);
         }
         return VOX_OK;
     } else if (w == "mega_trace") {

@@ -1523,12 +1523,13 @@ void DecodeMega::create(Session &s) {
     p.H = c.dec_heads;
     p.Hkv = c.dec_kv_heads;
     p.hd = c.dec_head_dim;
-    p.max_seq = s.out_ld;
-    p.page_table = s.d_page_table;
-    p.max_pages = s.kv_max_pages;
+    const KvView kv = s.kv.view(0, s.d_pos);   // the table, allocated once: launches capture its address
+    p.max_seq = kv.max_seq();
+    p.page_table = kv.page_table;
+    p.max_pages = kv.max_pages;
     p.window = c.dec_window;
     p.scale = powf((float)c.dec_head_dim, -0.5f);
-    p.ring = s.kv_ring ? 1 : 0;
+    p.ring = kv.ring ? 1 : 0;
     p.attn_out = s.attn_dec;
     p.emb_qs = m.tok_emb.qs;
     p.emb_d = m.tok_emb.d;
@@ -1563,7 +1564,7 @@ unsigned DecodeMega::prepare(const Session &s, int R) {
     for (int j = 0; j < c.dec_layers; ++j)
         if (!m.dec[j].wqkv.qs_tc || !m.dec[j].wo.qs_tc || !m.dec[j].w13.qs_tc || !m.dec[j].w2.qs_tc) return 0;
     const int max_pairs = std::max(std::max(mg_pairs(D), mg_pairs(H * hd)), mg_pairs(c.dec_ffn));
-    g.plan = decode_mega_plan(B, max_pairs, H, Hkv, hd, (int)kv_elem_bytes(s.kv_type));
+    g.plan = decode_mega_plan(B, max_pairs, H, Hkv, hd, (int)kv_elem_bytes(s.kv.type()));
     const int parts = (D + 15) / 16;
     std::vector<MegaOp> ops;
     bool ok = true;
@@ -1616,12 +1617,13 @@ unsigned DecodeMega::prepare(const Session &s, int R) {
         const DecLayerW &l = m.dec[j];
         // wqkv: its epilogue applies RoPE to q and k and appends k, v to layer j's cache
         matvec(l.wqkv, g.xf, s.qkv_dec, g.p.ld_qkv, nullptr, EPI_NONE, l.attn_norm, false, false, 1, none, nullptr);
-        ops.back().kc = kv_pool(s.kv_layer(s.kc, j), s.kv_type);
-        ops.back().vc = kv_pool(s.kv_layer(s.vc, j), s.kv_type);
+        const KvView kv = s.kv.view(j, s.d_pos);
+        ops.back().kc = kv.k;
+        ops.back().vc = kv.v;
         MegaOp a;
         a.kind = MG_ATTN;
-        a.kc = kv_pool(s.kv_layer(s.kc, j), s.kv_type);
-        a.vc = kv_pool(s.kv_layer(s.vc, j), s.kv_type);
+        a.kc = kv.k;
+        a.vc = kv.v;
         a.layer = j;
         ops.push_back(a);
         // wo: h += attn . Wo^T; leaves fragments of h x (ffn_norm x ADA) for w13

@@ -440,20 +440,9 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ri
         s->adapter_h = s->arena.alloc_n<float>(rows4 * c.dec_dim);
         s->audio = s->arena.alloc_n<float>(rows4 * c.dec_dim);
         // decoder
-        const int kv_cap = std::max(s->S4_max, s->M_max) + s->M_max;  // room for the incremental API
-        s->kv_max_pages = kv_ring ? (c.dec_window + s->M_max) / KV_PAGE + 1 : (kv_cap + KV_PAGE - 1) / KV_PAGE;
-        s->kv_n_pages = max_batch * s->kv_max_pages;
-        s->out_ld = s->kv_max_pages * KV_PAGE;
-        s->kv_ring = kv_ring;
+        s->kv.create(s->arena, c, max_batch, s->S4_max, s->M_max, kv_ring, kv_type);
+        s->out_ld = s->kv.capacity();
         s->dec_rope = m->dec_rope();
-        const size_t kv_elems = (size_t)c.dec_layers * s->kv_n_pages * c.dec_kv_heads * KV_PAGE * c.dec_head_dim;
-        s->kv_type = kv_type;
-        s->kc = s->arena.alloc(kv_elems * kv_elem_bytes(kv_type));
-        s->vc = s->arena.alloc(kv_elems * kv_elem_bytes(kv_type));
-        s->page_table_host.resize((size_t)max_batch * s->kv_max_pages);
-        for (int b = 0; b < max_batch; ++b)
-            for (int pg = 0; pg < s->kv_max_pages; ++pg) s->page_table_host[(size_t)b * s->kv_max_pages + pg] = b * s->kv_max_pages + pg;
-        s->d_page_table = s->arena.upload(s->page_table_host.data(), s->page_table_host.size());
         const size_t drows = B * s->M_max;
         const int qkvd = (c.dec_heads + 2 * c.dec_kv_heads) * c.dec_head_dim;
         s->x_dec = s->arena.alloc_n<float>(drows * c.dec_dim);
@@ -706,18 +695,6 @@ TcWork Session::tc_work(bool norm_in, bool ssq_out_) const {
     return w;
 }
 
-KvView Session::kv_view(int layer) const {
-    KvView v;
-    v.k = kv_pool(kv_layer(kc, layer), kv_type);
-    v.v = kv_pool(kv_layer(vc, layer), kv_type);
-    v.type = kv_type;
-    v.page_table = d_page_table;
-    v.max_pages = kv_max_pages;
-    v.ring = kv_ring;
-    v.pos = d_pos;
-    return v;
-}
-
 bool Session::decoder_forward(int B, int M) {
     const vox_model_info &c = m->info;
     const int D = c.dec_dim, H = c.dec_heads, Hkv = c.dec_kv_heads, hd = c.dec_head_dim;
@@ -731,7 +708,7 @@ bool Session::decoder_forward(int B, int M) {
     const bool fattn = fused && M == 1 && dec_attn_fused_supported(H, Hkv, hd);
     for (int j = 0; j < c.dec_layers; ++j) {
         const DecLayerW &l = m->dec[j];
-        const KvView kvl = kv_view(j);
+        const KvView kvl = kv.view(j, d_pos);
         linear(l.wqkv, x_dec, rows, qkv_dec, qkvd, nullptr, nullptr, EPI_NONE, l.attn_norm, h_dec, tc_norm);
         if (fattn) {
             launch_dec_attn_fused(qkv_dec, B, qkvd, H, Hkv, hd, kvl, c.dec_window, scale, dec_rope, attn_dec, st);
@@ -916,15 +893,12 @@ void Session::beam_start(int b) {
     CUDA_OK(cudaMemcpyAsync(beam.rank_row, rank_row.data(), sizeof(int) * rank_row.size(), cudaMemcpyHostToDevice, st));
     CUDA_OK(cudaMemsetAsync(beam.cum, 0, sizeof(double) * b * W, st));
     CUDA_OK(cudaStreamSynchronize(st));   // rank_row dies with this frame
-    page_table_forked = true;
     beam_step(b, 1);
 }
 
 void Session::beam_step(int b, int n_live) {
-    const vox_model_info &c = m->info;
     launch_beam_select(d_top_ids, d_top_lp, d_outpos, out_ld, b, beam_w, n_live, beam, d_tok, st);
-    launch_beam_fork(kc, vc, kv_type, kv_layer_stride(), c.dec_layers, d_page_table, kv_max_pages, d_pos, beam.src, b * beam_w,
-                     c.dec_kv_heads, c.dec_head_dim, st);
+    kv.fork(d_pos, beam.src, b * beam_w, st);
 }
 
 // Prefill of M positions for B streams (model.rs:894-923 with M = 38; also the incremental vox_prefill).
@@ -962,11 +936,7 @@ void Session::reset() {
     CUDA_OK(cudaMemsetAsync(d_outpos, 0, sizeof(int) * max_batch, st));
     std::fill(out_rows.begin(), out_rows.end(), 0);
     cache_len = 0;
-    if (page_table_forked) {
-        CUDA_OK(cudaMemcpyAsync(d_page_table, page_table_host.data(), sizeof(int) * page_table_host.size(),
-                                cudaMemcpyHostToDevice, st));
-        page_table_forked = false;
-    }
+    kv.restore_identity(st);
     clear_bias_history(-1);
     rebase_epoch();
 }
@@ -1213,7 +1183,6 @@ void Session::transcribe_ragged(const float *samples, const size_t *lens, int b,
             CUDA_OK(cudaMemcpyAsync(beam.rank_row, rank_row.data(), sizeof(int) * R0, cudaMemcpyHostToDevice, st));
             CUDA_OK(cudaMemsetAsync(beam.cum, 0, sizeof(double) * R0, st));
             CUDA_OK(cudaStreamSynchronize(st));   // rank_row dies with this frame
-            page_table_forked = true;
             beam_step(live, 1);
         }
         CUDA_OK(cudaEventRecord(ev[4], st));

@@ -14,6 +14,7 @@
 #include "gguf.h"
 #include "decode_mega.h"
 #include "kernels.h"
+#include "kv_cache.h"
 
 namespace vox {
 
@@ -150,18 +151,7 @@ struct Session {
     int *d_seg = nullptr;       // [max_batch + 1] encoder row of each stream's first frame (ragged encode)
     std::vector<int> seg_host;
     // decoder
-    // decoder KV cache: page pools [L][n_pages][Hkv][KV_PAGE][hd] + per-row page tables (kernels.h KvView).  Whole-
-    // utterance batches use the identity mapping (row b owns pages b*max_pages..); streaming sessions allocate pages
-    // of kv_type elements (vox_session_create_ex kv_dtype; fixed for the session's lifetime)
-    void *kc = nullptr, *vc = nullptr;
-    KvType kv_type = KvType::F32;
-    int kv_max_pages = 0, kv_n_pages = 0;
-    int *d_page_table = nullptr;          // [max_batch][kv_max_pages]
-    std::vector<int> page_table_host;
-    size_t kv_layer_stride() const { return (size_t)kv_n_pages * m->info.dec_kv_heads * KV_PAGE * m->info.dec_head_dim; }  // elements
-    void *kv_layer(void *pool, int layer) const { return (char *)pool + (size_t)layer * kv_layer_stride() * kv_elem_bytes(kv_type); }
-    bool kv_ring = false;                 // KvView::ring (Session::create)
-    KvView kv_view(int layer) const;
+    DecoderKv kv;                         // of max_batch rows (vox_session_create_ex kv_dtype)
     RopeView dec_rope;                    // the model's tables, or an unbounded stream pool's ring
     float *x_dec = nullptr, *h_dec = nullptr, *qkv_dec = nullptr, *attn_dec = nullptr, *act_dec = nullptr;
     float *last_h = nullptr, *logits = nullptr;
@@ -179,7 +169,7 @@ struct Session {
     std::vector<int> bound_streams;     // what the tables hold, per row
     std::vector<int64_t> bound_offs;
     int *d_pos = nullptr, *d_outpos = nullptr, *d_tok = nullptr, *d_ids = nullptr, *d_out = nullptr;
-    int out_ld = 0;
+    int out_ld = 0;     // row pitch of d_out and of the per-output buffers: kv.capacity()
     int cache_len = 0;  // host mirror of d_pos[] (all rows equal) for the incremental API
     // token confidences (vox_session_set_top_k): 0 = off (no launch, no memory).  k > 0: every prefill and decode step
     // ends with launch_token_scores over its rows into [max_batch][out_ld][TOPK_MAX] ids / log-probabilities, allocated
@@ -202,7 +192,6 @@ struct Session {
     BeamWork beam;
     int *d_nbest_ids = nullptr;     // every stream's [W][n] ids of the last transcribe, at NbestSpan::ids
     double *d_nbest_scores = nullptr;
-    bool page_table_forked = false; // a beam call has rewritten page-table rows: reset() re-uploads the identity table
     void set_beam(int w);
     void beam_start(int b);         // after the prefill of rows [0, b): start every beam row there, select position 0
     void beam_step(int b, int n_live);   // selection + KV fork after a step over the b * beam_w rows
@@ -258,9 +247,8 @@ struct Session {
     float *dbg_layers = nullptr;   // [enc_layers][B*S][enc_dim]
     float *dbg_conv = nullptr;
 
-    // kv_ring: each row's decoder KV is a ring of pages just long enough for the decoder window plus the rows one launch
-    // appends before reading (16 L > dec_window + M_max), and positions are unbounded (stream pools with no length
-    // limit; the pool owner points dec_rope at its RoPE ring)
+    // kv_ring: each row's decoder KV is a ring of pages (DecoderKv::create), and positions are unbounded (stream pools
+    // with no length limit; the pool owner points dec_rope at its RoPE ring)
     // kv_type: element type of the decoder KV cache
     static Session *create(Model *m, int max_batch, int max_mel_frames, bool kv_ring = false, KvType kv_type = KvType::F32);
     ~Session();

@@ -217,8 +217,6 @@ StreamPool *StreamPool::create(Model *m, int max_sessions, float max_seconds, Kv
             p->slide_tmp = s->arena.alloc_n<float>(most);
         }
         p->slots.resize(max_sessions);
-        // decoder KV pages: the session's identity tables are replaced by a free list
-        for (int i = s->kv_n_pages - 1; i >= 0; --i) p->free_pages.push_back(i);
     } catch (...) {
         delete p;
         throw;
@@ -291,7 +289,7 @@ void StreamPool::finish(int id) {
 
 void StreamPool::close(int id) {
     Slot &sl = slot(id);
-    for (int pg : sl.pages) free_pages.push_back(pg);
+    s->kv.release(id);
     sl = Slot();
 }
 
@@ -331,33 +329,21 @@ void StreamPool::encoder_rows(int R) {
     });
 }
 
-void StreamPool::ensure_pages(Slot &sl, int positions) {
-    int need = (positions + KV_PAGE - 1) / KV_PAGE;
-    if (unbounded) need = std::min(need, s->kv_max_pages);  // a full ring: logical page lp reuses slot lp % kv_max_pages
-    VOX_CHECK(need <= s->kv_max_pages, VOX_ECAPACITY, "stream session needs %d decoder positions > capacity %d", positions, s->out_ld);
-    while ((int)sl.pages.size() < need) {
-        VOX_CHECK(!free_pages.empty(), VOX_ECAPACITY, "decoder KV page pool exhausted (%d pages)", s->kv_n_pages);
-        sl.pages.push_back(free_pages.back());
-        free_pages.pop_back();
-    }
-}
-
 // rows[i] = slot id of batch row i: page tables, positions and fed-back tokens of this launch; the rows' slots and
 // their audio offsets for the session to bind (Session::bind_rows: ADA sets and audio embeddings)
 void StreamPool::upload_rows(const std::vector<int> &rows, bool with_tokens) {
     const vox_model_info &c = m->info;
-    const int nb = (int)rows.size(), mp = s->kv_max_pages;
-    std::vector<int> pt((size_t)nb * mp, 0), pos(nb), tok(nb), zero(nb, 0);
+    const int nb = (int)rows.size();
+    std::vector<int> pos(nb), tok(nb), zero(nb, 0);
     for (int i = 0; i < nb; ++i) {
         const Slot &sl = slots[rows[i]];
-        for (size_t k = 0; k < sl.pages.size(); ++k) pt[(size_t)i * mp + k] = sl.pages[k];
         pos[i] = sl.pos;
         tok[i] = sl.last_tok;
         // negative once the buffer has slid: position p's embedding sits at buffer row p - emb0
         s->audio_offs[rows[i]] = ((int64_t)rows[i] * s->S4_max - sl.emb0) * c.dec_dim;
     }
     s->row_streams = rows;
-    CUDA_OK(cudaMemcpyAsync(s->d_page_table, pt.data(), sizeof(int) * pt.size(), cudaMemcpyHostToDevice, s->st));
+    s->kv.bind(rows, s->st);
     CUDA_OK(cudaMemcpyAsync(s->d_pos, pos.data(), sizeof(int) * nb, cudaMemcpyHostToDevice, s->st));
     CUDA_OK(cudaMemcpyAsync(s->d_outpos, zero.data(), sizeof(int) * nb, cudaMemcpyHostToDevice, s->st));
     if (with_tokens) CUDA_OK(cudaMemcpyAsync(s->d_tok, tok.data(), sizeof(int) * nb, cudaMemcpyHostToDevice, s->st));
@@ -459,7 +445,7 @@ void StreamPool::tick(vox_stream_stats *st_out) {
             Slot &sl = slots[id];
             if (!sl.open || sl.drained || sl.pos != 0 || sl.n_emb < P) continue;
             VOX_CHECK(sl.emb0 == 0, VOX_ECAPACITY, "stream session %d: prefill embeddings were evicted", id);
-            ensure_pages(sl, P + 1);
+            s->kv.reserve(id, P + 1);
             if (unbounded) fill_rope(dec_rope_cos, dec_rope_sin, c.dec_head_dim, kDecRopeRing, 0, 0, P);
             upload_rows({id}, false);
             s->clear_bias_history(id);   // the slot's decoder cache starts empty
@@ -497,7 +483,7 @@ void StreamPool::tick(vox_stream_stats *st_out) {
             }
             if (rows.empty()) break;
             for (int id : rows) {
-                ensure_pages(slots[id], slots[id].pos + 1);
+                s->kv.reserve(id, slots[id].pos + 1);
                 if (unbounded) fill_rope(dec_rope_cos, dec_rope_sin, c.dec_head_dim, kDecRopeRing, 0, slots[id].pos, 1);
             }
             upload_rows(rows, true);
@@ -611,7 +597,7 @@ void StreamPool::session_info(int id, struct vox_stream_session_info *out) {
     out->first_audio_embed = sl.emb0;
     out->decoder_positions = sl.pos;
     out->ids_emitted = sl.n_ids;
-    out->kv_pages = (int32_t)sl.pages.size();
+    out->kv_pages = s->kv.pages(id);
 }
 
 // upload_rows resets every row's output position before a step, so its token and scores sit at position 0 of the row

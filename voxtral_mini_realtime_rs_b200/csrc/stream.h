@@ -24,7 +24,6 @@ struct StreamPool {
         std::vector<int32_t> top_ids;             // their scores, [ids.size()][s->top_k] (pool top_k > 0)
         std::vector<float> top_lp;
         int64_t n_ids = 0;                        // ids emitted (positions >= 38)
-        std::vector<int> pages;                   // decoder KV pages owned (page-table slot order)
         size_t pcm0 = 0;                          // absolute sample / frame / row of each buffer's row 0
         int mel0 = 0, c10 = 0, enc0 = 0, emb0 = 0;
     };
@@ -44,7 +43,6 @@ struct StreamPool {
     float *slide_tmp = nullptr;  // unbounded pools: bounce buffer of slide() (stream.cu), the size of the largest session buffer
     int *d_row_slot = nullptr, *d_row_pos = nullptr;
     std::vector<Slot> slots;
-    std::vector<int> free_pages;
 
     // max_seconds in [1, 60]: sessions up to that long, all their state resident.  0: sessions of any length.
     // kv_type: element type of the decoder KV pages every session of the pool shares (Session::create)
@@ -75,7 +73,6 @@ struct StreamPool {
   private:
     Slot &slot(int id);
     void encoder_rows(int R);
-    void ensure_pages(Slot &sl, int positions);
     void upload_rows(const std::vector<int> &rows, bool with_tokens);
     // enqueues the copy of the last step's scores of rows [0, n) (position 0 of each) into [n][top_k] host arrays
     void fetch_scores(int n, int32_t *top_ids, float *top_lp);
