@@ -343,7 +343,12 @@ int32_t vox_session_reset(vox_session *s);                                      
  * tiling of each persistent launch of the last decode step, 4 floats per launch {rows, token capacity,
  * keys per K/V tile, key chunks per (stream, kv head)} (none after a per-op step); "kv_k<l>" / "kv_v<l>" = decoder layer l's
  * cached K (after RoPE) or V for the rows of the last call, positions [0, cache length), as f32 [row][pos][kv_head][hd]
- * (an f16 cache widened exactly; not on the ring-indexed sessions of an unbounded stream pool); names of the form "<switch>_on|_off|_auto" (graph, tc, gemm_tc |
+ * (an f16 cache widened exactly; not on the ring-indexed sessions of an unbounded stream pool); "mel" = the log-mel of
+ * the last call that started from PCM (vox_transcribe_pcm, _dev, _ragged): time-major [sum of the streams' frames][128],
+ * stream after stream (each stream's frames = vox_mel_num_frames(its padded length)); after a call that took its mel
+ * from the caller (vox_encode_audio, vox_transcribe_streaming), that mel as [B][128][T]; VOX_ENOTFOUND before either;
+ * "pcm_pad" = the normalised, padded signal of each stream of the last PCM call (vox_pad_audio_len samples per stream),
+ * stream after stream; VOX_ENOTFOUND unless the last such call started from PCM; names of the form "<switch>_on|_off|_auto" (graph, tc, gemm_tc |
  * gemm_simt, enc_attn_tc | enc_attn_simt, mega, capture) flip a kernel-selection switch and return no
  * data (INTEGRATION.md section 5) */
 int32_t vox_session_debug_read(vox_session *s, const char *what, float *out, size_t cap_floats,
@@ -412,6 +417,11 @@ int32_t vox_stream_audio_embeds(vox_stream_pool *p, int32_t session, float *out,
  * resident (see vox_stream_session_info.first_audio_embed), VOX_EINVAL past the embeddings produced so far. */
 int32_t vox_stream_audio_embeds_range(vox_stream_pool *p, int32_t session, int64_t first, int64_t n, float *out,
                                       size_t cap_floats);
+/* log-mel frames [first, first + n) (absolute frame indices of the padded stream), [n][128] host: the frames the
+ * encoder's conv stem read.  VOX_ECAPACITY when `first` is no longer resident (an unbounded session keeps the frames
+ * its conv stem still reads, and slides them out when its buffer is full), VOX_EINVAL past
+ * vox_stream_session_info.mel_frames. */
+int32_t vox_stream_mel_range(vox_stream_pool *p, int32_t session, int64_t first, int64_t n, float *out, size_t cap_floats);
 /* a struct tag (not a typedef): the function below has the same name */
 struct vox_stream_session_info {
     int64_t samples;            /* padded signal samples known (left padding included; vox_stream_progress) */

@@ -130,6 +130,7 @@ extern "C" {
     // max_seconds = 0: sessions of any length (include/voxtral.h)
     pub fn vox_stream_audio_embeds_range(p: *mut vox_stream_pool, session: i32, first: i64, n: i64, out: *mut f32,
                                          cap: usize) -> i32;
+    pub fn vox_stream_mel_range(p: *mut vox_stream_pool, session: i32, first: i64, n: i64, out: *mut f32, cap: usize) -> i32;
     pub fn vox_stream_session_info(p: *mut vox_stream_pool, session: i32, out: *mut vox_stream_session_info) -> i32;
     pub fn vox_stream_encode_chunk(p: *mut vox_stream_pool, session: i32, mel: *const f32, t_frames: i32, audio_embeds: *mut f32,
                                    cap: usize, n: *mut i32) -> i32;

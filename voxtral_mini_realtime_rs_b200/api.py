@@ -164,6 +164,7 @@ _SIGS = {
                                            C.POINTER(C.c_int32)]),
     "vox_stream_audio_embeds": (C.c_int32, [_P, C.c_int32, _P, C.c_size_t, C.POINTER(C.c_int32)]),
     "vox_stream_audio_embeds_range": (C.c_int32, [_P, C.c_int32, C.c_int64, C.c_int64, _P, C.c_size_t]),
+    "vox_stream_mel_range": (C.c_int32, [_P, C.c_int32, C.c_int64, C.c_int64, _P, C.c_size_t]),
     "vox_stream_session_info": (C.c_int32, [_P, C.c_int32, _P]),
     "vox_stream_encode_chunk": (C.c_int32, [_P, C.c_int32, _P, C.c_int32, _P, C.c_size_t, C.POINTER(C.c_int32)]),
     "vox_stream_close": (C.c_int32, [_P, C.c_int32]),
@@ -993,6 +994,13 @@ class StreamingPool:
         _check(lib().vox_stream_audio_embeds(self._p, session, None, 0, C.byref(n)))
         out = np.empty((n.value, self.dec_dim), np.float32)
         _check(lib().vox_stream_audio_embeds(self._p, session, _ptr(out), out.size, C.byref(n)))
+        return out
+
+    def mel_range(self, session: int, first: int, n: int) -> np.ndarray:
+        """Resident log-mel frames [first, first + n) of the session's padded stream (absolute indices) -> float32
+        [n, 128] (vox_stream_mel_range)."""
+        out = np.empty((n, 128), np.float32)
+        _check(lib().vox_stream_mel_range(self._p, session, first, n, _ptr(out), out.size))
         return out
 
     def encode_audio_with_cache(self, session: int, mel) -> np.ndarray:

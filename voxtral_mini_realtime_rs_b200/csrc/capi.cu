@@ -542,6 +542,9 @@ static void upload_mel(Session *s, const float *mel, int b, int t) {
     VOX_CHECK(t >= 1 && t <= s->max_mel_frames, VOX_EINVAL, "mel frames %d exceed session max_mel_frames %d", t,
               s->max_mel_frames);
     CUDA_OK(cudaSetDevice(s->m->device));
+    s->front.frames.assign(b, t);
+    s->front.padded.clear();
+    s->front.pad_off.clear();
     CUDA_OK(cudaMemcpyAsync(s->mel, mel, sizeof(float) * (size_t)b * c.n_mels * t, cudaMemcpyHostToDevice, s->st));
     launch_transpose_mel(s->mel, s->mel_tm, b, c.n_mels, t, s->st);
 }
@@ -606,6 +609,10 @@ static int32_t transcribe_pcm_impl(Session *s, const float *host, const float *d
     VOX_CHECK(frames <= (size_t)s->max_mel_frames, VOX_EINVAL,
               "audio needs %zu mel frames > session max_mel_frames %d (chunk it: vox_chunk_plan)", frames, s->max_mel_frames);
     s->reserve_pcm(host ? (size_t)b * n : 0, (size_t)b * padded);
+    s->front.frames.assign(b, (int)frames);
+    s->front.padded.assign(b, padded);
+    s->front.pad_off.resize(b);
+    for (int i = 0; i < b; ++i) s->front.pad_off[i] = (size_t)i * padded;
     CUDA_OK(cudaEventRecord(s->ev[0], s->st));
     const float *src = dev;
     if (host) {
@@ -1030,9 +1037,29 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
             }
         }
         return VOX_OK;
-    } else if (w == "enc_out") { src = s->h_enc; n = rows * c.enc_dim; }
+    } else if (w == "pcm_pad") {
+        // each stream's normalised, padded signal of the last PCM call, stream after stream
+        const Session::FrontEnd &f = s->front;
+        VOX_CHECK(!f.padded.empty(), VOX_ENOTFOUND, "'pcm_pad': the last call did not start from PCM");
+        size_t cnt = 0;
+        for (size_t p : f.padded) cnt += p;
+        if (n_floats) *n_floats = cnt;
+        if (out) {
+            VOX_CHECK(cap >= cnt, VOX_ECAPACITY, "debug_read capacity %zu < %zu", cap, cnt);
+            CUDA_OK(cudaStreamSynchronize(s->st));
+            for (size_t i = 0, o = 0; i < f.padded.size(); o += f.padded[i], ++i)
+                CUDA_OK(cudaMemcpy(out + o, s->pcm_pad + f.pad_off[i], sizeof(float) * f.padded[i], cudaMemcpyDeviceToHost));
+        }
+        return VOX_OK;
+    } else if (w == "mel") {
+        // PCM call: the time-major mel every stream's frames were packed into; mel call: the caller's [B][128][T]
+        const Session::FrontEnd &f = s->front;
+        VOX_CHECK(!f.frames.empty(), VOX_ENOTFOUND, "'mel': no call has computed or uploaded a mel yet");
+        for (int t : f.frames) n += (size_t)t * c.n_mels;
+        src = f.padded.empty() ? s->mel : s->mel_tm;
+    }
+    else if (w == "enc_out") { src = s->h_enc; n = rows * c.enc_dim; }
     else if (w == "audio_embeds") { src = s->audio; n = (size_t)s->audio_n * c.dec_dim; }   // stream after stream
-    else if (w == "mel") { src = s->mel; n = 0; /* size unknown here */ }
     else if (w == "conv") { src = s->dbg_conv; n = rows * c.enc_dim; }
     else if (w == "logits") { src = s->logits; n = (size_t)s->cur_B * c.vocab; }
     else if (w == "ada") { src = s->ada_sets; n = (size_t)c.dec_layers * c.dec_dim; }   // stream 0's ADA scale
@@ -1165,6 +1192,19 @@ int32_t vox_stream_audio_embeds_range(vox_stream_pool *p, int32_t session, int64
     const size_t need = (size_t)n * p->p->m->info.dec_dim;
     if (need) REQUIRE(out);
     VOX_CHECK(cap >= need, VOX_ECAPACITY, "audio_embeds capacity %zu < %zu", cap, need);
+    CUDA_OK(cudaSetDevice(p->p->m->device));
+    CUDA_OK(cudaStreamSynchronize(p->p->s->st));
+    if (need) CUDA_OK(cudaMemcpy(out, src, sizeof(float) * need, cudaMemcpyDeviceToHost));
+    VOX_API_END
+}
+int32_t vox_stream_mel_range(vox_stream_pool *p, int32_t session, int64_t first, int64_t n, float *out, size_t cap) {
+    VOX_API_BEGIN
+    require_any_device();
+    REQUIRE(p);
+    const float *src = p->p->mel_range(session, first, n);
+    const size_t need = (size_t)n * p->p->m->info.n_mels;
+    if (need) REQUIRE(out);
+    VOX_CHECK(cap >= need, VOX_ECAPACITY, "mel capacity %zu < %zu", cap, need);
     CUDA_OK(cudaSetDevice(p->p->m->device));
     CUDA_OK(cudaStreamSynchronize(p->p->s->st));
     if (need) CUDA_OK(cudaMemcpy(out, src, sizeof(float) * need, cudaMemcpyDeviceToHost));

@@ -1156,6 +1156,10 @@ void Session::transcribe_ragged(const float *samples, const size_t *lens, int b,
         for (int w = 0; w < W; ++w) row_streams[(size_t)i * W + w] = order[i];
     }
 
+    front.frames = T;
+    front.padded.resize(b);
+    for (int s = 0; s < b; ++s) front.padded[s] = g[s].padded;
+    front.pad_off.assign(pad_off.begin(), pad_off.end() - 1);
     CUDA_OK(cudaEventRecord(ev[0], st));
     CUDA_OK(cudaMemcpyAsync(pcm, samples, sizeof(float) * in_off[b], cudaMemcpyHostToDevice, st));
     for (int s = 0, t0 = 0; s < b; t0 += T[s], ++s) {

@@ -136,6 +136,13 @@ struct Session {
     void reserve_pcm(size_t in_floats, size_t padded_floats);   // grows pcm / pcm_pad to hold that much
     float *mel = nullptr;     // [B][128][T] as handed in by callers (reference layout)
     float *mel_tm = nullptr;  // [B][T][128] time-major copy consumed by the conv1 implicit GEMM
+    // front end of the last call that started from PCM or from a caller's mel, for the "mel" / "pcm_pad" debug reads:
+    // per stream its mel frames (packed one after the other in mel_tm) and, from PCM, its padded length and offset in
+    // pcm_pad; a mel call leaves `padded` empty and its [B][128][T] input in `mel`
+    struct FrontEnd {
+        std::vector<int> frames;
+        std::vector<size_t> padded, pad_off;
+    } front;
     // encoder workspace
     float *h1 = nullptr, *x_enc = nullptr, *h_enc = nullptr, *qkv_enc = nullptr, *attn_enc = nullptr, *act_enc = nullptr;
     float *packed = nullptr, *adapter_h = nullptr, *audio = nullptr;

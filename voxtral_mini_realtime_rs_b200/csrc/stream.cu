@@ -587,6 +587,15 @@ const float *StreamPool::audio_embeds_range(int id, int64_t first, int64_t n) {
     return s->audio + ((size_t)id * s->S4_max + (size_t)(first - sl.emb0)) * m->info.dec_dim;
 }
 
+const float *StreamPool::mel_range(int id, int64_t first, int64_t n) {
+    Slot &sl = slot(id);
+    VOX_CHECK(first >= 0 && n >= 0 && first + n <= sl.n_mel, VOX_EINVAL, "stream session %d: mel frames [%lld, %lld) not produced yet (%d so far)",
+              id, (long long)first, (long long)(first + n), sl.n_mel);
+    VOX_CHECK(first >= sl.mel0, VOX_ECAPACITY, "stream session %d: mel frame %lld is no longer resident (first resident: %d)", id,
+              (long long)first, sl.mel0);
+    return s->mel_tm + ((size_t)id * s->max_mel_frames + (size_t)(first - sl.mel0)) * m->info.n_mels;
+}
+
 void StreamPool::session_info(int id, struct vox_stream_session_info *out) {
     const Slot &sl = slot(id);
     *out = {};

@@ -64,6 +64,8 @@ struct StreamPool {
     const float *audio_embeds(int id, int *n);   // device pointer [n][dec_dim]; fails once rows were evicted
     // device pointer to resident audio embeddings [first, first + n)
     const float *audio_embeds_range(int id, int64_t first, int64_t n);
+    // device pointer to resident log-mel frames [first, first + n), [n][n_mels]
+    const float *mel_range(int id, int64_t first, int64_t n);
     void session_info(int id, struct vox_stream_session_info *out);
     // encode_audio_with_cache (model.rs:790-799): one mel chunk [128][T] (host) through the conv stem ON ITS OWN (zero
     // padding at the chunk edges, as upstream) and the encoder layers over the session's K/V rings; returns the
