@@ -116,6 +116,29 @@ int32_t vox_q4_matmul(const vox_q4 *w, const float *x_dev, float *y_dev, int32_t
 /* host-buffer convenience (H2D, kernel, D2H, sync) -- what benches/q4_ops.rs:76-91 times */
 int32_t vox_q4_matmul_host(const vox_q4 *w, const float *x, float *y, int32_t b, int32_t m,
                            const float *bias /* nullable */);
+/* One linear layer of the model in any of its fused forms, on the kernel vox_q4_set_matvec_mode selects:
+ *   y[r,:] = epi(norm(x[r,:]) . W^T + bias) (+ res[r,:])
+ * x [rows][K] contiguous f32 (must not overlap y); y and res rows are ldy floats apart; res may equal y (in place).
+ * epi: VOX_EPI_* below.  SiLU*up reads output features (2i, 2i+1) as (gate_i, up_i) and writes N/2 columns.
+ * gamma_dev (nullable) selects the RMSNorm x / sqrt(mean(x^2) + eps) * gamma; ada_dev (nullable, needs gamma) is a
+ * device array of device pointers to K floats each: row r is further scaled by ada_dev[r / ada_m].  gamma and every
+ * ADA vector must be 16-byte aligned.
+ * ssq_in_dev (nullable, needs gamma): [ceil(K/16)][rows] partial sums of squares of x, each over 16 consecutive
+ * elements, from which the tensor-core matvec takes the norm.  ssq_out_dev (nullable, residual only):
+ * [ceil(N/16)][rows], written with the same partial sums of the new y rows.  Both need the tensor-core matvec
+ * (rows <= 8, mode bit 0 clear).  Refused with VOX_EINVAL (vox_last_error says why): rows < 1, an unknown epi, a
+ * residual without res or res with another epi, SiLU*up with an odd N, ldy < N/2 or a bias, any other epi with
+ * ldy < N, ADA without gamma or ada_m < 1, ssq_in without gamma, ssq_out without a residual, and either ssq pointer
+ * when the call would not run the tensor-core matvec.  The unfused norm goes through a [rows][K] scratch the handle
+ * owns; same reentrancy rule as vox_q4_matmul. */
+#define VOX_EPI_NONE 0
+#define VOX_EPI_RESIDUAL 1
+#define VOX_EPI_SILU_MUL 2
+#define VOX_EPI_GELU 3
+int32_t vox_q4_linear(const vox_q4 *w, const float *x_dev, float *y_dev, int32_t rows, int32_t ldy,
+                      const float *bias_dev, const float *res_dev, int32_t epi, const float *gamma_dev, float eps,
+                      const float *const *ada_dev, int32_t ada_m, const float *ssq_in_dev, float *ssq_out_dev,
+                      void *stream);
 void vox_q4_tensor_free(vox_q4 *w);
 /* kernel selection of the operator seam (bit mask, default 0): bit 0 = SIMT warp-reduce matvec instead of
  * the tensor-core-assisted one (M <= 8); bit 1 = SIMT tiled GEMM instead of the wgmma GEMM (M > 8).

@@ -100,6 +100,8 @@ _SIGS = {
     "vox_q4_tensor_dequantize": (C.c_int32, [_P, _P]),
     "vox_q4_matmul": (C.c_int32, [_P, _P, _P, C.c_int32, C.c_int32, _P, _P]),
     "vox_q4_matmul_host": (C.c_int32, [_P, _P, _P, C.c_int32, C.c_int32, _P]),
+    "vox_q4_linear": (C.c_int32, [_P, _P, _P, C.c_int32, C.c_int32, _P, _P, C.c_int32, _P, C.c_float, _P,
+                                  C.c_int32, _P, _P, _P]),
     "vox_q4_tensor_free": (None, [_P]),
     "vox_q4_set_matvec_mode": (C.c_int32, [C.c_int32]),
     "vox_dev_malloc": (C.c_int32, [C.c_int32, C.c_size_t, C.POINTER(_P)]),
@@ -561,6 +563,64 @@ def q4_matmul(x, weights: Q4Tensor, bias=None) -> np.ndarray:
         bp = _ptr(bias)
     _check(lib().vox_q4_matmul_host(weights._h, _ptr(x), _ptr(y), b, m, bp))
     return y
+
+
+EPILOGUES = {"none": 0, "residual": 1, "silu_mul": 2, "gelu": 3}   # include/voxtral.h VOX_EPI_*
+
+
+def q4_linear(weights: Q4Tensor, x, epi: str = "none", *, bias=None, res=None, gamma=None, eps: float = 1e-5,
+              ada=None, ada_m: int = 1, ssq_in=None, want_ssq_out: bool = False, ldy: int | None = None,
+              y_rows: int | None = None, sentinel: float = float("nan"), in_place: bool = False):
+    """One fused linear layer (vox_q4_linear) on host arrays: y[r] = epi(norm(x[r]) . W^T + bias) (+ res[r]).
+
+    x [rows, K].  ada: [streams, K], row r takes ada[r // ada_m].  res [rows, N] (residual only).  ssq_in
+    [ceil(K/16), rows].  y is a [y_rows, ldy] device buffer (defaults: rows, and N or N/2 for SiLU*up) pre-filled with
+    `sentinel`, and res is copied into its first rows when in_place (y == res).  Returns y whole, and with
+    want_ssq_out the [ceil(N/16), rows] partial sums of squares too."""
+    n, k = weights.shape()
+    x = _f32(x).reshape(-1, k)
+    rows = x.shape[0]
+    cols = n // 2 if epi == "silu_mul" else n
+    ldy = cols if ldy is None else ldy
+    y_rows = rows if y_rows is None else y_rows
+    dev = weights.device
+    keep = []
+
+    def up(a, dtype=np.float32):
+        if a is None:
+            return None
+        b = DeviceBuffer.from_numpy(np.ascontiguousarray(a, dtype), dev)
+        keep.append(b)
+        return b.ptr
+
+    y_host = np.full((y_rows, ldy), sentinel, np.float32)
+    if res is not None:
+        res = _f32(res).reshape(rows, n)
+        if in_place:
+            y_host[:rows, :n] = res
+    y = DeviceBuffer.from_numpy(y_host, dev)
+    keep.append(y)
+    res_ptr = None
+    if res is not None:
+        if in_place:
+            res_ptr = y.ptr
+        else:
+            r = np.full((rows, ldy), sentinel, np.float32)
+            r[:, :n] = res
+            res_ptr = up(r)
+    ada_ptr = None
+    if ada is not None:
+        vecs = [up(v) for v in _f32(ada).reshape(-1, k)]
+        ada_ptr = up(np.array([v.value for v in vecs], np.uint64), np.uint64)
+    ssq_shape = ((n + 15) // 16, rows)
+    ssq_out = DeviceBuffer.from_numpy(np.full(ssq_shape, sentinel, np.float32), dev) if want_ssq_out else None
+    _check(lib().vox_q4_linear(weights._h, up(x), y.ptr, rows, ldy, up(bias), res_ptr, EPILOGUES[epi], up(gamma),
+                               eps, ada_ptr, ada_m, up(ssq_in), ssq_out.ptr if ssq_out else None, None))
+    _check(lib().vox_dev_sync(dev))
+    out = y.to_numpy(np.float32, (y_rows, ldy))
+    if ssq_out is not None:
+        return out, ssq_out.to_numpy(np.float32, ssq_shape)
+    return out
 
 
 class Q4Linear:

@@ -58,6 +58,8 @@ struct vox_q4 {
     Q4Weight w;
     float *x = nullptr, *y = nullptr, *bias = nullptr;  // scratch for the host-buffer call
     size_t x_cap = 0, y_cap = 0;
+    float *norm = nullptr;  // [rows][K] output of the unfused RMSNorm (vox_q4_linear)
+    size_t norm_cap = 0;
     TcWork wk;  // split-K scratch of the tensor-core matvec (allocated with the tensor)
     void *xt = nullptr;  // split tiles for the wgmma GEMM (M > 8)
     size_t xt_elems = 0;
@@ -369,6 +371,52 @@ int32_t vox_q4_matmul_host(const vox_q4 *wc, const float *x, float *y, int32_t b
                      0.0f, nullptr, q4_scratch(w, (int)rows), g_q4_path, 0);
     CUDA_OK(cudaMemcpyAsync(y, w->y, sizeof(float) * yn, cudaMemcpyDeviceToHost, 0));
     CUDA_OK(cudaStreamSynchronize(0));
+    VOX_API_END
+}
+static_assert(VOX_EPI_NONE == EPI_NONE && VOX_EPI_RESIDUAL == EPI_RESIDUAL && VOX_EPI_SILU_MUL == EPI_SILU_MUL &&
+                  VOX_EPI_GELU == EPI_GELU,
+              "the header's epilogue codes are kernels.h Epi");
+int32_t vox_q4_linear(const vox_q4 *wc, const float *x_dev, float *y_dev, int32_t rows, int32_t ldy,
+                      const float *bias_dev, const float *res_dev, int32_t epi, const float *gamma_dev, float eps,
+                      const float *const *ada_dev, int32_t ada_m, const float *ssq_in_dev, float *ssq_out_dev,
+                      void *stream) {
+    VOX_API_BEGIN
+    vox_q4 *w = const_cast<vox_q4 *>(wc);
+    REQUIRE(w); REQUIRE(x_dev); REQUIRE(y_dev);
+    const int N = w->w.N, K = w->w.K;
+    VOX_CHECK(rows >= 1, VOX_EINVAL, "q4_linear: rows=%d must be positive", rows);
+    VOX_CHECK(epi >= VOX_EPI_NONE && epi <= VOX_EPI_GELU, VOX_EINVAL, "q4_linear: epilogue %d is not one of 0..3", epi);
+    VOX_CHECK((epi == VOX_EPI_RESIDUAL) == (res_dev != nullptr), VOX_EINVAL,
+              "q4_linear: a residual epilogue needs res, and res needs the residual epilogue (epi=%d)", epi);
+    if (epi == VOX_EPI_SILU_MUL) {
+        VOX_CHECK(N % 2 == 0, VOX_EINVAL, "q4_linear: SiLU*up needs (gate, up) row pairs, N=%d is odd", N);
+        VOX_CHECK(ldy >= N / 2, VOX_EINVAL, "q4_linear: ldy=%d < N/2=%d", ldy, N / 2);
+        VOX_CHECK(!bias_dev, VOX_EINVAL, "q4_linear: SiLU*up takes no bias (no kernel adds one there)");
+    } else {
+        VOX_CHECK(ldy >= N, VOX_EINVAL, "q4_linear: ldy=%d < N=%d", ldy, N);
+    }
+    VOX_CHECK(!ada_dev || gamma_dev, VOX_EINVAL, "q4_linear: per-row ADA vectors need a norm (gamma)");
+    VOX_CHECK(!ada_dev || ada_m >= 1, VOX_EINVAL, "q4_linear: ada_m=%d must be positive", ada_m);
+    VOX_CHECK(!ssq_in_dev || gamma_dev, VOX_EINVAL, "q4_linear: ssq_in feeds the norm and needs gamma");
+    VOX_CHECK(!ssq_out_dev || epi == VOX_EPI_RESIDUAL, VOX_EINVAL, "q4_linear: ssq_out is written by a residual epilogue only");
+    const bool tc = rows <= 8 && g_q4_path.matvec_tc && w->w.qs_tc;
+    VOX_CHECK(!(ssq_in_dev || ssq_out_dev) || tc, VOX_EINVAL,
+              "q4_linear: ssq_in / ssq_out need the tensor-core matvec (rows <= 8, matvec mode bit 0 clear), rows=%d",
+              rows);
+    CUDA_OK(cudaSetDevice(w->device));
+    const size_t xn = (size_t)rows * K;
+    if (gamma_dev && xn > w->norm_cap) {
+        w->norm = w->arena.alloc_n<float>(xn);
+        w->norm_cap = xn;
+    }
+    Q4Scratch sc = q4_scratch(w, rows);
+    TcWork wk = w->wk;
+    wk.ssq_in = ssq_in_dev;
+    wk.ssq_in_parts = ssq_in_dev ? (K + 15) / 16 : 0;
+    wk.ssq_out = ssq_out_dev;
+    sc.tc = &wk;
+    launch_q4_linear(w->w, x_dev, rows, y_dev, ldy, bias_dev, res_dev, epi, gamma_dev, eps, w->norm, sc, g_q4_path,
+                     (cudaStream_t)stream, AdaRows{ada_dev, ada_dev ? ada_m : 1, 0});
     VOX_API_END
 }
 void vox_q4_tensor_free(vox_q4 *w) {
