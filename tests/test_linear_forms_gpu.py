@@ -3,8 +3,8 @@
 The reference and its bound are tests/test_linear_forms_ref.py's (LinearRef): y = epi(norm(x) . W^T + bias) (+ res)
 with RMSNorm, per-stream ADA vectors, bias, in-place residual, GELU and SiLU*up.  Each (form, rows) case runs in mode
 "tc" (the tensor-core matvec at rows <= 8, the wgmma GEMM above on its shapes) and mode "simt" (the SIMT matvec and
-the SIMT GEMM), against one f64 reference shared by both.  Forms at their production shapes (csrc/model.cu
-encoder_layers, encode, decoder_forward, lm_head_rows and compute_ada; the lm_head with a reduced vocabulary so that its
+the SIMT GEMM), against one f64 reference shared by both.  Forms at their production shapes (csrc/encoder.cu layers
+and adapt, csrc/model.cu decoder_forward, lm_head_rows and compute_ada; the lm_head with a reduced vocabulary so that its
 f64 weights fit in host memory), plus odd shapes on the matvec and SIMT GEMM paths: N = 17 and 208 at K = 4192, and
 N = 18 at K = 96 (SiLU*up over a partial 16-row tile).  The activation sets rotate over the cases; N = 256, K = 3072
 runs every set with every form on each of the four kernels.

@@ -584,17 +584,11 @@ int32_t vox_session_set_delays(vox_session *s, const float *delays, int32_t b) {
     VOX_API_END
 }
 
-static void upload_mel(Session *s, const float *mel, int b, int t) {
-    const vox_model_info &c = s->m->info;
-    s->check_batch(b);
-    VOX_CHECK(t >= 1 && t <= s->max_mel_frames, VOX_EINVAL, "mel frames %d exceed session max_mel_frames %d", t,
-              s->max_mel_frames);
-    CUDA_OK(cudaSetDevice(s->m->device));
-    s->front.frames.assign(b, t);
-    s->front.padded.clear();
-    s->front.pad_off.clear();
-    CUDA_OK(cudaMemcpyAsync(s->mel, mel, sizeof(float) * (size_t)b * c.n_mels * t, cudaMemcpyHostToDevice, s->st));
-    launch_transpose_mel(s->mel, s->mel_tm, b, c.n_mels, t, s->st);
+// the uniform encode of b streams of t frames already in enc.mel_tm (vox_encode_audio, vox_forward_streaming)
+static void encode_uniform(Session *s, int b, int t) {
+    const std::vector<int> frames(b, t);
+    s->enc.encode(*s, b, frames.data());
+    s->cur_B = b;
 }
 
 int32_t vox_encode_audio(vox_session *sh, const float *mel, int32_t b, int32_t t, float *audio_embeds, size_t cap,
@@ -602,15 +596,15 @@ int32_t vox_encode_audio(vox_session *sh, const float *mel, int32_t b, int32_t t
     VOX_API_BEGIN
     REQUIRE(sh); REQUIRE(mel);
     Session *s = sh->s;
-    upload_mel(s, mel, b, t);
-    s->encode(b, t);
-    const size_t n = (size_t)b * s->cur_S4 * s->m->info.dec_dim;
+    s->enc.upload_mel(*s, mel, b, t);
+    encode_uniform(s, b, t);
+    const size_t n = (size_t)b * s->enc.positions * s->m->info.dec_dim;
     if (audio_embeds) {
         VOX_CHECK(cap >= n, VOX_ECAPACITY, "audio_embeds capacity %zu < %zu", cap, n);
-        if (n) CUDA_OK(cudaMemcpyAsync(audio_embeds, s->audio, sizeof(float) * n, cudaMemcpyDeviceToHost, s->st));
+        if (n) CUDA_OK(cudaMemcpyAsync(audio_embeds, s->enc.audio, sizeof(float) * n, cudaMemcpyDeviceToHost, s->st));
     }
     CUDA_OK(cudaStreamSynchronize(s->st));
-    if (seq_len) *seq_len = s->cur_S4;
+    if (seq_len) *seq_len = s->enc.positions;
     VOX_API_END
 }
 
@@ -636,7 +630,7 @@ int32_t vox_transcribe_streaming(vox_session *sh, const float *mel, int32_t b, i
     s->check_beam_bias();
     CUDA_OK(cudaSetDevice(s->m->device));
     CUDA_OK(cudaEventRecord(s->ev[0], s->st));
-    upload_mel(s, mel, b, t);
+    s->enc.upload_mel(*s, mel, b, t);
     CUDA_OK(cudaEventRecord(s->ev[1], s->st));
     *n_out = s->transcribe_from_mel(b, t, out_ids, cap, tm);
     fill_timings(s, tm);
@@ -651,25 +645,14 @@ static int32_t transcribe_pcm_impl(Session *s, const float *host, const float *d
     CUDA_OK(cudaSetDevice(s->m->device));
     vox_pad_config pc;
     pad_config_default(&pc);
-    const size_t padded = pad_audio_len(n, pc), left = pad_left(pc);
-    const size_t frames = mel_num_frames(padded);
+    const size_t frames = mel_num_frames(pad_audio_len(n, pc));
     VOX_CHECK(frames >= 1, VOX_EINVAL, "Audio too short to produce mel frames");
-    VOX_CHECK(frames <= (size_t)s->max_mel_frames, VOX_EINVAL,
-              "audio needs %zu mel frames > session max_mel_frames %d (chunk it: vox_chunk_plan)", frames, s->max_mel_frames);
-    s->reserve_pcm(host ? (size_t)b * n : 0, (size_t)b * padded);
-    s->front.frames.assign(b, (int)frames);
-    s->front.padded.assign(b, padded);
-    s->front.pad_off.resize(b);
-    for (int i = 0; i < b; ++i) s->front.pad_off[i] = (size_t)i * padded;
+    VOX_CHECK(frames <= (size_t)s->enc.max_mel_frames, VOX_EINVAL,
+              "audio needs %zu mel frames > session max_mel_frames %d (chunk it: vox_chunk_plan)", frames, s->enc.max_mel_frames);
+    const std::vector<size_t> lens(b, n);
+    s->enc.prepare_pcm(*s, lens.data(), b, host != nullptr);
     CUDA_OK(cudaEventRecord(s->ev[0], s->st));
-    const float *src = dev;
-    if (host) {
-        CUDA_OK(cudaMemcpyAsync(s->pcm, host, sizeof(float) * (size_t)b * n, cudaMemcpyHostToDevice, s->st));
-        src = s->pcm;
-    }
-    launch_peak_normalize_pad(src, b, n, 0.95f, normalize, s->pcm_pad, padded, left, s->peak_scale, s->st);
-    launch_mel(s->pcm_pad, b, padded, padded, s->m->mel.window, s->m->mel.fb_vals, s->m->mel.fb_start, s->m->mel.fb_len,
-               s->m->mel.fb_stride, s->mel_tm, (int)frames, 0, s->st);
+    s->enc.pcm_to_mel(*s, host, dev, lens.data(), b, normalize);
     CUDA_OK(cudaEventRecord(s->ev[1], s->st));
     *n_out = s->transcribe_from_mel(b, (int)frames, out_ids, cap, tm);
     fill_timings(s, tm);
@@ -700,9 +683,9 @@ int32_t vox_transcribe_pcm_ragged(vox_session *sh, const float *samples, const s
         VOX_CHECK(lens[i] >= 1, VOX_EINVAL, "stream %d is empty", i);
         const StreamGeom g = stream_geometry(c, lens[i]);
         VOX_CHECK(g.frames >= 1, VOX_EINVAL, "stream %d too short to produce mel frames", i);
-        VOX_CHECK(g.frames <= s->max_mel_frames, VOX_EINVAL,
+        VOX_CHECK(g.frames <= s->enc.max_mel_frames, VOX_EINVAL,
                   "stream %d needs %d mel frames > session max_mel_frames %d (chunk it: vox_chunk_plan)", i, g.frames,
-                  s->max_mel_frames);
+                  s->enc.max_mel_frames);
         total += (size_t)g.n_out;
         equal = equal && lens[i] == lens[0];
     }
@@ -755,9 +738,9 @@ int32_t vox_forward_streaming(vox_session *sh, const float *mel, int32_t b, int3
     REQUIRE(sh); REQUIRE(mel); REQUIRE(ids); REQUIRE(logits);
     Session *s = sh->s;
     const vox_model_info &c = s->m->info;
-    upload_mel(s, mel, b, t);
-    s->encode(b, t);
-    const int S4 = s->cur_S4;
+    s->enc.upload_mel(*s, mel, b, t);
+    encode_uniform(s, b, t);
+    const int S4 = s->enc.positions;
     VOX_CHECK(n_ids == S4, VOX_EINVAL, "forward_streaming needs one token id per audio position (%d), got %d", S4, n_ids);
     VOX_CHECK(S4 <= s->out_ld, VOX_EINVAL, "sequence %d exceeds the session KV capacity %d", S4, s->out_ld);
     s->check_ids(ids, (size_t)b * n_ids);
@@ -793,9 +776,9 @@ int32_t vox_prefill(vox_session *sh, const int32_t *ids, int32_t b, int32_t m, i
     VOX_CHECK(s->beam_w == 1, VOX_EINVAL, "vox_prefill runs greedy only: the session's beam width is %d", s->beam_w);
     VOX_CHECK(s->cache_len + m <= s->out_ld, VOX_EINVAL, "KV cache full (%d + %d > %d)", s->cache_len, m, s->out_ld);
     if (add_audio)
-        VOX_CHECK(b == (int)s->audio_offs.size() && s->cache_len + m <= s->cur_S4, VOX_EINVAL,
+        VOX_CHECK(b == (int)s->enc.audio_offs.size() && s->cache_len + m <= s->enc.positions, VOX_EINVAL,
                   "add_audio: positions %d..%d need audio embeddings of %d streams (have %d positions for %d streams; call vox_encode_audio first)",
-                  s->cache_len, s->cache_len + m, b, s->cur_S4, (int)s->audio_offs.size());
+                  s->cache_len, s->cache_len + m, b, s->enc.positions, (int)s->enc.audio_offs.size());
     s->check_ids(ids, (size_t)b * m);
     CUDA_OK(cudaSetDevice(s->m->device));
     s->step_incremental(b, m, ids, add_audio != 0);
@@ -811,9 +794,9 @@ int32_t vox_decode_step(vox_session *sh, const int32_t *tok, int32_t b, int32_t 
     VOX_CHECK(s->beam_w == 1, VOX_EINVAL, "vox_decode_step runs greedy only: the session's beam width is %d", s->beam_w);
     VOX_CHECK(s->cache_len + 1 <= s->out_ld, VOX_EINVAL, "KV cache full (%d + 1 > %d)", s->cache_len, s->out_ld);
     if (add_audio)
-        VOX_CHECK(b == (int)s->audio_offs.size() && s->cache_len < s->cur_S4, VOX_EINVAL,
-                  "add_audio: position %d has no audio embedding (%d positions, %d streams encoded)", s->cache_len, s->cur_S4,
-                  (int)s->audio_offs.size());
+        VOX_CHECK(b == (int)s->enc.audio_offs.size() && s->cache_len < s->enc.positions, VOX_EINVAL,
+                  "add_audio: position %d has no audio embedding (%d positions, %d streams encoded)", s->cache_len,
+                  s->enc.positions, (int)s->enc.audio_offs.size());
     CUDA_OK(cudaSetDevice(s->m->device));
     if (tok) {
         s->check_ids(tok, b);
@@ -977,17 +960,10 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
     const std::string w = what;
     const float *src = nullptr;
     size_t n = 0;
-    const size_t rows = (size_t)s->enc_rows;
-    if (w == "capture_on") {
-        if (!s->dbg_layers) {
-            s->dbg_layers = s->arena.alloc_n<float>((size_t)c.enc_layers * s->max_batch * s->S_max * c.enc_dim);
-            s->dbg_conv = s->arena.alloc_n<float>((size_t)s->max_batch * s->S_max * c.enc_dim);
-        }
-        s->debug_capture = true;
-        if (n_floats) *n_floats = 0;
-        return VOX_OK;
-    } else if (w == "capture_off") {
-        s->debug_capture = false;
+    AudioEncoder &e = s->enc;
+    const size_t rows = (size_t)e.rows;
+    if (w == "capture_on" || w == "capture_off") {
+        e.set_capture(*s, w == "capture_on");
         if (n_floats) *n_floats = 0;
         return VOX_OK;
     } else if (w == "graph_off" || w == "graph_on") {
@@ -995,7 +971,7 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
         if (n_floats) *n_floats = 0;
         return VOX_OK;
     } else if (w == "enc_attn_simt" || w == "enc_attn_tc") {
-        s->use_enc_attn_tc = (w == "enc_attn_tc");
+        e.use_attn_tc = (w == "enc_attn_tc");
         if (n_floats) *n_floats = 0;
         return VOX_OK;
     } else if (w == "gemm_simt" || w == "gemm_tc") {
@@ -1087,7 +1063,7 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
         return VOX_OK;
     } else if (w == "pcm_pad") {
         // each stream's normalised, padded signal of the last PCM call, stream after stream
-        const Session::FrontEnd &f = s->front;
+        const AudioEncoder::FrontEnd &f = e.front;
         VOX_CHECK(!f.padded.empty(), VOX_ENOTFOUND, "'pcm_pad': the last call did not start from PCM");
         size_t cnt = 0;
         for (size_t p : f.padded) cnt += p;
@@ -1096,25 +1072,25 @@ int32_t vox_session_debug_read(vox_session *sh, const char *what, float *out, si
             VOX_CHECK(cap >= cnt, VOX_ECAPACITY, "debug_read capacity %zu < %zu", cap, cnt);
             CUDA_OK(cudaStreamSynchronize(s->st));
             for (size_t i = 0, o = 0; i < f.padded.size(); o += f.padded[i], ++i)
-                CUDA_OK(cudaMemcpy(out + o, s->pcm_pad + f.pad_off[i], sizeof(float) * f.padded[i], cudaMemcpyDeviceToHost));
+                CUDA_OK(cudaMemcpy(out + o, e.pcm_pad + f.pad_off[i], sizeof(float) * f.padded[i], cudaMemcpyDeviceToHost));
         }
         return VOX_OK;
     } else if (w == "mel") {
         // PCM call: the time-major mel every stream's frames were packed into; mel call: the caller's [B][128][T]
-        const Session::FrontEnd &f = s->front;
+        const AudioEncoder::FrontEnd &f = e.front;
         VOX_CHECK(!f.frames.empty(), VOX_ENOTFOUND, "'mel': no call has computed or uploaded a mel yet");
         for (int t : f.frames) n += (size_t)t * c.n_mels;
-        src = f.padded.empty() ? s->mel : s->mel_tm;
+        src = f.padded.empty() ? e.mel : e.mel_tm;
     }
-    else if (w == "enc_out") { src = s->h_enc; n = rows * c.enc_dim; }
-    else if (w == "audio_embeds") { src = s->audio; n = (size_t)s->audio_n * c.dec_dim; }   // stream after stream
-    else if (w == "conv") { src = s->dbg_conv; n = rows * c.enc_dim; }
+    else if (w == "enc_out") { src = e.h_enc; n = rows * c.enc_dim; }
+    else if (w == "audio_embeds") { src = e.audio; n = (size_t)e.audio_n * c.dec_dim; }   // stream after stream
+    else if (w == "conv") { src = e.dbg_conv; n = rows * c.enc_dim; }
     else if (w == "logits") { src = s->logits; n = (size_t)s->cur_B * c.vocab; }
     else if (w == "ada") { src = s->ada_sets; n = (size_t)c.dec_layers * c.dec_dim; }   // stream 0's ADA scale
     else if (w.rfind("enc", 0) == 0 && w.size() > 3) {
         const int i = atoi(w.c_str() + 3);
-        VOX_CHECK(i >= 0 && i < c.enc_layers && s->dbg_layers, VOX_EINVAL, "no capture for '%s'", what);
-        src = s->dbg_layers + (size_t)i * rows * c.enc_dim;
+        VOX_CHECK(i >= 0 && i < c.enc_layers && e.dbg_layers, VOX_EINVAL, "no capture for '%s'", what);
+        src = e.dbg_layers + (size_t)i * rows * c.enc_dim;
         n = rows * c.enc_dim;
     }
     VOX_CHECK(src != nullptr, VOX_ENOTFOUND, "unknown debug buffer '%s'", what);

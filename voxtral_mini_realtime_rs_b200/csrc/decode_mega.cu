@@ -1674,7 +1674,7 @@ void DecodeMega::step(const Session &s, int R, bool add_audio) {
         p.d_outpos += b0;
         p.d_tok += b0;
         p.d_out += (size_t)b0 * p.out_ld;
-        p.audio = add_audio ? s.audio : nullptr;
+        p.audio = add_audio ? s.enc.audio : nullptr;
         p.logits_out = s.logits + (size_t)b0 * s.m->info.vocab;
         // read per launch: an unbounded stream pool points the session's RoPE tables at its ring after creating it
         p.cos_t = s.dec_rope.cos_t;

@@ -390,21 +390,6 @@ Model *Model::load(const Gguf &g, int device) {
 // ======================================================================================
 // Session
 // ======================================================================================
-static int conv_out(int t) { return (t + 2 - 3) / 2 + 1; }  // conv.rs:47-48
-
-StreamGeom stream_geometry(const vox_model_info &c, size_t n) {
-    vox_pad_config pc;
-    pad_config_default(&pc);
-    StreamGeom g;
-    g.padded = pad_audio_len(n, pc);
-    const size_t frames = mel_num_frames(g.padded);
-    g.frames = (int)std::min(frames, (size_t)1 << 30);
-    g.S = conv_out(conv_out(g.frames));
-    g.S4 = g.S / c.reshape_factor;
-    g.n_out = std::max(0, g.S4 - c.prefix_len);
-    return g;
-}
-
 Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ring, KvType kv_type) {
     VOX_CHECK(max_batch >= 1 && max_batch <= 64, VOX_EINVAL, "max_batch %d out of range [1,64]", max_batch);
     VOX_CHECK(max_mel_frames >= 16, VOX_EINVAL, "max_mel_frames %d too small", max_mel_frames);
@@ -415,32 +400,14 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ri
         s->m = m;
         s->arena.device = m->device;
         s->max_batch = max_batch;
-        s->max_mel_frames = max_mel_frames;
-        s->T1_max = conv_out(max_mel_frames);
-        s->S_max = conv_out(s->T1_max);
-        s->S4_max = s->S_max / c.reshape_factor;
         s->M_max = std::max(c.prefix_len, 64);
-        VOX_CHECK(s->S_max <= m->enc_rope_len, VOX_EINVAL, "max_mel_frames %d exceeds the encoder RoPE table", max_mel_frames);
+        s->enc.create(s->arena, *m, max_batch, max_mel_frames);
+        const int S_max = s->enc.S_max, S4_max = s->enc.S4_max;
         CUDA_OK(cudaStreamCreateWithFlags(&s->st, cudaStreamNonBlocking));
         for (auto &e : s->ev) CUDA_OK(cudaEventCreate(&e));
         const size_t B = max_batch;
-        const int hdq = c.enc_heads * c.enc_head_dim;
-        s->mel = s->arena.alloc_n<float>(B * c.n_mels * max_mel_frames);
-        s->mel_tm = s->arena.alloc_n<float>(B * c.n_mels * max_mel_frames);
-        s->peak_scale = s->arena.alloc_n<float>(B);
-        s->h1 = s->arena.alloc_n<float>(B * s->T1_max * c.enc_dim);
-        const size_t rows = B * s->S_max;
-        s->x_enc = s->arena.alloc_n<float>(rows * c.enc_dim);
-        s->h_enc = s->arena.alloc_n<float>(rows * c.enc_dim);
-        s->qkv_enc = s->arena.alloc_n<float>(rows * 3 * hdq);
-        s->attn_enc = s->arena.alloc_n<float>(rows * hdq);
-        s->act_enc = s->arena.alloc_n<float>(rows * c.enc_ffn);
-        const size_t rows4 = B * std::max(s->S4_max, 1);
-        s->packed = s->arena.alloc_n<float>(rows4 * c.enc_dim * c.reshape_factor);
-        s->adapter_h = s->arena.alloc_n<float>(rows4 * c.dec_dim);
-        s->audio = s->arena.alloc_n<float>(rows4 * c.dec_dim);
         // decoder
-        s->kv.create(s->arena, c, max_batch, s->S4_max, s->M_max, kv_ring, kv_type);
+        s->kv.create(s->arena, c, max_batch, S4_max, s->M_max, kv_ring, kv_type);
         s->out_ld = s->kv.capacity();
         s->dec_rope = m->dec_rope();
         const size_t drows = B * s->M_max;
@@ -462,16 +429,15 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ri
         s->ada_tmp = s->arena.alloc_n<float>(c.t_cond_dim);
         s->d_pos = s->arena.alloc_n<int>(B);      // per row (kernels.h KvView::pos)
         s->d_outpos = s->arena.alloc_n<int>(B);
-        s->d_seg = s->arena.alloc_n<int>(B + 1);
         s->d_tok = s->arena.alloc_n<int>(B);
         s->d_ids = s->arena.alloc_n<int>(drows);
         s->d_out = s->arena.alloc_n<int>(B * s->out_ld);
         {   // split-tile buffer of the wgmma GEMM: largest (rows, K) pair it is used with
-            const int rows_e = max_batch * s->S_max, rows_d = max_batch * s->M_max;
+            const int rows_e = max_batch * S_max, rows_d = max_batch * s->M_max;
             size_t e = 0;
             for (int K : {c.enc_dim, c.enc_heads * c.enc_head_dim, c.enc_ffn}) e = std::max(e, gemm_tc5_split_elems(rows_e, K / 64 * 64));
-            e = std::max(e, gemm_tc5_split_elems(max_batch * std::max(s->S4_max, 1), c.enc_dim * c.reshape_factor / 64 * 64));
-            for (int K : {c.dec_dim, c.dec_heads * c.dec_head_dim, c.dec_ffn}) e = std::max(e, gemm_tc5_split_elems(std::max(rows_d, max_batch * std::max(s->S4_max, 1)), K / 64 * 64));
+            e = std::max(e, gemm_tc5_split_elems(max_batch * std::max(S4_max, 1), c.enc_dim * c.reshape_factor / 64 * 64));
+            for (int K : {c.dec_dim, c.dec_heads * c.dec_head_dim, c.dec_ffn}) e = std::max(e, gemm_tc5_split_elems(std::max(rows_d, max_batch * std::max(S4_max, 1)), K / 64 * 64));
             s->xt_elems = e;
             s->xt_buf = s->arena.alloc(e * 2);
             s->gemm_work = gemm_tc5_work_size();
@@ -480,8 +446,6 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ri
             s->path.gemm_tc = !(gv && std::string(gv) == "simt");
             const char *tv = getenv("VOX_MATVEC");
             s->path.matvec_tc = !(tv && std::string(tv) == "simt");
-            const char *av = getenv("VOX_ENC_ATTN");
-            s->use_enc_attn_tc = !(av && std::string(av) == "simt");
         }
         {   // fused-decode scratch (see TcWork): split-K of the largest decoder / lm_head matvec
             std::vector<const Q4Weight *> ws{&m->tok_emb};
@@ -593,7 +557,7 @@ void Session::bind_rows(int B) {
     for (int r = 0; r < B; ++r) {
         const int s = row_streams.empty() ? r : row_streams[r];
         streams[r] = s;
-        offs[r] = s < (int)audio_offs.size() ? audio_offs[s] : 0;   // (a stream without embeddings reads none)
+        offs[r] = s < (int)enc.audio_offs.size() ? enc.audio_offs[s] : 0;   // (a stream without embeddings reads none)
     }
     if (bound_streams.size() >= (size_t)B && std::equal(streams.begin(), streams.end(), bound_streams.begin()) &&
         std::equal(offs.begin(), offs.end(), bound_offs.begin()))
@@ -612,72 +576,9 @@ void Session::bind_rows(int B) {
     bound_offs = std::move(offs);
 }
 
-void Session::reserve_pcm(size_t in_floats, size_t padded_floats) {
-    if (in_floats > pcm_cap) {
-        pcm = arena.alloc_n<float>(in_floats);
-        pcm_cap = in_floats;
-    }
-    if (padded_floats > pcm_pad_cap) {
-        pcm_pad = arena.alloc_n<float>(padded_floats);
-        pcm_pad_cap = padded_floats;
-    }
-}
-
 void Session::check_batch(int b) const { VOX_CHECK(b >= 1 && b <= max_batch, VOX_EINVAL, "batch %d exceeds session max_batch %d", b, max_batch); }
 void Session::check_ids(const int32_t *ids, size_t n) const {
     for (size_t i = 0; i < n; ++i) VOX_CHECK(ids[i] >= 0 && ids[i] < m->info.vocab, VOX_EINVAL, "token id %d out of range", ids[i]);
-}
-
-void Session::encoder_layers(int rows, const std::function<void(int)> &attn) {
-    const vox_model_info &c = m->info;
-    const int d = c.enc_dim;
-    for (int i = 0; i < c.enc_layers; ++i) {
-        const EncLayerW &l = m->enc[i];
-        linear(l.wqkv, x_enc, rows, qkv_enc, 3 * c.enc_heads * c.enc_head_dim, l.bqkv, nullptr, EPI_NONE, l.attn_norm, h_enc);
-        attn(i);
-        linear(l.wo, attn_enc, rows, x_enc, d, l.bo, x_enc, EPI_RESIDUAL);
-        linear(l.w13, x_enc, rows, act_enc, c.enc_ffn, nullptr, nullptr, EPI_SILU_MUL, l.ffn_norm, h_enc);
-        linear(l.w2, act_enc, rows, x_enc, d, l.b2, x_enc, EPI_RESIDUAL);
-        if (debug_capture && dbg_layers)
-            CUDA_OK(cudaMemcpyAsync(dbg_layers + (size_t)i * rows * d, x_enc, sizeof(float) * rows * d,
-                                    cudaMemcpyDeviceToDevice, st));
-    }
-    launch_rmsnorm(x_enc, m->enc_norm, h_enc, rows, d, m->norm_eps, st);
-}
-
-void Session::enc_rope_attention(int rows, int B, int S, const int *seg) {
-    const vox_model_info &c = m->info;
-    const int H = c.enc_heads, hd = c.enc_head_dim, hdq = H * hd;
-    const float scale = powf((float)hd, -0.5f);
-    launch_rope_inplace(qkv_enc, rows, 3 * hdq, 0, H, hdq, H, hd, S, 0, m->enc_cos, m->enc_sin, st, seg, seg ? B : 0);
-    const bool tc = use_enc_attn_tc && enc_attention_tc_supported(hd, 3 * hdq, 0, hdq, 2 * hdq);
-    (tc ? launch_enc_attention_tc : launch_enc_attention)(qkv_enc, attn_enc, B, S, H, hd, 3 * hdq, 0, hdq, 2 * hdq, c.enc_window,
-                                                          scale, st, seg);
-}
-
-// Q4VoxtralModel::encode_audio (model.rs:783-788): conv -> 32 layers -> norm -> reshape x4 -> adapter
-void Session::encode(int B, int T) {
-    const vox_model_info &c = m->info;
-    check_batch(B);
-    VOX_CHECK(T >= 1 && T <= max_mel_frames, VOX_EINVAL, "mel frames %d exceed session max_mel_frames %d", T, max_mel_frames);
-    const int T1 = conv_out(T), S = conv_out(T1), S4 = S / c.reshape_factor;
-    const int d = c.enc_dim, rows = B * S;
-    // conv1 + GELU as implicit GEMM over the time-major mel [B][T][128] (K = 3*128)
-    launch_conv2_gemm(mel_tm, m->conv1_w, m->conv1_b, h1, B, T, T1, c.n_mels, d, st);
-    launch_conv2_gemm(h1, m->conv2_w, m->conv2_b, x_enc, B, T1, S, d, d, st);
-    if (debug_capture && dbg_conv) CUDA_OK(cudaMemcpyAsync(dbg_conv, x_enc, sizeof(float) * rows * d, cudaMemcpyDeviceToDevice, st));
-    encoder_layers(rows, [&](int) { enc_rope_attention(rows, B, S, nullptr); });
-    cur_B = B;
-    cur_S4 = S4;
-    enc_rows = rows;
-    audio_n = B * S4;
-    audio_offs.resize(B);
-    for (int s = 0; s < B; ++s) audio_offs[s] = (int64_t)s * S4 * c.dec_dim;
-    if (S4 > 0) {
-        launch_reshape_rows(h_enc, packed, B, S, S4, d, c.reshape_factor, st);
-        linear(m->adapter0, packed, B * S4, adapter_h, c.dec_dim, nullptr, nullptr, EPI_GELU);
-        linear(m->adapter2, adapter_h, B * S4, audio, c.dec_dim, nullptr, nullptr, EPI_NONE);
-    }
 }
 
 // Q4LanguageModel::forward_hidden_with_cache (model.rs:665-677) over x_dec [B*M][D]; positions
@@ -736,7 +637,7 @@ void Session::lm_head_rows(int rows, bool norm_pending, float *dst) {
 void Session::forward_logits(int b, int M, const int *ids_host, bool with_audio, float *dst) {
     bind_rows(b);
     CUDA_OK(cudaMemcpyAsync(d_ids, ids_host, sizeof(int) * (size_t)b * M, cudaMemcpyHostToDevice, st));
-    launch_embed(m->tok_emb, d_ids, with_audio ? audio : nullptr, d_audio_off, b, M, d_pos, x_dec,
+    launch_embed(m->tok_emb, d_ids, with_audio ? enc.audio : nullptr, d_audio_off, b, M, d_pos, x_dec,
                  fused_decode(b * M) ? ssq_x : nullptr, st);
     const bool pending = decoder_forward(b, M);
     lm_head_rows(b * M, pending, dst);
@@ -757,7 +658,7 @@ unsigned Session::decode_step(int B, bool add_audio) {
     mega.attn_log.clear();
     if (mega_launches > 0) mega.step(*this, B, add_audio);
     else {
-        launch_embed(m->tok_emb, d_tok, add_audio ? audio : nullptr, d_audio_off, B, 1, d_pos, x_dec,
+        launch_embed(m->tok_emb, d_tok, add_audio ? enc.audio : nullptr, d_audio_off, B, 1, d_pos, x_dec,
                      fused_decode(B) ? ssq_x : nullptr, st);
         const bool pending = decoder_forward(B, 1);
         lm_head_rows(B, pending, logits);
@@ -906,7 +807,7 @@ void Session::prefill(int B, int M, const int *ids_host, bool add_audio) {
     const vox_model_info &c = m->info;
     bind_rows(B);
     CUDA_OK(cudaMemcpyAsync(d_ids, ids_host, sizeof(int) * (size_t)B * M, cudaMemcpyHostToDevice, st));
-    launch_embed(m->tok_emb, d_ids, add_audio ? audio : nullptr, d_audio_off, B, M, d_pos, x_dec,
+    launch_embed(m->tok_emb, d_ids, add_audio ? enc.audio : nullptr, d_audio_off, B, M, d_pos, x_dec,
                  fused_decode(B * M) ? ssq_x : nullptr, st);
     const bool pending = decoder_forward(B, M);
     if (pending) {   // decode-sized prefill (B*M <= 8): final norm still pending in x_dec
@@ -993,8 +894,8 @@ struct RowStreams {
 };
 }  // namespace
 
-// Q4VoxtralModel::transcribe_streaming (model.rs:873-963).  Expects the mel in s->mel; records
-// ev[1] (after encode) and ev[2] (after decode) on the stream.  Returns tokens per stream.
+// Q4VoxtralModel::transcribe_streaming (model.rs:873-963).  Expects the mel in enc.mel_tm; records
+// ev[2] (after encode), ev[4] (after the prefill) and ev[3] (after decode) on the stream.  Returns tokens per stream.
 int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids, vox_timings *tm) {
     const vox_model_info &c = m->info;
     const int W = beam_w, R = B * W;   // decode rows: beam w of stream s in row w * B + s
@@ -1002,9 +903,11 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
     RowStreams row_guard{this};
     if (W > 1)
         for (int r = 0; r < R; ++r) row_streams.push_back(r % B);
-    encode(B, T);
+    const std::vector<int> frames(B, T);
+    enc.encode(*this, B, frames.data());
+    cur_B = B;
     CUDA_OK(cudaEventRecord(ev[2], st));
-    const int S4 = cur_S4, P = c.prefix_len;
+    const int S4 = enc.positions, P = c.prefix_len;
     int n_out = 0;
     if (S4 >= P) {
         n_out = S4 - P;
@@ -1063,54 +966,6 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
 // Streams of different lengths in one call (vox_transcribe_pcm_ragged)
 // ======================================================================================
 
-// encode() on streams packed one after the other: the convolutions run per stream (their zero padding is at each
-// stream's own ends), the layers' linears run over all rows at once, RoPE and attention read the segment table, and
-// each stream keeps its own S / 4 embeddings.  Work follows the sum of the lengths, not b x the longest.
-void Session::encode_ragged(int b, const int *T) {
-    const vox_model_info &c = m->info;
-    check_batch(b);
-    const int d = c.enc_dim, f = c.reshape_factor, D = c.dec_dim;
-    std::vector<int> T1(b), S(b), S4(b);
-    seg_host.assign(b + 1, 0);
-    audio_offs.resize(b);
-    int S_long = 0, sum_T = 0, sum_S4 = 0, S4_short = S4_max;
-    for (int i = 0; i < b; ++i) {
-        VOX_CHECK(T[i] >= 1 && T[i] <= max_mel_frames, VOX_EINVAL, "mel frames %d exceed session max_mel_frames %d", T[i],
-                  max_mel_frames);
-        T1[i] = conv_out(T[i]);
-        S[i] = conv_out(T1[i]);
-        S4[i] = S[i] / f;
-        seg_host[i + 1] = seg_host[i] + S[i];
-        S_long = std::max(S_long, S[i]);
-        S4_short = std::min(S4_short, S4[i]);
-        sum_T += T[i];
-        audio_offs[i] = (int64_t)sum_S4 * D;
-        sum_S4 += S4[i];
-    }
-    const int rows = seg_host[b];
-    // b <= max_batch streams of <= max_mel_frames frames: the scratch Session::create sized for max_batch uniform streams
-    // holds them packed
-    if (!(sum_T <= max_batch * max_mel_frames && rows <= max_batch * S_max))
-        fail(VOX_EINVAL, "encode_ragged: packed streams exceed the session scratch");
-    CUDA_OK(cudaMemcpyAsync(d_seg, seg_host.data(), sizeof(int) * (b + 1), cudaMemcpyHostToDevice, st));
-    for (int i = 0, t0 = 0, t1 = 0; i < b; t0 += T[i], t1 += T1[i], ++i) {
-        launch_conv2_gemm(mel_tm + (size_t)t0 * c.n_mels, m->conv1_w, m->conv1_b, h1 + (size_t)t1 * d, 1, T[i], T1[i], c.n_mels,
-                          d, st);
-        launch_conv2_gemm(h1 + (size_t)t1 * d, m->conv2_w, m->conv2_b, x_enc + (size_t)seg_host[i] * d, 1, T1[i], S[i], d, d, st);
-    }
-    if (debug_capture && dbg_conv) CUDA_OK(cudaMemcpyAsync(dbg_conv, x_enc, sizeof(float) * rows * d, cudaMemcpyDeviceToDevice, st));
-    encoder_layers(rows, [&](int) { enc_rope_attention(rows, b, S_long, d_seg); });
-    enc_rows = rows;
-    cur_B = b * beam_w;   // the call's decoder rows, whose logits debug "logits" reads
-    cur_S4 = S4_short;    // positions every stream has
-    audio_n = sum_S4;
-    if (sum_S4 == 0) return;
-    for (int i = 0, o = 0; i < b; o += S4[i], ++i)
-        launch_reshape_rows(h_enc + (size_t)seg_host[i] * d, packed + (size_t)o * d * f, 1, S[i], S4[i], d, f, st);
-    linear(m->adapter0, packed, sum_S4, adapter_h, D, nullptr, nullptr, EPI_GELU);
-    linear(m->adapter2, adapter_h, sum_S4, audio, D, nullptr, nullptr, EPI_NONE);
-}
-
 // Streams sorted (stably) by decreasing output count own the rows: beams w of sorted stream i run in row i * W + w, so
 // the streams that still need tokens are always the rows [0, R).  Every stream with output takes the prefill; then the
 // steps run in segments, one per distinct output count, each over the rows still live.
@@ -1128,21 +983,13 @@ void Session::transcribe_ragged(const float *samples, const size_t *lens, int b,
     const int W = beam_w, P = c.prefix_len;
     check_batch(b);
     VOX_CHECK(W == 1 || b * W <= max_batch, VOX_EINVAL, "beam width %d x %d streams exceeds session max_batch %d", W, b, max_batch);
-    vox_pad_config pc;
-    pad_config_default(&pc);
-    const size_t left = pad_left(pc);
     std::vector<StreamGeom> g(b);
-    std::vector<size_t> in_off(b + 1, 0), pad_off(b + 1, 0);
-    std::vector<int> T(b);
     for (int s = 0; s < b; ++s) {
         g[s] = stream_geometry(c, lens[s]);
-        T[s] = g[s].frames;
         n_out[s] = g[s].n_out;
-        in_off[s + 1] = in_off[s] + lens[s];
-        pad_off[s + 1] = pad_off[s] + (g[s].padded + 3) / 4 * 4;   // each stream's padded signal 16-byte aligned
     }
     CUDA_OK(cudaSetDevice(m->device));
-    reserve_pcm(in_off[b], pad_off[b]);
+    enc.prepare_pcm(*this, lens, b, true);
     std::vector<int> order(b);
     for (int s = 0; s < b; ++s) order[s] = s;
     std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return g[x].n_out > g[y].n_out; });
@@ -1156,20 +1003,11 @@ void Session::transcribe_ragged(const float *samples, const size_t *lens, int b,
         for (int w = 0; w < W; ++w) row_streams[(size_t)i * W + w] = order[i];
     }
 
-    front.frames = T;
-    front.padded.resize(b);
-    for (int s = 0; s < b; ++s) front.padded[s] = g[s].padded;
-    front.pad_off.assign(pad_off.begin(), pad_off.end() - 1);
     CUDA_OK(cudaEventRecord(ev[0], st));
-    CUDA_OK(cudaMemcpyAsync(pcm, samples, sizeof(float) * in_off[b], cudaMemcpyHostToDevice, st));
-    for (int s = 0, t0 = 0; s < b; t0 += T[s], ++s) {
-        launch_peak_normalize_pad(pcm + in_off[s], 1, lens[s], 0.95f, normalize, pcm_pad + pad_off[s], g[s].padded, left,
-                                  peak_scale + s, st);
-        launch_mel(pcm_pad + pad_off[s], 1, g[s].padded, g[s].padded, m->mel.window, m->mel.fb_vals, m->mel.fb_start,
-                   m->mel.fb_len, m->mel.fb_stride, mel_tm + (size_t)t0 * c.n_mels, T[s], 0, st);
-    }
+    enc.pcm_to_mel(*this, samples, nullptr, lens, b, normalize);
     CUDA_OK(cudaEventRecord(ev[1], st));
-    encode_ragged(b, T.data());
+    enc.encode(*this, b, enc.front.frames.data());
+    cur_B = b * W;   // the call's decoder rows, whose logits debug "logits" reads
     CUDA_OK(cudaEventRecord(ev[2], st));
 
     const int n_max = live > 0 ? g[order[0]].n_out : 0;

@@ -5,7 +5,6 @@
 
 #include <algorithm>
 #include <cstdint>
-#include <functional>
 #include <string>
 #include <tuple>
 #include <vector>
@@ -13,6 +12,7 @@
 #include "audio_host.h"
 #include "gguf.h"
 #include "decode_mega.h"
+#include "encoder.h"
 #include "kernels.h"
 #include "kv_cache.h"
 
@@ -96,14 +96,6 @@ void rope_rows(int hd, float theta, int64_t p0, int n, float *cos_out, float *si
 Q4Weight upload_q4(DeviceArena &arena, const std::vector<const uint8_t *> &raw, const std::vector<int> &n_rows,
                    int K, bool interleave, bool tc_layout = false);
 
-// What a transcribe call makes of one stream of n samples: the padded length (pad_audio), mel frames, audio positions
-// after the two stride-2 convolutions and the reshape, and decoder outputs (positions after the prefix; 0 when shorter).
-struct StreamGeom {
-    size_t padded = 0;
-    int frames = 0, S = 0, S4 = 0, n_out = 0;
-};
-StreamGeom stream_geometry(const vox_model_info &c, size_t n);
-
 // transcription delay of a new session or stream session, in tokens of 80 ms: the CLI default --delay 6
 // (transcribe.rs:49-51)
 constexpr float kDefaultDelay = 6.0f;
@@ -125,38 +117,15 @@ struct StepGraph {
 
 struct Session {
     Model *m = nullptr;
-    int max_batch = 0, max_mel_frames = 0;
-    int T1_max = 0, S_max = 0, S4_max = 0, M_max = 0;
+    int max_batch = 0, M_max = 0;
     cudaStream_t st = nullptr;
     DeviceArena arena;
     cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-    // audio
-    float *pcm = nullptr, *pcm_pad = nullptr, *peak_scale = nullptr;
-    size_t pcm_cap = 0, pcm_pad_cap = 0;
-    void reserve_pcm(size_t in_floats, size_t padded_floats);   // grows pcm / pcm_pad to hold that much
-    float *mel = nullptr;     // [B][128][T] as handed in by callers (reference layout)
-    float *mel_tm = nullptr;  // [B][T][128] time-major copy consumed by the conv1 implicit GEMM
-    // front end of the last call that started from PCM or from a caller's mel, for the "mel" / "pcm_pad" debug reads:
-    // per stream its mel frames (packed one after the other in mel_tm) and, from PCM, its padded length and offset in
-    // pcm_pad; a mel call leaves `padded` empty and its [B][128][T] input in `mel`
-    struct FrontEnd {
-        std::vector<int> frames;
-        std::vector<size_t> padded, pad_off;
-    } front;
-    // encoder workspace
-    float *h1 = nullptr, *x_enc = nullptr, *h_enc = nullptr, *qkv_enc = nullptr, *attn_enc = nullptr, *act_enc = nullptr;
-    float *packed = nullptr, *adapter_h = nullptr, *audio = nullptr;
+    // audio encoder (encoder.h): its buffers, the embeddings of the last encode, the debug capture
+    AudioEncoder enc;
     // read on the host only (argument checks, step counts, debug reads), never by a launch: rows of the last call's
-    // logits, and positions every stream of the last encode has audio embeddings for
-    int cur_B = 0, cur_S4 = 0;
-    // stream s's audio embedding of position p is at audio + audio_offs[s] + p * dec_dim, for the streams of the last
-    // encode (s * S4 * dec_dim; a ragged encode packs them one after the other) or the slots of a stream pool;
-    // audio_n: the embeddings of the last encode, all its streams together
-    std::vector<int64_t> audio_offs;
-    int audio_n = 0;
-    int enc_rows = 0;           // encoder rows of the last encode: B * S, or the sum of the streams' S of a ragged one
-    int *d_seg = nullptr;       // [max_batch + 1] encoder row of each stream's first frame (ragged encode)
-    std::vector<int> seg_host;
+    // logits
+    int cur_B = 0;
     // decoder
     DecoderKv kv;                         // of max_batch rows (vox_session_create_ex kv_dtype)
     RopeView dec_rope;                    // the model's tables, or an unbounded stream pool's ring
@@ -246,13 +215,8 @@ struct Session {
     void *xt_buf = nullptr;   // f16 split tiles feeding the wgmma GEMM
     size_t xt_elems = 0;
     GemmWork gemm_work;       // split-K scratch of the wgmma GEMM
-    bool use_enc_attn_tc = true;  // tensor-core encoder attention (VOX_ENC_ATTN=simt disables)
     // tensor-core matvec for M <= 8 (VOX_MATVEC=simt disables), wgmma GEMM for M > 8 (VOX_GEMM=simt disables)
     Q4Path path;
-    std::vector<float> enc_debug;  // per-layer captures when debugging is enabled
-    bool debug_capture = false;
-    float *dbg_layers = nullptr;   // [enc_layers][B*S][enc_dim]
-    float *dbg_conv = nullptr;
 
     // kv_ring: each row's decoder KV is a ring of pages (DecoderKv::create), and positions are unbounded (stream pools
     // with no length limit; the pool owner points dec_rope at its RoPE ring)
@@ -269,14 +233,6 @@ struct Session {
     // copy-free when no row's stream or offset has changed (so it may run inside a stream capture); a delay change
     // rewrites the sets in place and needs no new binding.
     void bind_rows(int B);
-    // mel already on device, time-major, in s->mel_tm
-    void encode(int B, int T);
-    // The encoder layers over `rows` rows of x_enc, then the final norm into h_enc.  attn(layer) is the step between the
-    // layer's wqkv and wo: RoPE and attention from qkv_enc into attn_enc.
-    void encoder_layers(int rows, const std::function<void(int)> &attn);
-    // that step for B streams of up to S rows each: one after the other S rows apart, or, with a segment table `seg`
-    // (device, [B + 1]), packed at seg[b]
-    void enc_rope_attention(int rows, int B, int S, const int *seg);
     // launch_q4_linear with the session's GEMM scratch and path choice; `gamma`, `tmp`, `tc` and `ada_rows` as there
     void linear(const Q4Weight &w, const float *x, int M, float *y, int ldy, const float *bias, const float *res,
                 int epi, const float *gamma = nullptr, float *tmp = nullptr, const TcWork *tc = nullptr,
@@ -302,11 +258,8 @@ struct Session {
     void step_incremental(int b, int M, const int *ids_host, bool add_audio);
     void check_batch(int b) const;
     void check_ids(const int32_t *ids, size_t n) const;
-    // runs prefill + loop; returns tokens per stream
+    // encodes the B streams of T mel frames in enc.mel_tm, then runs prefill + loop; returns tokens per stream
     int transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids, vox_timings *tm);
-    // encode() of b streams of T[s] mel frames packed one after the other in mel_tm: frames, conv rows, encoder rows
-    // (d_seg) and audio embeddings (audio_offs) packed by stream
-    void encode_ragged(int b, const int *T);
     // vox_transcribe_pcm_ragged after its argument checks: b streams of lens[s] host samples, one after the other;
     // n_out[s] ids of stream s after those of stream s - 1 in out_ids.  Records ev[0..4] like the other transcribe calls.
     void transcribe_ragged(const float *samples, const size_t *lens, int b, int normalize, int32_t *out_ids,

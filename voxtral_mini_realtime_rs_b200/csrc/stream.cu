@@ -191,20 +191,19 @@ StreamPool *StreamPool::create(Model *m, int max_sessions, float max_seconds, Kv
         // unbounded: the frame buffers get a few frames beyond the resident audio for the rows their consumers still read
         p->s = Session::create(m, max_sessions, unbounded ? cap_mel + 16 : cap_mel, unbounded, kv_type);
         Session *s = p->s;
-        VOX_CHECK(s->S_max <= m->enc_rope_len, VOX_EINVAL, "max_seconds exceeds the encoder RoPE table");
+        VOX_CHECK(s->enc.S_max <= m->enc_rope_len, VOX_EINVAL, "max_seconds exceeds the encoder RoPE table");
         p->max_new = 256;
         p->ring = c.enc_window + p->max_new;
         const int HQ = c.enc_heads * c.enc_head_dim;
         const size_t B = max_sessions;
         p->pcm = s->arena.alloc_n<float>(B * p->cap_samples);
-        p->enc_out = s->arena.alloc_n<float>(B * s->S_max * c.enc_dim);
+        p->enc_out = s->arena.alloc_n<float>(B * s->enc.S_max * c.enc_dim);
         const size_t ring_elems = (size_t)c.enc_layers * B * p->ring * HQ;
         p->ek = s->arena.alloc_n<float>(ring_elems);
         p->ev = s->arena.alloc_n<float>(ring_elems);
         const size_t max_rows = (size_t)B * p->max_new;
         p->d_row_slot = s->arena.alloc_n<int>(max_rows);
         p->d_row_pos = s->arena.alloc_n<int>(max_rows);
-        s->audio_offs.assign(B, 0);   // slot id's embeddings: audio + (id * S4_max - emb0) * dec_dim, set per launch
         if (unbounded) {
             const size_t enc_rows = B * p->ring * (c.enc_head_dim / 2), dec_rows = (size_t)kDecRopeRing * (c.dec_head_dim / 2);
             p->enc_rope_cos = s->arena.alloc_n<float>(enc_rows);
@@ -212,8 +211,9 @@ StreamPool *StreamPool::create(Model *m, int max_sessions, float max_seconds, Kv
             p->dec_rope_cos = s->arena.alloc_n<float>(dec_rows);
             p->dec_rope_sin = s->arena.alloc_n<float>(dec_rows);
             s->dec_rope = RopeView{p->dec_rope_cos, p->dec_rope_sin, kDecRopeRing};
-            const size_t most = std::max({p->cap_samples, (size_t)s->max_mel_frames * c.n_mels, (size_t)s->T1_max * c.enc_dim,
-                                          (size_t)s->S_max * c.enc_dim, (size_t)s->S4_max * c.dec_dim});
+            const AudioEncoder &e = s->enc;
+            const size_t most = std::max({p->cap_samples, (size_t)e.max_mel_frames * c.n_mels, (size_t)e.T1_max * c.enc_dim,
+                                          (size_t)e.S_max * c.enc_dim, (size_t)e.S4_max * c.dec_dim});
             p->slide_tmp = s->arena.alloc_n<float>(most);
         }
         p->slots.resize(max_sessions);
@@ -312,35 +312,33 @@ size_t StreamPool::poll(int id, int32_t *ids, int32_t *top_ids, float *top_lp, s
     return n;
 }
 
-// Encoder layers over `R` gathered rows in s->x_enc (Q4EncoderLayer::forward_with_cache, model.rs:300-315).
+// Encoder layers over `R` gathered rows in s->enc.x_enc (Q4EncoderLayer::forward_with_cache, model.rs:300-315).
 void StreamPool::encoder_rows(int R) {
     const vox_model_info &c = m->info;
     const int HQ = c.enc_heads * c.enc_head_dim;
     const float scale = powf((float)c.enc_head_dim, -0.5f);
     const size_t ring_stride = (size_t)max_sessions * ring * HQ;
-    s->encoder_layers(R, [&](int i) {
-        stream_rope_append_kernel<<<R, 256, 0, s->st>>>(s->qkv_enc, 3 * HQ, c.enc_heads, c.enc_head_dim, d_row_slot, d_row_pos,
+    s->enc.layers(*s, R, [&](int i) {
+        stream_rope_append_kernel<<<R, 256, 0, s->st>>>(s->enc.qkv_enc, 3 * HQ, c.enc_heads, c.enc_head_dim, d_row_slot, d_row_pos,
                                                         ek + i * ring_stride, ev + i * ring_stride, ring,
                                                         unbounded ? enc_rope_cos : m->enc_cos, unbounded ? enc_rope_sin : m->enc_sin,
                                                         unbounded);
         cuda_check(cudaGetLastError(), "stream_rope_append launch");
-        launch_stream_attn(s->qkv_enc, R, 3 * HQ, c.enc_heads, c.enc_head_dim, d_row_slot, d_row_pos, ek + i * ring_stride,
-                           ev + i * ring_stride, ring, c.enc_window, scale, s->attn_enc, s->st);
+        launch_stream_attn(s->enc.qkv_enc, R, 3 * HQ, c.enc_heads, c.enc_head_dim, d_row_slot, d_row_pos, ek + i * ring_stride,
+                           ev + i * ring_stride, ring, c.enc_window, scale, s->enc.attn_enc, s->st);
     });
 }
 
 // rows[i] = slot id of batch row i: page tables, positions and fed-back tokens of this launch; the rows' slots and
 // their audio offsets for the session to bind (Session::bind_rows: ADA sets and audio embeddings)
 void StreamPool::upload_rows(const std::vector<int> &rows, bool with_tokens) {
-    const vox_model_info &c = m->info;
     const int nb = (int)rows.size();
     std::vector<int> pos(nb), tok(nb), zero(nb, 0);
     for (int i = 0; i < nb; ++i) {
         const Slot &sl = slots[rows[i]];
         pos[i] = sl.pos;
         tok[i] = sl.last_tok;
-        // negative once the buffer has slid: position p's embedding sits at buffer row p - emb0
-        s->audio_offs[rows[i]] = ((int64_t)rows[i] * s->S4_max - sl.emb0) * c.dec_dim;
+        s->enc.set_slot_offset(rows[i], sl.emb0);
     }
     s->row_streams = rows;
     s->kv.bind(rows, s->st);
@@ -354,6 +352,7 @@ void StreamPool::tick(vox_stream_stats *st_out) {
     const vox_model_info &c = m->info;
     CUDA_OK(cudaSetDevice(m->device));
     const int d = c.enc_dim, D = c.dec_dim, rf = c.reshape_factor, P = c.prefix_len;
+    AudioEncoder &e = s->enc;
     vox_stream_stats stats{};
     s->rebase_epoch();  // between ticks: no decode step is in flight
     cudaEvent_t e0 = s->ev[0], e1 = s->ev[1];
@@ -361,7 +360,7 @@ void StreamPool::tick(vox_stream_stats *st_out) {
     bool more = true;
     while (more) {
         more = false;
-        // ---- front end: mel -> conv1 -> conv2 for every session, new encoder rows gathered into s->x_enc
+        // ---- front end: mel -> conv1 -> conv2 for every session, new encoder rows gathered into s->enc.x_enc
         std::vector<int> row_slot, row_pos;
         struct Span { int slot, r0, n; };
         std::vector<Span> spans;
@@ -376,19 +375,18 @@ void StreamPool::tick(vox_stream_stats *st_out) {
                 enc_t = sl.n_enc + max_new;
                 more = true;
             }
-            float *mel_s = s->mel_tm + (size_t)id * s->max_mel_frames * c.n_mels;
-            float *c1_s = s->h1 + (size_t)id * s->T1_max * d;
+            float *mel_s = e.slot_mel(id), *c1_s = e.slot_conv1(id);
             // each buffer keeps from the first row its consumer still reads: conv1 output t reads mel 2t-1..2t+1, conv2
             // output t reads conv1 2t-1..2t+1
             if (mel_t > sl.n_mel) {
-                slide(mel_s, c.n_mels, s->max_mel_frames, sl.mel0, std::max(0, 2 * sl.n_c1 - 1), sl.n_mel, mel_t, false, slide_tmp, s->st);
+                slide(mel_s, c.n_mels, e.max_mel_frames, sl.mel0, std::max(0, 2 * sl.n_c1 - 1), sl.n_mel, mel_t, false, slide_tmp, s->st);
                 launch_mel(pcm + (size_t)id * cap_samples, 1, sl.n_samples, cap_samples, m->mel.window, m->mel.fb_vals, m->mel.fb_start,
                            m->mel.fb_len, m->mel.fb_stride, mel_s, mel_t, 0, s->st, sl.n_mel, sl.pcm0, sl.mel0);
                 stats.mel_frames += mel_t - sl.n_mel;
                 sl.n_mel = mel_t;
             }
             if (c1_t > sl.n_c1) {
-                slide(c1_s, d, s->T1_max, sl.c10, std::max(0, 2 * sl.n_enc - 1), sl.n_c1, c1_t, false, slide_tmp, s->st);
+                slide(c1_s, d, e.T1_max, sl.c10, std::max(0, 2 * sl.n_enc - 1), sl.n_c1, c1_t, false, slide_tmp, s->st);
                 launch_conv2_gemm(mel_s, m->conv1_w, m->conv1_b, c1_s + (size_t)(sl.n_c1 - sl.c10) * d, 1, sl.n_mel, c1_t - sl.n_c1, c.n_mels,
                                   d, s->st, sl.n_c1, sl.mel0);
                 sl.n_c1 = c1_t;
@@ -396,7 +394,7 @@ void StreamPool::tick(vox_stream_stats *st_out) {
             const int n_new = enc_t - sl.n_enc;
             if (n_new > 0) {
                 const int r0 = (int)row_slot.size();
-                launch_conv2_gemm(c1_s, m->conv2_w, m->conv2_b, s->x_enc + (size_t)r0 * d, 1, sl.n_c1, n_new, d, d, s->st, sl.n_enc,
+                launch_conv2_gemm(c1_s, m->conv2_w, m->conv2_b, e.x_enc + (size_t)r0 * d, 1, sl.n_c1, n_new, d, d, s->st, sl.n_enc,
                                   sl.c10);
                 if (unbounded)
                     fill_rope(enc_rope_cos, enc_rope_sin, c.enc_head_dim, ring, (size_t)id * ring, sl.n_enc, n_new);
@@ -417,9 +415,9 @@ void StreamPool::tick(vox_stream_stats *st_out) {
             stats.encoder_rows += R;
             for (const Span &sp : spans) {
                 Slot &sl = slots[sp.slot];
-                float *eo = enc_out + (size_t)sp.slot * s->S_max * d;
-                slide(eo, d, s->S_max, sl.enc0, (int64_t)sl.n_emb * rf, sl.n_enc, sl.n_enc + sp.n, false, slide_tmp, s->st);
-                CUDA_OK(cudaMemcpyAsync(eo + (size_t)(sl.n_enc - sl.enc0) * d, s->h_enc + (size_t)sp.r0 * d,
+                float *eo = enc_out + (size_t)sp.slot * e.S_max * d;
+                slide(eo, d, e.S_max, sl.enc0, (int64_t)sl.n_emb * rf, sl.n_enc, sl.n_enc + sp.n, false, slide_tmp, s->st);
+                CUDA_OK(cudaMemcpyAsync(eo + (size_t)(sl.n_enc - sl.enc0) * d, e.h_enc + (size_t)sp.r0 * d,
                                         sizeof(float) * (size_t)sp.n * d, cudaMemcpyDeviceToDevice, s->st));
                 sl.n_enc += sp.n;
             }
@@ -430,14 +428,12 @@ void StreamPool::tick(vox_stream_stats *st_out) {
             if (!sl.open || sl.drained) continue;
             const int emb_t = sl.n_enc / rf, n_new = emb_t - sl.n_emb;
             if (n_new <= 0) continue;
-            const float *src = enc_out + ((size_t)id * s->S_max + ((size_t)sl.n_emb * rf - sl.enc0)) * d;
+            const float *src = enc_out + ((size_t)id * e.S_max + ((size_t)sl.n_emb * rf - sl.enc0)) * d;
             // embeddings stay resident for audio_embeds_range as long as they can: when the buffer is full, the older
             // half goes -- never one the decoder has still to read (position pos reads embedding pos)
-            float *emb = s->audio + (size_t)id * s->S4_max * D;
-            slide(emb, D, s->S4_max, sl.emb0, std::min<int64_t>(sl.pos, emb_t - s->S4_max / 2), sl.n_emb, emb_t, false, slide_tmp, s->st);
-            float *dst = emb + (size_t)(sl.n_emb - sl.emb0) * D;
-            s->linear(m->adapter0, src, n_new, s->adapter_h, D, nullptr, nullptr, EPI_GELU);
-            s->linear(m->adapter2, s->adapter_h, n_new, dst, D, nullptr, nullptr, EPI_NONE);
+            float *emb = e.slot_audio(id);
+            slide(emb, D, e.S4_max, sl.emb0, std::min<int64_t>(sl.pos, emb_t - e.S4_max / 2), sl.n_emb, emb_t, false, slide_tmp, s->st);
+            e.adapt(*s, src, n_new, emb + (size_t)(sl.n_emb - sl.emb0) * D);
             sl.n_emb = emb_t;
         }
         // ---- decoder: prefill of sessions whose 38 prefix positions have their audio (model.rs:883-923)
@@ -530,35 +526,34 @@ int StreamPool::encode_chunk(int id, const float *mel, int T, float *out, size_t
     Slot &sl = slot(id);
     VOX_CHECK(!unbounded, VOX_EINVAL, "encode_chunk needs a pool with max_seconds > 0 (its output region is linear)");
     VOX_CHECK(sl.n_samples == pad_left(pad) && sl.n_audio == 0, VOX_EINVAL, "stream session %d is fed by push(): do not mix with encode_chunk", id);
-    VOX_CHECK(T >= 1 && T <= s->max_mel_frames, VOX_EINVAL, "mel chunk of %d frames exceeds the pool's capacity %d", T, s->max_mel_frames);
+    AudioEncoder &e = s->enc;
+    VOX_CHECK(T >= 1 && T <= e.max_mel_frames, VOX_EINVAL, "mel chunk of %d frames exceeds the pool's capacity %d", T, e.max_mel_frames);
     CUDA_OK(cudaSetDevice(m->device));
     const int d = c.enc_dim, D = c.dec_dim, rf = c.reshape_factor;
     const int T1 = conv_out(T), S = conv_out(T1), S4 = S / rf;
     VOX_CHECK(sl.n_enc + S <= m->enc_rope_len, VOX_ECAPACITY, "encoder positions %d exceed the RoPE table (%d)", sl.n_enc + S, m->enc_rope_len);
     VOX_CHECK(cap >= (size_t)S4 * D, VOX_ECAPACITY, "audio_embeds capacity %zu < %zu", cap, (size_t)S4 * D);
-    CUDA_OK(cudaMemcpyAsync(s->mel, mel, sizeof(float) * (size_t)c.n_mels * T, cudaMemcpyHostToDevice, s->st));
-    launch_transpose_mel(s->mel, s->mel_tm, 1, c.n_mels, T, s->st);
-    launch_conv2_gemm(s->mel_tm, m->conv1_w, m->conv1_b, s->h1, 1, T, T1, c.n_mels, d, s->st);
+    e.upload_mel(*s, mel, 1, T);
+    launch_conv2_gemm(e.mel_tm, m->conv1_w, m->conv1_b, e.h1, 1, T, T1, c.n_mels, d, s->st);
     // rows beyond the ring slack go through the layers in several passes; the conv output of the whole chunk waits in
     // the session's (otherwise unused in chunk mode) encoder-output region
-    float *conv = enc_out + (size_t)id * s->S_max * d;
-    launch_conv2_gemm(s->h1, m->conv2_w, m->conv2_b, conv, 1, T1, S, d, d, s->st);
+    float *conv = enc_out + (size_t)id * e.S_max * d;
+    launch_conv2_gemm(e.h1, m->conv2_w, m->conv2_b, conv, 1, T1, S, d, d, s->st);
     for (int r0 = 0; r0 < S; r0 += max_new) {
         const int R = std::min(max_new, S - r0);
         std::vector<int> rs(R, id), rp(R);
         for (int i = 0; i < R; ++i) rp[i] = sl.n_enc + r0 + i;
-        CUDA_OK(cudaMemcpyAsync(s->x_enc, conv + (size_t)r0 * d, sizeof(float) * (size_t)R * d, cudaMemcpyDeviceToDevice, s->st));
+        CUDA_OK(cudaMemcpyAsync(e.x_enc, conv + (size_t)r0 * d, sizeof(float) * (size_t)R * d, cudaMemcpyDeviceToDevice, s->st));
         CUDA_OK(cudaMemcpyAsync(d_row_slot, rs.data(), sizeof(int) * R, cudaMemcpyHostToDevice, s->st));
         CUDA_OK(cudaMemcpyAsync(d_row_pos, rp.data(), sizeof(int) * R, cudaMemcpyHostToDevice, s->st));
         CUDA_OK(cudaStreamSynchronize(s->st));
         encoder_rows(R);
-        CUDA_OK(cudaMemcpyAsync(s->packed + (size_t)r0 * d, s->h_enc, sizeof(float) * (size_t)R * d, cudaMemcpyDeviceToDevice, s->st));
+        CUDA_OK(cudaMemcpyAsync(e.packed + (size_t)r0 * d, e.h_enc, sizeof(float) * (size_t)R * d, cudaMemcpyDeviceToDevice, s->st));
     }
     sl.n_enc += S;
     if (S4 > 0) {
-        s->linear(m->adapter0, s->packed, S4, s->adapter_h, D, nullptr, nullptr, EPI_GELU);
-        s->linear(m->adapter2, s->adapter_h, S4, s->audio, D, nullptr, nullptr, EPI_NONE);
-        CUDA_OK(cudaMemcpyAsync(out, s->audio, sizeof(float) * (size_t)S4 * D, cudaMemcpyDeviceToHost, s->st));
+        e.adapt(*s, e.packed, S4, e.audio);
+        CUDA_OK(cudaMemcpyAsync(out, e.audio, sizeof(float) * (size_t)S4 * D, cudaMemcpyDeviceToHost, s->st));
     }
     CUDA_OK(cudaStreamSynchronize(s->st));
     return S4;
@@ -575,7 +570,7 @@ const float *StreamPool::audio_embeds(int id, int *n) {
     VOX_CHECK(sl.emb0 == 0, VOX_ECAPACITY, "stream session %d: audio embeddings before %d were evicted; use vox_stream_audio_embeds_range",
               id, sl.emb0);
     *n = sl.n_emb;
-    return s->audio + (size_t)id * s->S4_max * m->info.dec_dim;
+    return s->enc.slot_audio(id);
 }
 
 const float *StreamPool::audio_embeds_range(int id, int64_t first, int64_t n) {
@@ -584,7 +579,7 @@ const float *StreamPool::audio_embeds_range(int id, int64_t first, int64_t n) {
               id, (long long)first, (long long)(first + n), sl.n_emb);
     VOX_CHECK(first >= sl.emb0, VOX_ECAPACITY, "stream session %d: audio embedding %lld is no longer resident (first resident: %d)", id,
               (long long)first, sl.emb0);
-    return s->audio + ((size_t)id * s->S4_max + (size_t)(first - sl.emb0)) * m->info.dec_dim;
+    return s->enc.slot_audio(id) + (size_t)(first - sl.emb0) * m->info.dec_dim;
 }
 
 const float *StreamPool::mel_range(int id, int64_t first, int64_t n) {
@@ -593,7 +588,7 @@ const float *StreamPool::mel_range(int id, int64_t first, int64_t n) {
               id, (long long)first, (long long)(first + n), sl.n_mel);
     VOX_CHECK(first >= sl.mel0, VOX_ECAPACITY, "stream session %d: mel frame %lld is no longer resident (first resident: %d)", id,
               (long long)first, sl.mel0);
-    return s->mel_tm + ((size_t)id * s->max_mel_frames + (size_t)(first - sl.mel0)) * m->info.n_mels;
+    return s->enc.slot_mel(id) + (size_t)(first - sl.mel0) * m->info.n_mels;
 }
 
 void StreamPool::session_info(int id, struct vox_stream_session_info *out) {
