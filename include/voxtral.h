@@ -140,6 +140,42 @@ int32_t vox_q4_linear(const vox_q4 *w, const float *x_dev, float *y_dev, int32_t
                       const float *const *ada_dev, int32_t ada_m, const float *ssq_in_dev, float *ssq_out_dev,
                       void *stream);
 void vox_q4_tensor_free(vox_q4 *w);
+
+/* ------------------------------------------------------------------ attention operator seam
+ * Encoder attention (model.rs:77-122, masking.rs:9-107): for every (stream, head), query i attends to key j iff
+ * j <= i and i - j <= window, out = softmax(scale * q k^T) v.  All pointers are device pointers.
+ *   VOX_ATTN_ENC_TC   K4-TC (enc_attn_tc.cu), the encoder's production kernel;
+ *   VOX_ATTN_ENC_SIMT K4 (kernels.cu), its f32 SIMT cross-check;
+ *   VOX_ATTN_STREAM   K4-S (stream.cu), the streaming pools' attention over per-session K/V rings.
+ * Encoder kernels: stream t's rows are b * s + [0, s), or seg[t] .. seg[t + 1] - 1 when seg ([b + 1] ints) is given
+ * (then s is the longest stream); row r's q, k and v of head hh start at qkv + r * ld + {q,k,v}_off + hh * hd, and its
+ * output at out + r * h * hd + hh * hd.
+ * Ring kernel: row r (r < rows) is query position row_pos[r] of session row_slot[r]; its q of head hh starts at
+ * qkv + r * ld + hh * hd; key position p of that session is slot p % ring of k_ring / v_ring, [slots][ring][h * hd];
+ * its output is out + r * h * hd + hh * hd.  The caller keeps every key a row can see in the ring.
+ * The named kernel runs and no other.  Refused with VOX_EINVAL (vox_last_error says why): an unknown kernel, a null
+ * pointer the kernel reads, b, s, rows or h below 1, a negative window, operands that do not fit in ld; K4-TC: hd not
+ * 32 or 64, ld or an offset not a multiple of 4, qkv not 16-byte aligned; K4: hd not 32, 64 or 128; K4-S: hd not 32,
+ * 64 or 128, ring < 1 or window >= ring. */
+#define VOX_ATTN_ENC_TC 0
+#define VOX_ATTN_ENC_SIMT 1
+#define VOX_ATTN_STREAM 2
+typedef struct vox_attn_args {
+    const float *qkv;
+    int32_t ld;
+    int32_t q_off, k_off, v_off;          /* encoder kernels */
+    int32_t b, s, h, hd;                  /* b and s: encoder kernels */
+    const int32_t *seg;                   /* encoder kernels, nullable */
+    int32_t rows;                         /* ring kernel */
+    const int32_t *row_slot, *row_pos;    /* ring kernel, [rows] each */
+    const float *k_ring, *v_ring;         /* ring kernel */
+    int32_t ring;                         /* ring kernel */
+    int32_t window;
+    float scale;
+    float *out;
+} vox_attn_args;
+int32_t vox_attention(int32_t device, int32_t kernel, const vox_attn_args *args, void *stream);
+
 /* kernel selection of the operator seam (bit mask, default 0): bit 0 = SIMT warp-reduce matvec instead of
  * the tensor-core-assisted one (M <= 8); bit 1 = SIMT tiled GEMM instead of the wgmma GEMM (M > 8).
  * All implement the same contract; exposed for A/B measurement and parity tests. */

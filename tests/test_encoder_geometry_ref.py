@@ -11,7 +11,7 @@ the bounds that test imports.
     every f32 operand as two f16 pieces (hi + lo).  Keeping only hi -- Q, K, V and the softmax probabilities rounded to
     one f16 piece (against ENC_LAYER_REL_BOUND, the bound of the paths that check the attention kernels with the SIMT
     GEMM), or separately the normed operand of the Q/K/V and w1/w3 GEMMs (against WGMMA_LAYER_REL_BOUND) -- moves one
-    layer's output by > PIECE_SEPARATION x that bound (see the finding below the bounds).
+    layer's output by > PIECE_SEPARATION x that bound (see the note below the bounds).
 
 Errors are reported as max |got - ref| / max(1, max |ref|) over the whole compared tensor.
 """
@@ -35,10 +35,12 @@ WGMMA_LAYER_REL_BOUND = 7.5e-5 # a layer whose linears run the wgmma GEMM [2.45e
 ADAPTER_REL_BOUND = 1.3e-5     # adapter, fed the GPU's own encoder output [4.3e-6]
 EMBED_REL_BOUND = 3.5e-5       # audio embeddings end to end from the mel [1.1e-5 full size; 5.3e-6 at 2 layers]
 SEPARATION = 10                # the window pins exceed ENC_LAYER_REL_BOUND by at least this factor
-# Finding: the one-f16-piece pins do NOT reach SEPARATION.  Losing the low piece of Q/K/V/P moves layer 1 by 5.2e-5 =
-# 4.3x ENC_LAYER_REL_BOUND; losing the low piece of the normed GEMM operand moves a layer by >= 1.85e-4 = 2.5x
-# WGMMA_LAYER_REL_BOUND.  The wgmma GEMM's per-layer error is ~7x the SIMT GEMM's and shrinks when K is split into
-# slices, which points at its f32 accumulation over long K.  Until that is tightened, these pins hold at:
+# The one-f16-piece pins do not reach SEPARATION at layer level: losing the low piece of Q/K/V/P moves layer 1 by
+# 5.2e-5 = 4.3x ENC_LAYER_REL_BOUND, and losing the low piece of the normed GEMM operand moves a layer by >= 1.85e-4 =
+# 2.5x WGMMA_LAYER_REL_BOUND.  The attention's four pieces are pinned at operator level instead, each at >= 59x its
+# per-output bound (tests/test_attention_ref.py, test_planted_mistake_exceeds_the_bound; tests/test_attention_gpu.py
+# holds the kernels to that bound).  The wgmma GEMM's per-layer error is ~7x the SIMT GEMM's and shrinks when K is
+# split into slices, which points at its f32 accumulation over long K.  At layer level these pins hold at:
 PIECE_SEPARATION = 2
 
 GEOMETRY_SEED = 5

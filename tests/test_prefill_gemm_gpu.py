@@ -11,7 +11,8 @@ equal (split tiles are summed in slice order).
 
 Model level: on synth.decoder_geometry_config, a teacher-forced 38-row pass per stream (vox_generate_step_with_cache,
 the prefill's shapes: M = 38 * B through wqkv, wo and w2 with the in-place residual, w13 with SiLU * up) agrees with
-OracleModel(dtype=float64) within LOGIT_REL_BOUND at every one of the 38 rows, for B = 1..8.
+OracleModel(dtype=float64) within LOGIT_REL_BOUND at every one of the 38 rows, for B = 1..8 at decoder window 8192, and
+at B = 1, 3 and 8 at windows 40 and 8, where the mask of dec_attention_kernel bites inside the 38 prefill rows.
 """
 import numpy as np
 import pytest
@@ -61,16 +62,26 @@ def test_k3_matches_f64(vx, weights, name, m):
 
 @pytest.fixture(scope="module")
 def geometry(vx):
-    data = geometry_model_bytes(8192)
-    model = vx.Q4ModelLoader.from_bytes(data).load(0, max_batch=8, max_mel_frames=1200)
-    o64 = OracleModel(data, dtype=torch.float64)
-    yield model, o64
-    model.close()
+    """one model at a time, by decoder window"""
+    held = {}
+
+    def get(window):
+        if window not in held:
+            for m, _ in held.values():
+                m.close()
+            held.clear()
+            data = geometry_model_bytes(window)
+            held[window] = (vx.Q4ModelLoader.from_bytes(data).load(0, max_batch=8, max_mel_frames=1200),
+                            OracleModel(data, dtype=torch.float64))
+        return held[window]
+    yield get
+    for m, _ in held.values():
+        m.close()
 
 
-@pytest.mark.parametrize("B", range(1, 9))
-def test_prefill_rows_match_f64(geometry, B):
-    model, o64 = geometry
+@pytest.mark.parametrize("window,B", [(8192, b) for b in range(1, 9)] + [(w, b) for w in (40, 8) for b in (1, 3, 8)])
+def test_prefill_rows_match_f64(geometry, window, B):
+    model, o64 = geometry(window)
     vocab = model.info["vocab"]
     rng = np.random.default_rng(B)
     ids = rng.integers(0, vocab, (B, PREFIX_LEN)).astype(np.int32)

@@ -103,6 +103,7 @@ _SIGS = {
     "vox_q4_linear": (C.c_int32, [_P, _P, _P, C.c_int32, C.c_int32, _P, _P, C.c_int32, _P, C.c_float, _P,
                                   C.c_int32, _P, _P, _P]),
     "vox_q4_tensor_free": (None, [_P]),
+    "vox_attention": (C.c_int32, [C.c_int32, C.c_int32, _P, _P]),
     "vox_q4_set_matvec_mode": (C.c_int32, [C.c_int32]),
     "vox_dev_malloc": (C.c_int32, [C.c_int32, C.c_size_t, C.POINTER(_P)]),
     "vox_dev_free": (C.c_int32, [C.c_int32, _P]),
@@ -621,6 +622,59 @@ def q4_linear(weights: Q4Tensor, x, epi: str = "none", *, bias=None, res=None, g
     if ssq_out is not None:
         return out, ssq_out.to_numpy(np.float32, ssq_shape)
     return out
+
+
+ATTN_KERNELS = {"tc": 0, "simt": 1, "stream": 2}   # include/voxtral.h VOX_ATTN_*
+
+
+class _AttnArgs(C.Structure):
+    _fields_ = [("qkv", _P), ("ld", C.c_int32), ("q_off", C.c_int32), ("k_off", C.c_int32), ("v_off", C.c_int32),
+                ("b", C.c_int32), ("s", C.c_int32), ("h", C.c_int32), ("hd", C.c_int32), ("seg", _P),
+                ("rows", C.c_int32), ("row_slot", _P), ("row_pos", _P), ("k_ring", _P), ("v_ring", _P),
+                ("ring", C.c_int32), ("window", C.c_int32), ("scale", C.c_float), ("out", _P)]
+
+
+def attention(kernel: str, qkv, h: int, hd: int, window: int, scale: float, *, q_off: int = 0, k_off: int = 0,
+              v_off: int = 0, b: int = 1, s: int | None = None, seg=None, row_slot=None, row_pos=None, k_ring=None,
+              v_ring=None, out_rows: int | None = None, sentinel: float = float("nan"), device: int = 0) -> np.ndarray:
+    """One encoder attention launch (vox_attention) on host arrays, on the named kernel ("tc", "simt" or "stream").
+
+    qkv [rows, ld]: for "tc" / "simt" the q, k and v of head hh at columns {q,k,v}_off + hh * hd of each row; b
+    streams of s rows each, or the ragged streams seg[t] .. seg[t + 1] - 1 ([b + 1] offsets; s defaults to the longest).
+    For "stream", row r is query position row_pos[r] of session row_slot[r], with q at columns hh * hd; k_ring / v_ring
+    [slots, ring, h * hd] hold key position p at p % ring.  out is an [out_rows, h * hd] device buffer (default: the
+    rows of qkv) pre-filled with `sentinel`, returned whole."""
+    qkv = _f32(qkv)
+    rows, ld = qkv.shape
+    keep = []
+
+    def up(a, dtype):
+        if a is None:
+            return None
+        buf = DeviceBuffer.from_numpy(np.ascontiguousarray(a, dtype), device)
+        keep.append(buf)
+        return buf.ptr
+
+    a = _AttnArgs(qkv=up(qkv, np.float32), ld=ld, h=h, hd=hd, window=window, scale=scale)
+    if kernel == "stream":
+        k_ring = _f32(k_ring)
+        a.rows, a.ring = rows, k_ring.shape[1]
+        a.row_slot, a.row_pos = up(row_slot, np.int32), up(row_pos, np.int32)
+        a.k_ring, a.v_ring = up(k_ring, np.float32), up(v_ring, np.float32)
+    else:
+        a.q_off, a.k_off, a.v_off, a.b = q_off, k_off, v_off, b
+        if seg is not None:
+            seg = np.asarray(seg, np.int32)
+            a.seg = up(seg, np.int32)
+            s = int(np.diff(seg).max()) if s is None else s
+        a.s = rows // b if s is None else s
+    out_rows = rows if out_rows is None else out_rows
+    out = DeviceBuffer.from_numpy(np.full((out_rows, h * hd), sentinel, np.float32), device)
+    keep.append(out)
+    a.out = out.ptr
+    _check(lib().vox_attention(device, ATTN_KERNELS[kernel], C.byref(a), None))
+    _check(lib().vox_dev_sync(device))
+    return out.to_numpy(np.float32, (out_rows, h * hd))
 
 
 class Q4Linear:

@@ -425,6 +425,50 @@ void vox_q4_tensor_free(vox_q4 *w) {
     delete w;
 }
 
+int32_t vox_attention(int32_t device, int32_t kernel, const vox_attn_args *a, void *stream) {
+    VOX_API_BEGIN
+    REQUIRE(a);
+    VOX_CHECK(kernel >= VOX_ATTN_ENC_TC && kernel <= VOX_ATTN_STREAM, VOX_EINVAL, "attention: kernel %d is not one of 0..2",
+              kernel);
+    VOX_CHECK(a->qkv && a->out, VOX_EINVAL, "attention: qkv and out are required");
+    VOX_CHECK(a->h >= 1, VOX_EINVAL, "attention: h=%d must be positive", a->h);
+    VOX_CHECK(a->window >= 0, VOX_EINVAL, "attention: window=%d is negative", a->window);
+    const int hd = a->hd, hq = a->h * a->hd;
+    if (kernel == VOX_ATTN_STREAM) {
+        VOX_CHECK(hd == 32 || hd == 64 || hd == 128, VOX_EINVAL, "attention: the ring kernel takes hd 32, 64 or 128, not %d", hd);
+        VOX_CHECK(a->rows >= 1, VOX_EINVAL, "attention: rows=%d must be positive", a->rows);
+        VOX_CHECK(a->row_slot && a->row_pos && a->k_ring && a->v_ring, VOX_EINVAL,
+                  "attention: the ring kernel needs row_slot, row_pos, k_ring and v_ring");
+        VOX_CHECK(a->ld >= hq, VOX_EINVAL, "attention: ld=%d < h*hd=%d", a->ld, hq);
+        VOX_CHECK(a->ring >= 1 && a->window < a->ring, VOX_EINVAL,
+                  "attention: window=%d must be below ring=%d (keys older than the ring are overwritten)", a->window, a->ring);
+    } else {
+        const bool tc = kernel == VOX_ATTN_ENC_TC;
+        if (tc)
+            VOX_CHECK(hd == 32 || hd == 64, VOX_EINVAL, "attention: K4-TC takes hd 32 or 64, not %d", hd);
+        else
+            VOX_CHECK(hd == 32 || hd == 64 || hd == 128, VOX_EINVAL, "attention: K4 takes hd 32, 64 or 128, not %d", hd);
+        VOX_CHECK(a->b >= 1 && a->s >= 1, VOX_EINVAL, "attention: b=%d and s=%d must be positive", a->b, a->s);
+        for (const int off : {a->q_off, a->k_off, a->v_off})
+            VOX_CHECK(off >= 0 && off + hq <= a->ld, VOX_EINVAL, "attention: an operand at column %d of h*hd=%d does not fit in ld=%d",
+                      off, hq, a->ld);
+        VOX_CHECK(!tc || enc_attention_tc_supported(hd, a->ld, a->q_off, a->k_off, a->v_off), VOX_EINVAL,
+                  "attention: K4-TC loads float4s: ld=%d and the offsets (%d, %d, %d) must be multiples of 4", a->ld,
+                  a->q_off, a->k_off, a->v_off);
+        VOX_CHECK(!tc || (reinterpret_cast<uintptr_t>(a->qkv) & 15) == 0, VOX_EINVAL,
+                  "attention: K4-TC loads float4s: qkv must be 16-byte aligned");
+    }
+    require_device(device);
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (kernel == VOX_ATTN_STREAM)
+        launch_stream_attn(a->qkv, a->rows, a->ld, a->h, hd, a->row_slot, a->row_pos, a->k_ring, a->v_ring, a->ring,
+                           a->window, a->scale, a->out, st);
+    else
+        (kernel == VOX_ATTN_ENC_TC ? launch_enc_attention_tc : launch_enc_attention)(
+            a->qkv, a->out, a->b, a->s, a->h, hd, a->ld, a->q_off, a->k_off, a->v_off, a->window, a->scale, st, a->seg);
+    VOX_API_END
+}
+
 int32_t vox_dev_malloc(int32_t device, size_t bytes, void **p) {
     VOX_API_BEGIN
     REQUIRE(p);

@@ -4,10 +4,19 @@
 //
 // Flash-attention-2 data flow with mma.sync.m16n8k16 (f16 x f16 -> f32):
 //   CTA = 64 queries of one (stream, head), 4 warps x 16 query rows; key tiles of 64.
-//   Every f32 operand is split into two f16 pieces  x = hi + lo  (hi = f16(x), lo = f16(x - hi),
-//   22 mantissa bits) and every product is three MMAs  hi.hi + hi.lo + lo.hi  with f32 accumulation:
-//   the dropped lo.lo term is 2^-22 relative, below the f32 rounding of the dot products themselves
-//   (the SIMT kernel K4 in kernels.cu is the f32 cross-check; tests compare both against the oracle).
+//   Every f32 operand is split into two f16 pieces  x = hi + lo  (hi = f16(x), lo = f16(x - hi))
+//   and every product is three MMAs  hi.hi + hi.lo + lo.hi  with f32 accumulation.  The pieces carry
+//   22 mantissa bits only while lo stays in f16's normal range and hi below 65504, so each operand is
+//   first scaled by an exact power of two that brings its largest magnitude into [2^14, 2^15):
+//   Q per query row, K per key tile, P (in [0, 1]) by 2^15, and V by the running maximum over the
+//   key tiles the CTA has loaded (o is only ever scaled down, so it cannot overflow).  Keys no query
+//   of the CTA can see are loaded as zeros and do not count towards these maxima.  The S tile's
+//   factors are undone with `scale`, V's and P's as o is rescaled and stored.  So, whatever the
+//   overall scale of the operands, the representation error and the dropped lo.lo term are 2^-22
+//   relative to each operand, or 2^-39 relative to the largest Q of its row, K of its tile or V the
+//   CTA has loaded, whichever is larger: elements far below the largest in the same tile or block
+//   lose relative precision (tests/test_attention_ref.py models this arithmetic and bounds it; the
+//   SIMT kernel K4 in kernels.cu is the f32 cross-check).
 //   S = Q K^T : A = Q fragments (registers, loaded once), B = K tile [key][dim] from shared memory
 //               (ldmatrix, rows padded to 72 halves: conflict-free);
 //   online softmax in f32 registers (scale and mask applied to the f32 scores, exp in f32);
@@ -28,6 +37,7 @@ void tc_count_launch(const char *name);
 namespace {
 
 constexpr int ET_BQ = 64, ET_BK = 64, ET_THREADS = 128;
+constexpr float P_SCALE = 32768.0f;  // 2^15: softmax probabilities are split as P * 2^15
 constexpr int ET_PAD = 8;  // halves of row padding: row stride = HD + 8 halves (144 B for HD = 64)
 
 __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], const uint32_t b0, const uint32_t b1) {
@@ -56,6 +66,18 @@ __device__ __forceinline__ void split2(const float x, const float y, uint32_t &h
     hi = *reinterpret_cast<const uint32_t *>(&h);
     lo = *reinterpret_cast<const uint32_t *>(&l);
 }
+// 2^k for k in [-126, 127]
+__device__ __forceinline__ float pow2f(const int k) { return __uint_as_float((uint32_t)(k + 127) << 23); }
+// k such that 2^k maps m = max |x| into [2^14, 2^15), clamped to [-126, 126] so that 2^k and 2^-k are normal;
+// `keep` when m is 0 or not finite
+__device__ __forceinline__ int split_exp(const float m, const int keep) {
+    const int e = (int)((__float_as_uint(m) >> 23) & 0xff);
+    if (!(m > 0.0f) || e == 0xff) return keep;
+    return min(max(14 - (e - 127), -126), 126);
+}
+__device__ __forceinline__ float absmax4(const float a, const float b, const float c, const float d) {
+    return fmaxf(fmaxf(fabsf(a), fabsf(b)), fmaxf(fabsf(c), fabsf(d)));
+}
 
 template <int HD>
 __global__ void __launch_bounds__(ET_THREADS)
@@ -65,7 +87,10 @@ enc_attention_tc_kernel(const float *__restrict__ qkv, float *__restrict__ out, 
     constexpr int STR = HD + ET_PAD;  // halves per shared-memory row
     constexpr int KS = HD / 16;       // k-steps of Q K^T
     constexpr int ND = HD / 8;        // n-tiles of the output
+    constexpr int RL = HD / 4;        // threads per key row of the tile load (one float4 each)
+    constexpr int IT = ET_BK * RL / ET_THREADS;  // key rows each thread loads per tile
     __shared__ __align__(16) __half Kh[ET_BK * STR], Kl[ET_BK * STR], Vh[ET_BK * STR], Vl[ET_BK * STR];
+    __shared__ float tile_max[2][ET_THREADS / 32];  // per-warp max |k|, max |v| of the tile being loaded
     const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * ET_BQ;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int g = lane >> 2, t = lane & 3;
@@ -74,58 +99,106 @@ enc_attention_tc_kernel(const float *__restrict__ qkv, float *__restrict__ out, 
     if (q0 >= S) return;   // the grid covers the longest segment
     const float *base = qkv + (size_t)row0 * ld;
 
-    // ---- Q fragments (A operand), hi and lo pieces: rows q0 + 16*warp + {g, g+8}
+    // ---- Q fragments (A operand), hi and lo pieces: rows q0 + 16*warp + {g, g+8}, each row scaled by its power of two
+    //      (a row's elements sit in the 4 lanes of a quad)
     const int qr0 = q0 + warp * 16 + g, qr1 = qr0 + 8;
-    uint32_t qh[KS][4], ql[KS][4];
+    float2 qv[KS][4];
+    float qm0 = 0.0f, qm1 = 0.0f;
 #pragma unroll
     for (int ks = 0; ks < KS; ++ks) {
-        float2 v00 = make_float2(0.f, 0.f), v10 = v00, v01 = v00, v11 = v00;
+        qv[ks][0] = qv[ks][1] = qv[ks][2] = qv[ks][3] = make_float2(0.f, 0.f);
         if (qr0 < S) {
             const float *r = base + (size_t)qr0 * ld + q_off + h * HD + ks * 16 + 2 * t;
-            v00 = *reinterpret_cast<const float2 *>(r);
-            v01 = *reinterpret_cast<const float2 *>(r + 8);
+            qv[ks][0] = *reinterpret_cast<const float2 *>(r);
+            qv[ks][2] = *reinterpret_cast<const float2 *>(r + 8);
         }
         if (qr1 < S) {
             const float *r = base + (size_t)qr1 * ld + q_off + h * HD + ks * 16 + 2 * t;
-            v10 = *reinterpret_cast<const float2 *>(r);
-            v11 = *reinterpret_cast<const float2 *>(r + 8);
+            qv[ks][1] = *reinterpret_cast<const float2 *>(r);
+            qv[ks][3] = *reinterpret_cast<const float2 *>(r + 8);
         }
-        split2(v00.x, v00.y, qh[ks][0], ql[ks][0]);
-        split2(v10.x, v10.y, qh[ks][1], ql[ks][1]);
-        split2(v01.x, v01.y, qh[ks][2], ql[ks][2]);
-        split2(v11.x, v11.y, qh[ks][3], ql[ks][3]);
+        qm0 = fmaxf(qm0, absmax4(qv[ks][0].x, qv[ks][0].y, qv[ks][2].x, qv[ks][2].y));
+        qm1 = fmaxf(qm1, absmax4(qv[ks][1].x, qv[ks][1].y, qv[ks][3].x, qv[ks][3].y));
     }
+#pragma unroll
+    for (int x = 1; x <= 2; x <<= 1) {
+        qm0 = fmaxf(qm0, __shfl_xor_sync(0xffffffffu, qm0, x));
+        qm1 = fmaxf(qm1, __shfl_xor_sync(0xffffffffu, qm1, x));
+    }
+    const int eq0 = split_exp(qm0, 0), eq1 = split_exp(qm1, 0);
+    const float fq[4] = {pow2f(eq0), pow2f(eq1), pow2f(eq0), pow2f(eq1)};
+    // the rows' score factors: scale and the rows' Q powers of two undone (exactly: powers of two)
+    const float sc0 = scale * pow2f(-eq0), sc1 = scale * pow2f(-eq1);
+    uint32_t qh[KS][4], ql[KS][4];
+#pragma unroll
+    for (int ks = 0; ks < KS; ++ks)
+#pragma unroll
+        for (int a = 0; a < 4; ++a) split2(qv[ks][a].x * fq[a], qv[ks][a].y * fq[a], qh[ks][a], ql[ks][a]);
 
     float o[ND][4];
 #pragma unroll
     for (int n = 0; n < ND; ++n) o[n][0] = o[n][1] = o[n][2] = o[n][3] = 0.0f;
     float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.0f, 0.0f};
+    int ev_run = 126;  // o holds P V * 2^(15 + ev_run): P scaled by 2^15, V by the running power of two (never raised)
 
     const int q_last = min(q0 + ET_BQ - 1, S - 1);
-    int j_begin = q0 - window;
+    const int key_lo = q0 - window;  // keys [key_lo, q_last]: the keys some query of this CTA can see
+    int j_begin = key_lo;
     if (j_begin < 0) j_begin = 0;
     j_begin = (j_begin / ET_BK) * ET_BK;
     for (int j0 = j_begin; j0 <= q_last; j0 += ET_BK) {
         __syncthreads();  // previous tile fully consumed
-        // ---- K, V tile: f32 global -> f16 hi/lo shared, [key][dim]
-        for (int i = tid; i < ET_BK * (HD / 4); i += ET_THREADS) {
-            const int kk = i / (HD / 4), d4 = (i - kk * (HD / 4)) * 4;
-            const int gj = j0 + kk;
+        // ---- K, V tile: f32 global -> f16 hi/lo shared, [key][dim]; K scaled by the tile's power of two, V by the running
+        //      one.  Keys outside [key_lo, q_last] load as zeros.  A first pass takes the block-wide maxima; the split
+        //      pass reads the tile again (from L1).
+        float km = 0.0f, vm = 0.0f;
+#pragma unroll 2
+        for (int it = 0; it < IT; ++it) {
+            const int i = tid + it * ET_THREADS;
+            const int kk = i / RL, d4 = (i - kk * RL) * 4;
+            if (j0 + kk >= key_lo && j0 + kk <= q_last) {
+                const float *r = base + (size_t)(j0 + kk) * ld + h * HD + d4;
+                const float4 kv = *reinterpret_cast<const float4 *>(r + k_off), vv = *reinterpret_cast<const float4 *>(r + v_off);
+                km = fmaxf(km, absmax4(kv.x, kv.y, kv.z, kv.w));
+                vm = fmaxf(vm, absmax4(vv.x, vv.y, vv.z, vv.w));
+            }
+        }
+#pragma unroll
+        for (int x = 16; x > 0; x >>= 1) {
+            km = fmaxf(km, __shfl_xor_sync(0xffffffffu, km, x));
+            vm = fmaxf(vm, __shfl_xor_sync(0xffffffffu, vm, x));
+        }
+        if (lane == 0) {
+            tile_max[0][warp] = km;
+            tile_max[1][warp] = vm;
+        }
+        __syncthreads();
+        // V's power of two only falls (an all-zero tile keeps it): o is never scaled up
+        const int ek = split_exp(fmaxf(fmaxf(tile_max[0][0], tile_max[0][1]), fmaxf(tile_max[0][2], tile_max[0][3])), 0);
+        const int ev = min(ev_run, split_exp(fmaxf(fmaxf(tile_max[1][0], tile_max[1][1]), fmaxf(tile_max[1][2], tile_max[1][3])), ev_run));
+        const float fk = pow2f(ek), fv = pow2f(ev);
+#pragma unroll 2
+        for (int it = 0; it < IT; ++it) {
+            const int i = tid + it * ET_THREADS;
+            const int kk = i / RL, d4 = (i - kk * RL) * 4;
             float4 kv = make_float4(0.f, 0.f, 0.f, 0.f), vv = kv;
-            if (gj < S) {
-                kv = *reinterpret_cast<const float4 *>(base + (size_t)gj * ld + k_off + h * HD + d4);
-                vv = *reinterpret_cast<const float4 *>(base + (size_t)gj * ld + v_off + h * HD + d4);
+            if (j0 + kk >= key_lo && j0 + kk <= q_last) {
+                const float *r = base + (size_t)(j0 + kk) * ld + h * HD + d4;
+                kv = *reinterpret_cast<const float4 *>(r + k_off);
+                vv = *reinterpret_cast<const float4 *>(r + v_off);
             }
             uint2 a, bq;
-            split2(kv.x, kv.y, a.x, bq.x);
-            split2(kv.z, kv.w, a.y, bq.y);
+            split2(kv.x * fk, kv.y * fk, a.x, bq.x);
+            split2(kv.z * fk, kv.w * fk, a.y, bq.y);
             *reinterpret_cast<uint2 *>(&Kh[kk * STR + d4]) = a;
             *reinterpret_cast<uint2 *>(&Kl[kk * STR + d4]) = bq;
-            split2(vv.x, vv.y, a.x, bq.x);
-            split2(vv.z, vv.w, a.y, bq.y);
+            split2(vv.x * fv, vv.y * fv, a.x, bq.x);
+            split2(vv.z * fv, vv.w * fv, a.y, bq.y);
             *reinterpret_cast<uint2 *>(&Vh[kk * STR + d4]) = a;
             *reinterpret_cast<uint2 *>(&Vl[kk * STR + d4]) = bq;
         }
+        // the rows' score factors for this tile: scale and the row's and the tile's powers of two undone (exactly)
+        const float st0 = sc0 * pow2f(-ek), st1 = sc1 * pow2f(-ek);
         __syncthreads();
 
         // ---- S = Q K^T (16 x 64 per warp), three MMAs per product
@@ -148,7 +221,8 @@ enc_attention_tc_kernel(const float *__restrict__ qkv, float *__restrict__ out, 
                 mma16816(s[n], ql[2 * kp + 1], kh[2], kh[3]);
             }
         }
-        // ---- scale, mask, online softmax (rows g and g+8; a row's 64 scores live in the 4 lanes of a quad)
+        // ---- scale (powers of two undone), mask, online softmax (rows g and g+8; a row's
+        //      64 scores live in the 4 lanes of a quad)
         float m_t[2] = {-INFINITY, -INFINITY};
 #pragma unroll
         for (int n = 0; n < 8; ++n) {
@@ -157,7 +231,7 @@ enc_attention_tc_kernel(const float *__restrict__ qkv, float *__restrict__ out, 
                 const int gi = (e < 2) ? qr0 : qr1;
                 const int gj = j0 + n * 8 + 2 * t + (e & 1);
                 const bool valid = (gj < S) && (gj <= gi) && (gi - gj <= window);
-                s[n][e] = valid ? s[n][e] * scale : -INFINITY;
+                s[n][e] = valid ? s[n][e] * ((e < 2) ? st0 : st1) : -INFINITY;
                 m_t[e >> 1] = fmaxf(m_t[e >> 1], s[n][e]);
             }
         }
@@ -181,18 +255,23 @@ enc_attention_tc_kernel(const float *__restrict__ qkv, float *__restrict__ out, 
                 pv[e] = (mr == -INFINITY) ? 0.0f : expf(s[n][e] - mr);
                 psum[e >> 1] += pv[e];
             }
-            // C layout {row g: c0 c1, row g+8: c2 c3} of n-tile n -> A regs {a0, a1} (n even) or {a2, a3} (n odd)
-            split2(pv[0], pv[1], ph[n >> 1][(n & 1) * 2 + 0], pl[n >> 1][(n & 1) * 2 + 0]);
-            split2(pv[2], pv[3], ph[n >> 1][(n & 1) * 2 + 1], pl[n >> 1][(n & 1) * 2 + 1]);
+            // C layout {row g: c0 c1, row g+8: c2 c3} of n-tile n -> A regs {a0, a1} (n even) or {a2, a3} (n odd).
+            // P in [0, 1] is split as P * 2^15: its lo piece stays in f16's normal range down to P = 2^-18
+            split2(pv[0] * P_SCALE, pv[1] * P_SCALE, ph[n >> 1][(n & 1) * 2 + 0], pl[n >> 1][(n & 1) * 2 + 0]);
+            split2(pv[2] * P_SCALE, pv[3] * P_SCALE, ph[n >> 1][(n & 1) * 2 + 1], pl[n >> 1][(n & 1) * 2 + 1]);
         }
 #pragma unroll
         for (int r = 0; r < 2; ++r) l_run[r] = l_run[r] * alpha[r] + psum[r];  // quad-partial sums; reduced at the end
+        // o moves to this tile's V power of two with the softmax rescale
+        const int dv = ev - ev_run;  // in [-239, 0]: two exact power-of-two factors
+        const float r0 = alpha[0] * pow2f(dv / 2) * pow2f(dv - dv / 2), r1 = alpha[1] * pow2f(dv / 2) * pow2f(dv - dv / 2);
+        ev_run = ev;
 #pragma unroll
         for (int n = 0; n < ND; ++n) {
-            o[n][0] *= alpha[0];
-            o[n][1] *= alpha[0];
-            o[n][2] *= alpha[1];
-            o[n][3] *= alpha[1];
+            o[n][0] *= r0;
+            o[n][1] *= r0;
+            o[n][2] *= r1;
+            o[n][3] *= r1;
         }
         // ---- O += P V
 #pragma unroll
@@ -220,14 +299,16 @@ enc_attention_tc_kernel(const float *__restrict__ qkv, float *__restrict__ out, 
         l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
     }
     const float inv0 = 1.0f / l_run[0], inv1 = 1.0f / l_run[1];
+    const int eo = -(15 + ev_run);  // undo P's and V's powers of two (eo in [-141, 98]: two exact factors)
+    const float fo0 = pow2f(eo / 2), fo1 = pow2f(eo - eo / 2);
 #pragma unroll
     for (int n = 0; n < ND; ++n) {
         if (qr0 < S)
             *reinterpret_cast<float2 *>(out + ((size_t)row0 + qr0) * (H * HD) + h * HD + n * 8 + 2 * t) =
-                make_float2(o[n][0] * inv0, o[n][1] * inv0);
+                make_float2(o[n][0] * inv0 * fo0 * fo1, o[n][1] * inv0 * fo0 * fo1);
         if (qr1 < S)
             *reinterpret_cast<float2 *>(out + ((size_t)row0 + qr1) * (H * HD) + h * HD + n * 8 + 2 * t) =
-                make_float2(o[n][2] * inv1, o[n][3] * inv1);
+                make_float2(o[n][2] * inv1 * fo0 * fo1, o[n][3] * inv1 * fo0 * fo1);
     }
 }
 

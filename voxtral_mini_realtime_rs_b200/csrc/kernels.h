@@ -259,7 +259,10 @@ void launch_rope_inplace(float *buf, int rows, int ld, int q_off, int n_q, int k
 // longest stream's length; a stream's band never reaches into another stream's rows.
 void launch_enc_attention(const float *qkv, float *out, int B, int S, int H, int hd, int ld, int q_off,
                           int k_off, int v_off, int window, float scale, cudaStream_t st, const int *seg = nullptr);
-// same contract on the tensor cores (enc_attn_tc.cu): mma.sync with two-piece f16 operands, f32-grade accuracy
+// same contract on the tensor cores (enc_attn_tc.cu): mma.sync with two-piece f16 operands, each operand scaled by a
+// power of two first (Q per row, K per key tile, V by the running tile maximum, P by 2^15), so 22-bit pieces at any
+// overall operand scale (relative to the largest element of the row, tile or block: enc_attn_tc.cu); hd 32 or 64,
+// ld and the offsets multiples of 4, qkv 16-byte aligned
 bool enc_attention_tc_supported(int hd, int ld, int q_off, int k_off, int v_off);
 void launch_enc_attention_tc(const float *qkv, float *out, int B, int S, int H, int hd, int ld, int q_off,
                              int k_off, int v_off, int window, float scale, cudaStream_t st, const int *seg = nullptr);

@@ -128,6 +128,8 @@ stream_enc_attn_kernel(const float *__restrict__ qkv, const int ld, const int H,
     }
 }
 
+}  // namespace
+
 void launch_stream_attn(const float *qkv, int R, int ld, int H, int hd, const int *row_slot, const int *row_pos, const float *kr,
                         const float *vr, int ring, int window, float scale, float *out, cudaStream_t st) {
     dim3 grid(H, R);
@@ -139,6 +141,8 @@ void launch_stream_attn(const float *qkv, int R, int ld, int H, int hd, const in
     }
     cuda_check(cudaGetLastError(), "stream_enc_attn launch");
 }
+
+namespace {
 
 int conv_out(int t) { return t > 0 ? (t + 2 - 3) / 2 + 1 : 0; }
 

@@ -11,6 +11,12 @@ namespace vox {
 // buffers hold this much and slide forward as the session advances.
 constexpr float kResidentSeconds = 30.0f;
 
+// K4-S: encoder attention of R rows, each at (session row_slot[r], absolute position row_pos[r]), over the sessions' K/V
+// rings kr / vr [slot][ring][H*hd] (position p at p % ring): keys max(0, p - window) .. p.  q of row r at qkv + r * ld,
+// out [R][H*hd].  hd in {32, 64, 128}.
+void launch_stream_attn(const float *qkv, int R, int ld, int H, int hd, const int *row_slot, const int *row_pos, const float *kr,
+                        const float *vr, int ring, int window, float scale, float *out, cudaStream_t st);
+
 struct StreamPool {
     // Counters are absolute (since the session opened).  Every audio-side buffer of a session holds a window of rows
     // starting at absolute row *0 (pcm0, mel0, ...): always 0 in a bounded pool, whose buffers hold the whole stream.
