@@ -39,6 +39,9 @@ extern "C" {
 #define VOX_DTYPE_F32 0 /* GgmlDtype, src/gguf/reader.rs:18-49 */
 #define VOX_DTYPE_F16 1
 #define VOX_DTYPE_Q4_0 2
+/* decoder KV cache only (vox_session_create_ex): int8 with an f16 scale per 16 head dims.  Outside GGML's type table,
+ * so it never collides with a vox_gguf_tensor_info code (GGUF's Q8_0, type 8, has blocks of 32 and rounds differently). */
+#define VOX_DTYPE_KV_Q8 100
 
 const char *vox_last_error(void);
 int32_t vox_version(void);
@@ -237,6 +240,16 @@ int32_t vox_session_create(vox_model *m, int32_t max_batch, int32_t max_mel_fram
  *     per-op paths) reads the stored values, including the current position's own key and value, widens them exactly to
  *     f32 and computes as with an f32 cache, so all paths compute the same function.  Nothing else changes:
  *     activations, logits, weights, the encoder and its K/V rings, token scores, beams and bias work as before.
+ *   VOX_DTYPE_KV_Q8: 1.125 bytes per cached value, 9/32 of the f32 KV memory and 9/16 of the f16.  Each block of 16
+ *     consecutive head dims x[0..16) of one (position, kv head) vector (f32: K after RoPE, or V) is stored as
+ *       a   = max_i |x_i|
+ *       d   = f16_rn(min(a / 127, 65504))          (a / 127 an f32 division; f16_rn rounds to nearest even)
+ *       q_i = 0 if d == 0, else clamp(rint(x_i / (float)d), -127, 127)
+ *                                                  (f32 division; rint to nearest even; -128 is never stored)
+ *     A block holding a NaN stores d = NaN and q_i = 0: the whole block decodes to NaN.  The decoded value is
+ *     (float)d * q_i, exact in f32.  As for f16, every attention path reads the decoded values, including the current
+ *     position's own key and value, and computes as with an f32 cache holding them; vox_session_debug_read("kv_k<l>" /
+ *     "kv_v<l>") returns them as f32.  Nothing else changes.
  *   Any other kv_dtype: VOX_EINVAL, and *out is left untouched. */
 int32_t vox_session_create_ex(vox_model *m, int32_t max_batch, int32_t max_mel_frames, int32_t kv_dtype, vox_session **out);
 /* bytes of device memory the session allocated (all of it at creation; the first set_top_k / set_beam / set_bias and
@@ -439,7 +452,8 @@ typedef struct {
  * would exceed those 30 s; encode_chunk is not available.  Absolute positions stay int32: ~248 days of audio. */
 int32_t vox_stream_pool_create(vox_model *m, int32_t max_sessions, float max_seconds, vox_stream_pool **out);
 /* kv_dtype as vox_session_create_ex: every session of the pool shares its page pool, so they share the element type.
- * An unbounded pool's state is dominated by the decoder KV ring; VOX_DTYPE_F16 halves it (INTEGRATION.md section 3b). */
+ * An unbounded pool's state is dominated by the decoder KV ring; VOX_DTYPE_F16 halves it and VOX_DTYPE_KV_Q8 takes it to
+ * 9/32 of f32 (INTEGRATION.md section 3b). */
 int32_t vox_stream_pool_create_ex(vox_model *m, int32_t max_sessions, float max_seconds, int32_t kv_dtype,
                                   vox_stream_pool **out);
 /* bytes of device memory the pool allocated (its session's arena, which holds every per-session buffer) */

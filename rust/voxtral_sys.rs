@@ -16,6 +16,11 @@ use std::os::raw::{c_char, c_void};
 #[repr(C)] pub struct vox_tokenizer { _p: [u8; 0] }
 #[repr(C)] pub struct vox_stream_pool { _p: [u8; 0] }
 
+// decoder KV cache element types (vox_session_create_ex / vox_stream_pool_create_ex kv_dtype)
+pub const VOX_DTYPE_F32: i32 = 0;
+pub const VOX_DTYPE_F16: i32 = 1;
+pub const VOX_DTYPE_KV_Q8: i32 = 100;   // int8 with an f16 scale per 16 head dims (include/voxtral.h)
+
 #[repr(C)] #[derive(Default, Clone, Copy)]
 pub struct vox_timings {
     pub preprocess_ms: f32, pub encode_ms: f32, pub decode_ms: f32, pub total_ms: f32,
@@ -48,7 +53,7 @@ extern "C" {
     // src/gguf/model.rs
     pub fn vox_session_create(m: *mut vox_model, max_batch: i32, max_mel_frames: i32,
                               out: *mut *mut vox_session) -> i32;
-    // kv_dtype: VOX_DTYPE_F32 (0) or VOX_DTYPE_F16 (1), the decoder KV cache's element type
+    // kv_dtype: VOX_DTYPE_F32 (0), VOX_DTYPE_F16 (1) or VOX_DTYPE_KV_Q8 (100), the decoder KV cache's element type
     pub fn vox_session_create_ex(m: *mut vox_model, max_batch: i32, max_mel_frames: i32, kv_dtype: i32,
                                  out: *mut *mut vox_session) -> i32;
     pub fn vox_session_device_bytes(s: *const vox_session, bytes: *mut u64) -> i32;

@@ -1,18 +1,22 @@
 #!/usr/bin/env python
-"""What the f16 decoder KV cache saves, on the full-size synthetic model (seed 42, the weights bench.py runs).
+"""What the f16 and 8-bit (q8) decoder KV caches save, on the full-size synthetic model (seed 42, the weights bench.py
+runs).
 
-  * Memory: device_bytes of unbounded stream pools of 1 and 2 sessions at f32 and f16; their difference is the bytes
-    of one session slot, and (80 GB - the model - the pool's fixed part) / slot the slots that fit in 80 GB.  Computed
-    from the handles' own counts, never by allocating.
+  * Memory: device_bytes of unbounded stream pools of 1 and 2 sessions at f32, f16 and q8; their difference is the
+    bytes of one session slot, and (80 GB - the model - the pool's fixed part) / slot the slots that fit in 80 GB.
+    Computed from the handles' own counts, never by allocating.
   * Soak: an unbounded pool of 8 sessions, every session fed 160 ms of audio per tick (as scripts/stream_soak.py
-    does, without waiting for the wall clock), f32 and f16 pools in turn.  Per-tick device time (vox_stream_stats.gpu_ms)
-    p50 / p95 over the ticks of the first minute of audio and over the ticks after the decoder's 8192-position window
-    has filled.  The decoder advances 6.25 positions per second of audio, so 8192 positions take about 1310 s: the
-    default --soak-seconds 1500 reaches the window; a shorter soak reports the second figure as null.
-  * Offline: the 16 s B = 8 and B = 1 decode step, f32 and f16 sessions alternating, --rounds rounds, medians
-    (vox_timings: decode_ms - prefill_ms over the graph-replayed steps).
+    does, without waiting for the wall clock), one pool per --soak-dtypes entry in turn.  Per-tick device time
+    (vox_stream_stats.gpu_ms) p50 / p95 over the ticks of the first minute of audio and over the ticks after the
+    decoder's 8192-position window has filled.  The decoder advances 6.25 positions per second of audio, so 8192
+    positions take about 1310 s: the default --soak-seconds 1500 reaches the window; a shorter soak reports the second
+    figure as null.
+  * Offline: the 16 s B = 8 and B = 1 decode step, one session per --step-dtypes entry, alternating, --rounds rounds,
+    medians and ranges (vox_timings: decode_ms - prefill_ms over the graph-replayed steps), and the share of ids each
+    type agrees with the first one on.
 
-    python scripts/kv_half_bench.py [--rounds 5] [--soak-seconds 1500] [--out DIR]
+    python scripts/kv_half_bench.py [--rounds 5] [--soak-seconds 1500] [--soak-dtypes f16,q8]
+                                    [--step-dtypes f16,q8] [--out DIR]
 
 Prints one JSON line with the card's name and power limit; with --out also writes it there.
 """
@@ -68,8 +72,11 @@ def main():
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--seconds", type=float, default=16.0)
     ap.add_argument("--soak-seconds", type=float, default=1500.0)
+    ap.add_argument("--soak-dtypes", default="f16,q8")
+    ap.add_argument("--step-dtypes", default="f16,q8")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
+    soak_dtypes, step_dtypes = args.soak_dtypes.split(","), args.step_dtypes.split(",")
     import voxtral_mini_realtime_rs_b200 as vx
     from voxtral_mini_realtime_rs_b200 import synth
     from oracle import mel as omel
@@ -84,10 +91,11 @@ def main():
         synth.write_synthetic_gguf(path, synth.VoxtralConfig(), seed=42)
         loader = vx.Q4ModelLoader.from_file(path)
         m = loader.load(0, max_batch=8, max_mel_frames=int(args.seconds * 100) + 1200)
-        m16 = loader.load(0, max_batch=8, max_mel_frames=int(args.seconds * 100) + 1200, kv_dtype="f16")
+        sessions = {dt: loader.load(0, max_batch=8, max_mel_frames=int(args.seconds * 100) + 1200, kv_dtype=dt)
+                    for dt in step_dtypes}
         model_bytes = int(m.info["device_bytes"])
 
-        for dt in ("f32", "f16"):
+        for dt in ("f32", "f16", "q8"):
             sizes = []
             for n in (1, 2):
                 p = vx.StreamingPool(m, max_sessions=n, max_seconds=None, kv_dtype=dt)
@@ -100,7 +108,7 @@ def main():
         res["memory"]["model_bytes"] = model_bytes
 
         audio = [omel.peak_normalize(omel.speechlike(60.0, 40 + i)).astype(np.float32) for i in range(8)]
-        for dt in ("f32", "f16"):
+        for dt in soak_dtypes:
             early, late = soak(vx, m, audio, dt, args.soak_seconds)
             res["soak_ms"][dt] = {"first_minute_p50": pct(early, 50), "first_minute_p95": pct(early, 95),
                                   "window_full_p50": pct(late, 50), "window_full_p95": pct(late, 95),
@@ -115,20 +123,25 @@ def main():
             return (tm.decode_ms - tm.prefill_ms) / (ids.shape[1] - 1), ids
 
         for B in (8, 1):
-            t32, t16, agree = [], [], 0.0
-            step_ms(m, B)
-            step_ms(m16, B)
+            times, ids = {dt: [] for dt in step_dtypes}, {}
+            for dt in step_dtypes:
+                step_ms(sessions[dt], B)
             for _ in range(args.rounds):
-                a, i32 = step_ms(m, B)
-                b, i16 = step_ms(m16, B)
-                t32.append(a)
-                t16.append(b)
-                agree = float(np.mean(i32 == i16))
+                for dt in step_dtypes:
+                    t, ids[dt] = step_ms(sessions[dt], B)
+                    times[dt].append(t)
             med = statistics.median
-            res["step_ms"][f"B{B}"] = {"f32": med(t32), "f16": med(t16), "f32_range": [min(t32), max(t32)],
-                                       "f16_range": [min(t16), max(t16)], "ids_agree": agree}
+            row = {}
+            for dt in step_dtypes:
+                row[dt] = med(times[dt])
+                row[f"{dt}_range"] = [min(times[dt]), max(times[dt])]
+                a, b = ids[step_dtypes[0]], ids[dt]
+                n = min(a.shape[1], b.shape[1])
+                row[f"{dt}_ids_agree"] = float(np.mean(a[:, :n] == b[:, :n]))
+            res["step_ms"][f"B{B}"] = row
         m.close()
-        m16.close()
+        for s_ in sessions.values():
+            s_.close()
     line = json.dumps(res)
     print(line)
     if args.out:

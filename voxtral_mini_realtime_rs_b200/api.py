@@ -696,8 +696,8 @@ def q4_matmul_bench(weights, m: int, iters: int = 200, warmup: int = 20) -> floa
     return ms.value
 
 
-# decoder KV cache element types (include/voxtral.h vox_session_create_ex): VOX_DTYPE_F32, VOX_DTYPE_F16
-KV_DTYPES = {"f32": 0, "f16": 1}
+# decoder KV cache element types (include/voxtral.h vox_session_create_ex): VOX_DTYPE_F32, VOX_DTYPE_F16, VOX_DTYPE_KV_Q8
+KV_DTYPES = {"f32": 0, "f16": 1, "q8": 100}
 
 
 def _kv_dtype(kv_dtype: str) -> int:
@@ -1016,7 +1016,7 @@ class StreamingPool:
 
     def __init__(self, model: "Q4VoxtralModel", max_sessions: int = 8, max_seconds: float | None = 30.0,
                  kv_dtype: str = "f32"):
-        """kv_dtype: element type of the decoder KV cache the sessions share, "f32" or "f16" (include/voxtral.h)."""
+        """kv_dtype: element type of the decoder KV cache the sessions share, "f32", "f16" or "q8" (include/voxtral.h)."""
         self._model = model
         self._p = _P()
         _check(lib().vox_stream_pool_create_ex(model._m, max_sessions, 0.0 if max_seconds is None else max_seconds,
@@ -1168,7 +1168,7 @@ class Q4ModelLoader:
 
     def load(self, device: int = 0, max_batch: int = 1, max_mel_frames: int = 3000,
              kv_dtype: str = "f32") -> Q4VoxtralModel:
-        """kv_dtype: element type of the session's decoder KV cache, "f32" or "f16" (include/voxtral.h)."""
+        """kv_dtype: element type of the session's decoder KV cache, "f32", "f16" or "q8" (include/voxtral.h)."""
         _kv_dtype(kv_dtype)
         h = _P()
         _check(lib().vox_model_load_gguf_handle(self._reader._h, device, C.byref(h)))

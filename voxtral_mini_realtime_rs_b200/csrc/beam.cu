@@ -102,6 +102,23 @@ beam_fork_kernel(KV *kc, KV *vc, size_t layer_stride, int *page_table, int max_p
     if (layer == 0)
         for (int lp = threadIdx.x; lp < c; lp += blockDim.x) dst_pt[lp] = src_pt[lp];
     if (rem == 0) return;
+    if constexpr (kv_type_of<KV>() == KvType::Q8) {
+        // a (page, kv head) unit of layer_stride-byte layers: values [KV_PAGE][hd], then scales [KV_PAGE][hd / 16] f16;
+        // positions [0, rem) are the first rem rows of each plane (values in 16-byte chunks, scales in 4-byte words)
+        const size_t ub = kv_unit_bytes(KvType::Q8, hd);
+        const int n16 = rem * hd / 16, n4 = rem * (hd / KV_Q8_BLOCK) / 2;
+        for (int kv = 0; kv < 2; ++kv) {
+            KV *base = (kv ? vc : kc) + (size_t)layer * layer_stride;
+            for (int h = 0; h < Hkv; ++h) {
+                const KV *s = base + ((size_t)from * Hkv + h) * ub;
+                KV *d = base + ((size_t)own * Hkv + h) * ub;
+                for (int i = threadIdx.x; i < n16; i += blockDim.x) reinterpret_cast<uint4 *>(d)[i] = reinterpret_cast<const uint4 *>(s)[i];
+                for (int i = threadIdx.x; i < n4; i += blockDim.x)
+                    reinterpret_cast<uint32_t *>(d + (size_t)KV_PAGE * hd)[i] = reinterpret_cast<const uint32_t *>(s + (size_t)KV_PAGE * hd)[i];
+            }
+        }
+        return;
+    }
     const int n4 = rem * hd / (16 / (int)sizeof(KV));   // 16-byte chunks: positions [0, rem) of one kv head are contiguous in a page
     for (int kv = 0; kv < 2; ++kv) {
         KV *base = (kv ? vc : kc) + (size_t)layer * layer_stride;
@@ -113,13 +130,16 @@ beam_fork_kernel(KV *kc, KV *vc, size_t layer_stride, int *page_table, int max_p
     }
 }
 
-void launch_beam_fork(void *kc, void *vc, KvType type, size_t layer_stride, int layers, int *page_table, int max_pages,
+void launch_beam_fork(void *kc, void *vc, KvType type, size_t layer_bytes, int layers, int *page_table, int max_pages,
                       const int *pos, const int *src, int rows, int Hkv, int hd, cudaStream_t st) {
-    if (type == KvType::F16)
-        beam_fork_kernel<__half><<<dim3(rows, layers), 256, 0, st>>>((__half *)kc, (__half *)vc, layer_stride, page_table,
+    if (type == KvType::Q8)
+        beam_fork_kernel<int8_t><<<dim3(rows, layers), 256, 0, st>>>((int8_t *)kc, (int8_t *)vc, layer_bytes, page_table,
+                                                                     max_pages, pos, src, Hkv, hd);
+    else if (type == KvType::F16)
+        beam_fork_kernel<__half><<<dim3(rows, layers), 256, 0, st>>>((__half *)kc, (__half *)vc, layer_bytes / 2, page_table,
                                                                      max_pages, pos, src, Hkv, hd);
     else
-        beam_fork_kernel<float><<<dim3(rows, layers), 256, 0, st>>>((float *)kc, (float *)vc, layer_stride, page_table,
+        beam_fork_kernel<float><<<dim3(rows, layers), 256, 0, st>>>((float *)kc, (float *)vc, layer_bytes / 4, page_table,
                                                                     max_pages, pos, src, Hkv, hd);
     tc_count_launch("beam_fork");
 }

@@ -593,9 +593,9 @@ void vox_model_free(vox_model *m) {
 // ---------------------------------------------------------------- session
 // the element type vox_session_create_ex / vox_stream_pool_create_ex accept
 static KvType kv_type_of(int32_t kv_dtype) {
-    VOX_CHECK(kv_dtype == VOX_DTYPE_F32 || kv_dtype == VOX_DTYPE_F16, VOX_EINVAL,
-              "kv_dtype %d: VOX_DTYPE_F32 or VOX_DTYPE_F16", (int)kv_dtype);
-    return kv_dtype == VOX_DTYPE_F16 ? KvType::F16 : KvType::F32;
+    VOX_CHECK(kv_dtype == VOX_DTYPE_F32 || kv_dtype == VOX_DTYPE_F16 || kv_dtype == VOX_DTYPE_KV_Q8, VOX_EINVAL,
+              "kv_dtype %d: VOX_DTYPE_F32, VOX_DTYPE_F16 or VOX_DTYPE_KV_Q8", (int)kv_dtype);
+    return kv_dtype == VOX_DTYPE_F16 ? KvType::F16 : (kv_dtype == VOX_DTYPE_KV_Q8 ? KvType::Q8 : KvType::F32);
 }
 int32_t vox_session_create(vox_model *m, int32_t max_batch, int32_t max_mel_frames, vox_session **out) {
     return vox_session_create_ex(m, max_batch, max_mel_frames, VOX_DTYPE_F32, out);

@@ -54,7 +54,15 @@ dec_attn_fused_kernel(const float *__restrict__ qkv, const int ld, const int H, 
         v[1] = xr * s + xi * c;
     }
     __syncthreads();
-    {
+    if constexpr (kv_type_of<KV>() == KvType::Q8) {
+        // the whole head vector is in kvs: a thread per 16-element block of K, then of V
+        constexpr int NB = HD / KV_Q8_BLOCK;
+        if (threadIdx.x < 2 * NB) {
+            const int kv_i = threadIdx.x / NB, blk = threadIdx.x - kv_i * NB;
+            const KvQ8Row r = kv_q8_row<RING>(kv_ptr<int8_t>(kv_i ? kv.v : kv.k), kv, b, Hkv, kvh, pos, HD);
+            kv_q8_store16(r.q + blk * KV_Q8_BLOCK, r.d + blk, &kvs[kv_i][blk * KV_Q8_BLOCK]);
+        }
+    } else {
         const size_t at = kv_index<RING>(kv, b, Hkv, kvh, pos, HD);
         for (int i = threadIdx.x; i < HD; i += DA_THREADS) {
             kv_store(kv_ptr<KV>(kv.k) + at + i, kvs[0][i]);
@@ -81,13 +89,25 @@ dec_attn_fused_kernel(const float *__restrict__ qkv, const int ld, const int H, 
         float kk[DPL], vv[DPL];
         const int pg = RING ? (j / KV_PAGE) % kv.max_pages : j / KV_PAGE;
         const int phys = pg < 64 ? pts[pg] : kv.page_table[(size_t)b * kv.max_pages + pg];
-        const size_t at = (((size_t)phys * Hkv + kvh) * KV_PAGE + (j % KV_PAGE)) * HD + lane * DPL;
-        const KV *kr = kv_ptr<KV>(kv.k) + at;
-        const KV *vr = kv_ptr<KV>(kv.v) + at;
+        if constexpr (kv_type_of<KV>() == KvType::Q8) {
+            // this lane's DPL dims lie in one scale block
+            const KvQ8Row kr = kv_q8_at(kv_ptr<int8_t>(kv.k), (size_t)phys * Hkv + kvh, j % KV_PAGE, HD);
+            const KvQ8Row vr = kv_q8_at(kv_ptr<int8_t>(kv.v), (size_t)phys * Hkv + kvh, j % KV_PAGE, HD);
+            const float kd = __half2float(kr.d[lane * DPL / KV_Q8_BLOCK]), vd = __half2float(vr.d[lane * DPL / KV_Q8_BLOCK]);
 #pragma unroll
-        for (int i = 0; i < DPL; ++i) {
-            kk[i] = kv_load(kr[i]);
-            vv[i] = kv_load(vr[i]);
+            for (int i = 0; i < DPL; ++i) {
+                kk[i] = kv_q8_load(kr.q[lane * DPL + i], kd);
+                vv[i] = kv_q8_load(vr.q[lane * DPL + i], vd);
+            }
+        } else {
+            const size_t at = (((size_t)phys * Hkv + kvh) * KV_PAGE + (j % KV_PAGE)) * HD + lane * DPL;
+            const KV *kr = kv_ptr<KV>(kv.k) + at;
+            const KV *vr = kv_ptr<KV>(kv.v) + at;
+#pragma unroll
+            for (int i = 0; i < DPL; ++i) {
+                kk[i] = kv_load(kr[i]);
+                vv[i] = kv_load(vr[i]);
+            }
         }
         float s[G];
 #pragma unroll
@@ -163,6 +183,18 @@ void launch_dec_attn_fused(float *qkv, int B, int ld, int H, int Hkv, int hd, co
     VOX_CHECK(dec_attn_fused_supported(H, Hkv, hd), VOX_EINVAL, "dec_attn_fused: unsupported shape");
     const int G = H / Hkv, dpl = hd / 32;
     dim3 grid(Hkv, B);
+    if (kv.type == KvType::Q8) {
+        switch (G * 2 + (kv.ring ? 1 : 0)) {
+            case 2: launch_g<1, false, int8_t>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+            case 3: launch_g<1, true, int8_t>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+            case 4: launch_g<2, false, int8_t>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+            case 5: launch_g<2, true, int8_t>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+            case 8: launch_g<4, false, int8_t>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+            default: launch_g<4, true, int8_t>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;
+        }
+        tc_count_launch("dec_attn_fused");
+        return;
+    }
     const bool f16 = kv.type == KvType::F16;
     switch (G * 4 + (kv.ring ? 2 : 0) + (f16 ? 1 : 0)) {
         case 4: launch_g<1, false, float>(dpl, grid, st, qkv, ld, H, Hkv, kv, window, scale, rope, out); break;

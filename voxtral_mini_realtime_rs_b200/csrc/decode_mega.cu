@@ -79,7 +79,7 @@ struct MegaOp {
     float *ssq_out = nullptr;       // [n_tiles][B]
     int track_argmax = 0;
     // MG_ATTN, and the layer's qkv MG_MATVEC, whose epilogue applies RoPE to the q and k rows and appends k and v
-    KvPool kc, vc;   // this layer's KV page pools [n_pages][Hkv][KV_PAGE][hd] of MegaPlan::kv_bytes elements (kernels.h)
+    KvPool kc, vc;   // this layer's KV page pools [n_pages][Hkv] of MegaPlan::kv_type units (kernels.h kv_unit_bytes)
     int layer = 0;
     // MG_MATVEC whose output fragments take layer j's ffn_norm x ADA scale (wo): j, else -1.  Token b's fragments are
     // scaled by MegaParams::ffn_ada_rows[b] + j * D (fout_gamma is unset).
@@ -148,7 +148,7 @@ struct MegaPlan {
     int scratch_bytes = 0;
     int nstage = 0;
     int attn_tile = 0;      // keys per K/V tile of the attention phase (what the scratch region holds)
-    int kv_bytes = 4;       // KV cache element: 4 (f32) or 2 (f16); selects the kernel instantiation
+    KvType kv_type = KvType::F32;   // KV cache element type; selects the kernel instantiation
     size_t smem_bytes = 0;
 };
 
@@ -195,14 +195,18 @@ __host__ __device__ constexpr int mg_misc_bytes(int MT) {
 }
 __host__ __device__ constexpr int mg_pair_bytes(int MT) { return 272 * MT; }  // fragments + offsets of one block pair
 // Attention phase in the scratch region: q [G][HD] + per-warp maxima [MG_CWARPS][G], then per key of a tile its G scores,
-// its K row padded by one 16-byte chunk (HD + 16 / KB elements of KB bytes: 4 f32 or 8 f16) and its V row.  Keys per
-// tile: what the scratch holds, in whole warps (one key per consumer thread, at most MG_CTHREADS).
+// its K row padded by one 16-byte chunk (HD + 16 / KB elements of KB bytes: 4 f32, 8 f16 or 16 int8) and its V row;
+// Q8 adds the K and V rows' scales (HD / 16 f16 each).  Keys per tile: what the scratch holds, in whole warps (one key
+// per consumer thread, at most MG_CTHREADS).
 __host__ __device__ constexpr int mg_attn_fixed_bytes(int G, int HD) { return (G * HD + MG_CWARPS * G) * 4; }
-__host__ __device__ constexpr int mg_attn_key_bytes(int G, int HD, int KB) { return G * 4 + (2 * HD + 16 / KB) * KB; }
-__host__ __device__ constexpr int mg_attn_tile(int scratch_bytes, int G, int HD, int KB) {
-    return (scratch_bytes - mg_attn_fixed_bytes(G, HD)) / mg_attn_key_bytes(G, HD, KB) / 32 * 32 > MG_CTHREADS
+__host__ __device__ constexpr int mg_attn_key_bytes(int G, int HD, KvType t) {
+    return t == KvType::Q8 ? G * 4 + (2 * HD + 16) + 2 * (HD / KV_Q8_BLOCK) * 2
+                           : G * 4 + (2 * HD + 16 / (t == KvType::F16 ? 2 : 4)) * (t == KvType::F16 ? 2 : 4);
+}
+__host__ __device__ constexpr int mg_attn_tile(int scratch_bytes, int G, int HD, KvType t) {
+    return (scratch_bytes - mg_attn_fixed_bytes(G, HD)) / mg_attn_key_bytes(G, HD, t) / 32 * 32 > MG_CTHREADS
                ? MG_CTHREADS
-               : (scratch_bytes - mg_attn_fixed_bytes(G, HD)) / mg_attn_key_bytes(G, HD, KB) / 32 * 32;
+               : (scratch_bytes - mg_attn_fixed_bytes(G, HD)) / mg_attn_key_bytes(G, HD, t) / 32 * 32;
 }
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -644,9 +648,16 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                                 const int j0 = j_lo + ch * per, j1 = min(pos, j0 + per);  // row `pos` is not written yet
                                 for (int pg = j0 / KV_PAGE; pg * KV_PAGE < j1; ++pg) {     // pages are the contiguous unit
                                     const int ka = max(j0, pg * KV_PAGE), ke = min(j1, (pg + 1) * KV_PAGE);
-                                    const size_t off = (((size_t)p.page_table[(size_t)b * p.max_pages + (RING ? pg % p.max_pages : pg)] * p.Hkv + kvh) * KV_PAGE + (ka - pg * KV_PAGE)) * HD;
-                                    bulk_prefetch_l2(kv_ptr<KV>(nx.kc) + off, (uint32_t)(ke - ka) * HD * (uint32_t)sizeof(KV));
-                                    bulk_prefetch_l2(kv_ptr<KV>(nx.vc) + off, (uint32_t)(ke - ka) * HD * (uint32_t)sizeof(KV));
+                                    if constexpr (kv_type_of<KV>() == KvType::Q8) {   // the whole unit: its rows and their scales
+                                        constexpr uint32_t UB = (uint32_t)kv_unit_bytes(KvType::Q8, HD);
+                                        const size_t off = ((size_t)p.page_table[(size_t)b * p.max_pages + (RING ? pg % p.max_pages : pg)] * p.Hkv + kvh) * UB;
+                                        bulk_prefetch_l2(kv_ptr<KV>(nx.kc) + off, UB);
+                                        bulk_prefetch_l2(kv_ptr<KV>(nx.vc) + off, UB);
+                                    } else {
+                                        const size_t off = (((size_t)p.page_table[(size_t)b * p.max_pages + (RING ? pg % p.max_pages : pg)] * p.Hkv + kvh) * KV_PAGE + (ka - pg * KV_PAGE)) * HD;
+                                        bulk_prefetch_l2(kv_ptr<KV>(nx.kc) + off, (uint32_t)(ke - ka) * HD * (uint32_t)sizeof(KV));
+                                        bulk_prefetch_l2(kv_ptr<KV>(nx.vc) + off, (uint32_t)(ke - ka) * HD * (uint32_t)sizeof(KV));
+                                    }
                                 }
                             }
                         }
@@ -782,13 +793,15 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                                                     out = make_float4(out.x * c.x - out.y * sn.x, out.x * sn.x + out.y * c.x,
                                                                       out.z * c.y - out.w * sn.y, out.z * sn.y + out.w * c.y);
                                                 }
-                                                if (r_row >= p.H * HD) {
-                                                    KvView kvw;
-                                                    kvw.page_table = p.page_table;
-                                                    kvw.max_pages = p.max_pages;
-                                                    const int kvh = ((r_row - p.H * HD) / HD) % p.Hkv;
-                                                    KV *dst = (r_row < qk_rows ? kv_ptr<KV>(vop->kc) : kv_ptr<KV>(vop->vc)) + kv_index<RING>(kvw, q_tok, p.Hkv, kvh, pos, HD) + hrow;
-                                                    kv_store4(dst, out);
+                                                if constexpr (kv_type_of<KV>() != KvType::Q8) {   // (Q8: below, a block at a time)
+                                                    if (r_row >= p.H * HD) {
+                                                        KvView kvw;
+                                                        kvw.page_table = p.page_table;
+                                                        kvw.max_pages = p.max_pages;
+                                                        const int kvh = ((r_row - p.H * HD) / HD) % p.Hkv;
+                                                        KV *dst = (r_row < qk_rows ? kv_ptr<KV>(vop->kc) : kv_ptr<KV>(vop->vc)) + kv_index<RING>(kvw, q_tok, p.Hkv, kvh, pos, HD) + hrow;
+                                                        kv_store4(dst, out);
+                                                    }
                                                 }
                                             }
                                         }
@@ -815,6 +828,32 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                                             vd[MT] = out.y;
                                             vd[2 * MT] = out.z;
                                             vd[3 * MT] = out.w;
+                                        }
+                                    }
+                                    if constexpr (kv_type_of<KV>() == KvType::Q8) {
+                                        // the qkv phase's append to an 8-bit cache: a tile's 16 rows are one scale block of one
+                                        // token's k or v head vector, held by four consecutive lanes (q_r0 = 0, 4, 8, 12); its
+                                        // absmax takes the same two shuffles as the sum of squares below.  Each lane stores its
+                                        // 4 values, lane q_r0 == 0 the scale.
+                                        if (kv_ptr<KV>(vop->kc) != nullptr) {
+                                            unsigned ab = kv_q8_abits4(out);
+                                            ab = max(ab, __shfl_xor_sync(0xffffffffu, ab, 2));
+                                            ab = max(ab, __shfl_xor_sync(0xffffffffu, ab, 1));
+                                            if (live && r_row < N && r_row >= p.H * HD) {
+                                                const int pos = p.d_pos[q_tok];
+                                                if (RING || pos < p.max_seq) {
+                                                    const int hrow = r_row % HD, qk_rows = (p.H + p.Hkv) * HD;
+                                                    KvView kvw;
+                                                    kvw.page_table = p.page_table;
+                                                    kvw.max_pages = p.max_pages;
+                                                    const int kvh = ((r_row - p.H * HD) / HD) % p.Hkv;
+                                                    const KvQ8Row kr = kv_q8_row<RING>(r_row < qk_rows ? kv_ptr<KV>(vop->kc) : kv_ptr<KV>(vop->vc), kvw,
+                                                                                       q_tok, p.Hkv, kvh, pos, HD);
+                                                    const __half dh = kv_q8_scale(ab);
+                                                    *reinterpret_cast<uint32_t *>(kr.q + hrow) = kv_q8_pack4(out, __half2float(dh));
+                                                    if (q_r0 == 0) kr.d[hrow / KV_Q8_BLOCK] = dh;
+                                                }
+                                            }
                                         }
                                     }
                                     if (ssq_out) {   // sum of squares of the tile's 16 rows: 4 in this thread, 4 lanes per tile
@@ -1064,15 +1103,21 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
             // key j against the G heads (q read as a broadcast; K rows padded to HD + 4 floats, an odd number of float4, so
             // the 8 threads of a quarter-warp read 8 distinct bank groups), one CTA-wide max per head, then P.V with
             // thread = (head, dim).  An f16 cache is staged as stored (EPC = 8 elements per 16-byte copy, K rows padded
-            // by 8 halves: again an odd number of chunks at HD 128 and 32) and widened exactly where it is read.
+            // by 8 halves: again an odd number of chunks at HD 128 and 32) and widened exactly where it is read.  A Q8 cache
+            // is staged as stored too: int8 rows (K padded by 16 bytes) and their f16 scales behind the V rows, decoded to
+            // f32 where a key is scored and where P.V reads V.
+            constexpr bool Q8 = kv_type_of<KV>() == KvType::Q8;
             constexpr int EPC = 16 / (int)sizeof(KV);
-            const int KT = mg_attn_tile(p.scratch_bytes, G, HD, (int)sizeof(KV));
+            const int KT = mg_attn_tile(p.scratch_bytes, G, HD, kv_type_of<KV>());
             constexpr int KLD = HD + EPC;
+            constexpr int NB = HD / KV_Q8_BLOCK;              // Q8: scale blocks per row
             float *qs = reinterpret_cast<float *>(scratch);  // [G][HD]
             float *red_m = qs + G * HD;                       // [MG_CWARPS][G] tile max per warp
             float *ps = red_m + MG_CWARPS * G;                // [G][KT] scores, then probabilities
             KV *ks = reinterpret_cast<KV *>(ps + G * KT);     // [KT][KLD]
             KV *vs = ks + KT * KLD;                           // [KT][HD]
+            __half *kds = reinterpret_cast<__half *>(vs + KT * HD);   // Q8: [KT][NB] K scales
+            __half *vds = kds + KT * NB;                              // Q8: [KT][NB] V scales
             const int H = p.H, Hkv = p.Hkv, NC = p.attn_chunks;
             KvView kvw;
             kvw.k = op.kc;
@@ -1099,16 +1144,42 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                     if (jt == j0)
                         for (int i = tid; i < G * HD / 4; i += MG_CTHREADS)
                             cp_async16(qs + 4 * i, p.qkv + (size_t)b * p.ld_qkv + (size_t)kvh * G * HD + 4 * i);
-                    for (int f = tid; f < n * (HD / EPC); f += MG_CTHREADS) {
-                        const int jj = f / (HD / EPC), c4 = f - jj * (HD / EPC);
-                        cp_async16(ks + jj * KLD + EPC * c4, kv_ptr<KV>(kvw.k) + kv_index<RING>(kvw, b, Hkv, kvh, jt + jj, HD) + EPC * c4);
+                    if constexpr (Q8) {
+                        // rows in 16-byte chunks; a row's scales are HD / 8 bytes: one 16-byte copy at HD 128, a 4-byte
+                        // load at HD 32 (stored before the barrier below)
+                        static_assert(NB * 2 == 16 || NB * 2 == 4, "Q8 scale row of 16 or 4 bytes");
+                        for (int f = tid; f < n * (HD / EPC); f += MG_CTHREADS) {
+                            const int jj = f / (HD / EPC), c4 = f - jj * (HD / EPC);
+                            cp_async16(ks + jj * KLD + EPC * c4, kv_q8_row<RING>(kv_ptr<KV>(kvw.k), kvw, b, Hkv, kvh, jt + jj, HD).q + EPC * c4);
+                        }
+                        for (int f = tid; f < n; f += MG_CTHREADS) {
+                            const __half *src = kv_q8_row<RING>(kv_ptr<KV>(kvw.k), kvw, b, Hkv, kvh, jt + f, HD).d;
+                            if constexpr (NB * 2 == 16) cp_async16(kds + f * NB, src);
+                            else *reinterpret_cast<unsigned *>(kds + f * NB) = __ldcg(reinterpret_cast<const unsigned *>(src));
+                        }
+                        cp_async_commit();
+                        for (int f = tid; f < n * (HD / EPC); f += MG_CTHREADS) {
+                            const int jj = f / (HD / EPC), c4 = f - jj * (HD / EPC);
+                            cp_async16(vs + jj * HD + EPC * c4, kv_q8_row<RING>(kv_ptr<KV>(kvw.v), kvw, b, Hkv, kvh, jt + jj, HD).q + EPC * c4);
+                        }
+                        for (int f = tid; f < n; f += MG_CTHREADS) {
+                            const __half *src = kv_q8_row<RING>(kv_ptr<KV>(kvw.v), kvw, b, Hkv, kvh, jt + f, HD).d;
+                            if constexpr (NB * 2 == 16) cp_async16(vds + f * NB, src);
+                            else *reinterpret_cast<unsigned *>(vds + f * NB) = __ldcg(reinterpret_cast<const unsigned *>(src));
+                        }
+                        cp_async_commit();
+                    } else {
+                        for (int f = tid; f < n * (HD / EPC); f += MG_CTHREADS) {
+                            const int jj = f / (HD / EPC), c4 = f - jj * (HD / EPC);
+                            cp_async16(ks + jj * KLD + EPC * c4, kv_ptr<KV>(kvw.k) + kv_index<RING>(kvw, b, Hkv, kvh, jt + jj, HD) + EPC * c4);
+                        }
+                        cp_async_commit();
+                        for (int f = tid; f < n * (HD / EPC); f += MG_CTHREADS) {
+                            const int jj = f / (HD / EPC), c4 = f - jj * (HD / EPC);
+                            cp_async16(vs + jj * HD + EPC * c4, kv_ptr<KV>(kvw.v) + kv_index<RING>(kvw, b, Hkv, kvh, jt + jj, HD) + EPC * c4);
+                        }
+                        cp_async_commit();
                     }
-                    cp_async_commit();
-                    for (int f = tid; f < n * (HD / EPC); f += MG_CTHREADS) {
-                        const int jj = f / (HD / EPC), c4 = f - jj * (HD / EPC);
-                        cp_async16(vs + jj * HD + EPC * c4, kv_ptr<KV>(kvw.v) + kv_index<RING>(kvw, b, Hkv, kvh, jt + jj, HD) + EPC * c4);
-                    }
-                    cp_async_commit();
                     cp_async_wait<1>();
                     cbar();  // q and the K tile have landed
                     if (jt == j0) {
@@ -1124,6 +1195,27 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                         float d0[G], d1[G];   // two chains per head
 #pragma unroll
                         for (int h = 0; h < G; ++h) d0[h] = d1[h] = 0.0f;
+                        if constexpr (Q8) {
+                            // one 16-byte row load and one scale per block; the chains see the elements in the f32 order
+                            const __half *kd = kds + tid * NB;
+#pragma unroll 2
+                            for (int blk = 0; blk < NB; ++blk) {
+                                const uint4 u = reinterpret_cast<const uint4 *>(kr)[blk];
+                                const float dk = __half2float(kd[blk]);
+#pragma unroll
+                                for (int hf = 0; hf < 2; ++hf) {
+                                    const int c = 4 * blk + 2 * hf;
+                                    const float4 ka = kv_q8_load4(hf ? u.z : u.x, dk), kb = kv_q8_load4(hf ? u.w : u.y, dk);
+#pragma unroll
+                                    for (int h = 0; h < G; ++h) {
+                                        const float4 qa = reinterpret_cast<const float4 *>(qs + h * HD)[c];
+                                        const float4 qb = reinterpret_cast<const float4 *>(qs + h * HD)[c + 1];
+                                        d0[h] = fmaf(qa.x, ka.x, fmaf(qa.y, ka.y, fmaf(qa.z, ka.z, fmaf(qa.w, ka.w, d0[h]))));
+                                        d1[h] = fmaf(qb.x, kb.x, fmaf(qb.y, kb.y, fmaf(qb.z, kb.z, fmaf(qb.w, kb.w, d1[h]))));
+                                    }
+                                }
+                            }
+                        } else {
 #pragma unroll 4
                         for (int c = 0; c < HD / 4; c += 2) {
                             float4 ka, kb;
@@ -1135,6 +1227,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                                 d0[h] = fmaf(qa.x, ka.x, fmaf(qa.y, ka.y, fmaf(qa.z, ka.z, fmaf(qa.w, ka.w, d0[h]))));
                                 d1[h] = fmaf(qb.x, kb.x, fmaf(qb.y, kb.y, fmaf(qb.z, kb.z, fmaf(qb.w, kb.w, d1[h]))));
                             }
+                        }
                         }
 #pragma unroll
                         for (int h = 0; h < G; ++h) {
@@ -1176,6 +1269,21 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                         const KV *vc = vs + od;
                         float a0 = 0.0f, a1 = 0.0f, s0 = 0.0f, s1 = 0.0f;
                         int j = 0;
+                        if constexpr (Q8) {
+                            const __half *vd = vds + od / KV_Q8_BLOCK;
+#pragma unroll 4
+                            for (; j + 1 < n; j += 2) {
+                                const float2 pj = *reinterpret_cast<const float2 *>(pr + j);
+                                a0 = fmaf(pj.x, kv_q8_load(vc[j * HD], __half2float(vd[j * NB])), a0);
+                                a1 = fmaf(pj.y, kv_q8_load(vc[(j + 1) * HD], __half2float(vd[(j + 1) * NB])), a1);
+                                s0 += pj.x;
+                                s1 += pj.y;
+                            }
+                            if (j < n) {
+                                a0 = fmaf(pr[j], kv_q8_load(vc[j * HD], __half2float(vd[j * NB])), a0);
+                                s0 += pr[j];
+                            }
+                        } else {
 #pragma unroll 4
                         for (; j + 1 < n; j += 2) {
                             const float2 pj = *reinterpret_cast<const float2 *>(pr + j);
@@ -1187,6 +1295,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaPa
                         if (j < n) {
                             a0 = fmaf(pr[j], kv_load(vc[j * HD]), a0);
                             s0 += pr[j];
+                        }
                         }
                         o_acc = fmaf(o_acc, alpha, a0 + a1);
                         o_sum = fmaf(o_sum, alpha, s0 + s1);
@@ -1406,7 +1515,8 @@ void launch_t(const MegaParams &p, const MegaPlan &plan, int grid, cudaStream_t 
 
 template <int MT, int G, int DPL>
 void launch_g(const MegaParams &p, const MegaPlan &plan, int grid, cudaStream_t st) {
-    if (plan.kv_bytes == 2) (p.ring ? launch_t<MT, G, DPL, true, __half> : launch_t<MT, G, DPL, false, __half>)(p, plan, grid, st);
+    if (plan.kv_type == KvType::Q8) (p.ring ? launch_t<MT, G, DPL, true, int8_t> : launch_t<MT, G, DPL, false, int8_t>)(p, plan, grid, st);
+    else if (plan.kv_type == KvType::F16) (p.ring ? launch_t<MT, G, DPL, true, __half> : launch_t<MT, G, DPL, false, __half>)(p, plan, grid, st);
     else (p.ring ? launch_t<MT, G, DPL, true, float> : launch_t<MT, G, DPL, false, float>)(p, plan, grid, st);
 }
 
@@ -1427,14 +1537,13 @@ MegaLaunch find_launch(int MT, int H, int Hkv, int hd) {
 }
 
 // Shared-memory plan for B streams given the largest K (in block pairs) of any matvec of the step and the KV cache's
-// element size in bytes (4: f32, 2: f16).
-MegaPlan decode_mega_plan(int B, int max_pairs, int H, int Hkv, int hd, int kv_bytes) {
-    VOX_CHECK(kv_bytes == 4 || kv_bytes == 2, VOX_EINVAL, "decode_mega: KV element of %d bytes", kv_bytes);
+// element type.
+MegaPlan decode_mega_plan(int B, int max_pairs, int H, int Hkv, int hd, KvType kv_type) {
     MegaPlan pl;
-    pl.kv_bytes = kv_bytes;
+    pl.kv_type = kv_type;
     pl.MT = B <= 1 ? 1 : (B <= 2 ? 2 : (B <= 4 ? 4 : 8));
     const int G = H / Hkv;
-    const int attn_bytes = mg_attn_fixed_bytes(G, hd) + 32 * mg_attn_key_bytes(G, hd, kv_bytes);   // a tile of at least 32 keys
+    const int attn_bytes = mg_attn_fixed_bytes(G, hd) + 32 * mg_attn_key_bytes(G, hd, kv_type);   // a tile of at least 32 keys
     const int per_pair = mg_pair_bytes(pl.MT);
     int cap_pairs = MG_SCRATCH_CAP / per_pair;
     if (cap_pairs >= MG_CHUNK) cap_pairs = cap_pairs / MG_CHUNK * MG_CHUNK;
@@ -1443,7 +1552,7 @@ MegaPlan decode_mega_plan(int B, int max_pairs, int H, int Hkv, int hd, int kv_b
     int scratch = pl.Ps_cap * per_pair;
     if (scratch < attn_bytes) scratch = attn_bytes;
     pl.scratch_bytes = (scratch + 127) & ~127;
-    pl.attn_tile = mg_attn_tile(pl.scratch_bytes, G, hd, kv_bytes);
+    pl.attn_tile = mg_attn_tile(pl.scratch_bytes, G, hd, kv_type);
     const int left = MG_SMEM_MAX - mg_misc_bytes(pl.MT) - pl.scratch_bytes;
     const int stage_bytes = mg_nt(pl.MT) * MG_SLOT_BYTES;
     int ns = left / stage_bytes;
@@ -1564,7 +1673,7 @@ unsigned DecodeMega::prepare(const Session &s, int R) {
     for (int j = 0; j < c.dec_layers; ++j)
         if (!m.dec[j].wqkv.qs_tc || !m.dec[j].wo.qs_tc || !m.dec[j].w13.qs_tc || !m.dec[j].w2.qs_tc) return 0;
     const int max_pairs = std::max(std::max(mg_pairs(D), mg_pairs(H * hd)), mg_pairs(c.dec_ffn));
-    g.plan = decode_mega_plan(B, max_pairs, H, Hkv, hd, (int)kv_elem_bytes(s.kv.type()));
+    g.plan = decode_mega_plan(B, max_pairs, H, Hkv, hd, s.kv.type());
     const int parts = (D + 15) / 16;
     std::vector<MegaOp> ops;
     bool ok = true;

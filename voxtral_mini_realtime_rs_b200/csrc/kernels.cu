@@ -689,17 +689,41 @@ __global__ void dec_rope_append_kernel(float *qkv, int M, int ld, int H, int Hkv
     }
     const float *krow = row + H * hd;
     const float *vrow = krow + Hkv * hd;
-    for (int t = threadIdx.x; t < Hkv * half; t += blockDim.x) {
-        const int h = t / half, p = t - h * half;
-        const float xr = krow[h * hd + 2 * p], xi = krow[h * hd + 2 * p + 1];
-        KV *dst = kv_ptr<KV>(kv.k) + kv_index<RING>(kv, b, Hkv, h, pos, hd) + 2 * p;
-        kv_store(dst, xr * cr[p] - xi * sr[p]);
-        kv_store(dst + 1, xr * sr[p] + xi * cr[p]);
-    }
-    for (int t = threadIdx.x; t < Hkv * hd; t += blockDim.x) {
-        const int h = t / hd, d = t - h * hd;
-        const float x = vrow[t];
-        kv_store(kv_ptr<KV>(kv.v) + kv_index<RING>(kv, b, Hkv, h, pos, hd) + d, x);
+    if constexpr (kv_type_of<KV>() == KvType::Q8) {
+        // a thread per 16-element block of one kv head's K after RoPE (then of V): the block's scale is local to it
+        const int nb = hd / KV_Q8_BLOCK;
+        for (int t = threadIdx.x; t < 2 * Hkv * nb; t += blockDim.x) {
+            const bool is_v = t >= Hkv * nb;
+            const int u = is_v ? t - Hkv * nb : t, h = u / nb, blk = u - h * nb;
+            float x[KV_Q8_BLOCK];
+            if (is_v) {
+#pragma unroll
+                for (int i = 0; i < KV_Q8_BLOCK; ++i) x[i] = vrow[h * hd + blk * KV_Q8_BLOCK + i];
+            } else {
+#pragma unroll
+                for (int i = 0; i < KV_Q8_BLOCK / 2; ++i) {
+                    const int p = blk * (KV_Q8_BLOCK / 2) + i;
+                    const float xr = krow[h * hd + 2 * p], xi = krow[h * hd + 2 * p + 1];
+                    x[2 * i] = xr * cr[p] - xi * sr[p];
+                    x[2 * i + 1] = xr * sr[p] + xi * cr[p];
+                }
+            }
+            const KvQ8Row r = kv_q8_row<RING>(kv_ptr<int8_t>(is_v ? kv.v : kv.k), kv, b, Hkv, h, pos, hd);
+            kv_q8_store16(r.q + blk * KV_Q8_BLOCK, r.d + blk, x);
+        }
+    } else {
+        for (int t = threadIdx.x; t < Hkv * half; t += blockDim.x) {
+            const int h = t / half, p = t - h * half;
+            const float xr = krow[h * hd + 2 * p], xi = krow[h * hd + 2 * p + 1];
+            KV *dst = kv_ptr<KV>(kv.k) + kv_index<RING>(kv, b, Hkv, h, pos, hd) + 2 * p;
+            kv_store(dst, xr * cr[p] - xi * sr[p]);
+            kv_store(dst + 1, xr * sr[p] + xi * cr[p]);
+        }
+        for (int t = threadIdx.x; t < Hkv * hd; t += blockDim.x) {
+            const int h = t / hd, d = t - h * hd;
+            const float x = vrow[t];
+            kv_store(kv_ptr<KV>(kv.v) + kv_index<RING>(kv, b, Hkv, h, pos, hd) + d, x);
+        }
     }
 }
 
@@ -707,7 +731,11 @@ void launch_dec_rope_append(float *qkv, int B, int M, int ld, int H, int Hkv, in
                             const RopeView &rope, cudaStream_t st) {
     dim3 grid(M, B);
     const bool f16 = kv.type == KvType::F16;
-    if (kv.ring && f16) dec_rope_append_kernel<true, __half><<<grid, 256, 0, st>>>(qkv, M, ld, H, Hkv, hd, kv, rope);
+    if (kv.type == KvType::Q8) {
+        VOX_CHECK(hd % KV_Q8_BLOCK == 0, VOX_EINVAL, "dec_rope_append: head_dim %d is not a multiple of %d", hd, KV_Q8_BLOCK);
+        if (kv.ring) dec_rope_append_kernel<true, int8_t><<<grid, 256, 0, st>>>(qkv, M, ld, H, Hkv, hd, kv, rope);
+        else dec_rope_append_kernel<false, int8_t><<<grid, 256, 0, st>>>(qkv, M, ld, H, Hkv, hd, kv, rope);
+    } else if (kv.ring && f16) dec_rope_append_kernel<true, __half><<<grid, 256, 0, st>>>(qkv, M, ld, H, Hkv, hd, kv, rope);
     else if (kv.ring) dec_rope_append_kernel<true, float><<<grid, 256, 0, st>>>(qkv, M, ld, H, Hkv, hd, kv, rope);
     else if (f16) dec_rope_append_kernel<false, __half><<<grid, 256, 0, st>>>(qkv, M, ld, H, Hkv, hd, kv, rope);
     else dec_rope_append_kernel<false, float><<<grid, 256, 0, st>>>(qkv, M, ld, H, Hkv, hd, kv, rope);
@@ -735,16 +763,28 @@ __global__ void dec_attention_kernel(const float *__restrict__ qkv, int M, int l
     const int base = RING ? j_lo : 0;
     float mx = -INFINITY;
     for (int j = j_lo + lane; j <= pos; j += 32) {
-        const KV *kr = kv_ptr<KV>(kv.k) + kv_index<RING>(kv, b, Hkv, kvh, j, hd);
         const float4 *q4 = reinterpret_cast<const float4 *>(qsm);
         float acc = 0.0f;
-        for (int d = 0; d < (hd >> 2); ++d) {
-            const float4 kk = kv_load4(kr, d);
-            const float4 qv = q4[d];
-            acc = fmaf(qv.x, kk.x, acc);
-            acc = fmaf(qv.y, kk.y, acc);
-            acc = fmaf(qv.z, kk.z, acc);
-            acc = fmaf(qv.w, kk.w, acc);
+        if constexpr (kv_type_of<KV>() == KvType::Q8) {
+            const KvQ8Row kr = kv_q8_row<RING>(kv_ptr<int8_t>(kv.k), kv, b, Hkv, kvh, j, hd);
+            for (int d = 0; d < (hd >> 2); ++d) {
+                const float4 kk = kv_q8_load4(reinterpret_cast<const uint32_t *>(kr.q)[d], __half2float(kr.d[d >> 2]));
+                const float4 qv = q4[d];
+                acc = fmaf(qv.x, kk.x, acc);
+                acc = fmaf(qv.y, kk.y, acc);
+                acc = fmaf(qv.z, kk.z, acc);
+                acc = fmaf(qv.w, kk.w, acc);
+            }
+        } else {
+            const KV *kr = kv_ptr<KV>(kv.k) + kv_index<RING>(kv, b, Hkv, kvh, j, hd);
+            for (int d = 0; d < (hd >> 2); ++d) {
+                const float4 kk = kv_load4(kr, d);
+                const float4 qv = q4[d];
+                acc = fmaf(qv.x, kk.x, acc);
+                acc = fmaf(qv.y, kk.y, acc);
+                acc = fmaf(qv.z, kk.z, acc);
+                acc = fmaf(qv.w, kk.w, acc);
+            }
         }
         acc *= scale;
         sc[j - base] = acc;
@@ -763,8 +803,15 @@ __global__ void dec_attention_kernel(const float *__restrict__ qkv, int M, int l
     float *orow = out + ((size_t)b * M + i) * (H * hd) + h * hd;
     for (int d = lane; d < hd; d += 32) {
         float acc = 0.0f;
-        for (int j = j_lo; j <= pos; ++j)
-            acc = fmaf(sc[j - base], kv_load(kv_ptr<KV>(kv.v)[kv_index<RING>(kv, b, Hkv, kvh, j, hd) + d]), acc);
+        if constexpr (kv_type_of<KV>() == KvType::Q8) {
+            for (int j = j_lo; j <= pos; ++j) {
+                const KvQ8Row vr = kv_q8_row<RING>(kv_ptr<int8_t>(kv.v), kv, b, Hkv, kvh, j, hd);
+                acc = fmaf(sc[j - base], kv_q8_load(vr.q[d], __half2float(vr.d[d / KV_Q8_BLOCK])), acc);
+            }
+        } else {
+            for (int j = j_lo; j <= pos; ++j)
+                acc = fmaf(sc[j - base], kv_load(kv_ptr<KV>(kv.v)[kv_index<RING>(kv, b, Hkv, kvh, j, hd) + d]), acc);
+        }
         orow[d] = acc * inv;
     }
 }
@@ -775,14 +822,18 @@ void launch_dec_attention(const float *qkv, int B, int M, int ld, int H, int Hkv
     dim3 grid(Hkv, M, B);
     const size_t smem = (size_t)G * (hd + kv.max_seq()) * sizeof(float);
     VOX_CHECK(smem <= 200 * 1024, VOX_EINVAL, "dec_attention: max_seq %d too large for the v1 kernel", kv.max_seq());
-    static SmemAttr attr, attr_ring, attr16, attr_ring16;
+    static SmemAttr attr, attr_ring, attr16, attr_ring16, attr8, attr_ring8;
     if (kv.ring) VOX_CHECK(window < kv.max_seq(), VOX_EINVAL, "dec_attention: window %d does not fit the KV ring", window);
     auto go = [&](auto kernel, SmemAttr &a) {
         if (smem > 48 * 1024) smem_attr_check(ensure_dyn_smem(kernel, smem, a), "dec_attention");
         kernel<<<grid, 32 * G, smem, st>>>(qkv, M, ld, H, Hkv, hd, kv, window, scale, out);
     };
     const bool f16 = kv.type == KvType::F16;
-    if (kv.ring && f16) go(dec_attention_kernel<true, __half>, attr_ring16);
+    if (kv.type == KvType::Q8) {
+        VOX_CHECK(hd % KV_Q8_BLOCK == 0, VOX_EINVAL, "dec_attention: head_dim %d is not a multiple of %d", hd, KV_Q8_BLOCK);
+        if (kv.ring) go(dec_attention_kernel<true, int8_t>, attr_ring8);
+        else go(dec_attention_kernel<false, int8_t>, attr8);
+    } else if (kv.ring && f16) go(dec_attention_kernel<true, __half>, attr_ring16);
     else if (kv.ring) go(dec_attention_kernel<true, float>, attr_ring);
     else if (f16) go(dec_attention_kernel<false, __half>, attr16);
     else go(dec_attention_kernel<false, float>, attr);

@@ -96,36 +96,57 @@ TcWork q4_matvec_tc_work_size(int N, int K);
 // Decoder KV cache of ONE layer as the attention kernels see it: PAGED (KVCache semantics of kv_cache.rs:52-142 --
 // append at the stream's position, read keys 0..pos -- over fixed-size pages so that sessions of different ages
 // share one pool).  Batch row b owns logical pages page_table[b][0..max_pages); logical position j lives at
-//   pool + ((phys(b, j / KV_PAGE) * Hkv + kv_head) * KV_PAGE + j % KV_PAGE) * hd.
+//   pool + ((phys(b, j / KV_PAGE) * Hkv + kv_head) * KV_PAGE + j % KV_PAGE) * hd  (Q8: kv_q8_row below).
 // Positions are per row (pos[b] = number of cached positions of row b = position of its next token): whole-utterance
 // batches keep them equal, streaming sessions do not.
 // ring: the page table row is a RING -- logical page lp lives in slot lp % max_pages and positions are unbounded (the
 // sessions of an unbounded stream pool, stream.cu; safe while max_pages * KV_PAGE > window + the rows a prefill writes
 // before reading).  The kernels take it as a template flag, so the non-ring code is the plain table walk.
 constexpr int KV_PAGE = 16;
-// Element type of the decoder KV cache, fixed for a session's lifetime (vox_session_create_ex kv_dtype): f32, or IEEE
-// binary16 (__half).  Kernels take the C++ type as a template parameter KV next to RING; every load and store of a
-// cached K or V element goes through kv_load / kv_store below, the one place the f16 format is decided.
-enum class KvType : uint8_t { F32 = 0, F16 = 1 };
-inline size_t kv_elem_bytes(KvType t) { return t == KvType::F16 ? 2 : 4; }
+// Element type of the decoder KV cache, fixed for a session's lifetime (vox_session_create_ex kv_dtype): f32, IEEE
+// binary16 (__half), or Q8: int8 with one f16 scale per 16 consecutive head dims (int8_t).  Kernels take the C++ type
+// as a template parameter KV next to RING; every load and store of a cached K or V element goes through kv_load /
+// kv_store and the kv_q8_* helpers below, the one place the formats are decided.
+enum class KvType : uint8_t { F32 = 0, F16 = 1, Q8 = 2 };
+// Q8 pages: each (page, kv head) unit holds its values [KV_PAGE][hd] int8 and then their scales [KV_PAGE][hd / 16] f16,
+// contiguous -- 2304 bytes at hd 128, 576 at hd 32, both multiples of 16, so one unit's rows and scales stage with
+// 16-byte copies.  Scale block i of a row covers its head dims [16i, 16i + 16).
+constexpr int KV_Q8_BLOCK = 16;
+// bytes of one (page, kv head) unit: KV_PAGE positions of hd values
+__host__ __device__ constexpr size_t kv_unit_bytes(KvType t, int hd) {
+    return t == KvType::Q8 ? (size_t)KV_PAGE * hd + (size_t)KV_PAGE * (hd / KV_Q8_BLOCK) * 2
+                           : (size_t)KV_PAGE * hd * (t == KvType::F16 ? 2 : 4);
+}
+template <typename KV> __host__ __device__ constexpr KvType kv_type_of() {
+    return sizeof(KV) == 1 ? KvType::Q8 : (sizeof(KV) == 2 ? KvType::F16 : KvType::F32);
+}
 // Base address of a KV page pool, typed by its element: kv_pool sets the member of the pool's KvType, kv_ptr<KV> reads
 // the member of the kernel's KV (the same type: a kernel instantiation is chosen by the view's KvType).
 union KvPool {
     float *f32 = nullptr;
     __half *f16;
+    int8_t *q8;   // byte address of the pool's (page, kv head) units
 };
 inline KvPool kv_pool(void *p, KvType t) {
     KvPool r;
     if (t == KvType::F16) r.f16 = static_cast<__half *>(p);
+    else if (t == KvType::Q8) r.q8 = static_cast<int8_t *>(p);
     else r.f32 = static_cast<float *>(p);
     return r;
 }
 template <typename KV> __host__ __device__ __forceinline__ KV *kv_ptr(const KvPool &p);
 template <> __host__ __device__ __forceinline__ float *kv_ptr<float>(const KvPool &p) { return p.f32; }
 template <> __host__ __device__ __forceinline__ __half *kv_ptr<__half>(const KvPool &p) { return p.f16; }
+template <> __host__ __device__ __forceinline__ int8_t *kv_ptr<int8_t>(const KvPool &p) { return p.q8; }
 template <typename KV> __host__ __device__ __forceinline__ KV *kv_ptr(const volatile KvPool &p);
 template <> __host__ __device__ __forceinline__ float *kv_ptr<float>(const volatile KvPool &p) { return p.f32; }
 template <> __host__ __device__ __forceinline__ __half *kv_ptr<__half>(const volatile KvPool &p) { return p.f16; }
+template <> __host__ __device__ __forceinline__ int8_t *kv_ptr<int8_t>(const volatile KvPool &p) { return p.q8; }
+// Q8 storage rule of one block x[0..16) (include/voxtral.h VOX_DTYPE_KV_Q8):
+//   a = max |x_i|, d = f16_rn(min(a / 127, 65504)), q_i = clamp(rint(x_i / d), -127, 127) (q_i = 0 when d == 0);
+//   a block holding a NaN stores d = NaN and q_i = 0.  Decoded value: (float)d * q_i, exact in f32.
+// The host mirror (DecoderKv::read) decodes with the same product.
+inline float kv_q8_decode_host(const int8_t q, const __half d) { return __half2float(d) * (float)q; }
 struct KvView {
     KvPool k, v;                       // [n_pages][Hkv][KV_PAGE][hd] of `type`
     const int *page_table = nullptr;   // [B][max_pages] physical page ids
@@ -181,6 +202,67 @@ __device__ __forceinline__ void kv_load8(const __half *row, const int c, float4 
     const float2 f3 = __half22float2(*reinterpret_cast<const __half2 *>(&u.w));
     a = make_float4(f0.x, f0.y, f1.x, f1.y);
     b = make_float4(f2.x, f2.y, f3.x, f3.y);
+}
+// ---- Q8: position j of (row b, kv head kvh) in a pool of (page, kv head) units (kv_unit_bytes): its hd values and
+// its hd / 16 scales
+struct KvQ8Row {
+    int8_t *q;
+    __half *d;
+};
+// row r of unit u = phys * Hkv + kv head
+__device__ __forceinline__ KvQ8Row kv_q8_at(int8_t *pool, const size_t u, const int r, const int hd) {
+    int8_t *unit = pool + u * kv_unit_bytes(KvType::Q8, hd);
+    return KvQ8Row{unit + (size_t)r * hd, reinterpret_cast<__half *>(unit + (size_t)KV_PAGE * hd) + r * (hd / KV_Q8_BLOCK)};
+}
+template <bool RING = false>
+__device__ __forceinline__ KvQ8Row kv_q8_row(int8_t *pool, const KvView &kv, const int b, const int Hkv, const int kvh, const int j,
+                                             const int hd) {
+    const int lp = j / KV_PAGE;
+    const int phys = kv.page_table[(size_t)b * kv.max_pages + (RING ? lp % kv.max_pages : lp)];
+    return kv_q8_at(pool, (size_t)phys * Hkv + kvh, j % KV_PAGE, hd);
+}
+// |x| as bits: ordered like the magnitudes, and any NaN compares above +inf (0x7f800000), so an integer max over a block
+// is its absmax with NaN propagated
+__device__ __forceinline__ unsigned kv_q8_abits(const float x) { return __float_as_uint(x) & 0x7fffffffu; }
+__device__ __forceinline__ unsigned kv_q8_abits4(const float4 x) {
+    return max(max(kv_q8_abits(x.x), kv_q8_abits(x.y)), max(kv_q8_abits(x.z), kv_q8_abits(x.w)));
+}
+// the block's scale from its absmax bits: f16_rn(min(a / 127, 65504)) (IEEE f32 division), NaN for a NaN block
+__device__ __forceinline__ __half kv_q8_scale(const unsigned abits) {
+    const float a = __uint_as_float(abits);
+    return abits > 0x7f800000u ? __float2half_rn(a) : __float2half_rn(fminf(a / 127.0f, 65504.0f));
+}
+// q = clamp(rint(x / d), -127, 127); 0 when d is 0 or NaN
+__device__ __forceinline__ int kv_q8_quant(const float x, const float d) {
+    if (!(d > 0.0f)) return 0;
+    return (int)fminf(fmaxf(rintf(x / d), -127.0f), 127.0f);
+}
+// four quantised values of scale d packed as the 4 bytes they are stored in
+__device__ __forceinline__ uint32_t kv_q8_pack4(const float4 x, const float d) {
+    return (uint32_t)(kv_q8_quant(x.x, d) & 0xff) | (uint32_t)(kv_q8_quant(x.y, d) & 0xff) << 8 |
+           (uint32_t)(kv_q8_quant(x.z, d) & 0xff) << 16 | (uint32_t)(kv_q8_quant(x.w, d) & 0xff) << 24;
+}
+// stores one whole block x[0..16) at q (16-byte aligned) and its scale at *d
+__device__ __forceinline__ void kv_q8_store16(int8_t *q, __half *d, const float *x) {
+    unsigned ab = 0;
+#pragma unroll
+    for (int i = 0; i < KV_Q8_BLOCK; ++i) ab = max(ab, kv_q8_abits(x[i]));
+    const __half dh = kv_q8_scale(ab);
+    const float df = __half2float(dh);
+    uint4 u;
+    u.x = kv_q8_pack4(make_float4(x[0], x[1], x[2], x[3]), df);
+    u.y = kv_q8_pack4(make_float4(x[4], x[5], x[6], x[7]), df);
+    u.z = kv_q8_pack4(make_float4(x[8], x[9], x[10], x[11]), df);
+    u.w = kv_q8_pack4(make_float4(x[12], x[13], x[14], x[15]), df);
+    *reinterpret_cast<uint4 *>(q) = u;
+    *d = dh;
+}
+// decoded value: (float)d * q, exact in f32
+__device__ __forceinline__ float kv_q8_load(const int8_t q, const float d) { return d * (float)q; }
+// four decoded values from their 4 stored bytes
+__device__ __forceinline__ float4 kv_q8_load4(const uint32_t u, const float d) {
+    return make_float4(d * (float)(int8_t)(u & 0xff), d * (float)(int8_t)((u >> 8) & 0xff), d * (float)(int8_t)((u >> 16) & 0xff),
+                       d * (float)(int8_t)(u >> 24));
 }
 #endif
 // Decoder RoPE tables as the kernels read them: cos / sin [rows][hd/2], position p at row p -- or, for a ring KvView, at
@@ -323,8 +405,8 @@ struct BeamWork {
 };
 void launch_beam_select(const int *top_ids, const float *top_lp, const int *out_pos, int out_ld, int b, int W, int n_live,
                         const BeamWork &w, int *tok, cudaStream_t st);
-// kc / vc: KV page pools of element type `type`, layer_stride elements per layer
-void launch_beam_fork(void *kc, void *vc, KvType type, size_t layer_stride, int layers, int *page_table, int max_pages,
+// kc / vc: KV page pools of element type `type`, layer_bytes bytes per layer
+void launch_beam_fork(void *kc, void *vc, KvType type, size_t layer_bytes, int layers, int *page_table, int max_pages,
                       const int *pos, const int *src, int rows, int Hkv, int hd, cudaStream_t st);
 void launch_beam_traceback(const BeamWork &w, int b, int W, int n, int out_ld, int *ids, double *scores, int *out,
                            int *top_ids, float *top_lp, cudaStream_t st, int s0 = 0, int out_stride = 1);

@@ -17,7 +17,7 @@ void DecoderKv::create(DeviceArena &arena, const vox_model_info &c, int rows, in
     hd = c.dec_head_dim;
     max_pages = ring ? (c.dec_window + launch) / KV_PAGE + 1 : (cap + KV_PAGE - 1) / KV_PAGE;
     n_pages = rows * max_pages;
-    const size_t bytes = (size_t)layers * layer_elems() * kv_elem_bytes(type);
+    const size_t bytes = (size_t)layers * layer_bytes();
     kc = arena.alloc(bytes);
     vc = arena.alloc(bytes);
     identity.resize((size_t)n_pages);
@@ -28,7 +28,7 @@ void DecoderKv::create(DeviceArena &arena, const vox_model_info &c, int rows, in
 }
 
 void *DecoderKv::pool(bool v, int layer) const {
-    return (char *)(v ? vc : kc) + (size_t)layer * layer_elems() * kv_elem_bytes(type_);
+    return (char *)(v ? vc : kc) + (size_t)layer * layer_bytes();
 }
 
 KvView DecoderKv::view(int layer, const int *pos) const {
@@ -44,7 +44,7 @@ KvView DecoderKv::view(int layer, const int *pos) const {
 }
 
 void DecoderKv::fork(const int *pos, const int *src, int rows, cudaStream_t st) {
-    launch_beam_fork(kc, vc, type_, layer_elems(), layers, table, max_pages, pos, src, rows, Hkv, hd, st);
+    launch_beam_fork(kc, vc, type_, layer_bytes(), layers, table, max_pages, pos, src, rows, Hkv, hd, st);
     forked = true;
 }
 
@@ -81,16 +81,26 @@ void DecoderKv::read(int layer, bool v, int B, int L, float *out) const {
     VOX_CHECK(!ring, VOX_EINVAL, "'kv_%c%d': not on ring-indexed sessions", v ? 'v' : 'k', layer);
     std::vector<int> pt((size_t)B * max_pages);
     CUDA_OK(cudaMemcpy(pt.data(), table, sizeof(int) * pt.size(), cudaMemcpyDeviceToHost));
-    std::vector<unsigned char> bytes(layer_elems() * kv_elem_bytes(type_));
+    std::vector<unsigned char> bytes(layer_bytes());
     CUDA_OK(cudaMemcpy(bytes.data(), pool(v, layer), bytes.size(), cudaMemcpyDeviceToHost));
-    const float *f32 = reinterpret_cast<const float *>(bytes.data());
-    const __half *f16 = reinterpret_cast<const __half *>(bytes.data());
+    const size_t unit_bytes = kv_unit_bytes(type_, hd);
     size_t o = 0;
     for (int b = 0; b < B; ++b)
         for (int j = 0; j < L; ++j)
             for (int h = 0; h < Hkv; ++h) {
-                const size_t at = (((size_t)pt[(size_t)b * max_pages + j / KV_PAGE] * Hkv + h) * KV_PAGE + j % KV_PAGE) * hd;
-                for (int d = 0; d < hd; ++d, ++o) out[o] = type_ == KvType::F16 ? __half2float(f16[at + d]) : f32[at + d];
+                const unsigned char *unit = bytes.data() + ((size_t)pt[(size_t)b * max_pages + j / KV_PAGE] * Hkv + h) * unit_bytes;
+                const int r = j % KV_PAGE;
+                if (type_ == KvType::Q8) {
+                    const int8_t *q = reinterpret_cast<const int8_t *>(unit) + (size_t)r * hd;
+                    const __half *d = reinterpret_cast<const __half *>(unit + (size_t)KV_PAGE * hd) + (size_t)r * (hd / KV_Q8_BLOCK);
+                    for (int i = 0; i < hd; ++i, ++o) out[o] = kv_q8_decode_host(q[i], d[i / KV_Q8_BLOCK]);
+                } else if (type_ == KvType::F16) {
+                    const __half *f16 = reinterpret_cast<const __half *>(unit) + (size_t)r * hd;
+                    for (int i = 0; i < hd; ++i, ++o) out[o] = __half2float(f16[i]);
+                } else {
+                    const float *f32 = reinterpret_cast<const float *>(unit) + (size_t)r * hd;
+                    for (int i = 0; i < hd; ++i, ++o) out[o] = f32[i];
+                }
             }
 }
 

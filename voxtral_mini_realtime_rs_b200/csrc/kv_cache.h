@@ -11,7 +11,8 @@ namespace vox {
 
 struct DeviceArena;
 
-// A session's decoder KV cache: page pools [layers][n_pages][Hkv][KV_PAGE][hd] of `type` for K and V, and a page table
+// A session's decoder KV cache: page pools [layers][n_pages][Hkv] of (page, kv head) units (kernels.h kv_unit_bytes: KV_PAGE
+// positions x hd of `type`) for K and V, and a page table
 // [rows][max_pages] of physical page ids.  Whole-utterance batches use the identity table (row b owns pages
 // b * max_pages ..), which beams fork through; a stream pool gives its streams pages from a free list and binds them to
 // the rows of each launch.  The element type is fixed for the cache's lifetime.
@@ -46,7 +47,7 @@ struct DecoderKv {
 
   private:
     void *pool(bool v, int layer) const;   // base of one layer's K or V pool
-    size_t layer_elems() const { return (size_t)n_pages * Hkv * KV_PAGE * hd; }
+    size_t layer_bytes() const { return (size_t)n_pages * Hkv * kv_unit_bytes(type_, hd); }
 
     KvType type_ = KvType::F32;
     bool ring = false;
