@@ -17,7 +17,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(CSRC, "build")
 LIB = os.path.join(HERE, "libvoxtral_b200.so")
 
-CU_SOURCES = ["kernels.cu", "matvec_tc.cu", "decode_attn.cu", "decode_mega.cu", "enc_attn_tc.cu", "gemm_tc5.cu", "beam.cu", "bias.cu", "kv_cache.cu", "encoder.cu", "model.cu", "stream.cu", "capi.cu"]
+CU_SOURCES = ["kernels.cu", "matvec_tc.cu", "decode_attn.cu", "decode_mega.cu", "enc_attn_tc.cu", "gemm_tc5.cu", "beam.cu", "bias.cu", "kv_cache.cu", "encoder.cu", "token_select.cu", "model.cu", "stream.cu", "capi.cu"]
 CXX_SOURCES = ["gguf.cpp", "audio_host.cpp", "tokenizer.cpp"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=default"]

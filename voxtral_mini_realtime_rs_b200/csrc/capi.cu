@@ -671,7 +671,7 @@ int32_t vox_transcribe_streaming(vox_session *sh, const float *mel, int32_t b, i
     VOX_API_BEGIN
     REQUIRE(sh); REQUIRE(mel); REQUIRE(out_ids); REQUIRE(n_out);
     Session *s = sh->s;
-    s->check_beam_bias();
+    s->sel.check_beam_bias();
     CUDA_OK(cudaSetDevice(s->m->device));
     CUDA_OK(cudaEventRecord(s->ev[0], s->st));
     s->enc.upload_mel(*s, mel, b, t);
@@ -681,10 +681,11 @@ int32_t vox_transcribe_streaming(vox_session *sh, const float *mel, int32_t b, i
     VOX_API_END
 }
 
+// `total`: the getters report the counts over all streams (a ragged call)
 static int32_t transcribe_pcm_impl(Session *s, const float *host, const float *dev, int b, size_t n, int normalize,
-                                   int32_t *out_ids, size_t cap, int32_t *n_out, vox_timings *tm) {
+                                   int32_t *out_ids, size_t cap, int32_t *n_out, vox_timings *tm, bool total = false) {
     s->check_batch(b);
-    s->check_beam_bias();
+    s->sel.check_beam_bias();
     VOX_CHECK(n >= 1, VOX_EINVAL, "empty audio");
     CUDA_OK(cudaSetDevice(s->m->device));
     vox_pad_config pc;
@@ -698,7 +699,7 @@ static int32_t transcribe_pcm_impl(Session *s, const float *host, const float *d
     CUDA_OK(cudaEventRecord(s->ev[0], s->st));
     s->enc.pcm_to_mel(*s, host, dev, lens.data(), b, normalize);
     CUDA_OK(cudaEventRecord(s->ev[1], s->st));
-    *n_out = s->transcribe_from_mel(b, (int)frames, out_ids, cap, tm);
+    *n_out = s->transcribe_from_mel(b, (int)frames, out_ids, cap, tm, total);
     fill_timings(s, tm);
     return VOX_OK;
 }
@@ -718,9 +719,8 @@ int32_t vox_transcribe_pcm_ragged(vox_session *sh, const float *samples, const s
     const vox_model_info &c = s->m->info;
     // every argument on the host, before any device work
     s->check_batch(b);
-    VOX_CHECK(s->beam_w == 1 || b * s->beam_w <= s->max_batch, VOX_EINVAL, "beam width %d x %d streams exceeds session max_batch %d",
-              s->beam_w, b, s->max_batch);
-    s->check_beam_bias();
+    s->sel.check_rows(b);
+    s->sel.check_beam_bias();
     size_t total = 0;
     bool equal = true;
     for (int i = 0; i < b; ++i) {
@@ -736,10 +736,9 @@ int32_t vox_transcribe_pcm_ragged(vox_session *sh, const float *samples, const s
     VOX_CHECK(cap >= total, VOX_ECAPACITY, "out_ids capacity %zu < %zu", cap, total);
     if (equal) {   // the batched [b][n] path: its layouts of ids, scores and n-best are the packed ones
         int32_t n = 0;
-        const int32_t rc = transcribe_pcm_impl(s, samples, nullptr, b, lens[0], normalize, out_ids, cap, &n, tm);
+        const int32_t rc = transcribe_pcm_impl(s, samples, nullptr, b, lens[0], normalize, out_ids, cap, &n, tm, true);
         for (int i = 0; i < b; ++i) n_out[i] = n;
-        s->scores_n = s->nbest_n = b * n;   // a ragged call reports the total over its streams
-        if (s->beam_w == 1) {   // like a ragged call, leave the decoder cache empty
+        if (s->sel.beam_w == 1) {   // like a ragged call, leave the decoder cache empty
             s->reset();
             CUDA_OK(cudaStreamSynchronize(s->st));
         }
@@ -817,7 +816,7 @@ int32_t vox_prefill(vox_session *sh, const int32_t *ids, int32_t b, int32_t m, i
     Session *s = sh->s;
     s->check_batch(b);
     VOX_CHECK(m >= 1 && m <= s->M_max, VOX_EINVAL, "M=%d out of range [1,%d]", m, s->M_max);
-    VOX_CHECK(s->beam_w == 1, VOX_EINVAL, "vox_prefill runs greedy only: the session's beam width is %d", s->beam_w);
+    s->sel.check_greedy("vox_prefill");
     VOX_CHECK(s->cache_len + m <= s->out_ld, VOX_EINVAL, "KV cache full (%d + %d > %d)", s->cache_len, m, s->out_ld);
     if (add_audio)
         VOX_CHECK(b == (int)s->enc.audio_offs.size() && s->cache_len + m <= s->enc.positions, VOX_EINVAL,
@@ -835,7 +834,7 @@ int32_t vox_decode_step(vox_session *sh, const int32_t *tok, int32_t b, int32_t 
     REQUIRE(sh);
     Session *s = sh->s;
     s->check_batch(b);
-    VOX_CHECK(s->beam_w == 1, VOX_EINVAL, "vox_decode_step runs greedy only: the session's beam width is %d", s->beam_w);
+    s->sel.check_greedy("vox_decode_step");
     VOX_CHECK(s->cache_len + 1 <= s->out_ld, VOX_EINVAL, "KV cache full (%d + 1 > %d)", s->cache_len, s->out_ld);
     if (add_audio)
         VOX_CHECK(b == (int)s->enc.audio_offs.size() && s->cache_len < s->enc.positions, VOX_EINVAL,
@@ -855,7 +854,7 @@ static_assert(VOX_MAX_TOP_K == TOPK_MAX, "the score buffers hold VOX_MAX_TOP_K e
 int32_t vox_session_set_top_k(vox_session *s, int32_t k) {
     VOX_API_BEGIN
     REQUIRE(s);
-    s->s->set_top_k(k);
+    s->s->sel.set_top_k(k);
     VOX_API_END
 }
 int32_t vox_session_token_scores(vox_session *sh, int32_t *top_ids, float *top_logprobs, size_t cap, int32_t *b, int32_t *n,
@@ -863,38 +862,14 @@ int32_t vox_session_token_scores(vox_session *sh, int32_t *top_ids, float *top_l
     VOX_API_BEGIN
     REQUIRE(sh);
     Session *s = sh->s;
-    const int K = s->scores_k;
-    VOX_CHECK(K > 0, VOX_EINVAL, "no token scores: the last transcribe, prefill or decode step ran with top_k 0 (vox_session_set_top_k)");
-    if (b) *b = (int32_t)s->score_spans.size();
-    if (n) *n = s->scores_n;
-    if (k) *k = K;
-    if (!top_ids && !top_logprobs) return VOX_OK;
-    REQUIRE(top_ids); REQUIRE(top_logprobs);
-    size_t need = 0;
-    for (const Session::ScoreSpan &r : s->score_spans) need += (size_t)r.n * K;
-    VOX_CHECK(cap >= need, VOX_ECAPACITY, "token scores capacity %zu < %zu", cap, need);
-    CUDA_OK(cudaSetDevice(s->m->device));
-    CUDA_OK(cudaStreamSynchronize(s->st));
-    // one stream after the other: entries [pos0, pos0 + n) of its row of the device's [row][out_ld][VOX_MAX_TOP_K]
-    // buffers, the first K of each
-    const size_t pitch = sizeof(int32_t) * VOX_MAX_TOP_K;
-    size_t dst = 0;
-    for (const Session::ScoreSpan &r : s->score_spans) {
-        if (r.n == 0) continue;
-        const size_t at = ((size_t)r.row * s->out_ld + r.pos0) * VOX_MAX_TOP_K;
-        CUDA_OK(cudaMemcpy2D(top_ids + dst, sizeof(int32_t) * K, s->d_top_ids + at, pitch, sizeof(int32_t) * K, r.n,
-                             cudaMemcpyDeviceToHost));
-        CUDA_OK(cudaMemcpy2D(top_logprobs + dst, sizeof(float) * K, s->d_top_lp + at, pitch, sizeof(float) * K, r.n,
-                             cudaMemcpyDeviceToHost));
-        dst += (size_t)r.n * K;
-    }
+    s->sel.read_scores(top_ids, top_logprobs, cap, b, n, k, s->st);
     VOX_API_END
 }
 static_assert(VOX_MAX_BEAM == BEAM_MAX, "the beam kernels handle up to VOX_MAX_BEAM beams per stream");
 int32_t vox_session_set_beam(vox_session *s, int32_t width) {
     VOX_API_BEGIN
     REQUIRE(s);
-    s->s->set_beam(width);
+    s->s->sel.set_beam(width);
     VOX_API_END
 }
 static_assert(VOX_MAX_BIAS_PHRASES == BIAS_MAX_PHRASES && VOX_MAX_BIAS_LEN == BIAS_MAX_LEN &&
@@ -960,25 +935,7 @@ int32_t vox_session_nbest(vox_session *sh, int32_t *ids, double *scores, size_t 
     VOX_API_BEGIN
     REQUIRE(sh);
     Session *s = sh->s;
-    const int W = s->nbest_w;
-    VOX_CHECK(W > 0, VOX_EINVAL, "no n-best list: the last transcribe ran at beam width 1 (vox_session_set_beam)");
-    if (b) *b = (int32_t)s->nbest_spans.size();
-    if (w) *w = W;
-    if (n) *n = s->nbest_n;
-    if (!ids && !scores) return VOX_OK;
-    REQUIRE(ids); REQUIRE(scores);
-    size_t need = 0;
-    for (const Session::NbestSpan &r : s->nbest_spans) need += (size_t)W * r.n;
-    VOX_CHECK(cap >= need, VOX_ECAPACITY, "n-best capacity %zu < %zu", cap, need);
-    CUDA_OK(cudaSetDevice(s->m->device));
-    CUDA_OK(cudaStreamSynchronize(s->st));
-    // one stream after the other: its W hypotheses of n ids each, and its W scores
-    for (const Session::NbestSpan &r : s->nbest_spans) {
-        if (r.n > 0) CUDA_OK(cudaMemcpy(ids, s->d_nbest_ids + r.ids, sizeof(int32_t) * W * r.n, cudaMemcpyDeviceToHost));
-        CUDA_OK(cudaMemcpy(scores, s->d_nbest_scores + r.scores, sizeof(double) * W, cudaMemcpyDeviceToHost));
-        ids += (size_t)W * r.n;
-        scores += W;
-    }
+    s->sel.read_nbest(ids, scores, cap, b, w, n, s->st);
     VOX_API_END
 }
 int32_t vox_session_cache_len(const vox_session *s, int32_t *len) {
@@ -1223,7 +1180,7 @@ int32_t vox_stream_poll_scored(vox_stream_pool *p, int32_t session, int32_t *ids
                                size_t cap, size_t *n, int32_t *done) {
     VOX_API_BEGIN
     REQUIRE(p); REQUIRE(n);
-    VOX_CHECK(p->p->s->top_k > 0, VOX_EINVAL, "no token scores: the pool's top_k is 0 (vox_stream_pool_set_top_k)");
+    VOX_CHECK(p->p->s->sel.top_k > 0, VOX_EINVAL, "no token scores: the pool's top_k is 0 (vox_stream_pool_set_top_k)");
     if (cap) { REQUIRE(ids); REQUIRE(top_ids); REQUIRE(top_logprobs); }
     bool d = false;
     *n = p->p->poll(session, ids, top_ids, top_logprobs, cap, &d);

@@ -409,6 +409,7 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ri
         // decoder
         s->kv.create(s->arena, c, max_batch, S4_max, s->M_max, kv_ring, kv_type);
         s->out_ld = s->kv.capacity();
+        s->sel.create(s->arena, m->device, max_batch, s->out_ld, c.vocab);
         s->dec_rope = m->dec_rope();
         const size_t drows = B * s->M_max;
         const int qkvd = (c.dec_heads + 2 * c.dec_kv_heads) * c.dec_head_dim;
@@ -421,7 +422,6 @@ Session *Session::create(Model *m, int max_batch, int max_mel_frames, bool kv_ri
         s->logits = s->arena.alloc_n<float>(B * c.vocab);
         s->ada_sets = s->arena.alloc_n<float>(B * s->ada_set_floats());
         s->delays.assign(B, 0.0f);
-        s->bias_n.assign(B, 0);
         s->d_ada_rows = (const float **)s->arena.alloc(sizeof(float *) * B);
         s->d_fga_rows = (const float **)s->arena.alloc(sizeof(float *) * B);
         s->d_audio_off = s->arena.alloc_n<int64_t>(B);
@@ -570,7 +570,7 @@ void Session::bind_rows(int B) {
     CUDA_OK(cudaMemcpyAsync(d_ada_rows, a.data(), sizeof(float *) * B, cudaMemcpyHostToDevice, st));
     CUDA_OK(cudaMemcpyAsync(d_fga_rows, f.data(), sizeof(float *) * B, cudaMemcpyHostToDevice, st));
     CUDA_OK(cudaMemcpyAsync(d_audio_off, offs.data(), sizeof(int64_t) * B, cudaMemcpyHostToDevice, st));
-    if (d_row_stream) CUDA_OK(cudaMemcpyAsync(d_row_stream, streams.data(), sizeof(int) * B, cudaMemcpyHostToDevice, st));
+    sel.bind_rows(streams, st);
     CUDA_OK(cudaStreamSynchronize(st));   // the staging vectors die with this frame
     bound_streams = std::move(streams);
     bound_offs = std::move(offs);
@@ -665,141 +665,12 @@ unsigned Session::decode_step(int B, bool add_audio) {
         launch_argmax_multi(logits, B, m->info.vocab, d_tok, d_out, out_ld, d_outpos, am_vals, am_idx, am_cnt, st);
         launch_advance(d_pos, 1, d_outpos, 1, B, st);
     }
-    bias_select(B);    // one launch over every row (every group of the persistent kernel's) ...
-    token_scores(B);   // ... and so is this one
+    sel.after_step(*this, B);   // over every row (every group of the persistent kernel's)
     return mega_launches;
 }
 
-void Session::set_top_k(int k) {
-    VOX_CHECK(k >= 0 && k <= TOPK_MAX, VOX_EINVAL, "top_k %d out of range [0,%d]", k, TOPK_MAX);
-    if (k > 0) alloc_scores();
-    top_k = k;
-}
-
-void Session::alloc_scores() {
-    if (d_top_ids) return;
-    CUDA_OK(cudaSetDevice(m->device));
-    const size_t n = (size_t)max_batch * out_ld * TOPK_MAX, parts = (size_t)max_batch * ARGMAX_PARTS;
-    d_top_ids = arena.alloc_n<int>(n);
-    d_top_lp = arena.alloc_n<float>(n);
-    score_work.m = arena.alloc_n<float>(parts);
-    score_work.l = arena.alloc_n<float>(parts);
-    score_work.vals = arena.alloc_n<float>(parts * TOPK_MAX);
-    score_work.idx = arena.alloc_n<int>(parts * TOPK_MAX);
-    score_work.counters = arena.alloc_n<int>(max_batch);
-    CUDA_OK(cudaMemset(score_work.counters, 0, sizeof(int) * max_batch));
-}
-
-// after the step's argmax and counter advance: row b's scores land at its output position d_outpos[b] - 1
-void Session::token_scores(int B) {
-    // at W > 1 every step belongs to a beam call (the incremental calls refuse to run), whose selection reads W candidates
-    const int k = std::max(top_k, beam_w > 1 ? beam_w : 0);
-    if (k > 0) launch_token_scores(logits, B, m->info.vocab, k, d_outpos, out_ld, d_top_ids, d_top_lp, score_work, st);
-}
-
 void Session::set_bias(int stream, const int32_t *ids, const int32_t *lens, const float *boosts, int n) {
-    VOX_CHECK(stream >= -1 && stream < max_batch, VOX_EINVAL, "set_bias: stream %d out of range [0,%d) (or -1 for every stream)",
-              stream, max_batch);
-    VOX_CHECK(n >= 0 && n <= BIAS_MAX_PHRASES, VOX_EINVAL, "set_bias: %d phrases out of range [0,%d]", n, BIAS_MAX_PHRASES);
-    VOX_CHECK(n == 0 || (ids && lens && boosts), VOX_EINVAL, "set_bias: NULL ids, lens or boosts with %d phrases", n);
-    // phrase p is ids[off_p .. off_p + lens[p]), padded to BIAS_MAX_LEN ids in the device layout
-    std::vector<int> packed((size_t)n * BIAS_MAX_LEN, 0), hist(BIAS_HIST + 1, 0);
-    for (int p = 0, off = 0; p < n; off += lens[p], ++p) {
-        VOX_CHECK(lens[p] >= 1 && lens[p] <= BIAS_MAX_LEN, VOX_EINVAL, "set_bias: phrase %d has %d ids (1..%d)", p, lens[p],
-                  BIAS_MAX_LEN);
-        VOX_CHECK(std::isfinite(boosts[p]) && boosts[p] > 0.0f, VOX_EINVAL, "set_bias: boost %g of phrase %d must be finite and > 0",
-                  boosts[p], p);
-        for (int j = 0; j < lens[p]; ++j) {
-            const int t = ids[off + j];
-            VOX_CHECK(t >= BIAS_FIRST_TEXT_ID && t < m->info.vocab, VOX_EINVAL, "set_bias: id %d of phrase %d outside [%d,%d)", t, p,
-                      BIAS_FIRST_TEXT_ID, m->info.vocab);
-            packed[(size_t)p * BIAS_MAX_LEN + j] = t;
-        }
-    }
-    if (n == 0 && !bias.ids) return;   // nothing was ever set: nothing to clear
-    CUDA_OK(cudaSetDevice(m->device));
-    if (!bias.ids) {
-        const size_t S = max_batch;
-        bias.ids = arena.alloc_n<int>(S * BIAS_MAX_PHRASES * BIAS_MAX_LEN);
-        bias.lens = arena.alloc_n<int>(S * BIAS_MAX_PHRASES);
-        bias.boosts = arena.alloc_n<float>(S * BIAS_MAX_PHRASES);
-        bias.n_phrases = arena.alloc_n<int>(S);
-        bias.hist = arena.alloc_n<int>(S * (BIAS_HIST + 1));
-        d_row_stream = arena.alloc_n<int>(S);
-        CUDA_OK(cudaMemsetAsync(bias.n_phrases, 0, sizeof(int) * S, st));
-        CUDA_OK(cudaMemsetAsync(bias.hist, 0, sizeof(int) * S * (BIAS_HIST + 1), st));
-        bound_streams.clear();   // the next bind_rows fills the row table
-    }
-    for (int s = stream < 0 ? 0 : stream; s < (stream < 0 ? max_batch : stream + 1); ++s) {
-        const size_t p0 = (size_t)s * BIAS_MAX_PHRASES;
-        if (n > 0) {
-            CUDA_OK(cudaMemcpyAsync(bias.ids + p0 * BIAS_MAX_LEN, packed.data(), sizeof(int) * packed.size(), cudaMemcpyHostToDevice, st));
-            CUDA_OK(cudaMemcpyAsync(bias.lens + p0, lens, sizeof(int) * n, cudaMemcpyHostToDevice, st));
-            CUDA_OK(cudaMemcpyAsync(bias.boosts + p0, boosts, sizeof(float) * n, cudaMemcpyHostToDevice, st));
-        }
-        CUDA_OK(cudaMemcpyAsync(bias.n_phrases + s, &n, sizeof(int), cudaMemcpyHostToDevice, st));
-        CUDA_OK(cudaMemcpyAsync(bias.hist + (size_t)s * (BIAS_HIST + 1), hist.data(), sizeof(int) * hist.size(),
-                                cudaMemcpyHostToDevice, st));
-        bias_n[s] = n;
-    }
-    CUDA_OK(cudaStreamSynchronize(st));   // the staging vectors and the caller's buffers
-}
-
-void Session::clear_bias_history(int stream) {
-    if (!bias.hist) return;
-    const size_t per = BIAS_HIST + 1;
-    if (stream < 0) CUDA_OK(cudaMemsetAsync(bias.hist, 0, sizeof(int) * max_batch * per, st));
-    else CUDA_OK(cudaMemsetAsync(bias.hist + (size_t)stream * per, 0, sizeof(int) * per, st));
-}
-
-void Session::bias_select(int B) {
-    if (bias_on()) launch_bias_select(logits, B, m->info.vocab, d_row_stream, bias, d_tok, d_out, out_ld, d_outpos, st);
-}
-
-void Session::check_beam_bias() const {
-    VOX_CHECK(beam_w == 1 || !bias_on(), VOX_EINVAL, "beam search (width %d) does not take phrase boosting: clear the bias lists",
-              beam_w);
-}
-
-static_assert(BEAM_MAX <= TOPK_MAX, "a beam's candidates are the first W entries of its row's top-k list");
-
-void Session::set_beam(int w) {
-    VOX_CHECK(w >= 1 && w <= BEAM_MAX, VOX_EINVAL, "beam width %d out of range [1,%d]", w, BEAM_MAX);
-    if (w > 1 && !beam.rank_row) {
-        alloc_scores();
-        const size_t rows = max_batch, hist = (size_t)max_batch * out_ld;
-        beam.rank_row = arena.alloc_n<int>(rows);
-        beam.cum = arena.alloc_n<double>(rows);
-        beam.src = arena.alloc_n<int>(rows);
-        beam.hist_tok = arena.alloc_n<int>(hist);
-        beam.hist_par = arena.alloc_n<int>(hist);
-        d_nbest_ids = arena.alloc_n<int>(hist);   // b * W <= max_batch hypotheses of n <= out_ld ids
-        d_nbest_scores = arena.alloc_n<double>(rows);
-    }
-    beam_w = w;
-}
-
-// The prefill left stream s's prefix in row s.  Beam rows w * b + s take stream s's step counters (and read its audio
-// embeddings through row_streams); the selection at position 0 has one live rank per stream (the prefix, score 0), whose
-// top-W ids become the W beams, and the fork hands the prefix's KV to the other rows.
-void Session::beam_start(int b) {
-    const int W = beam_w;
-    for (int w = 1; w < W; ++w) {
-        CUDA_OK(cudaMemcpyAsync(d_pos + w * b, d_pos, sizeof(int) * b, cudaMemcpyDeviceToDevice, st));
-        CUDA_OK(cudaMemcpyAsync(d_outpos + w * b, d_outpos, sizeof(int) * b, cudaMemcpyDeviceToDevice, st));
-    }
-    std::vector<int> rank_row((size_t)b * W);
-    for (int s = 0; s < b; ++s)
-        for (int w = 0; w < W; ++w) rank_row[(size_t)s * W + w] = w * b + s;
-    CUDA_OK(cudaMemcpyAsync(beam.rank_row, rank_row.data(), sizeof(int) * rank_row.size(), cudaMemcpyHostToDevice, st));
-    CUDA_OK(cudaMemsetAsync(beam.cum, 0, sizeof(double) * b * W, st));
-    CUDA_OK(cudaStreamSynchronize(st));   // rank_row dies with this frame
-    beam_step(b, 1);
-}
-
-void Session::beam_step(int b, int n_live) {
-    launch_beam_select(d_top_ids, d_top_lp, d_outpos, out_ld, b, beam_w, n_live, beam, d_tok, st);
-    kv.fork(d_pos, beam.src, b * beam_w, st);
+    if (sel.set_bias(stream, ids, lens, boosts, n, st)) bound_streams.clear();   // the next bind_rows fills the row table
 }
 
 // Prefill of M positions for B streams (model.rs:894-923 with M = 38; also the incremental vox_prefill).
@@ -818,18 +689,15 @@ void Session::prefill(int B, int M, const int *ids_host, bool add_audio) {
     linear(m->tok_emb, last_h, B, logits, c.vocab, nullptr, nullptr, EPI_NONE);
     launch_argmax(logits, B, c.vocab, d_tok, d_out, out_ld, d_outpos, st);
     launch_advance(d_pos, M, d_outpos, 1, B, st);
-    bias_select(B);
-    token_scores(B);
+    sel.after_step(*this, B);
 }
 
 void Session::step_incremental(int b, int M, const int *ids_host, bool add_audio) {
     if (ids_host) prefill(b, M, ids_host, add_audio);
     else decode_step(b, add_audio);
     cache_len += M;
-    scores_k = top_k;
-    scores_n = 1;
-    score_spans.resize(b);
-    for (int r = 0; r < b; ++r) score_spans[r] = {r, out_rows[r]++, 1};   // each row's output just emitted
+    sel.record_step(b, out_rows.data());   // each row's output just emitted
+    for (int r = 0; r < b; ++r) ++out_rows[r];
 }
 
 void Session::reset() {
@@ -838,7 +706,7 @@ void Session::reset() {
     std::fill(out_rows.begin(), out_rows.end(), 0);
     cache_len = 0;
     kv.restore_identity(st);
-    clear_bias_history(-1);
+    sel.clear_bias_history(-1, st);
     rebase_epoch();
 }
 
@@ -849,7 +717,7 @@ template <class Step>
 void Session::run_steps(int R, int n, Step step) {
     if (n <= 0) return;
     prepare_step(R);
-    const StepKey key{R, top_k, beam_w, path.matvec_tc, path.gemm_tc, use_mega, bias_on()};
+    const StepKey key{R, sel.top_k, sel.beam_w, path.matvec_tc, path.gemm_tc, use_mega, sel.bias_on()};
     if (use_graph && !(step_graph.exec && step_graph.key == key)) {
         // first step eagerly (also performs any one-time kernel attribute setup), then capture one step and replay it
         step();
@@ -896,10 +764,10 @@ struct RowStreams {
 
 // Q4VoxtralModel::transcribe_streaming (model.rs:873-963).  Expects the mel in enc.mel_tm; records
 // ev[2] (after encode), ev[4] (after the prefill) and ev[3] (after decode) on the stream.  Returns tokens per stream.
-int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids, vox_timings *tm) {
+int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids, vox_timings *tm, bool total) {
     const vox_model_info &c = m->info;
-    const int W = beam_w, R = B * W;   // decode rows: beam w of stream s in row w * B + s
-    VOX_CHECK(W == 1 || R <= max_batch, VOX_EINVAL, "beam width %d x %d streams exceeds session max_batch %d", W, B, max_batch);
+    const int W = sel.beam_w, R = B * W;   // decode rows: beam w of stream s in row w * B + s
+    sel.check_rows(B);
     RowStreams row_guard{this};
     if (W > 1)
         for (int r = 0; r < R; ++r) row_streams.push_back(r % B);
@@ -917,18 +785,28 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
         std::vector<int> prefix((size_t)B * P, 32);
         for (int b = 0; b < B; ++b) prefix[(size_t)b * P] = 1;
         prefill(B, P, prefix.data(), true);
-        if (W > 1) beam_start(B);
+        if (W > 1) {
+            // beam rows w * B + s take stream s's step counters (and read its audio embeddings through row_streams); the
+            // selection at position 0 has one live rank per stream (the prefix, score 0), whose top-W ids become the W
+            // beams, and the fork hands the prefix's KV to the other rows
+            for (int w = 1; w < W; ++w) {
+                CUDA_OK(cudaMemcpyAsync(d_pos + w * B, d_pos, sizeof(int) * B, cudaMemcpyDeviceToDevice, st));
+                CUDA_OK(cudaMemcpyAsync(d_outpos + w * B, d_outpos, sizeof(int) * B, cudaMemcpyDeviceToDevice, st));
+            }
+            std::vector<int> rank_row((size_t)B * W);
+            for (int s = 0; s < B; ++s)
+                for (int w = 0; w < W; ++w) rank_row[(size_t)s * W + w] = w * B + s;
+            sel.beam_begin(*this, rank_row, B);
+        }
         CUDA_OK(cudaEventRecord(ev[4], st));
         run_steps(R, S4 - P - 1, [&] {
             const unsigned launches = decode_step(R);
-            if (W > 1) beam_step(B, W);
+            if (W > 1) sel.beam_step(*this, B, W);
             return launches;
         });
-        if (W > 1)
-            launch_beam_traceback(beam, B, W, n_out, out_ld, d_nbest_ids, d_nbest_scores, d_out, top_k > 0 ? d_top_ids : nullptr,
-                                  d_top_lp, st);
+        if (W > 1) sel.traceback(*this, std::vector<int>(B, n_out).data(), B, 1);
     } else if (W > 1) {
-        CUDA_OK(cudaMemsetAsync(d_nbest_scores, 0, sizeof(double) * R, st));
+        sel.zero_nbest_scores(0, B, st);
     }
     if (S4 < P) CUDA_OK(cudaEventRecord(ev[4], st));
     CUDA_OK(cudaEventRecord(ev[3], st));
@@ -946,15 +824,9 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
         if (S4 >= P)   // the prefill's output and one per step
             for (int b = 0; b < B; ++b) out_rows[b] = std::max(n_out, 1);
     }
-    scores_k = top_k;
-    nbest_w = W > 1 ? W : 0;
-    scores_n = nbest_n = n_out;
-    score_spans.resize(B);
-    nbest_spans.resize(B);
-    for (int b = 0; b < B; ++b) {   // stream b's rank 0 beam is row b, the traceback's ids are [B][W][n_out]
-        score_spans[b] = {b, 0, n_out};
-        nbest_spans[b] = {(size_t)b * W * n_out, b * W, n_out};
-    }
+    std::vector<int> order(B), n(B, n_out);   // stream b's rank 0 beam is row b, the traceback's ids are [B][W][n_out]
+    for (int b = 0; b < B; ++b) order[b] = b;
+    sel.record_transcribe(B, order.data(), n.data(), 1, total);
     if (tm) {
         tm->seq_len = S4;
         tm->decode_tokens = n_out;
@@ -971,7 +843,7 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
 // steps run in segments, one per distinct output count, each over the rows still live.
 //
 // transcribe_from_mel is not this function at equal lengths, and moving it here would change what it costs and computes:
-//   - it prefills b rows and replicates them to the beam rows (beam_start).  Here the rows are stream-major, so that the
+//   - it prefills b rows and replicates them to the beam rows (then beam_begin).  Here the rows are stream-major, so that the
 //     live streams stay a prefix of the rows; a prefill row is then both a fork source and another stream's fork
 //     destination, and all b * W rows take the prefill: the prefill GEMMs' M grows W-fold (38 -> 304 at 1 stream x 8
 //     beams; not measured for that case).
@@ -980,9 +852,9 @@ int Session::transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids,
 void Session::transcribe_ragged(const float *samples, const size_t *lens, int b, int normalize, int32_t *out_ids,
                                 int32_t *n_out, vox_timings *tm) {
     const vox_model_info &c = m->info;
-    const int W = beam_w, P = c.prefix_len;
+    const int W = sel.beam_w, P = c.prefix_len;
     check_batch(b);
-    VOX_CHECK(W == 1 || b * W <= max_batch, VOX_EINVAL, "beam width %d x %d streams exceeds session max_batch %d", W, b, max_batch);
+    sel.check_rows(b);
     std::vector<StreamGeom> g(b);
     for (int s = 0; s < b; ++s) {
         g[s] = stream_geometry(c, lens[s]);
@@ -1022,10 +894,7 @@ void Session::transcribe_ragged(const float *samples, const size_t *lens, int b,
         if (W > 1) {
             std::vector<int> rank_row(R0);
             for (int r = 0; r < R0; ++r) rank_row[r] = r;
-            CUDA_OK(cudaMemcpyAsync(beam.rank_row, rank_row.data(), sizeof(int) * R0, cudaMemcpyHostToDevice, st));
-            CUDA_OK(cudaMemsetAsync(beam.cum, 0, sizeof(double) * R0, st));
-            CUDA_OK(cudaStreamSynchronize(st));   // rank_row dies with this frame
-            beam_step(live, 1);
+            sel.beam_begin(*this, rank_row, live);
         }
         CUDA_OK(cudaEventRecord(ev[4], st));
         for (int t = 1; t < n_max;) {   // outputs [0, t) of every live stream are done
@@ -1034,28 +903,22 @@ void Session::transcribe_ragged(const float *samples, const size_t *lens, int b,
             const int t_end = g[order[L - 1]].n_out;
             run_steps(L * W, t_end - t, [&] {
                 const unsigned launches = decode_step(L * W);
-                if (W > 1) beam_step(L, W);
+                if (W > 1) sel.beam_step(*this, L, W);
                 return launches;
             });
             t = t_end;
         }
-        if (W > 1)
-            for (int i0 = 0, off = 0; i0 < live;) {   // one traceback per output count
-                const int n = g[order[i0]].n_out;
-                int i1 = i0;
-                while (i1 < live && g[order[i1]].n_out == n) ++i1;
-                launch_beam_traceback(beam, i1 - i0, W, n, out_ld, d_nbest_ids + off, d_nbest_scores, d_out,
-                                      top_k > 0 ? d_top_ids : nullptr, d_top_lp, st, i0, W);
-                off += (i1 - i0) * W * n;
-                i0 = i1;
-            }
+        if (W > 1) {
+            std::vector<int> n_sorted(live);
+            for (int i = 0; i < live; ++i) n_sorted[i] = g[order[i]].n_out;
+            sel.traceback(*this, n_sorted.data(), live, W);
+        }
     } else {
         CUDA_OK(cudaEventRecord(ev[4], st));
     }
     CUDA_OK(cudaEventRecord(ev[3], st));
 
-    if (W > 1 && live < b)   // a stream without output has no hypotheses: scores 0
-        CUDA_OK(cudaMemsetAsync(d_nbest_scores + live * W, 0, sizeof(double) * (b - live) * W, st));
+    if (W > 1 && live < b) sel.zero_nbest_scores(live, b, st);   // a stream without output has no hypotheses
 
     // ids back in the caller's stream order: stream s's outputs are in the row of its rank 0 beam, row0[s]
     std::vector<int> host((size_t)live * W * out_ld);
@@ -1064,18 +927,8 @@ void Session::transcribe_ragged(const float *samples, const size_t *lens, int b,
     size_t total = 0;
     for (int s = 0; s < b; total += g[s].n_out, ++s)
         for (int i = 0; i < g[s].n_out; ++i) out_ids[total + i] = host[(size_t)row0[s] * out_ld + i];
-    // scores and n-best stay on the device: the tracebacks packed sorted stream i's W hypotheses after those of sorted
-    // stream i - 1, and its W scores at i * W
-    scores_k = top_k;
-    nbest_w = W > 1 ? W : 0;
-    scores_n = nbest_n = (int)total;
-    score_spans.resize(b);
-    nbest_spans.resize(b);
-    for (size_t i = 0, off = 0; i < (size_t)b; off += (size_t)W * g[order[i]].n_out, ++i) {
-        const int s = order[i];
-        score_spans[s] = {row0[s], 0, g[s].n_out};
-        nbest_spans[s] = {off, (int)i * W, g[s].n_out};
-    }
+    // scores and n-best stay on the device, sorted stream i's in row i * W and at the traceback's i-th list
+    sel.record_transcribe(b, order.data(), n_out, W, true);
     // the cache holds streams of different lengths (and perhaps beams): the incremental API starts over
     reset();
     CUDA_OK(cudaStreamSynchronize(st));

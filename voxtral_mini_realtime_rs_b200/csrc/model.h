@@ -15,6 +15,7 @@
 #include "encoder.h"
 #include "kernels.h"
 #include "kv_cache.h"
+#include "token_select.h"
 
 namespace vox {
 
@@ -147,54 +148,13 @@ struct Session {
     int *d_pos = nullptr, *d_outpos = nullptr, *d_tok = nullptr, *d_ids = nullptr, *d_out = nullptr;
     int out_ld = 0;     // row pitch of d_out and of the per-output buffers: kv.capacity()
     int cache_len = 0;  // host mirror of d_pos[] (all rows equal) for the incremental API
-    // token confidences (vox_session_set_top_k): 0 = off (no launch, no memory).  k > 0: every prefill and decode step
-    // ends with launch_token_scores over its rows into [max_batch][out_ld][TOPK_MAX] ids / log-probabilities, allocated
-    // by the first set_top_k(k > 0)
-    int top_k = 0;
-    int *d_top_ids = nullptr;
-    float *d_top_lp = nullptr;
-    ScoreWork score_work;
-    void set_top_k(int k);
-    void alloc_scores();        // the score buffers above (first use)
-    // launch over rows [0, B) of the step that just ran at k = max(top_k, beam width when it is > 1); no-op at 0
-    void token_scores(int B);
-    // beam search (vox_session_set_beam): beam_w beams per stream for the transcribe calls; 1 = greedy (no launch, no
-    // memory).  A call over b streams at W > 1 runs rows w * b + s (beam w of stream s; kernels.h BeamWork), allocated
-    // with the n-best results by the first set_beam(W > 1).
-    int beam_w = 1;
     // the stream of each decoder row while a transcribe call runs whose rows are not its streams in order (beams, a
     // ragged call's sorted streams), or the slot of each row of a stream pool's launch; empty: row r belongs to stream r
     std::vector<int> row_streams;
-    BeamWork beam;
-    int *d_nbest_ids = nullptr;     // every stream's [W][n] ids of the last transcribe, at NbestSpan::ids
-    double *d_nbest_scores = nullptr;
-    void set_beam(int w);
-    void beam_start(int b);         // after the prefill of rows [0, b): start every beam row there, select position 0
-    void beam_step(int b, int n_live);   // selection + KV fork after a step over the b * beam_w rows
-    // phrase boosting (vox_session_set_bias): per-stream lists and histories at fixed offsets (kernels.h BiasLists),
-    // allocated by the first non-empty list, with the stream of each row (bind_rows fills it once they exist).  While
-    // some stream has a list, every prefill and decode step ends with one launch_bias_select over its rows.
-    BiasLists bias;
-    std::vector<int> bias_n;        // phrases per stream
-    int *d_row_stream = nullptr;    // [max_batch]
-    bool bias_on() const { return std::any_of(bias_n.begin(), bias_n.end(), [](int n) { return n > 0; }); }
-    // stream's list (-1: every stream's) := the n phrases of ids / lens / boosts (vox_session_set_bias), its history
-    // cleared; every argument is checked before anything changes
+    // token scores, beam search, phrase boosting and the record of the last call's results (token_select.h)
+    TokenSelect sel;
+    // sel.set_bias, and a new binding of rows once it has created the row table
     void set_bias(int stream, const int32_t *ids, const int32_t *lens, const float *boosts, int n);
-    void clear_bias_history(int stream);   // -1: every stream's; on st
-    void bias_select(int B);               // rows [0, B) of the step that just ran; no-op while no stream has a list
-    void check_beam_bias() const;          // a beam transcribe call with a list set is refused
-    // Where the results of the last call are, per stream in the caller's order; the getters copy them from the device
-    // when asked (the buffers outlive reset()).  Token scores, of the last transcribe or incremental call: entries
-    // [pos0, pos0 + n) of row `row` of d_top_ids / d_top_lp, scored with k = scores_k (0: that call ran with scores
-    // off).  N-best lists, of the last transcribe: W x n ids at d_nbest_ids + ids, W scores at d_nbest_scores + scores
-    // (nbest_w == 0: that transcribe ran greedy).  scores_n / nbest_n are the counts the getters report: per stream, or
-    // the total over the streams after vox_transcribe_pcm_ragged.
-    struct ScoreSpan { int row, pos0, n; };
-    struct NbestSpan { size_t ids; int scores, n; };
-    std::vector<ScoreSpan> score_spans;
-    std::vector<NbestSpan> nbest_spans;
-    int scores_k = 0, scores_n = 0, nbest_w = 0, nbest_n = 0;
     // host mirror of d_outpos[] (the stream pool's session aside): outputs per row since reset (incremental calls /
     // transcribe)
     std::vector<int> out_rows;
@@ -258,8 +218,9 @@ struct Session {
     void step_incremental(int b, int M, const int *ids_host, bool add_audio);
     void check_batch(int b) const;
     void check_ids(const int32_t *ids, size_t n) const;
-    // encodes the B streams of T mel frames in enc.mel_tm, then runs prefill + loop; returns tokens per stream
-    int transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids, vox_timings *tm);
+    // encodes the B streams of T mel frames in enc.mel_tm, then runs prefill + loop; returns tokens per stream.  `total`:
+    // the getters report the counts over all streams (vox_transcribe_pcm_ragged at equal lengths)
+    int transcribe_from_mel(int B, int T, int32_t *out_ids, size_t cap_ids, vox_timings *tm, bool total = false);
     // vox_transcribe_pcm_ragged after its argument checks: b streams of lens[s] host samples, one after the other;
     // n_out[s] ids of stream s after those of stream s - 1 in out_ids.  Records ev[0..4] like the other transcribe calls.
     void transcribe_ragged(const float *samples, const size_t *lens, int b, int normalize, int32_t *out_ids,

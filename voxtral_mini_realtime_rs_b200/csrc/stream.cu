@@ -241,7 +241,7 @@ int StreamPool::open() {
             CUDA_OK(cudaSetDevice(m->device));
             CUDA_OK(cudaMemsetAsync(pcm + (size_t)i * cap_samples, 0, sizeof(float) * cap_samples, s->st));
             s->set_stream_delay(i, kDefaultDelay);   // a reused slot does not inherit the previous session's delay ...
-            if (s->bias_n[i] > 0) s->set_bias(i, nullptr, nullptr, nullptr, 0);   // ... or its phrase list
+            if (s->sel.bias_n[i] > 0) s->set_bias(i, nullptr, nullptr, nullptr, 0);   // ... or its phrase list
             return i;
         }
     fail(VOX_ECAPACITY, fmt("all %d stream sessions are in use", max_sessions));
@@ -300,12 +300,12 @@ void StreamPool::close(int id) {
 void StreamPool::set_top_k(int k) {
     for (int i = 0; i < max_sessions; ++i)
         VOX_CHECK(!slots[i].open, VOX_EINVAL, "top_k of a stream pool can only change while no session is open (session %d is)", i);
-    s->set_top_k(k);
+    s->sel.set_top_k(k);
 }
 
 size_t StreamPool::poll(int id, int32_t *ids, int32_t *top_ids, float *top_lp, size_t cap, bool *done) {
     Slot &sl = slot(id);
-    const size_t n = std::min(cap, sl.ids.size()), nk = n * (size_t)s->top_k;
+    const size_t n = std::min(cap, sl.ids.size()), nk = n * (size_t)s->sel.top_k;
     if (n) memcpy(ids, sl.ids.data(), sizeof(int32_t) * n);
     if (nk && top_ids) memcpy(top_ids, sl.top_ids.data(), sizeof(int32_t) * nk);
     if (nk && top_lp) memcpy(top_lp, sl.top_lp.data(), sizeof(float) * nk);
@@ -448,15 +448,15 @@ void StreamPool::tick(vox_stream_stats *st_out) {
             s->kv.reserve(id, P + 1);
             if (unbounded) fill_rope(dec_rope_cos, dec_rope_sin, c.dec_head_dim, kDecRopeRing, 0, 0, P);
             upload_rows({id}, false);
-            s->clear_bias_history(id);   // the slot's decoder cache starts empty
+            s->sel.clear_bias_history(id, s->st);   // the slot's decoder cache starts empty
             std::vector<int> prefix((size_t)P, 32);
             prefix[0] = 1;
             s->prefill(1, P, prefix.data(), true);
             int tok = 0;
-            std::vector<int32_t> top((size_t)s->top_k);
-            std::vector<float> lp((size_t)s->top_k);
+            std::vector<int32_t> top((size_t)s->sel.top_k);
+            std::vector<float> lp((size_t)s->sel.top_k);
             CUDA_OK(cudaMemcpyAsync(&tok, s->d_tok, sizeof(int), cudaMemcpyDeviceToHost, s->st));
-            fetch_scores(1, top.data(), lp.data());
+            s->sel.fetch_rows(1, top.data(), lp.data(), s->st);
             CUDA_OK(cudaStreamSynchronize(s->st));
             sl.last_tok = tok;
             sl.ids.push_back(tok);
@@ -486,19 +486,19 @@ void StreamPool::tick(vox_stream_stats *st_out) {
                 s->kv.reserve(id, slots[id].pos + 1);
                 if (unbounded) fill_rope(dec_rope_cos, dec_rope_sin, c.dec_head_dim, kDecRopeRing, 0, slots[id].pos, 1);
             }
-            upload_rows(rows, true);
+            upload_rows(rows, true);   // every row's output position starts at 0: its token and scores land there
             s->decode_step((int)rows.size(), true);
             std::vector<int> toks(rows.size());
-            std::vector<int32_t> top(rows.size() * s->top_k);
-            std::vector<float> lp(rows.size() * s->top_k);
+            std::vector<int32_t> top(rows.size() * s->sel.top_k);
+            std::vector<float> lp(rows.size() * s->sel.top_k);
             CUDA_OK(cudaMemcpyAsync(toks.data(), s->d_tok, sizeof(int) * rows.size(), cudaMemcpyDeviceToHost, s->st));
-            fetch_scores((int)rows.size(), top.data(), lp.data());
+            s->sel.fetch_rows((int)rows.size(), top.data(), lp.data(), s->st);
             CUDA_OK(cudaStreamSynchronize(s->st));
             for (size_t i = 0; i < rows.size(); ++i) {
                 Slot &sl = slots[rows[i]];
                 sl.last_tok = toks[i];
                 sl.ids.push_back(toks[i]);
-                append_scores(sl, top.data() + i * s->top_k, lp.data() + i * s->top_k);
+                append_scores(sl, top.data() + i * s->sel.top_k, lp.data() + i * s->sel.top_k);
                 sl.n_ids += 1;
                 sl.pos += 1;
             }
@@ -608,20 +608,9 @@ void StreamPool::session_info(int id, struct vox_stream_session_info *out) {
     out->kv_pages = s->kv.pages(id);
 }
 
-// upload_rows resets every row's output position before a step, so its token and scores sit at position 0 of the row
-void StreamPool::fetch_scores(int n, int32_t *top_ids, float *top_lp) {
-    const int k = s->top_k;
-    if (k == 0) return;
-    const size_t row = (size_t)s->out_ld * TOPK_MAX;
-    CUDA_OK(cudaMemcpy2DAsync(top_ids, sizeof(int32_t) * k, s->d_top_ids, sizeof(int32_t) * row, sizeof(int32_t) * k, n,
-                              cudaMemcpyDeviceToHost, s->st));
-    CUDA_OK(cudaMemcpy2DAsync(top_lp, sizeof(float) * k, s->d_top_lp, sizeof(float) * row, sizeof(float) * k, n,
-                              cudaMemcpyDeviceToHost, s->st));
-}
-
 void StreamPool::append_scores(Slot &sl, const int32_t *top_ids, const float *top_lp) {
-    sl.top_ids.insert(sl.top_ids.end(), top_ids, top_ids + s->top_k);
-    sl.top_lp.insert(sl.top_lp.end(), top_lp, top_lp + s->top_k);
+    sl.top_ids.insert(sl.top_ids.end(), top_ids, top_ids + s->sel.top_k);
+    sl.top_lp.insert(sl.top_lp.end(), top_lp, top_lp + s->sel.top_k);
 }
 
 // RoPE rows of positions [p0, p0 + n) into a ring table of `rows` rows starting at row `row0`: position p at row p % rows

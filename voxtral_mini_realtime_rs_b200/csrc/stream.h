@@ -27,7 +27,7 @@ struct StreamPool {
         int pos = 0;                              // decoder positions cached (0: prefill pending)
         int last_tok = 0;
         std::vector<int32_t> ids;                 // emitted ids not yet polled
-        std::vector<int32_t> top_ids;             // their scores, [ids.size()][s->top_k] (pool top_k > 0)
+        std::vector<int32_t> top_ids;             // their scores, [ids.size()][s->sel.top_k] (pool top_k > 0)
         std::vector<float> top_lp;
         int64_t n_ids = 0;                        // ids emitted (positions >= 38)
         size_t pcm0 = 0;                          // absolute sample / frame / row of each buffer's row 0
@@ -82,8 +82,6 @@ struct StreamPool {
     Slot &slot(int id);
     void encoder_rows(int R);
     void upload_rows(const std::vector<int> &rows, bool with_tokens);
-    // enqueues the copy of the last step's scores of rows [0, n) (position 0 of each) into [n][top_k] host arrays
-    void fetch_scores(int n, int32_t *top_ids, float *top_lp);
     void append_scores(Slot &sl, const int32_t *top_ids, const float *top_lp);
     int final_enc(const Slot &sl) const;
     void fill_rope(float *cos_d, float *sin_d, int hd, int rows, size_t row0, int64_t p0, int n);
