@@ -179,6 +179,45 @@ typedef struct vox_attn_args {
 } vox_attn_args;
 int32_t vox_attention(int32_t device, int32_t kernel, const vox_attn_args *args, void *stream);
 
+/* Decoder attention (model.rs:125-197, rope.rs:103-141, kv_cache.rs:116-142) over one layer's paged K/V cache.  Row
+ * r = bb * m + i (bb < b, i < m) is position pos[bb] + i of stream bb; its q of head hh, k and v of kv head g start at
+ * qkv + r * ld + hh * hd, + (h + g) * hd and + (h + hkv + g) * hd.  The call rotates q and k by the RoPE row of the
+ * position (row p of cos / sin [rope_rows][hd / 2], or p % rope_rows for a ring), appends k after RoPE and v to the
+ * cache at that position, and writes out + r * h * hd + hh * hd = softmax(scale q k^T) v over the keys
+ * max(0, p - window) .. p of kv head hh / (h / hkv).  All pointers are device pointers.
+ *   VOX_DEC_ATTN_FUSED   K5 (decode_attn.cu): one launch fused with RoPE and the append, m == 1; qkv is left unchanged;
+ *   VOX_DEC_ATTN_PREFILL K5 prefill (kernels.cu): dec_rope_append, which rotates q in place, then dec_attention.
+ * Cache: kv_dtype VOX_DTYPE_F32, VOX_DTYPE_F16 or VOX_DTYPE_KV_Q8, each value stored by the rule of
+ * vox_session_create_ex.  k_pool / v_pool are [pages][hkv] units of 16 positions: [16][hd] values, and for q8 [16][hd]
+ * int8 followed by [16][hd / 16] f16 scales.  Position p of stream bb is slot p % 16 of physical page
+ * page_table[bb * max_pages + p / 16], or with ring != 0 page_table[bb * max_pages + (p / 16) % max_pages], so that
+ * positions are unbounded.
+ * The named kernel runs and no other.  Refused with VOX_EINVAL (vox_last_error says why), before any launch: an unknown
+ * kernel or kv_dtype, a null pointer the kernel reads, b, m, h, hkv, hd, max_pages or rope_rows below 1, h % hkv != 0,
+ * ld < (h + 2 hkv) hd, a negative window; fused: m != 1 or a shape it has no instantiation for (hd 32, 64 or 128,
+ * h / hkv 1, 2 or 4), a ring with window >= 16 max_pages; prefill: hd not a multiple of 4 (16 for q8), shared memory
+ * 4 (h / hkv) (hd + 16 max_pages) above 200 KB, a ring with window + m > 16 max_pages; without a ring, a negative
+ * pos[bb] or pos[bb] + m above 16 max_pages or rope_rows (pos is downloaded to check). */
+#define VOX_DEC_ATTN_FUSED 0
+#define VOX_DEC_ATTN_PREFILL 1
+typedef struct vox_dec_attn_args {
+    float *qkv;                           /* [b * m][ld]; prefill rotates its q columns in place */
+    int32_t ld;
+    int32_t b, m, h, hkv, hd;
+    int32_t kv_dtype;
+    void *k_pool, *v_pool;
+    const int32_t *page_table;            /* [b][max_pages] */
+    int32_t max_pages;
+    int32_t ring;
+    const int32_t *pos;                   /* [b] */
+    const float *cos, *sin;               /* [rope_rows][hd / 2] */
+    int32_t rope_rows;
+    int32_t window;
+    float scale;
+    float *out;                           /* [b * m][h * hd] */
+} vox_dec_attn_args;
+int32_t vox_dec_attention(int32_t device, int32_t kernel, const vox_dec_attn_args *args, void *stream);
+
 /* kernel selection of the operator seam (bit mask, default 0): bit 0 = SIMT warp-reduce matvec instead of
  * the tensor-core-assisted one (M <= 8); bit 1 = SIMT tiled GEMM instead of the wgmma GEMM (M > 8).
  * All implement the same contract; exposed for A/B measurement and parity tests. */

@@ -16,7 +16,7 @@ import of the test oracle -- a missing library or missing GPU raises.
 """
 from .api import (  # noqa: F401
     VoxtralError, lib, lib_path, device_count,
-    GgufReader, Q4ModelLoader, Q4VoxtralModel, Q4Tensor, Q4Linear, q4_matmul, q4_linear, attention,
+    GgufReader, Q4ModelLoader, Q4VoxtralModel, Q4Tensor, Q4Linear, q4_matmul, q4_linear, attention, dec_attention,
     MelSpectrogram, PadConfig, pad_audio, peak_normalize, chunk_audio, needs_chunking, stream_progress,
     stream_n_out, frames_n_out, join_chunk_texts,
     TimeEmbedding, VoxtralTokenizer, Timings, DeviceBuffer, PinnedArray, q4_matmul_bench, StreamingPool,
@@ -24,7 +24,7 @@ from .api import (  # noqa: F401
 
 __all__ = [
     "VoxtralError", "lib", "lib_path", "device_count", "GgufReader", "Q4ModelLoader", "Q4VoxtralModel", "Q4Tensor",
-    "Q4Linear", "q4_matmul", "q4_linear", "attention", "MelSpectrogram", "PadConfig", "pad_audio", "peak_normalize",
+    "Q4Linear", "q4_matmul", "q4_linear", "attention", "dec_attention", "MelSpectrogram", "PadConfig", "pad_audio", "peak_normalize",
     "chunk_audio", "needs_chunking", "stream_progress", "stream_n_out", "frames_n_out", "join_chunk_texts",
     "TimeEmbedding", "VoxtralTokenizer", "Timings", "DeviceBuffer", "q4_matmul_bench", "PinnedArray", "StreamingPool",
 ]

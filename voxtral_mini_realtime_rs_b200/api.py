@@ -104,6 +104,7 @@ _SIGS = {
                                   C.c_int32, _P, _P, _P]),
     "vox_q4_tensor_free": (None, [_P]),
     "vox_attention": (C.c_int32, [C.c_int32, C.c_int32, _P, _P]),
+    "vox_dec_attention": (C.c_int32, [C.c_int32, C.c_int32, _P, _P]),
     "vox_q4_set_matvec_mode": (C.c_int32, [C.c_int32]),
     "vox_dev_malloc": (C.c_int32, [C.c_int32, C.c_size_t, C.POINTER(_P)]),
     "vox_dev_free": (C.c_int32, [C.c_int32, _P]),
@@ -675,6 +676,49 @@ def attention(kernel: str, qkv, h: int, hd: int, window: int, scale: float, *, q
     _check(lib().vox_attention(device, ATTN_KERNELS[kernel], C.byref(a), None))
     _check(lib().vox_dev_sync(device))
     return out.to_numpy(np.float32, (out_rows, h * hd))
+
+
+DEC_ATTN_KERNELS = {"fused": 0, "prefill": 1}   # include/voxtral.h VOX_DEC_ATTN_*
+
+
+class _DecAttnArgs(C.Structure):
+    _fields_ = [("qkv", _P), ("ld", C.c_int32), ("b", C.c_int32), ("m", C.c_int32), ("h", C.c_int32),
+                ("hkv", C.c_int32), ("hd", C.c_int32), ("kv_dtype", C.c_int32), ("k_pool", _P), ("v_pool", _P),
+                ("page_table", _P), ("max_pages", C.c_int32), ("ring", C.c_int32), ("pos", _P), ("cos", _P),
+                ("sin", _P), ("rope_rows", C.c_int32), ("window", C.c_int32), ("scale", C.c_float), ("out", _P)]
+
+
+def dec_attention(kernel: str, qkv, *, b: int, m: int, h: int, hkv: int, hd: int, kv_dtype: str, k_pool, v_pool,
+                  page_table, pos, cos, sin, window: int, scale: float, ring: bool = False, out_rows: int | None = None,
+                  sentinel: float = float("nan"), device: int = 0):
+    """One decoder attention launch (vox_dec_attention) on host arrays, on the named kernel ("fused" or "prefill").
+
+    qkv [b * m, ld] f32; k_pool / v_pool: the cache's pages in their stored form (any dtype, uploaded as bytes);
+    page_table [b, max_pages] and pos [b] int32; cos / sin [rope_rows, hd / 2] f32.  out is an [out_rows, h * hd]
+    device buffer (default b * m rows) pre-filled with `sentinel`.  Returns (out, qkv, k_pool, v_pool), each as it is on
+    the device after the call, in the dtype and shape it was given."""
+    qkv = _f32(qkv)
+    keep = []
+
+    def up(a):
+        buf = DeviceBuffer.from_numpy(a, device)
+        keep.append(buf)
+        return buf
+
+    page_table = np.ascontiguousarray(page_table, np.int32)
+    k_pool, v_pool = np.ascontiguousarray(k_pool), np.ascontiguousarray(v_pool)
+    bufs = [up(qkv), up(k_pool), up(v_pool)]
+    out_rows = b * m if out_rows is None else out_rows
+    out = up(np.full((out_rows, h * hd), sentinel, np.float32))
+    a = _DecAttnArgs(qkv=bufs[0].ptr, ld=qkv.shape[1], b=b, m=m, h=h, hkv=hkv, hd=hd, kv_dtype=_kv_dtype(kv_dtype),
+                     k_pool=bufs[1].ptr, v_pool=bufs[2].ptr, page_table=up(page_table).ptr,
+                     max_pages=page_table.shape[1], ring=int(ring), pos=up(np.ascontiguousarray(pos, np.int32)).ptr,
+                     cos=up(_f32(cos)).ptr, sin=up(_f32(sin)).ptr, rope_rows=np.shape(cos)[0], window=window,
+                     scale=scale, out=out.ptr)
+    _check(lib().vox_dec_attention(device, DEC_ATTN_KERNELS[kernel], C.byref(a), None))
+    _check(lib().vox_dev_sync(device))
+    return (out.to_numpy(np.float32, (out_rows, h * hd)),
+            *(buf.to_numpy(arr.dtype, arr.shape) for buf, arr in zip(bufs, (qkv, k_pool, v_pool))))
 
 
 class Q4Linear:

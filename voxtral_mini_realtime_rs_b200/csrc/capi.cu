@@ -4,6 +4,7 @@
 #include <cuda_profiler_api.h>
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstring>
 #include <memory>
 #include <string>
@@ -466,6 +467,59 @@ int32_t vox_attention(int32_t device, int32_t kernel, const vox_attn_args *a, vo
     else
         (kernel == VOX_ATTN_ENC_TC ? launch_enc_attention_tc : launch_enc_attention)(
             a->qkv, a->out, a->b, a->s, a->h, hd, a->ld, a->q_off, a->k_off, a->v_off, a->window, a->scale, st, a->seg);
+    VOX_API_END
+}
+
+int32_t vox_dec_attention(int32_t device, int32_t kernel, const vox_dec_attn_args *a, void *stream) {
+    VOX_API_BEGIN
+    REQUIRE(a);
+    VOX_CHECK(kernel == VOX_DEC_ATTN_FUSED || kernel == VOX_DEC_ATTN_PREFILL, VOX_EINVAL,
+              "dec_attention: kernel %d is not one of 0..1", kernel);
+    VOX_CHECK(a->kv_dtype == VOX_DTYPE_F32 || a->kv_dtype == VOX_DTYPE_F16 || a->kv_dtype == VOX_DTYPE_KV_Q8, VOX_EINVAL,
+              "dec_attention: kv_dtype %d is not f32, f16 or q8", a->kv_dtype);
+    VOX_CHECK(a->qkv && a->k_pool && a->v_pool && a->page_table && a->pos && a->cos && a->sin && a->out, VOX_EINVAL,
+              "dec_attention: qkv, k_pool, v_pool, page_table, pos, cos, sin and out are required");
+    VOX_CHECK(a->b >= 1 && a->m >= 1 && a->h >= 1 && a->hkv >= 1 && a->hd >= 1 && a->max_pages >= 1 && a->rope_rows >= 1,
+              VOX_EINVAL, "dec_attention: b=%d, m=%d, h=%d, hkv=%d, hd=%d, max_pages=%d and rope_rows=%d must be positive",
+              a->b, a->m, a->h, a->hkv, a->hd, a->max_pages, a->rope_rows);
+    VOX_CHECK(a->h % a->hkv == 0, VOX_EINVAL, "dec_attention: h=%d is not a multiple of hkv=%d", a->h, a->hkv);
+    VOX_CHECK((int64_t)a->ld >= (int64_t)(a->h + 2 * a->hkv) * a->hd, VOX_EINVAL, "dec_attention: ld=%d < (h + 2 hkv) hd=%d",
+              a->ld, (a->h + 2 * a->hkv) * a->hd);
+    VOX_CHECK(a->window >= 0, VOX_EINVAL, "dec_attention: window=%d is negative", a->window);
+    const bool fused = kernel == VOX_DEC_ATTN_FUSED;
+    if (fused) {
+        VOX_CHECK(a->m == 1, VOX_EINVAL, "dec_attention: the fused kernel takes m = 1, not %d", a->m);
+        VOX_CHECK(dec_attn_fused_supported(a->h, a->hkv, a->hd), VOX_EINVAL,
+                  "dec_attention: the fused kernel has no instantiation for h=%d, hkv=%d, hd=%d", a->h, a->hkv, a->hd);
+    }
+    KvView kv;
+    const KvType type = a->kv_dtype == VOX_DTYPE_F16 ? KvType::F16 : (a->kv_dtype == VOX_DTYPE_KV_Q8 ? KvType::Q8 : KvType::F32);
+    kv.k = kv_pool(a->k_pool, type);
+    kv.v = kv_pool(a->v_pool, type);
+    kv.page_table = a->page_table;
+    kv.max_pages = a->max_pages;
+    kv.ring = a->ring != 0;
+    kv.type = type;
+    kv.pos = a->pos;
+    const RopeView rope{a->cos, a->sin, a->rope_rows};
+    require_device(device);
+    if (!kv.ring) {
+        // the kernels skip a row past the capacity and leave its output as it was
+        std::vector<int32_t> pos(a->b);
+        CUDA_OK(cudaMemcpy(pos.data(), a->pos, sizeof(int32_t) * a->b, cudaMemcpyDeviceToHost));
+        for (int bb = 0; bb < a->b; ++bb)
+            VOX_CHECK(pos[bb] >= 0 && (int64_t)pos[bb] + a->m <= std::min(kv.max_seq(), a->rope_rows), VOX_EINVAL,
+                      "dec_attention: row %d at pos %d + m=%d runs past the capacity %d or rope_rows %d", bb, pos[bb], a->m,
+                      kv.max_seq(), a->rope_rows);
+    }
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (fused) {
+        launch_dec_attn_fused(a->qkv, a->b, a->ld, a->h, a->hkv, a->hd, kv, a->window, a->scale, rope, a->out, st);
+    } else {
+        dec_attention_check(a->m, a->h, a->hkv, a->hd, kv, a->window);
+        launch_dec_rope_append(a->qkv, a->b, a->m, a->ld, a->h, a->hkv, a->hd, kv, rope, st);
+        launch_dec_attention(a->qkv, a->b, a->m, a->ld, a->h, a->hkv, a->hd, kv, a->window, a->scale, a->out, st);
+    }
     VOX_API_END
 }
 

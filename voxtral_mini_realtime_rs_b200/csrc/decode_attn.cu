@@ -181,6 +181,10 @@ bool dec_attn_fused_supported(int H, int Hkv, int hd) {
 void launch_dec_attn_fused(float *qkv, int B, int ld, int H, int Hkv, int hd, const KvView &kv, int window, float scale,
                            const RopeView &rope, float *out, cudaStream_t st) {
     VOX_CHECK(dec_attn_fused_supported(H, Hkv, hd), VOX_EINVAL, "dec_attn_fused: unsupported shape");
+    // the key at pos - window must still be in the ring after the append at pos
+    if (kv.ring)
+        VOX_CHECK(window < kv.max_seq(), VOX_EINVAL, "dec_attn_fused: window %d does not fit the KV ring of %d", window,
+                  kv.max_seq());
     const int G = H / Hkv, dpl = hd / 32;
     dim3 grid(Hkv, B);
     if (kv.type == KvType::Q8) {

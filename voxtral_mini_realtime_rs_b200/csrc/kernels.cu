@@ -816,21 +816,30 @@ __global__ void dec_attention_kernel(const float *__restrict__ qkv, int M, int l
     }
 }
 
+void dec_attention_check(int M, int H, int Hkv, int hd, const KvView &kv, int window) {
+    const size_t smem = (size_t)(H / Hkv) * (hd + kv.max_seq()) * sizeof(float);
+    VOX_CHECK(smem <= 200 * 1024, VOX_EINVAL, "dec_attention: max_seq %d too large for the v1 kernel", kv.max_seq());
+    VOX_CHECK(hd % (kv.type == KvType::Q8 ? KV_Q8_BLOCK : 4) == 0, VOX_EINVAL,
+              "dec_attention: head_dim %d is not a multiple of %d", hd, kv.type == KvType::Q8 ? KV_Q8_BLOCK : 4);
+    // all M rows are appended before any row reads: row 0's oldest key must outlive the append of row M - 1
+    if (kv.ring)
+        VOX_CHECK(window + M <= kv.max_seq(), VOX_EINVAL, "dec_attention: window %d + %d rows does not fit the KV ring of %d",
+                  window, M, kv.max_seq());
+}
+
 void launch_dec_attention(const float *qkv, int B, int M, int ld, int H, int Hkv, int hd, const KvView &kv, int window,
                           float scale, float *out, cudaStream_t st) {
     const int G = H / Hkv;
     dim3 grid(Hkv, M, B);
     const size_t smem = (size_t)G * (hd + kv.max_seq()) * sizeof(float);
-    VOX_CHECK(smem <= 200 * 1024, VOX_EINVAL, "dec_attention: max_seq %d too large for the v1 kernel", kv.max_seq());
+    dec_attention_check(M, H, Hkv, hd, kv, window);
     static SmemAttr attr, attr_ring, attr16, attr_ring16, attr8, attr_ring8;
-    if (kv.ring) VOX_CHECK(window < kv.max_seq(), VOX_EINVAL, "dec_attention: window %d does not fit the KV ring", window);
     auto go = [&](auto kernel, SmemAttr &a) {
         if (smem > 48 * 1024) smem_attr_check(ensure_dyn_smem(kernel, smem, a), "dec_attention");
         kernel<<<grid, 32 * G, smem, st>>>(qkv, M, ld, H, Hkv, hd, kv, window, scale, out);
     };
     const bool f16 = kv.type == KvType::F16;
     if (kv.type == KvType::Q8) {
-        VOX_CHECK(hd % KV_Q8_BLOCK == 0, VOX_EINVAL, "dec_attention: head_dim %d is not a multiple of %d", hd, KV_Q8_BLOCK);
         if (kv.ring) go(dec_attention_kernel<true, int8_t>, attr_ring8);
         else go(dec_attention_kernel<false, int8_t>, attr8);
     } else if (kv.ring && f16) go(dec_attention_kernel<true, __half>, attr_ring16);

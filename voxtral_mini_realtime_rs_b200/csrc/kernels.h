@@ -352,7 +352,10 @@ void launch_enc_attention_tc(const float *qkv, float *out, int B, int S, int H, 
 // qkv rows [B*M][ld].
 void launch_dec_rope_append(float *qkv, int B, int M, int ld, int H, int Hkv, int hd, const KvView &kv,
                             const RopeView &rope, cudaStream_t st);
-// decoder GQA attention over the cache (keys 0..kv.pos[b]+i, window), out [B*M][H*hd].
+// decoder GQA attention over the cache (keys 0..kv.pos[b]+i, window), out [B*M][H*hd].  dec_attention_check throws
+// what launch_dec_attention refuses (shared memory, head_dim, a ring that cannot hold window + M positions), so a caller
+// can refuse before it launches dec_rope_append.
+void dec_attention_check(int M, int H, int Hkv, int hd, const KvView &kv, int window);
 void launch_dec_attention(const float *qkv, int B, int M, int ld, int H, int Hkv, int hd, const KvView &kv, int window,
                           float scale, float *out, cudaStream_t st);
 // x[r][:] = audio[audio_off[b] + (pos[b] + i)*K ..] + dequant(E[ids[r]]),  r = b*M + i; without audio (nullptr) the
